@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — wake_up latency (s) and H2D GB/s of the sleep/wake weight-movement path on B200.
+"""bench.py — wake_up latency (s) and H2D GB/s of the sleep/wake weight-movement path on H100.
 
   python bench.py [--gpus N] [--steps K] [--warmup W]            this repo's engine (C-ABI libfma_b200.so)
   python bench.py --impl reference [--gpus N] ...                the reference data path: vLLM's OWN
@@ -10,7 +10,7 @@
               --master-port P bench.py --gpus N --steps K --warmup W
 
 A "step" is one level-1 sleep -> wake_up round trip of one rank's model shard (weights offloaded,
-kv_cache discarded and remapped): BASELINE.json config[1] (Llama-3-8B, 1xB200, host-DRAM tier) at N=1,
+kv_cache discarded and remapped): BASELINE.json config[1] (Llama-3-8B, 1xH100, host-DRAM tier) at N=1,
 config[2] (Llama-3-70B TP=8 per-rank shard, every rank concurrently, no collective) at N>1.
 
   value          aggregate wake H2D GB/s = N*W / max_ranks(mean device time of the wake pipeline, CUDA events)
@@ -28,9 +28,13 @@ config[2] (Llama-3-70B TP=8 per-rank shard, every rank concurrently, no collecti
   --incremental 1   sleeps whose weights still match the image in the host store release the device side without a copy
   --extras packed,incremental   (any N, opt-in) after the main line, on the same engines: bf16 refill, PACKED cycles, then
                     INCREMENTAL cycles, aggregated like the main line (reported under `extras`)
+  --dump-outputs DIR   after the timed steps, write what the last wake handed back to the caller as .npy files (rank r of N > 1
+                    prefixes rank<r>_): weights_digest.npy (float64 [n, 2]: high and low 32 bits of each weight segment's K3 digest),
+                    weights_sample.npy (float32 [k, 4096]: the bytes of k seeded 4 KiB windows of the weights) and
+                    weights_sample_index.npy (float64 [k, 2]: segment index and byte offset of each window)
 
 Synthetic data: counter-based splitmix64 bytes (seed 1234 + rank); the working set (>= 15 GiB per rank) is far
-larger than the 126 MB L2, so no L2 flush is needed between iterations.
+larger than the 50 MB L2, so no L2 flush is needed between iterations.
 """
 from __future__ import annotations
 
@@ -48,9 +52,9 @@ if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
 GiB = 1 << 30
-PCIE_GEN5_X16_GBS = 64.0      # north_star's PCIe roofline, per direction per GPU
-NVLINK5_GBS = 900.0           # north_star's NVLink roofline, per direction per GPU
-HBM_FALLBACK_GBS = 6650.0     # /opt/skills/guides/B200_PROFILING.md fallback
+PCIE_GEN5_X16_GBS = 64.0      # PCIe Gen5 x16, per direction per GPU
+NVLINK4_GBS = 450.0           # H100 SXM NVLink 4: 900 GB/s in both directions together, per GPU
+HBM_DATASHEET_GBS = 3350.0    # H100 SXM HBM3 (NVIDIA data sheet)
 
 
 def hbm_peak() -> tuple[float, str]:
@@ -58,7 +62,7 @@ def hbm_peak() -> tuple[float, str]:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return HBM_FALLBACK_GBS, "fallback (B200_PROFILING.md)"
+        return HBM_DATASHEET_GBS, "fallback (H100 SXM data sheet)"
 
 
 def workload_for(n_gpus: int, override: str | None) -> str:
@@ -68,7 +72,7 @@ def workload_for(n_gpus: int, override: str | None) -> str:
 
 
 # --------------------------------------------------------------------------------------------------
-# clocks: sample nvidia-smi DURING the timed region (B200_PROFILING.md recipe)
+# clocks: sample nvidia-smi DURING the timed region
 # --------------------------------------------------------------------------------------------------
 class ClockSampler:
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
@@ -120,6 +124,37 @@ class ClockSampler:
         return {"sm_mhz": statistics.median(sm) if sm else None, "sm_max_mhz": max(mx) if mx else None,
                 "power_w_max": max(power) if power else None, "samples": len(sm), "reasons": sorted(reasons),
                 "note": "PCIe-bound path: SMs only run the short K1/K2 page copies, so SM clocks are not the limiter"}
+
+
+def gpu_identity(index: int) -> dict:
+    """Name and power limit of the card the numbers were measured on (a power-capped card runs lower clocks)."""
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader,nounits", "-i", str(index)],
+                             capture_output=True, text=True, timeout=30).stdout.strip().split(",")
+        return {"name": out[0].strip(), "power_limit_w": float(out[1])}
+    except Exception:
+        return {"name": None, "power_limit_w": None}
+
+
+def dump_outputs(eng, table, out_dir: str, prefix: str, windows_per_segment: int = 4, window: int = 4096) -> None:
+    """What the last wake handed back to the caller: the K3 digest of every weight segment (all of its bytes) and the bytes
+    of `windows_per_segment` 4 KiB windows per weight segment at offsets drawn from a fixed seed (the same for every run
+    with the same table), as float32 / float64 arrays."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    weights = [i for i, s in enumerate(table) if s.tag == "weights"]
+    dg = eng.digest_all(["weights"])
+    np.save(os.path.join(out_dir, prefix + "weights_digest.npy"),
+            np.array([[dg[i] >> 32, dg[i] & 0xFFFFFFFF] for i in weights], dtype=np.float64))
+    rng = np.random.default_rng(20240601)
+    rows, index = [], []
+    for i in weights:
+        for o in sorted(rng.choice(table[i].bytes // window, size=min(windows_per_segment, table[i].bytes // window), replace=False)):
+            rows.append(np.frombuffer(eng.read(i, window, offset=int(o) * window), dtype=np.uint8))
+            index.append((i, int(o) * window))
+    np.save(os.path.join(out_dir, prefix + "weights_sample.npy"), np.stack(rows).astype(np.float32))
+    np.save(os.path.join(out_dir, prefix + "weights_sample_index.npy"), np.array(index, dtype=np.float64))
 
 
 # --------------------------------------------------------------------------------------------------
@@ -208,6 +243,8 @@ def run_ours(args) -> None:
 
     after = eng.digest_all(["weights"])
     bit_exact = after == before
+    if args.dump_outputs:
+        dump_outputs(eng, table, args.dump_outputs, f"rank{rank}_" if world > 1 else "")
 
     mean = lambda xs: sum(xs) / len(xs)
     k2_s = sum(r[1]["kernel_seconds"] for r in rows); k2_b = sum(r[1]["kernel_bytes"] for r in rows)
@@ -260,21 +297,9 @@ def run_ours(args) -> None:
         peak, peak_src = hbm_peak()
         achieved = (k2_b / k2_s / 1e9) if k2_s > 0 else None
         bytes_per_launch = int(k2_b / k2_n) if k2_n else 0
-        traffic, traffic_src = None, None
-        tp = os.path.join(ROOT, "profiles", "k2_traffic.json")
-        if os.path.exists(tp):      # NOT measured in this run: the ncu --set full capture of the same kernel, kept under profiles/
-            try:
-                tj = json.load(open(tp))
-                if abs(tj.get("algorithmic_bytes_per_launch", 0) - bytes_per_launch) <= 0.02 * max(bytes_per_launch, 1):
-                    traffic = tj.get("dram_bytes_per_launch")
-                    traffic_src = "profiles/k2_traffic.json: dram__bytes_read+write of one launch of this size under ncu --set full (kept capture, profiles/k2_full_r2.md; a constant, not measured in this run)"
-                else:
-                    traffic_src = "no ncu capture for this launch size (profiles/k2_traffic.json is for 512 MiB slots)"
-            except Exception:
-                traffic = None
         e2e_gbs = W_total / wake_wall_med / 1e9
         e2e_mean_gbs = W_total / wake_wall_m / 1e9
-        link_peak = PCIE_GEN5_X16_GBS if tier == L.FMA_TIER_HOST else NVLINK5_GBS
+        link_peak = PCIE_GEN5_X16_GBS if tier == L.FMA_TIER_HOST else NVLINK4_GBS
         out = {
             "metric": "wake_h2d_gbs", "value": round(W_total / wake_dev_med / 1e9, 3), "unit": "GB/s",
             "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
@@ -300,19 +325,19 @@ def run_ours(args) -> None:
             "gpu_launches": launches_total,
             "roofline": {"bound": "hbm", "kernel": "fma_k_page_copy_tma (K2 scatter, wake)" if args.kernel == "tma" else "fma_k_page_copy_ldg (K2)",
                          "achieved": round(achieved, 1) if achieved else None, "peak": peak, "unit": "GB/s",
-                         "frac": round(achieved / peak, 4) if achieved else None, "traffic": traffic, "traffic_source": traffic_src,
+                         "frac": round(achieved / peak, 4) if achieved else None, "traffic": None, "traffic_source": "not measured",
                          "launches": k2_n, "bytes_per_launch": bytes_per_launch,
                          "avg_launch_us": round(k2_s / k2_n * 1e6, 2) if k2_n else None, "peak_source": peak_src,
                          "k1_gather_achieved": round(k1_b / k1_s / 1e9, 1) if k1_s > 0 else None, "k1_launches": k1_n},
             "pcie" if tier == L.FMA_TIER_HOST else "nvlink": {
-                "bound": "pcie_gen5_x16" if tier == L.FMA_TIER_HOST else "nvlink5",
+                "bound": "pcie_gen5_x16" if tier == L.FMA_TIER_HOST else "nvlink4",
                 "achieved_per_gpu": round(e2e_gbs / world, 3), "device_timed_per_gpu": round(W_total / wake_dev_med / 1e9 / world, 3),
                 "peak": link_peak, "unit": "GB/s", "frac": round(e2e_gbs / world / link_peak, 4),
                 "naive_pinned_h2d_per_gpu": round(ceiling, 3) if ceiling else None,
                 "vs_naive_pinned_h2d": round(e2e_gbs / world / ceiling, 4) if ceiling else None,
                 "naive_note": "min over ranks of a plain 8 GiB cudaMemcpyAsync from a torch pin_memory buffer, all ranks at once "
                               "(no NUMA placement, best of 3): the box's sustained copy-engine rate on the slowest rank's link"},
-            "clocks": clocks,
+            "clocks": clocks, "gpu": gpu_identity(local_rank),
         }
         if peer:
             out["peer_tier"] = peer
@@ -347,7 +372,7 @@ def bench_config(args, workload: str, weight_bytes: int, n_segments: int, world:
             "contents": "splitmix64 bytes (incompressible)" if args.contents == "prng" else "bf16 U(-1e-3, 1e-3) (vLLM dummy weights)",
             "pack": packed, "incremental_sleep": bool(args.incremental),
             "phases": "executor semantics: every rank finishes sleeping before any rank wakes (host-side barrier between the phases)",
-            "l2": "working set >> 126 MB L2 (no flush needed)", "parallelism": f"{world} independent ranks"}
+            "l2": "working set >> 50 MB L2 (no flush needed)", "parallelism": f"{world} independent ranks"}
 
 
 def load_model(eng, W, model: str, kv_gib: float, seed: int):
@@ -363,7 +388,7 @@ def load_model(eng, W, model: str, kv_gib: float, seed: int):
 
 
 def measure_swap(args, L, W, cycles: int = 10) -> dict:
-    """BASELINE config 4: Llama-3-8B <-> Mistral-7B under one owner on one B200.  `fma_swap` = sleep(out) || wake(in): the D2H of
+    """BASELINE config 4: Llama-3-8B <-> Mistral-7B under one owner on one GPU.  `fma_swap` = sleep(out) || wake(in): the D2H of
     the outgoing model and the H2D of the incoming one use the two PCIe directions at once.  Beside it, the serial form (sleep,
     then wake: what two independent reconciles of the reference controller produce, SURVEY.md section 3.4).  Medians over `cycles`."""
     import fma_b200
@@ -390,7 +415,7 @@ def measure_swap(args, L, W, cycles: int = 10) -> dict:
         A.swap_out_for(B, ["weights"]); ok = ok and B.digest_all(["weights"]) == db
         A.close(); B.close()
         med = statistics.median
-        return {"models": f"{ma} ({wa / GiB:.2f} GiB) <-> {mb} ({wb / GiB:.2f} GiB), {args.extras_kv_gib:g} GiB kv_cache each, 1xB200, host tier",
+        return {"models": f"{ma} ({wa / GiB:.2f} GiB) <-> {mb} ({wb / GiB:.2f} GiB), {args.extras_kv_gib:g} GiB kv_cache each, 1 GPU, host tier",
                 "swap_s_median": round(med(swap), 4), "swap_s_min_max": [round(min(swap), 4), round(max(swap), 4)],
                 "serial_sleep_then_wake_s_median": round(med(serial), 4), "serial_s_min_max": [round(min(serial), 4), round(max(serial), 4)],
                 "speedup_vs_serial": round(med(serial) / med(swap), 3),
@@ -402,7 +427,7 @@ def measure_swap(args, L, W, cycles: int = 10) -> dict:
 
 def measure_multipath(args, L, W, cfg, workload: str, n_visible: int, cycles: int = 6) -> dict:
     """MULTI-PATH wake (fma_paths_set) at N=1 with idle peers on the box: the same table, host tier; helpers = GPUs 1..k lend their
-    PCIe links, K2 on GPU 0 gathers their staging slots over NVLink.  The single-link ceiling (55.6 GB/s measured) stops applying."""
+    PCIe links, K2 on GPU 0 gathers their staging slots over NVLink, so one link's ceiling stops applying."""
     import fma_b200
 
     try:
@@ -517,7 +542,7 @@ def measure_roundrobin(args, L, W, local_rank, rank, world, group, torch, rounds
         out = {"models": half, "model": f"{args.swap_models.split(',')[0]} ({w8 / GiB:.2f} GiB)", "placement": f"rank r < {half} parks on GPU r + {half}",
                "roundrobin_wake_s_median": round(med(single), 5), "roundrobin_wake_s_min_max": [round(min(single), 5), round(max(single), 5)],
                "roundrobin_gbs_e2e": round(w8 / med(single) / 1e9, 1), "roundrobin_gbs_device": round(w8 / med(single_dev) / 1e9, 1),
-               "frac_of_nvlink_900": round(w8 / med(single) / 1e9 / NVLINK5_GBS, 4), "wakes": len(single),
+               "frac_of_nvlink": round(w8 / med(single) / 1e9 / NVLINK4_GBS, 4), "wakes": len(single),
                "all_at_once_wake_s_median": round(med(together), 5), "all_at_once_aggregate_gbs": round(half * w8 / med(together) / 1e9, 1),
                "bit_exact": bool(ok)}
     except Exception as e:
@@ -720,7 +745,7 @@ def measure_peer(eng, L, Wb, local_rank, world, barrier, max_over_ranks, before,
         sleep_dev = max_over_ranks(mean([r[0]["sleep_copy_seconds"] for r in rows]))
         return {"wake_latency_s": round(wake_wall, 5), "wake_gbs_per_gpu_e2e": round(Wb / wake_wall / 1e9, 1),
                 "wake_gbs_per_gpu_device": round(Wb / wake_dev / 1e9, 1), "sleep_gbs_per_gpu_device": round(Wb / sleep_dev / 1e9, 1),
-                "frac_of_nvlink_900": round(Wb / wake_dev / 1e9 / NVLINK5_GBS, 4), "bit_exact": bool(ok),
+                "frac_of_nvlink": round(Wb / wake_dev / 1e9 / NVLINK4_GBS, 4), "bit_exact": bool(ok),
                 "placement": "rank r parks on GPU (r + N/2) % N"}
     except Exception as e:  # the peer tier is extra evidence; never fail the host-tier line because of it
         return {"error": str(e)[:200]}
@@ -934,6 +959,8 @@ def main() -> None:
     ap.add_argument("--scaling-workload", default="llama-3-70b-tp8", help="table of the scaling_base extra (= the N>1 workload)")
     ap.add_argument("--extras-kv-gib", type=float, default=16.0, help="kv_cache bytes per model in the swap / roundrobin extras")
     ap.add_argument("--timeline", default="", help="directory: every rank writes the per-phase timeline (fma_timeline) of its last timed sleep and wake there")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="after the timed steps, write the woken weights' digests and a seeded sample of their bytes to DIR/*.npy")
     ap.add_argument("--packed-child", action="store_true", help=argparse.SUPPRESS)
     args = ap.parse_args()
     if args.packed_child:

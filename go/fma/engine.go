@@ -1,4 +1,4 @@
-// Package fma is the cgo binding of the B200 sleep/wake weight-movement engine (include/fma_engine.h).
+// Package fma is the cgo binding of the H100 sleep/wake weight-movement engine (include/fma_engine.h).
 //
 // NOT COMPILED OR TESTED IN THIS REPOSITORY'S CI: the build image has no Go toolchain (SURVEY.md §0).  It is the
 // reference-side binding a maintainer of llm-d-fast-model-actuation would add for a Go-hosted engine owner

@@ -1,5 +1,5 @@
 /*
- * fma_engine.h — C-ABI of the B200-native sleep / wake / hot-swap weight-movement engine.
+ * fma_engine.h — C-ABI of the H100-native sleep / wake / hot-swap weight-movement engine.
  *
  * This is the drop-in boundary (SURVEY.md §8b, surface B3) for the ONE hot path of
  * llm-d-fast-model-actuation: moving an inference server's weight segments HBM -> host (or
@@ -51,7 +51,7 @@ extern "C" {
 
 /* ---- units ------------------------------------------------------------------------ */
 /* The engine's unit of placement is the 2 MiB VMM page (cuMemGetAllocationGranularity
- * minimum on B200).  Every segment handed out by my_malloc / fma_alloc is a whole number
+ * minimum on H100).  Every segment handed out by my_malloc / fma_alloc is a whole number
  * of pages, so the packed image of a sleeping model is a concatenation of pages and
  * gather / scatter are page-table driven (K1/K2, csrc/fma_kernels.cu).                  */
 #define FMA_PAGE_BYTES  ((size_t)2u << 20)
@@ -59,7 +59,7 @@ extern "C" {
 
 /* ---- tiers ------------------------------------------------------------------------ */
 #define FMA_TIER_HOST   0   /* pinned host-DRAM store over PCIe Gen5 (copy engines)      */
-#define FMA_TIER_PEER   1   /* peer-GPU HBM parking buffer over NVLink 5 / NVSwitch      */
+#define FMA_TIER_PEER   1   /* peer-GPU HBM parking buffer over NVLink / NVSwitch        */
 #define FMA_TIER_LOCAL  2   /* parking buffer in the SAME GPU's HBM (kernel roofline/test)*/
 
 /* ---- data-path modes (how bytes cross the link) ----------------------------------- */
@@ -235,7 +235,7 @@ FMA_API int  fma_peer_release(fma_engine_t* e);
  * restores the weights at PCIe speed instead of re-reading a checkpoint.  The fd may also be a regular FILE holding
  * the same bytes (Engine.image_save / image_load in the Python binding): if its mapping cannot be pinned in place the
  * image is copied once into an anonymous pinned store.  A PACKED image travels with its page table (descriptor v2).
- * Status: green on a B200 (in-process and cross-process, plain and PACKED: tests/test_gpu_parity.py, profiles/gpu_suite_all_gates_open_r2.log). */
+ * Tests: in-process and cross-process, plain and PACKED (tests/test_gpu_parity.py). */
 FMA_API int  fma_image_export(fma_engine_t* e, int* out_fd);          /* caller owns (closes) the returned fd          */
 /* flags: FMA_FLAG_VERIFY = "sleep by adoption": the engine holds the weights itself (another replica of the model the image
  * came from) and its device bytes must match the image's digests — then its device side is released and it shares that

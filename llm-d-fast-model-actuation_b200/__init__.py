@@ -1,4 +1,4 @@
-"""B200-native sleep / wake / hot-swap weight-movement engine (host-side Python mirror).
+"""H100-native sleep / wake / hot-swap weight-movement engine (host-side Python mirror).
 
 The directory name follows the repo layout contract; import it as ``fma_b200`` (the loader
 ``fma_b200.py`` at the repo root registers this directory under that name).

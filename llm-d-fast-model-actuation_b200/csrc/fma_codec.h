@@ -6,7 +6,7 @@
 // weights simply stays raw, so the round trip stays bit-identical to the reference's (SURVEY.md §8c invariant).
 //
 // This header is the single definition of the format's per-lane arithmetic.  It is compiled three ways: into the
-// sm_100a kernels K4/K5 (csrc/fma_pack_kernels.cu: one warp per tile, one lane per 8 values), into the host
+// sm_90a kernels K4/K5 (csrc/fma_pack_kernels.cu: one warp per tile, one lane per 8 values), into the host
 // simulation's stand-ins (tests/cpp/hostsim/hostsim_kernels.cpp: the same lane functions in a loop), and it is
 // restated independently, value by value, in oracle/fma_oracle.c (the checker).
 //

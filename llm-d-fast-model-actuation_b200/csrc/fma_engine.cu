@@ -1,4 +1,4 @@
-// fma_engine.cu — host side of the B200 sleep/wake weight-movement engine (C-ABI in
+// fma_engine.cu — host side of the H100 sleep/wake weight-movement engine (C-ABI in
 // include/fma_engine.h).  No kernels live here; see fma_kernels.cu.
 //
 // What it replaces in the reference's hot path (SURVEY.md §8a):
@@ -8,7 +8,7 @@
 //   a5 my_malloc/my_free/create_and_map/unmap_and_release (cumem_allocator.abi3.so, T3)
 //   a6 blocking cudaMemcpy       cuda_wrapper.py:168-173                  -> multi-stream async copy engines / K1,K2
 //
-// Design (B200-first, not a port):
+// Design (H100-first, not a port):
 //   * one Engine per GPU / process (rank); segments are CUDA-VMM ranges whose VA reservation
 //     outlives unmap so every tensor keeps its device address across sleep -> wake;
 //   * a sleeping model is a PACKED IMAGE: its offloaded segments concatenated page by page
@@ -123,7 +123,7 @@ CUmemAllocationProp device_prop(int device) {
 }
 
 // create + map + set access, then drop the handle: the physical memory stays alive until cuMemUnmap
-// (verified on B200, scripts/vmm_span_probe.py), which makes teardown a single driver call per range.
+// (scripts/vmm_span_probe.py checks this), which makes teardown a single driver call per range.
 int vmm_create_and_map(int device, CUdeviceptr va, size_t bytes) {
     CUmemAllocationProp prop = device_prop(device);
     CUmemGenericAllocationHandle h = 0;
@@ -263,9 +263,10 @@ int ensure_pack_bufs(fma_engine_t* e, size_t n_pages) {
     return FMA_OK;
 }
 
-// DMA chunk for DIRECT (round-robin over copy streams) and ring-slot size for STAGED.  Defaults come from the
-// sweeps in profiles/: H2D saturates from 32 MiB chunks; a K1/K2 launch issued while a copy engine is busy pays a
-// fixed ~25 us (H2D) / ~40 us (D2H) of launch latency, so slots of 512 MiB keep that under 15% of the launch.
+// DMA chunk for DIRECT (round-robin over copy streams) and ring-slot size for STAGED.  H2D over PCIe Gen5 saturates
+// well below 32 MiB per copy; a K1/K2 launch issued while a copy engine is busy pays a fixed launch latency of tens of
+// microseconds, which large (512 MiB) ring slots keep a small fraction of each launch (scripts/staged_sweep.py,
+// scripts/k_contention.py measure both).
 size_t direct_chunk(const fma_engine_t* e) {
     return e->cfg.chunk_bytes ? round_up((size_t)e->cfg.chunk_bytes, FMA_PAGE_BYTES) : ((size_t)32 << 20);
 }
@@ -284,7 +285,7 @@ void release_ring(fma_engine_t* e) {
 }
 
 // The HBM staging ring lives from the start of a wake to the end of the next sleep: a serving model keeps it
-// (1 GiB of 180 GB) so that /sleep needs no allocation, a SLEEPING model does not hold it (FMA_RING_PERSIST=1 keeps
+// (1 GiB of 80 GB) so that /sleep needs no allocation, a SLEEPING model does not hold it (FMA_RING_PERSIST=1 keeps
 // it, trading 1 GiB of a sleeper's HBM for one driver call less at wake).  It is freed at the END of sleep,
 // synchronously: on these shared hosts a cudaFree of 1 GiB takes anywhere from 0.8 ms to 300 ms (driver stalls), which
 // must never sit inside the wake latency — and freeing it from a background thread was measured to block the next
@@ -427,8 +428,8 @@ int host_store_reserve(fma_engine_t* e, size_t bytes) {
             madvise(p, bytes, MADV_HUGEPAGE);
             // MULTI-PATH wake configured (fma_paths_set): stripe the store over the NUMA nodes of the paths' GPUs in proportion
             // to the number of paths on each node, so that every path can pull chunks that are LOCAL to its GPU's socket.
-            // Measured on a B200 box whose helpers sat on the other socket: 3 helpers dragging a node-0 store across the
-            // interconnect got 26 GB/s each (78 GB/s together) instead of 55 (profiles/multipath_r2.md).
+            // Helpers on the other socket than a store they read from pull it across the socket interconnect and lose about
+            // half of their link rate.
             std::map<int, int> per_node;
             if (want_bind)
                 for (const WakePath& wp : e->paths)

@@ -61,8 +61,7 @@ bool pid_alive(int32_t pid) {
 
 void open_gate() {
     const char* on = getenv("FMA_VMM_GATE");
-    // On unless FMA_VMM_GATE=0.  A/B at N=8 on one lease (profiles/bench_n8_gate_v2_r2.json vs bench_n8_nogate_r2.json): host tier
-    // 433.3 vs 430.4 GB/s (every rank 323-326 ms under the gate), peer tier with all ranks waking at once 0.087 vs 0.120 s.
+    // On unless FMA_VMM_GATE=0 (the A/B switch: bench.py at N > 1 with and without it).
     if (on && *on && atoi(on) == 0) return;
     char name[128];
     const char* forced = getenv("FMA_VMM_GATE_NAME");

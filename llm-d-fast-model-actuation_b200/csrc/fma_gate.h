@@ -1,14 +1,14 @@
 // fma_gate.h — cross-process VMM gate (internal; host only).
 //
 // cuMemCreate / cuMemMap / cuMemSetAccess / cuMemUnmap of ALL processes on one host serialise inside the driver
-// (profiles/vmm_span_probe_r1.json), in arrival order.  When N ranks wake at once that order is wrong: the call that gates
+// (scripts/vmm_span_probe.py), in arrival order.  When N ranks wake at once that order is wrong: the call that gates
 // a rank's first H2D (its 1 GiB staging ring, then the first piece of its weights run) can queue behind another rank's
 // 32 GiB kv_cache remap, which nothing waits for.  The reference has the same property, only worse (three calls per
 // segment, cumem.py:240 -> create_and_map).  The gate is a priority lock in POSIX shared memory that every engine on the
 // host takes around its VMM calls: the driver serialises them anyway, so holding our own lock costs nothing and decides
 // the ORDER — class 0 (gates a first copy) before the weights pieces in round robin across ranks (class = piece index) before
-// remap-only runs (the whole copy time of slack) before sleep-side unmaps — and, measured at N=8 (profiles/wake_timeline_r2.md),
-// un-contended calls are 5-6x FASTER: a 2 GiB piece maps in 0.65 ms under the gate against 3-8 ms when eight ranks' calls collide.
+// remap-only runs (the whole copy time of slack) before sleep-side unmaps — and un-contended calls are faster than calls of
+// several ranks that collide in the driver (bench.py --timeline shows the per-call times).
 //
 // Failure model: everything is bounded.  A waiter gives up waiting for higher classes after `max_wait_s` and a lock that
 // cannot be had within 2 s is skipped (the driver's own lock still serialises), so a dead or wedged peer can delay a

@@ -192,7 +192,7 @@ constexpr int kMaxPaths = 8;
 
 // MULTI-PATH wake (fma_paths_set): one PCIe path into the waking GPU per entry.  Path 0 is the engine's own link; every other
 // path is an idle peer GPU whose copy engine pulls chunks of the host image over ITS x16 link into a small staging buffer in
-// ITS HBM, from where K2 on the waking GPU gathers them over NVLink / NVSwitch (900 GB/s >> k x 55 GB/s) straight into the
+// ITS HBM, from where K2 on the waking GPU gathers them over NVLink / NVSwitch (450 GB/s per direction on H100 >> k x ~55 GB/s) straight into the
 // destination pages.  A lone wake is then bounded by k links instead of one (DESIGN.md section 3).
 struct WakePath {
     int device = -1;                         // -1 for a REMOTE path: a helper GPU this process cannot see (fma_paths_attach)
@@ -288,8 +288,8 @@ struct fma_engine {
     void* load_ring = nullptr;
     size_t load_ring_bytes = 0;
     std::vector<cudaEvent_t> ev_load;
-    int load_threads = 12;               // sweep on B200 (profiles/load_bench_llama3_8b_r1.json): 4 -> 22, 8 -> 31-38,
-    size_t load_chunk = (size_t)16 << 20;  // 12 -> 48.7, 16 -> 46.9 GB/s from the page cache (pread is the limiter)
+    int load_threads = 12;               // pread from the page cache is the limiter: enough readers to keep
+    size_t load_chunk = (size_t)16 << 20;  // one PCIe Gen5 link busy (tests/tools/load_bench.py measures it)
     int load_slots = 24;
 
     // MULTI-PATH wake

@@ -1,4 +1,4 @@
-// fma_kernels.cu — sm_100a kernels of the sleep/wake weight-movement path.
+// fma_kernels.cu — sm_90a kernels of the sleep/wake weight-movement path.
 //
 //   K0  fma_k_fill         counter-based splitmix64 fill of pages (synthetic weight blobs)
 //   K1/K2 fma_k_page_copy_* page-table driven gather / scatter of 2 MiB VMM pages:
@@ -37,7 +37,7 @@ __device__ __forceinline__ uint64_t fmix64(uint64_t z) {
 
 #if !defined(FMA_CUDA_EMU)
 // ------------------------------------------------------------------------------------
-// PTX wrappers (sm_90+/sm_100a bulk async copy + mbarrier)
+// PTX wrappers (sm_90 bulk async copy + mbarrier)
 // ------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
     return static_cast<uint32_t>(__cvta_generic_to_shared(p));
@@ -181,44 +181,47 @@ fma_k_page_copy_tma(const uint64_t* __restrict__ src_tab, uint64_t src_base, con
 }
 
 // ------------------------------------------------------------------------------------
-// K1/K2 (LDG variant): 256 threads, each moves UNROLL x 32 B per tile with streaming hints.
+// K1/K2 (LDG variant): 256 threads, each moves 2 x UNROLL x 16 B per tile with streaming hints.
 // ------------------------------------------------------------------------------------
-// 256-bit streaming load/store (sm_100: LDG.E.256 / STG.E.256); the L2::evict_first qualifier is only
-// accepted by ptxas on the .v4.b64 / .v8.b32 forms.
-struct __align__(32) u64x4 { uint64_t a, b, c, d; };
+// 128-bit streaming load/store (LDG.E.128 / STG.E.128, the widest global access sm_90 has): vector v of a tile
+// is at byte 16 * v, thread t takes v = t, t + 256, ... so every warp instruction covers 512 contiguous bytes.
+// Nothing is allocated in L1, and the L2 policy marks the lines evict-first: the data is touched once.
+struct __align__(16) u64x2 { uint64_t a, b; };
 #if !defined(FMA_CUDA_EMU)
-__device__ __forceinline__ u64x4 ld_stream(const u64x4* p) {
-    u64x4 v;
-    asm volatile("ld.global.nc.L1::no_allocate.L2::evict_first.v4.b64 {%0,%1,%2,%3}, [%4];"
-                 : "=l"(v.a), "=l"(v.b), "=l"(v.c), "=l"(v.d) : "l"(p));
+__device__ __forceinline__ u64x2 ld_stream(const u64x2* p, uint64_t pol) {
+    u64x2 v;
+    asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v2.u64 {%0,%1}, [%2], %3;"
+                 : "=l"(v.a), "=l"(v.b) : "l"(p), "l"(pol));
     return v;
 }
-__device__ __forceinline__ void st_stream(u64x4* p, const u64x4& v) {
-    asm volatile("st.global.L1::no_allocate.L2::evict_first.v4.b64 [%0], {%1,%2,%3,%4};" ::"l"(p), "l"(v.a), "l"(v.b),
-                 "l"(v.c), "l"(v.d) : "memory");
+__device__ __forceinline__ void st_stream(u64x2* p, const u64x2& v, uint64_t pol) {
+    asm volatile("st.global.L1::no_allocate.L2::cache_hint.v2.u64 [%0], {%1,%2}, %3;" ::"l"(p), "l"(v.a), "l"(v.b),
+                 "l"(pol) : "memory");
 }
 #else
-inline u64x4 ld_stream(const u64x4* p) { return *p; }
-inline void st_stream(u64x4* p, const u64x4& v) { *p = v; }
+inline u64x2 ld_stream(const u64x2* p, uint64_t) { return *p; }
+inline void st_stream(u64x2* p, const u64x2& v, uint64_t) { *p = v; }
 #endif
 
 template <int UNROLL>
 __global__ void __launch_bounds__(256)
 fma_k_page_copy_ldg(const uint64_t* __restrict__ src_tab, uint64_t src_base, const uint64_t* __restrict__ dst_tab,
                     uint64_t dst_base, uint32_t n_pages) {
-    constexpr uint32_t kTile = 256u * 32u * UNROLL;
+    constexpr int kVecs = 2 * UNROLL;  // 16-byte vectors per thread and tile
+    constexpr uint32_t kTile = 256u * 16u * kVecs;
     constexpr uint32_t kTilesPerPage = FMA_K_PAGE_BYTES / kTile;
+    const uint64_t pol = policy_evict_first();
     const uint64_t n_tiles = (uint64_t)n_pages * kTilesPerPage;
     for (uint64_t t = blockIdx.x; t < n_tiles; t += gridDim.x) {
         const uint32_t p = (uint32_t)(t / kTilesPerPage);
         const uint32_t o = (uint32_t)(t % kTilesPerPage) * kTile;
-        const u64x4* __restrict__ s = reinterpret_cast<const u64x4*>(page_addr(src_tab, src_base, p) + o) + threadIdx.x;
-        u64x4* __restrict__ d = reinterpret_cast<u64x4*>(page_addr(dst_tab, dst_base, p) + o) + threadIdx.x;
-        u64x4 v[UNROLL];
+        const u64x2* __restrict__ s = reinterpret_cast<const u64x2*>(page_addr(src_tab, src_base, p) + o) + threadIdx.x;
+        u64x2* __restrict__ d = reinterpret_cast<u64x2*>(page_addr(dst_tab, dst_base, p) + o) + threadIdx.x;
+        u64x2 v[kVecs];
 #pragma unroll
-        for (int u = 0; u < UNROLL; ++u) v[u] = ld_stream(s + u * 256);
+        for (int u = 0; u < kVecs; ++u) v[u] = ld_stream(s + u * 256, pol);
 #pragma unroll
-        for (int u = 0; u < UNROLL; ++u) st_stream(d + u * 256, v[u]);
+        for (int u = 0; u < kVecs; ++u) st_stream(d + u * 256, v[u], pol);
     }
 }
 
@@ -227,29 +230,28 @@ fma_k_page_copy_ldg(const uint64_t* __restrict__ src_tab, uint64_t src_base, con
 // over the page's 2^18 little-endian 64-bit words; sums are mod 2^64 so any reduction order
 // is exact.  out[p] must be zero on entry (atomicAdd accumulation, one per CTA-tile).
 // ------------------------------------------------------------------------------------
-constexpr int kDigUnroll = 4;
+constexpr int kDigVecs = 8;  // 16-byte vectors per thread and tile
 __global__ void __launch_bounds__(256)
 fma_k_page_digest(const fma_k_page_desc* __restrict__ pages, uint32_t n_pages, unsigned long long* __restrict__ out) {
-    constexpr uint32_t kTile = 256u * 32u * kDigUnroll;  // 32 KiB
+    constexpr uint32_t kTile = 256u * 16u * kDigVecs;  // 32 KiB
     constexpr uint32_t kTilesPerPage = FMA_K_PAGE_BYTES / kTile;
     __shared__ unsigned long long warp_sums[8];
+    const uint64_t pol = policy_evict_first();
     const uint64_t n_tiles = (uint64_t)n_pages * kTilesPerPage;
     for (uint64_t t = blockIdx.x; t < n_tiles; t += gridDim.x) {
         const uint32_t p = (uint32_t)(t / kTilesPerPage);
         const uint32_t o = (uint32_t)(t % kTilesPerPage) * kTile;
         const fma_k_page_desc pd = pages[p];
-        const u64x4* __restrict__ s = reinterpret_cast<const u64x4*>(pd.addr + o) + threadIdx.x;
-        u64x4 v[kDigUnroll];
+        const u64x2* __restrict__ s = reinterpret_cast<const u64x2*>(pd.addr + o) + threadIdx.x;
+        u64x2 v[kDigVecs];
 #pragma unroll
-        for (int u = 0; u < kDigUnroll; ++u) v[u] = ld_stream(s + u * 256);
+        for (int u = 0; u < kDigVecs; ++u) v[u] = ld_stream(s + u * 256, pol);
         uint64_t acc = 0;
 #pragma unroll
-        for (int u = 0; u < kDigUnroll; ++u) {
-            const uint64_t j = pd.first_word + (uint64_t)(o / 8) + (uint64_t)(u * 256 + threadIdx.x) * 4;
+        for (int u = 0; u < kDigVecs; ++u) {
+            const uint64_t j = pd.first_word + (uint64_t)(o / 8) + (uint64_t)(u * 256 + threadIdx.x) * 2;
             acc += fmix64(v[u].a + (j + 1) * FMA_GOLDEN);
             acc += fmix64(v[u].b + (j + 2) * FMA_GOLDEN);
-            acc += fmix64(v[u].c + (j + 3) * FMA_GOLDEN);
-            acc += fmix64(v[u].d + (j + 4) * FMA_GOLDEN);
         }
 #pragma unroll
         for (int off = 16; off > 0; off >>= 1) acc += __shfl_down_sync(0xffffffffu, acc, off);
@@ -270,23 +272,23 @@ fma_k_page_digest(const fma_k_page_desc* __restrict__ pages, uint32_t n_pages, u
 // ------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
 fma_k_fill(const fma_k_page_desc* __restrict__ pages, uint32_t n_pages, uint64_t seed) {
-    constexpr uint32_t kTile = 256u * 32u * 4;
+    constexpr int kVecs = 8;  // 16-byte vectors per thread and tile
+    constexpr uint32_t kTile = 256u * 16u * kVecs;
     constexpr uint32_t kTilesPerPage = FMA_K_PAGE_BYTES / kTile;
+    const uint64_t pol = policy_evict_first();
     const uint64_t n_tiles = (uint64_t)n_pages * kTilesPerPage;
     for (uint64_t t = blockIdx.x; t < n_tiles; t += gridDim.x) {
         const uint32_t p = (uint32_t)(t / kTilesPerPage);
         const uint32_t o = (uint32_t)(t % kTilesPerPage) * kTile;
         const fma_k_page_desc pd = pages[p];
-        u64x4* __restrict__ d = reinterpret_cast<u64x4*>(pd.addr + o) + threadIdx.x;
+        u64x2* __restrict__ d = reinterpret_cast<u64x2*>(pd.addr + o) + threadIdx.x;
 #pragma unroll
-        for (int u = 0; u < 4; ++u) {
-            const uint64_t k = pd.first_word + (uint64_t)(o / 8) + (uint64_t)(u * 256 + threadIdx.x) * 4;
-            u64x4 v;
+        for (int u = 0; u < kVecs; ++u) {
+            const uint64_t k = pd.first_word + (uint64_t)(o / 8) + (uint64_t)(u * 256 + threadIdx.x) * 2;
+            u64x2 v;
             v.a = fmix64(seed + (k + 1) * FMA_GOLDEN);
             v.b = fmix64(seed + (k + 2) * FMA_GOLDEN);
-            v.c = fmix64(seed + (k + 3) * FMA_GOLDEN);
-            v.d = fmix64(seed + (k + 4) * FMA_GOLDEN);
-            st_stream(d + u * 256, v);
+            st_stream(d + u * 256, v, pol);
         }
     }
 }
@@ -298,7 +300,7 @@ int sm_count() {
         int dev = 0;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&g_sm_count, cudaDevAttrMultiProcessorCount, dev);
-        if (g_sm_count <= 0) g_sm_count = 148;
+        if (g_sm_count <= 0) g_sm_count = 132;  // H100 SXM
     }
     return g_sm_count;
 }
@@ -309,9 +311,9 @@ int sm_count() {
 // launch wrappers (internal C++ interface used by fma_engine.cu)
 // ------------------------------------------------------------------------------------
 fma_k_tma_cfg fma_k_default_tma_cfg() {
-    // Picked from the launch-size sweep on B200 (profiles/k_size_sweep_r1.md): 2 pipes x 3 stages x 16 KiB =
-    // 96 KiB in flight per SM is the best or within 1% of the best from 256 MiB to 4 GiB per launch
-    // (6.22 -> 6.62 TB/s read+write); deeper rings or 2 CTAs/SM lose 3-6% (more DRAM page conflicts).
+    // 2 pipes x 3 stages x 16 KiB = 96 KiB of smem per SM, 64 KiB of loads in flight: on H100 (132 SMs,
+    // 3.35 TB/s HBM3) that is about 8.4 MiB in flight against the ~2.5 MiB that bandwidth x ~0.7 us of DRAM
+    // latency needs, with the smem well inside the 227 KiB a block may use.
     fma_k_tma_cfg c;
     c.tile_bytes = 16u << 10;
     c.stages = 3;
@@ -360,7 +362,7 @@ cudaError_t fma_k_launch_page_copy(const uint64_t* src_tab, uint64_t src_base, c
 cudaError_t fma_k_launch_page_digest(const fma_k_page_desc* pages, uint32_t n_pages, uint64_t* out_zeroed,
                                      cudaStream_t stream) {
     if (n_pages == 0) return cudaSuccess;
-    const uint64_t n_tiles = (uint64_t)n_pages * (FMA_K_PAGE_BYTES / (256u * 32u * kDigUnroll));
+    const uint64_t n_tiles = (uint64_t)n_pages * (FMA_K_PAGE_BYTES / (256u * 16u * kDigVecs));
     uint64_t grid = (uint64_t)sm_count() * 8;
     if (grid > n_tiles) grid = n_tiles;
     FMA_LAUNCH(fma_k_page_digest, (unsigned)grid, 256, 0, stream, pages, n_pages, reinterpret_cast<unsigned long long*>(out_zeroed));

@@ -1,4 +1,4 @@
-// fma_kernels.h — internal C++ interface between the host engine and the sm_100a kernels.
+// fma_kernels.h — internal C++ interface between the host engine and the sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

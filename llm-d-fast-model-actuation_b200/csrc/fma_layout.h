@@ -13,9 +13,8 @@ namespace fma_layout {
 
 // One VA arena per tag: segments of a tag are bump-allocated next to each other, so that after a sleep the whole tag
 // can be re-created with ONE cuMemCreate + cuMemMap + cuMemSetAccess (a "run") instead of three driver calls per
-// segment.  Measured on B200: 15 GiB as 131 pieces = 8 ms map + 17 ms unmap alone, 16 + 22 ms with a second process
-// making VMM calls, and 325 ms inside a 2-rank wake; as one run = 1.4 ms + 5 ms, contention-proof
-// (profiles/vmm_span_probe_r1.json).
+// segment.  Driver VMM calls serialise across processes, so the number of calls, not the bytes, sets the cost of a remap
+// when other processes make VMM calls too (scripts/vmm_span_probe.py compares pieces with one run).
 struct Arena {
     uint64_t base = 0;                  // device VA of the reservation
     size_t cap = 0;

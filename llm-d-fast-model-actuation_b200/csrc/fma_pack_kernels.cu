@@ -1,4 +1,4 @@
-// fma_pack_kernels.cu — sm_100a kernels of the PACKED host image (format: fma_codec.h).
+// fma_pack_kernels.cu — sm_90a kernels of the PACKED host image (format: fma_codec.h).
 //
 //   K4p fma_k_pack_probe   per page: would it pack?  -> stored size (kPackedBytes or 2 MiB raw)
 //   K4  fma_k_pack         gather + encode: scattered 2 MiB device pages -> packed pages in a contiguous ring slot
@@ -14,9 +14,8 @@
 // low 24 bits of the page descriptor's `state` word; the high 8 bits count finished parts and the part that finishes last
 // writes the page header); each part stages its 512 B slice of the emax plane in shared memory.  K5: each part decodes its
 // tiles and then patches the exceptions that fall into its value range.
-// Why parts (round 2, B200): with one CTA per page a ring slot's worth of pages (256-337) is 1.7-2.3 waves of 148 SMs at
-// 28 % of the warps an SM can hold — K5 ran at 2.7-3.3 TB/s per slot-sized launch against 5.6 TB/s for 1024 pages
-// (profiles/pack_sweep_r2.json, profiles/k5_full_r2.md); 8 x as many, 8 x smaller work items fill the machine at every size.
+// Why parts: with one CTA per page a ring slot's worth of pages (256-337) is only about two waves of H100's 132 SMs, each
+// SM holding a fraction of the warps it could; 8 x as many, 8 x smaller work items fill the machine at every slot size.
 // HBM-bound: reads 2 MiB, writes 1.52 MiB per page, all accesses whole 32-byte sectors except the (rare) exception patches.  All arithmetic is in fma_codec.h, shared with the CPU stand-in that the host-simulated engine
 // tests run, and restated in oracle/fma_oracle.c.
 #include <cuda_runtime.h>

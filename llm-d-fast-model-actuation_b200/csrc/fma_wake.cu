@@ -570,10 +570,9 @@ int do_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags) {
             view.push_back(fma_layout::SegView{i, s.arena, (uint64_t)s.va, s.bytes, s.has_backup, s.packed_off});
         }
         // FMA_MAP_PIECE_MIB (default 2048; 0 = whole runs): backed-up runs are mapped in pieces of about that size, cut at segment
-        // boundaries.  One 15 GiB mapping has only the ring's ~19 ms of slack, and 20-30 % of the wakes on these hosts hit a
-        // 10-190 ms stall in one driver call; with pieces K2 starts on the first piece and every later call has the copy time
-        // of the pieces before it as slack.  B200, 8B table, 16 wakes: 0.2898-0.2937 s (mean 0.2904) vs 0.290-0.349 s (mean
-        // 0.2992) for whole runs (profiles/bench_n1_pieces_r2.json).
+        // boundaries.  One 15 GiB mapping has only the ring's slack of a few milliseconds, and a shared host's driver calls
+        // sometimes stall for tens of milliseconds; with pieces K2 starts on the first piece and every later call has the copy
+        // time of the pieces before it as slack.
         runs = fma_layout::plan_runs(view, env_int("FMA_MERGE_RUNS", 1) != 0, (size_t)std::max(env_int("FMA_MAP_PIECE_MIB", 2048), 0) << 20);
     }
     const int tier = e->image_tier;

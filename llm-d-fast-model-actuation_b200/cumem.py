@@ -2,7 +2,7 @@
 
 Same class name, singleton accessor, method names, argument meaning and error behaviour as the
 reference's allocator shim, so vLLM's ``Worker.sleep`` / ``Worker.wake_up`` / ``load_model``
-(vllm:v1/worker/gpu_worker.py:157-209,335-342) run unchanged on top of the B200 engine:
+(vllm:v1/worker/gpu_worker.py:157-209,335-342) run unchanged on top of the H100 engine:
 
     reference (vllm:device_allocator/cumem.py)            this module
     ------------------------------------------            -----------------------------------

@@ -396,7 +396,7 @@ def create_app(agent: NodeAgent) -> FastAPI:
 
     @app.get("/")
     def index():
-        return JSONResponse({"name": "B200 node agent (launcher-compatible instance management + node-scoped actuation)", "version": "2.0",
+        return JSONResponse({"name": "H100 node agent (launcher-compatible instance management + node-scoped actuation)", "version": "2.0",
                              "endpoints": {"index": "GET /", "health": "GET /health",
                                            "create_instance": "POST /v2/vllm/instances",
                                            "create_named_instance": "PUT /v2/vllm/instances/{instance_id}",
@@ -529,7 +529,7 @@ def create_app(agent: NodeAgent) -> FastAPI:
 def main() -> None:
     import uvicorn
 
-    ap = argparse.ArgumentParser(description="B200 node agent (launcher-compatible)")
+    ap = argparse.ArgumentParser(description="H100 node agent (launcher-compatible)")
     ap.add_argument("--mock-gpus", action="store_true")
     ap.add_argument("--mock-gpu-count", type=int, default=8)   # accepted for CLI compatibility with launcher.py:857-899
     ap.add_argument("--host", default="0.0.0.0")

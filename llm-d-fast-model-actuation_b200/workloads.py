@@ -74,8 +74,8 @@ def _llama_tensors(*, hidden: int, inter: int, heads: int, kv_heads: int, head_d
     """Fused vLLM layouts per TP rank: qkv_proj, o_proj, gate_up_proj, down_proj, two RMSNorm weights — plus, with ``max_pos``, the
     non-parameter buffers a live vLLM allocates under the ``weights`` tag (SURVEY.md §8d): the rotary embedding built right after
     layer 0's o_proj (``inv_freq``: the first small-pool allocation; ``cos_sin_cache`` = max_pos x head_dim x dtype: 1-10 MiB, so a
-    20 MiB large-pool segment), shared by all layers.  Validated against a live vLLM 0.22 + torch 2.11 weights pool on a B200
-    (Llama-3-8B shapes, ``profiles/e2e_table_validation_llama3_8b_r2.json``): 132 segments, 16 083 058 688 bytes, order
+    20 MiB large-pool segment), shared by all layers.  What a live vLLM 0.22 + torch 2.11 weights pool holds for Llama-3-8B
+    shapes (``scripts/e2e_launcher_vllm.py`` compares the two): 132 segments, 16 083 058 688 bytes, order
     [1002, 48, 32, 2, 20, 224, 112, ...] MiB."""
     b = dtype_bytes
     q_rows = heads * head_dim // tp

@@ -21,7 +21,7 @@
  * PARITY PINNING: the reference's own tests hold no golden vector for this path (SURVEY.md
  * §8c: vLLM is MagicMock'ed, test_launcher.py:32-38).  Pins used instead:
  *   (1) splitmix64 published known-answer vector (seed 1234567) — tests/test_oracle.py;
- *   (2) golden fixtures produced by running vLLM's OWN CuMemAllocator on a B200
+ *   (2) golden fixtures produced by running vLLM's OWN CuMemAllocator on an H100
  *       (tests/golden/make_vllm_cumem_golden.py -> tests/golden/vllm_cumem_roundtrip.json):
  *       segment sizes/tags and before/after digests of the real reference data path.
  */

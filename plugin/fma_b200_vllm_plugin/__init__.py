@@ -1,4 +1,4 @@
-"""vLLM general plugin: routes vLLM's sleep/wake allocator to the B200 engine when FMA_B200=1.
+"""vLLM general plugin: routes vLLM's sleep/wake allocator to the H100 engine when FMA_B200=1.
 
 vLLM calls every entry point of group ``vllm.general_plugins`` in the API-server, engine-core and worker
 processes (vllm:plugins/__init__.py:69-82, v1/engine/core.py:108, v1/worker/worker_base.py:247) before a worker

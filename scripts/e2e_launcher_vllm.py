@@ -1,5 +1,5 @@
-"""End-to-end drop-in check on a GPU box (SURVEY.md §7 step 7, BASELINE.md §3): the UNMODIFIED reference launcher
-(baseline/_ref/launcher/launcher.py, staged by __graft_entry__.build()) forks a real vLLM server with a dummy-weight
+"""End-to-end drop-in check on a GPU machine (SURVEY.md §7 step 7, BASELINE.md §3): the UNMODIFIED reference launcher
+(inference_server/launcher/ of a reference checkout, named by REFERENCE_LAUNCHER_DIR) forks a real vLLM server with a dummy-weight
 Llama model; the same HTTP calls the dual-pods controller makes (`POST /sleep`, `GET /is_sleeping`, `POST /wake_up`,
 pkg/controller/dual-pods/inference-server.go:1329-1339,1595-1607,1118-1137) are timed by wall clock, once with vLLM's
 own allocator and once with FMA_B200=1 in the instance's env_vars (-> plugin/ -> fma_b200.cumem).  A generation
@@ -18,6 +18,7 @@ cfg = dict(architectures=["LlamaForCausalLM"], model_type="llama", hidden_act="s
            rope_theta=500000.0, tie_word_embeddings=False, torch_dtype="bfloat16", bos_token_id=128000, eos_token_id=128001, **CFGS[MODEL])
 json.dump(cfg, open(f"{mdir}/config.json", "w"))
 OUT = os.path.join(ROOT, "gpurun_out", "e2e"); os.makedirs(OUT, exist_ok=True)
+LAUNCHER_DIR = os.environ.get("REFERENCE_LAUNCHER_DIR", "")
 LPORT, VPORT = 8001, 8005
 # Arms (E2E_ARMS=comma list).  Default: vLLM's allocator vs the engine, dummy weights.  Extra arms:
 #   fma_b200_packed  the engine with the PACKED host image (FMA_PACK=1; dummy weights are bf16 U(-1e-3, 1e-3): they code)
@@ -82,8 +83,8 @@ if USE_AGENT:   # this repo's launcher-compatible node agent, owning the parking
     launcher = subprocess.Popen([sys.executable, os.path.join(ROOT, "scripts", "run_node_agent.py"), "--port", str(LPORT), "--host", "127.0.0.1", "--parking",
                                  "--log-dir", OUT], env=env, cwd=ROOT, stdout=open(f"{OUT}/launcher.log", "w"), stderr=subprocess.STDOUT)
 else:
-    launcher = subprocess.Popen([sys.executable, os.path.join(ROOT, "baseline", "_ref", "launcher", "launcher.py"), "--port", str(LPORT), "--host", "127.0.0.1"],
-                                env=env, cwd=os.path.join(ROOT, "baseline", "_ref", "launcher"), stdout=open(f"{OUT}/launcher.log", "w"), stderr=subprocess.STDOUT)
+    launcher = subprocess.Popen([sys.executable, os.path.join(LAUNCHER_DIR, "launcher.py"), "--port", str(LPORT), "--host", "127.0.0.1"],
+                                env=env, cwd=LAUNCHER_DIR, stdout=open(f"{OUT}/launcher.log", "w"), stderr=subprocess.STDOUT)
 results = {}
 try:
     for _ in range(240):

@@ -1,4 +1,4 @@
-"""Round-2 probe (a few seconds on a B200): does VA alignment / handle size change what a run costs to map?
+"""Probe (a few seconds on one GPU): does VA alignment / handle size change what a run costs to map?
 Prints cuMemGetAllocationGranularity (minimum vs recommended) and times cuMemCreate / Map / SetAccess / Unmap of one
 16 GiB run for VA reservations aligned to 2 MiB, 32 MiB, 512 MiB and 1 GiB (the engine's arenas are aligned to the
 minimum granularity today, csrc/fma_engine.cu arena_take).  Output: gpurun_out/vmm/gran_probe.json."""

@@ -1,6 +1,6 @@
 """BASELINE config 5: four sleeping Llama-3-8B models parked in idle GPUs' HBM over NVSwitch, round-robin wake.
 One process drives 4 engines (GPUs 0-3); each parks its image on GPU 4-7 (FMA_TIER_PEER: cuMemCreate on the peer +
-cuMemMap/SetAccess into the owner, K1/K2 move pages over NVLink 5).  Reports wake latency and GB/s vs 900 GB/s."""
+cuMemMap/SetAccess into the owner, K1/K2 move pages over NVLink).  Reports wake latency and GB/s vs 450 GB/s (H100 NVLink 4, per direction)."""
 import os, sys, json, time, threading
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import fma_b200

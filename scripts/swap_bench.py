@@ -1,4 +1,4 @@
-"""BASELINE config 4: model swap under one process, Llama-3-8B <-> Mistral-7B on 1xB200.
+"""BASELINE config 4: model swap under one process, Llama-3-8B <-> Mistral-7B on one GPU.
 Serial (sleep A, then wake B: what two independent reconciles of the reference do, SURVEY.md §3.4) vs
 fma_swap (D2H of A overlapped with H2D of B on opposite PCIe directions)."""
 import os, sys, json, time

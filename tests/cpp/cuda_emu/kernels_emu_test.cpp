@@ -1,6 +1,6 @@
 // Runs the ACTUAL kernel source csrc/fma_kernels.cu — K0 fill, K1/K2 page copy (the TMA pipeline and the LDG variant), K3
 // digest — on the CPU execution model of cuda_emu.h (lazy async proxy included) and checks it against the oracle
-// (oracle/fma_oracle.c).  These kernels are validated on B200 hardware (tests -m gpu, compute-sanitizer, ncu); this adds
+// (oracle/fma_oracle.c).  These kernels are tested on the H100 (tests -m gpu); this adds
 // what the GPU cannot show cheaply: ThreadSanitizer over their shared-memory traffic, and a standing CPU regression test
 // of the exact source that ships.  Built by tests/test_kernels_emulated.py with g++ -DFMA_CUDA_EMU -include cuda_emu.h.
 #include <cassert>

@@ -4,7 +4,7 @@
 // with g++ -DFMA_CUDA_EMU -include cuda_emu.h, plain and under ThreadSanitizer (missing barriers = data races).
 //
 // The SAME file is the GPU-side kernel test: `nvcc -x cu -DFMA_GPU_TEST ...` (tests/cpp/cuda_emu/Makefile ->
-// tests/cpp/cuda_emu/pack_kernels_gpu_test, run on a B200 by tests/test_gpu_parity.py::test_pack_kernels_binary_on_the_device) compiles the real kernels and
+// tests/cpp/cuda_emu/pack_kernels_gpu_test, run on an H100 by tests/test_gpu_parity.py::test_pack_kernels_binary_on_the_device) compiles the real kernels and
 // keeps every buffer in managed memory, so a mismatch on the device is reported with the page it happened in,
 // without the engine in the way.
 #include <algorithm>

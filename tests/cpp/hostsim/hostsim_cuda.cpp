@@ -9,7 +9,7 @@
 // "Device memory" is host memory.  VMM is modelled with mmap so that the semantics the engine relies on are REAL:
 //   cuMemAddressReserve -> PROT_NONE reservation; cuMemMap -> fresh zero pages at that VA (MAP_FIXED);
 //   cuMemUnmap -> the pages are gone (PROT_NONE again; touching them faults) and only WHOLE mappings may be unmapped,
-//   a range spanning several whole mappings is accepted, a sub-range is CUDA_ERROR_INVALID_VALUE (as measured on B200,
+//   a range spanning several whole mappings is accepted, a sub-range is CUDA_ERROR_INVALID_VALUE (as the driver does,
 //   scripts/vmm_span_probe.py); memory lives until unmap even if the handle was released right after cuMemMap.
 // Streams execute eagerly (a copy has happened when cudaMemcpyAsync returns); events record wall-clock time.
 #include <cuda.h>

@@ -1,8 +1,8 @@
-"""Generates tests/golden/vllm_cumem_roundtrip.json ON A GPU BOX by running the reference data path itself:
+"""Generates tests/golden/vllm_cumem_roundtrip.json on a GPU machine with vLLM by running the reference data path itself:
 vLLM's unmodified CuMemAllocator (vllm:device_allocator/cumem.py:177-249, the code POST /sleep and /wake_up
 reach through inference_server/launcher/launcher.py) over the tensors of the `tiny-llama-test` model (torch's caching allocator turns them into segments).
 
-    gpurun -- 'python tests/golden/make_vllm_cumem_golden.py'    # writes gpurun_out/golden/..., copy into tests/golden/
+    python tests/golden/make_vllm_cumem_golden.py [OUT_DIR]    # writes OUT_DIR/vllm_cumem_roundtrip.json (default: tests/golden)
 
 Every weight tensor is loaded with the oracle's splitmix64 stream (seed 1234, word index continuing across
 tensors), sent through sleep(offload_tags=("weights",)) -> wake_up(), read back, and hashed with SHA-256
@@ -55,8 +55,9 @@ for (name, nbytes), t, fw in zip(tensors, weights, firsts):
 for t in kvs:
     b = t.cpu().numpy()
     out["kv_cache"].append({"bytes": int(b.size), "restored": bool((b == 0x5A).all())})
-os.makedirs(os.path.join(ROOT, "gpurun_out", "golden"), exist_ok=True)
-p = os.path.join(ROOT, "gpurun_out", "golden", "vllm_cumem_roundtrip.json")
+out_dir = sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "tests", "golden")
+os.makedirs(out_dir, exist_ok=True)
+p = os.path.join(out_dir, "vllm_cumem_roundtrip.json")
 json.dump(out, open(p, "w"), indent=1)
 print("wrote", p, "same_va", out["same_device_addresses"], "n_weights", len(weights), "segments", len(seg_sizes),
       "kv restored", [k["restored"] for k in out["kv_cache"]])

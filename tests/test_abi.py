@@ -1,4 +1,4 @@
-"""The C-ABI library builds for sm_100a, loads on a CPU-only box, exports every symbol include/*.h
+"""The C-ABI library builds for sm_90a, loads on a CPU-only box, exports every symbol include/*.h
 declares, matches the ctypes mirror byte for byte, and refuses to run without a GPU (no CPU fallback)."""
 import ctypes as C
 import os
@@ -60,13 +60,14 @@ def test_struct_layouts_match_the_header(built, tmp_path):
 
 
 def test_sass_contains_tma_bulk_copies(built):
-    """K1/K2 are Blackwell-native: the SASS must show UBLKCP (cp.async.bulk) and 256-bit LDG/STG."""
+    """K1/K2 are Hopper-native: the SASS must show UBLKCP (cp.async.bulk), mbarrier waits (SYNCS) and 128-bit
+    streaming LDG/STG, the widest global access sm_90 has."""
     import fma_b200
 
     sass = subprocess.check_output(["cuobjdump", "-sass", fma_b200.lib_path()], text=True)
-    assert "sm_100a" in sass
+    assert "sm_90a" in sass
     assert "UBLKCP" in sass and "SYNCS" in sass
-    assert ".256" in sass
+    assert "LDG.E.NA.128" in sass and "STG.E.NA.128" in sass
 
 
 def _has_gpu():

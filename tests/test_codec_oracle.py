@@ -1,6 +1,6 @@
 """The "FMP4" page code of packed host images: the oracle's value-by-value restatement (oracle/fma_oracle.c) against
 the format's algebra.  The engine's kernels are compared with this oracle in tests/test_gpu_parity.py (on the CUDA host
-simulation here, on a B200 with -m gpu)."""
+simulation here, on an H100 with -m gpu)."""
 import numpy as np
 import pytest
 

@@ -1,6 +1,7 @@
-"""BASELINE config 0 (plumbing, no GPU): the UNMODIFIED reference launcher (staged into baseline/_ref by build())
-creates an instance from the same JSON the Go controller sends (pkg/controller/dual-pods/launcherclient.go:72-78),
-forks the child, and the controller's sleep -> is_sleeping -> wake_up sequence works against the child's port.
+"""BASELINE config 0 (plumbing, no GPU): the launcher-compatible node agent (scripts/run_node_agent.py; its REST contract is
+pinned to the reference launcher's answers by tests/test_node_agent_differential.py) creates an instance from the same JSON
+the Go controller sends (pkg/controller/dual-pods/launcherclient.go:72-78), forks the child, and the controller's
+sleep -> is_sleeping -> wake_up sequence works against the child's port.
 The child is the route-compatible stand-in of SURVEY.md §8c-iv (CPU-worker semantics: nothing moves)."""
 import json
 import os
@@ -11,10 +12,9 @@ import time
 import urllib.error
 import urllib.request
 
-import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-LAUNCHER = os.path.join(ROOT, "baseline", "_ref", "launcher", "launcher.py")
+LAUNCHER = os.path.join(ROOT, "scripts", "run_node_agent.py")
 
 
 def _port():
@@ -45,9 +45,7 @@ def _wait(url, seconds):
     return False
 
 
-def test_unmodified_launcher_drives_sleep_wake(built, tmp_path):
-    if not os.path.exists(LAUNCHER):
-        pytest.skip("reference launcher not staged (no /root/reference at build time)")
+def test_launcher_compatible_agent_drives_sleep_wake(built, tmp_path):
     lport, vport = _port(), _port()
     env = dict(os.environ)
     env["PYTHONPATH"] = os.pathsep.join([os.path.join(ROOT, "scripts", "vllm_cpu_standin"), os.path.join(ROOT, "scripts", "k8s_stub"),

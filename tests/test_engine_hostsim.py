@@ -12,8 +12,10 @@ streams) and host stand-ins for the kernel launch wrappers, then
 
 The product library contains none of this: without a GPU it refuses to run (tests/test_abi.py)."""
 import os
+import shutil
 import subprocess
 import sys
+import tempfile
 
 import pytest
 
@@ -23,6 +25,14 @@ CSRC = os.path.join(ROOT, "llm-d-fast-model-actuation_b200", "csrc")
 INC = ["-I/usr/local/cuda/include", "-I" + CSRC, "-I" + os.path.join(ROOT, "include")]
 HOST_TUS = ["fma_engine.cu", "fma_sleep.cu", "fma_wake.cu", "fma_load.cu", "fma_image.cu", "fma_gate.cu", "fma_pull.cu"]   # the host engine (no kernels): csrc/Makefile HOST_SRCS
 SRCS = ["-x", "c++", *[os.path.join(CSRC, f) for f in HOST_TUS], os.path.join(SIM, "hostsim_cuda.cpp"), os.path.join(SIM, "hostsim_kernels.cpp")]
+
+
+@pytest.fixture()
+def sock_dir():
+    """A unix socket path may be at most 107 bytes and pytest's tmp_path can be longer: sockets go to a short directory."""
+    d = tempfile.mkdtemp(prefix="fma-", dir="/tmp")
+    yield d
+    shutil.rmtree(d, ignore_errors=True)
 
 
 def _have_cuda_headers():
@@ -302,14 +312,14 @@ else:
 """
 
 
-def test_node_level_parking_service_keeps_a_dead_instances_image(hostsim_lib, tmp_path):
+def test_node_level_parking_service_keeps_a_dead_instances_image(hostsim_lib, tmp_path, sock_dir):
     """fma_b200.parking: the node agent's ParkingService owns exportable parking buffers and serves fds over a unix socket; an
     instance parks its weights there, deposits the descriptor and DIES; a fresh instance with the same ID finds the image, attaches,
     adopts and wakes with identical K3 digests; the owner's accounting (MiB per GPU — what a sleeper budget needs,
     inference-server.go:1609-1636) follows.  Host-simulated engine; the C-ABI underneath is GPU-tested in tests/test_gpu_parity.py."""
     import json
 
-    env = dict(os.environ, FMA_B200_LIB=hostsim_lib, FMA_HOSTSIM="1", HOSTSIM_DEVICES="3", FMA_NODE_AGENT_SOCK=str(tmp_path / "park.sock"))
+    env = dict(os.environ, FMA_B200_LIB=hostsim_lib, FMA_HOSTSIM="1", HOSTSIM_DEVICES="3", FMA_NODE_AGENT_SOCK=os.path.join(sock_dir, "park.sock"))
     owner = r"""
 import os, sys, json, subprocess
 sys.path.insert(0, %r)

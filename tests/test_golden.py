@@ -1,5 +1,5 @@
 """The oracle vs the golden fixture produced by the reference data path itself (vLLM's CuMemAllocator run
-on a B200 by tests/golden/make_vllm_cumem_golden.py): weight bytes after the reference's sleep -> wake are
+on an H100 by tests/golden/make_vllm_cumem_golden.py): weight bytes after the reference's sleep -> wake are
 exactly the bytes that went in, at the same device addresses; segment sizes follow the 2 MiB rounding the
 allocation tables assume; non-offloaded tags do not come back."""
 import hashlib

@@ -1,4 +1,4 @@
-"""The controller's three HTTP calls against an engine on a real B200 (SURVEY.md section 8 a9 / B1).
+"""The controller's three HTTP calls against an engine on a real H100 (SURVEY.md section 8 a9 / B1).
 
 The dual-pods controller drives an inference server with exactly POST /sleep (inference-server.go:1329-1339, default client, must
 be 200), GET /is_sleeping (:1595-1607) and POST /wake_up (:1118-1137, 5 s timeout, retried => must be idempotent); the executable

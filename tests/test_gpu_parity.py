@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on a B200): the CUDA path through the C-ABI vs the CPU oracle on the
+"""GPU parity tests (run with -m gpu on an H100): the CUDA path through the C-ABI vs the CPU oracle on the
 same seeded inputs — bit-exact, since everything on this path is byte movement and integer arithmetic."""
 import ctypes as C
 import hashlib
@@ -324,7 +324,7 @@ def test_cumem_shim_with_torch_pool(built, oracle):
     cumem.CuMemAllocator.instance = None
 
 
-# ---- the reference's own round trip (golden fixture produced by vLLM's CuMemAllocator on a B200) -------
+# ---- the reference's own round trip (golden fixture produced by vLLM's CuMemAllocator on an H100) -----
 def test_shim_roundtrip_equals_reference_golden(built, oracle):
     """Same torch allocation sequence, same bytes, through THIS allocator: every tensor must hash to what the
     reference's sleep -> wake produced, at an unchanged data_ptr, with the same segment sizes."""
@@ -946,7 +946,7 @@ def test_full_size_llama3_70b_tp8_shard_roundtrip_properties(engine, oracle):
     assert engine.read(coded[0], 4 << 20) == np.resize(page, 4 << 20).tobytes()
 
 
-# ---- image hand-over between processes (memfd host store).  Green on a B200 since round 2 (profiles/gpu_suite_all_gates_open_r2.log).
+# ---- image hand-over between processes (memfd host store).
 
 _ADOPT_CHILD = r"""
 import os, sys, json

@@ -11,7 +11,7 @@ def _large(table):
 
 def test_llama3_8b_table():
     t = W.allocation_table("llama-3-8b")
-    assert len(t) == 132 and len(_large(t)) == 130                     # 130 large tensors + the small-pool segment + the rotary cache's 20 MiB segment: what a LIVE vLLM allocates (profiles/e2e_table_validation_llama3_8b_r2.json)
+    assert len(t) == 132 and len(_large(t)) == 130                     # 130 large tensors + the small-pool segment + the rotary cache's 20 MiB segment: what a LIVE vLLM allocates
     sizes = sorted({s.bytes // MiB for s in _large(t)})
     assert sizes == [32, 48, 112, 224, 1002]                            # o, qkv, down, gate_up, embed/lm_head
     assert W.weight_bytes(t) == 15338 * MiB == 16083058688              # 14.958 GiB of tensors + the small-pool segment + 20 MiB for the rotary cache: vLLM's own "14.98 GiB is backed up"
