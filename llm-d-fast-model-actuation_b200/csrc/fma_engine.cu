@@ -304,6 +304,10 @@ int ensure_ring_events(fma_engine_t* e, int n) {
     return FMA_OK;
 }
 
+// FMA_NO_RING=1 (read at every sleep and wake): behave as if HBM were too full for a staging ring.  Test and A/B knob: it
+// reaches the ring-less paths, e.g. K5 decoding a packed image straight from pinned host memory, without filling the GPU.
+bool no_ring() { return env_int("FMA_NO_RING", 0) != 0; }
+
 int ensure_ring(fma_engine_t* e, size_t image_bytes) {
     size_t slot = ring_slot_for(e, image_bytes);
     int n = ring_slots_for(e);
@@ -708,6 +712,18 @@ int resolve_mode(const fma_engine_t* e, int tier) {
     return m;
 }
 
+// A sleep or wake that may launch K1 / K2 checks the engine's TMA shape before it unmaps, maps or copies anything: the
+// launch wrapper refuses a shape that cannot run, and by the time of the first launch a sleep has already discarded
+// segments while others are still mapped.  set_option checks one key at a time (a shape is set key by key, through
+// combinations that do not fit), and FMA_TMA_* only seeds the same fields, so both are checked here.
+int check_tma_shape(const fma_engine_t* e, int tier) {
+    if (e->cfg.kernel != FMA_KERNEL_TMA || resolve_mode(e, tier) == FMA_MODE_DIRECT) return FMA_OK;
+    fma_k_tma_cfg c = e->tma;
+    if (fma_k_tma_shape_fits(&c)) return FMA_OK;
+    return fail(FMA_EINVAL, "TMA shape does not fit (tile %u B, %u stages, %u pipes): the tile must be >= 1 KiB, a multiple of 16 dividing "
+                "2 MiB, and pipes x stages x tile + 128 B <= 227 KiB of shared memory", e->tma.tile_bytes, c.stages, c.pipes);
+}
+
 uint64_t store_dev_base(const fma_engine_t* e, int tier) {
     return tier == FMA_TIER_HOST ? (uint64_t)(uintptr_t)e->host.dev_alias : (uint64_t)e->park.va;
 }
@@ -1046,6 +1062,11 @@ int fma_swap(fma_engine_t* out_e, uint64_t offload_tag_mask, int tier, fma_engin
              uint32_t flags) {
     if (check_engine(out_e) != FMA_OK || check_engine(in_e) != FMA_OK) return FMA_EINVAL;
     if (out_e == in_e) return fail(FMA_EINVAL, "swap needs two different engines");
+    {  // neither half starts when the other would refuse its shape
+        int rc = check_tma_shape(out_e, tier);
+        if (rc == FMA_OK) rc = check_tma_shape(in_e, in_e->image_tier);
+        if (rc != FMA_OK) return rc;
+    }
     int rc_sleep = FMA_OK;
     char sleep_msg[512] = "";
     std::thread t([&] {

@@ -352,6 +352,7 @@ size_t ring_slot_for(const fma_engine_t* e, size_t image_bytes);
 int ring_slots_for(const fma_engine_t* e);
 int ensure_ring_events(fma_engine_t* e, int n);
 int ensure_ring(fma_engine_t* e, size_t image_bytes);
+bool no_ring();
 int ensure_event_pool(fma_engine_t* e, size_t n);
 // ---- stores (fma_engine.cu) ----
 void host_store_free(HostStore& h);
@@ -448,6 +449,7 @@ struct KernelTimes {  // event pairs around each K1/K2 launch on the kernel stre
 
 int flush_kernel_times(fma_engine_t* e);
 int resolve_mode(const fma_engine_t* e, int tier);
+int check_tma_shape(const fma_engine_t* e, int tier);
 uint64_t store_dev_base(const fma_engine_t* e, int tier);
 void* store_copy_base(const fma_engine_t* e, int tier);
 int digest_segments(fma_engine_t* e, const std::vector<size_t>& idx, std::vector<uint64_t>* out);

@@ -328,15 +328,9 @@ cudaError_t fma_k_launch_page_copy(const uint64_t* src_tab, uint64_t src_base, c
     if (n_pages == 0) return cudaSuccess;
     if (variant == FMA_K_VARIANT_TMA) {
         fma_k_tma_cfg c = cfg_in ? *cfg_in : fma_k_default_tma_cfg();
-        if (c.stages < 2) c.stages = 2;
-        if (c.stages > kMaxStages) c.stages = kMaxStages;
-        if (c.pipes < 1) c.pipes = 1;
-        if (c.pipes > kMaxPipes) c.pipes = kMaxPipes;
-        if (c.ctas_per_sm < 1) c.ctas_per_sm = 1;
-        if (c.tile_bytes < 1024 || (FMA_K_PAGE_BYTES % c.tile_bytes) != 0 || (c.tile_bytes % 16) != 0)
-            return cudaErrorInvalidValue;
+        if (!fma_k_tma_shape_fits(&c)) return cudaErrorInvalidValue;
+        static_assert(kMaxStages == 8 && kMaxPipes == 4, "fma_k_tma_shape_fits clamps to these");
         const size_t smem = (size_t)c.pipes * c.stages * c.tile_bytes + 128;
-        if (smem > 227u * 1024u) return cudaErrorInvalidValue;
 #if !defined(FMA_CUDA_EMU)
         cudaError_t err = cudaFuncSetAttribute(fma_k_page_copy_tma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (err != cudaSuccess) return err;

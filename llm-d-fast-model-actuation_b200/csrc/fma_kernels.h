@@ -21,6 +21,20 @@ struct fma_k_tma_cfg {
 
 fma_k_tma_cfg fma_k_default_tma_cfg();
 
+// The shape rules of the TMA page copy, shared by its launch wrapper and by the engine, which checks a shape before a
+// sleep or wake starts: stages are clamped to 2..8, pipes to 1..4 and ctas_per_sm to >= 1; the tile must be at least 1 KiB,
+// a multiple of 16 and divide the 2 MiB page, and pipes x stages x tile (+ 128 B of alignment slack) must fit the 227 KiB
+// of shared memory a block may use.  Clamps *c in place; false = the shape cannot run.
+inline bool fma_k_tma_shape_fits(fma_k_tma_cfg* c) {
+    if (c->stages < 2) c->stages = 2;
+    if (c->stages > 8) c->stages = 8;
+    if (c->pipes < 1) c->pipes = 1;
+    if (c->pipes > 4) c->pipes = 4;
+    if (c->ctas_per_sm < 1) c->ctas_per_sm = 1;
+    if (c->tile_bytes < 1024 || (FMA_K_PAGE_BYTES % c->tile_bytes) != 0 || (c->tile_bytes % 16) != 0) return false;
+    return (uint64_t)c->pipes * c->stages * c->tile_bytes + 128 <= 227u * 1024u;
+}
+
 // K1/K2: tables are DEVICE arrays of device addresses (nullptr => contiguous from *_base).
 cudaError_t fma_k_launch_page_copy(const uint64_t* src_tab, uint64_t src_base, const uint64_t* dst_tab,
                                    uint64_t dst_base, uint32_t n_pages, int variant, const fma_k_tma_cfg* cfg,

@@ -239,7 +239,7 @@ int pack_sm_count() {
         int dev = 0;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&g_pack_sm_count, cudaDevAttrMultiProcessorCount, dev);
-        if (g_pack_sm_count <= 0) g_pack_sm_count = 148;
+        if (g_pack_sm_count <= 0) g_pack_sm_count = 132;  // H100 SXM
     }
     return g_pack_sm_count;
 }

@@ -553,6 +553,8 @@ int do_sleep(fma_engine_t* e, uint64_t offload_mask, int tier, uint32_t flags) {
     bool any_unmapped = false, any_mapped = false;
     for (const Segment& s : e->segs) (s.mapped ? any_mapped : any_unmapped) = true;
     if (any_unmapped || !any_mapped) return FMA_OK;
+    rc = check_tma_shape(e, tier);
+    if (rc != FMA_OK) return rc;
     e->tl_begin("sleep", t_entry);
 
     // plan: offloaded segments -> packed image, in (arena, VA) order.  Arenas are bump-allocated per tag, so this is
@@ -629,7 +631,7 @@ int do_sleep(fma_engine_t* e, uint64_t offload_mask, int tier, uint32_t flags) {
             partial_packed = dirty_pages.size() <= e->img_bytes.size();
             for (size_t q = 0; q < k && partial_packed; ++q)
                 partial_packed = dirty_pages[q] < e->img_bytes.size() && e->h_psize[q] == e->img_bytes[dirty_pages[q]];
-            if (partial_packed && ensure_ring(e, W) != FMA_OK) partial_packed = false;  // no HBM for a ring: full sleep through the plain path
+            if (partial_packed && (no_ring() || ensure_ring(e, W) != FMA_OK)) partial_packed = false;  // no HBM for a ring: full sleep through the plain path
         }
     }
     if (clean) flags |= kFlagAdopt;                  // release the device side only: not a byte moves
@@ -638,7 +640,7 @@ int do_sleep(fma_engine_t* e, uint64_t offload_mask, int tier, uint32_t flags) {
     // MULTI-PATH (fma_paths_set): a full, plain host-tier sleep is striped over the paths' links; every path has its own staging slots
     const bool multipath = !e->paths.empty() && !e->mbox && tier == FMA_TIER_HOST && mode == FMA_MODE_STAGED && !partial && !partial_packed && !clean &&
                            !(flags & kFlagAdopt) && !e->cfg.pack && env_int("FMA_MULTIPATH_SLEEP", 1) != 0;
-    if (W && !(flags & kFlagAdopt) && mode == FMA_MODE_STAGED && !multipath && ensure_ring(e, W) != FMA_OK) mode = FMA_MODE_DIRECT;  // HBM too full for a ring
+    if (W && !(flags & kFlagAdopt) && mode == FMA_MODE_STAGED && !multipath && (no_ring() || ensure_ring(e, W) != FMA_OK)) mode = FMA_MODE_DIRECT;  // HBM too full for a ring
     // PACKED image (config.pack): decide per page what its stored form is BEFORE the store is sized
     bool packed = false;
     uint64_t Wp = W;

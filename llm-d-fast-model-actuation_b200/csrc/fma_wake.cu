@@ -559,6 +559,8 @@ int do_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags) {
             cand.push_back(i);
         }
         if (cand.empty()) return FMA_OK;
+        rc = check_tma_shape(e, e->image_tier);
+        if (rc != FMA_OK) return rc;
         e->tl_begin("wake", t_entry);
         std::sort(cand.begin(), cand.end(), [&](size_t a, size_t b) {
             const Segment &x = e->segs[a], &y = e->segs[b];
@@ -598,6 +600,8 @@ int do_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags) {
             if (r.has_backup) w_bytes += r.bytes;
         if (w_bytes && mode == FMA_MODE_STAGED && multipath) {
             // every path brings its own staging slots: no ring
+        } else if (w_bytes && mode == FMA_MODE_STAGED && no_ring()) {
+            mode = FMA_MODE_DIRECT;  // as when HBM is too full for a ring
         } else if (w_bytes && mode == FMA_MODE_STAGED && !e->n_ring) {
             const Run& r0 = runs[0];
             Arena& a = e->arenas[r0.arena];

@@ -28,6 +28,13 @@ struct DevAlloc {  // managed memory: the host-side checks read what the kernels
     template <class U> bool operator!=(const DevAlloc<U>&) const { return false; }
 };
 #define DEVICE_SYNC() do { cudaError_t _e = cudaDeviceSynchronize(); if (_e != cudaSuccess) { fprintf(stderr, "CUDA error: %s\n", cudaGetErrorString(_e)); return 2; } } while (0)
+static unsigned char* host_mapped(size_t n, unsigned char** dev) {  // pinned host memory the device reads over the link
+    void *h = nullptr, *d = nullptr;
+    if (cudaHostAlloc(&h, n, cudaHostAllocMapped) != cudaSuccess || cudaHostGetDevicePointer(&d, h, 0) != cudaSuccess) throw std::bad_alloc();
+    *dev = static_cast<unsigned char*>(d);
+    return static_cast<unsigned char*>(h);
+}
+static const bool kOnDevice = true;
 #else
 // the runtime calls the launch wrappers make
 extern "C" cudaError_t cudaGetDevice(int* d) { *d = 0; return cudaSuccess; }
@@ -35,6 +42,8 @@ extern "C" cudaError_t cudaDeviceGetAttribute(int* v, cudaDeviceAttr, int) { *v 
 extern "C" cudaError_t cudaGetLastError(void) { return cudaSuccess; }
 template <class T> using DevAlloc = std::allocator<T>;
 #define DEVICE_SYNC() do { } while (0)
+static unsigned char* host_mapped(size_t n, unsigned char** dev) { *dev = static_cast<unsigned char*>(malloc(n)); return *dev; }
+static const bool kOnDevice = false;
 #endif
 
 #include "../../../llm-d-fast-model-actuation_b200/csrc/fma_pack_kernels.cu"
@@ -79,6 +88,32 @@ static int run_all() {
     { Page p(N); for (auto& v : p) v = (uint16_t)rnd(); pages.push_back(p); }                                                   // noise -> raw
     pages.push_back(Page(N, 0));                                        // zeros
     { Page p = weights(120, 6); p[5] = 0x7F80; p[300000] = 0xFFC1; p[N - 1] = 0x0001; pages.push_back(p); }                    // inf / nan / denormal at the edges
+    // K4 shares one exception counter among the 8 parts of a page and the last part to finish writes the header; K5 gives an
+    // exception to the part whose value range (kValuesPart = 131072 values) holds its index.  0x3F80 has exponent 127,
+    // 0x00D5 exponent 1: one exception each.
+    { Page p(N, 0x3F80); for (int k = 0; k < 2048; ++k) p[3 * kValuesPart + (size_t)k * 64 + 17] = 0x00D5; pages.push_back(p); }   // all 2048 in part 3
+    { Page p(N, 0x3F80); for (size_t q = 0; q < kParts; ++q) for (int k = 0; k < 256; ++k) p[q * kValuesPart + (size_t)k * 512 + 5] = 0x00D5; pages.push_back(p); }  // 256 per part
+    { Page p = weights(118, 9); for (size_t q = 0; q < kParts; ++q) { p[q * kValuesPart] = 0x00D5; p[q * kValuesPart + kValuesPart - 1] = 0x80D5; } pages.push_back(p); }  // first + last value of every part
+    {   // tile maxima 0, 1, 13, 14, 15, 255 and 127, with values exactly 13 (code 13) and 14 (code 14 for zeros, else an exception)
+        // binades below them; tiles of emax 0 hold only zeros and denormals
+        Page p(N);
+        const uint32_t emax_of[8] = {0, 1, 13, 14, 15, 255, 127, 0};
+        for (uint32_t t = 0; t < fma_codec::kTiles; ++t) {
+            const uint32_t em = emax_of[t % 8];
+            for (uint32_t i = 0; i < fma_codec::kTileValues; ++i) {
+                const uint32_t x = rnd();
+                uint32_t e = em;
+                switch (i % 4) {
+                    case 0: e = em; break;
+                    case 1: e = em >= 13 ? em - 13 : 0; break;                // code 13 (em = 13: a zero / denormal coded 13)
+                    case 2: e = 0; break;                                      // zero / denormal: code <= 13, or 14
+                    case 3: e = i == 3 && em >= 14 ? em - 14 : em >= 13 ? em - 13 : em; break;  // one value per tile 14 binades down
+                }
+                p[t * fma_codec::kTileValues + i] = (uint16_t)(((x >> 31) << 15) | (e << 7) | ((x >> 16) & 0x7F));
+            }
+        }
+        pages.push_back(p);
+    }
     if (getenv("FMA_EMU_FAST")) pages.resize(5);                        // sanitizer runs: the first five pages cover every branch but noise / inf
     const uint32_t n = (uint32_t)pages.size();
 
@@ -99,7 +134,7 @@ static int run_all() {
 
     // K4: gather in a permuted order into one contiguous store
     std::vector<uint32_t> perm(n);
-    for (uint32_t k = 0; k < n; ++k) perm[k] = (3 * k + 3) % n;          // a permutation for n = 5 and n = 8
+    for (uint32_t k = 0; k < n; ++k) perm[k] = (7 * k + 3) % n;          // a permutation for n = 5 and n = 12
     uint64_t total = 0;
     for (uint32_t p : perm) total += sizes[p];
     Bytes store(total, 0xEE);
@@ -137,6 +172,72 @@ static int run_all() {
     for (uint32_t k = 0; k < n; ++k) {
         Page out(N);
         assert(fma_oracle_unpack_page(store.data() + off[k], sizes[perm[k]], out.data()) == 0 && out == pages[perm[k]]);
+    }
+
+    // K5 reads the stored pages straight from mapped pinned host memory (the zero-copy packed wake)
+    {
+        unsigned char* h_dev = nullptr;
+        unsigned char* h = host_mapped(total, &h_dev);
+        memcpy(h, store.data(), total);
+        for (uint32_t k = 0; k < n; ++k) { d[k].src = (uint64_t)(uintptr_t)(h_dev + off[k]); std::fill(back[perm[k]].begin(), back[perm[k]].end(), 0x5A5A); }
+        err = 0;
+        assert(fma_k_launch_unpack(d.data(), n, &err, nullptr) == cudaSuccess);
+        DEVICE_SYNC();
+        assert(err == 0);
+        for (uint32_t p = 0; p < n; ++p)
+            if (back[p] != pages[p]) { fprintf(stderr, "page %u: K5 from mapped host memory differs\n", p); return 1; }
+#if defined(FMA_GPU_TEST)
+        cudaFreeHost(h);
+#else
+        free(h);
+#endif
+    }
+
+    // RAW and coded descriptors alternate in one launch with more work items than CTAs: every CTA strides over items of both
+    // kinds (K4p / K5 reuse their shared state across items, K4 its emax slice).  The CPU model's grid is 3 SMs x 8 CTAs;
+    // on the device FMA_PACK_CTAS_PER_SM=1 makes it 132 CTAs, and then the launch must reach 2 items per CTA.
+    {
+        std::vector<uint32_t> raw, coded;
+        for (uint32_t p = 0; p < n; ++p) (sizes[p] == PAGE ? raw : coded).push_back(p);
+        const uint32_t cap = pack_grid(0xFFFFFFFFu);
+        const uint32_t n_alt = std::min<uint32_t>((2 * cap + kParts - 1) / kParts + 1, 40);
+        std::vector<uint32_t> src(n_alt);
+        for (uint32_t k = 0; k < n_alt; ++k) src[k] = k % 2 ? coded[(k / 2) % coded.size()] : raw[(k / 2) % raw.size()];
+        DVec<uint64_t> atab(n_alt);
+        for (uint32_t k = 0; k < n_alt; ++k) atab[k] = tab[src[k]];
+        DVec<uint32_t> asz(n_alt, 0);
+        assert(fma_k_launch_pack_probe(atab.data(), n_alt, asz.data(), nullptr) == cudaSuccess);
+        DEVICE_SYNC();
+        std::vector<uint64_t> aoff(n_alt);
+        uint64_t atotal = 0;
+        for (uint32_t k = 0; k < n_alt; ++k) {
+            if (asz[k] != sizes[src[k]]) { fprintf(stderr, "strided probe: page %u says %u\n", k, asz[k]); return 1; }
+            aoff[k] = atotal;
+            atotal += asz[k];
+        }
+        Bytes astore(atotal, 0xEE);
+        DVec<fma_k_pack_desc> ad(n_alt);
+        for (uint32_t k = 0; k < n_alt; ++k)
+            ad[k] = fma_k_pack_desc{atab[k], (uint64_t)(uintptr_t)(astore.data() + aoff[k]), asz[k] == PAGE ? (uint32_t)FMA_K_PACK_RAW : (uint32_t)FMA_K_PACK_BF16, 0};
+        err = 0;
+        assert(fma_k_launch_pack(ad.data(), n_alt, &err, nullptr) == cudaSuccess);
+        DEVICE_SYNC();
+        assert(err == 0);
+        for (uint32_t k = 0; k < n_alt; ++k) {
+            if (!same_stored(astore.data() + aoff[k], want[src[k]].data(), asz[k])) { fprintf(stderr, "strided K4: stored page %u differs from the oracle's\n", k); return 1; }
+            Page out(N);
+            if (fma_oracle_unpack_page(astore.data() + aoff[k], asz[k], out.data()) != 0 || out != pages[src[k]]) { fprintf(stderr, "strided K4: the oracle cannot decode page %u\n", k); return 1; }
+        }
+        std::vector<Page> aback(n_alt, Page(N, 0xABCD));
+        for (uint32_t k = 0; k < n_alt; ++k) { ad[k].src = (uint64_t)(uintptr_t)(astore.data() + aoff[k]); ad[k].dst = (uint64_t)(uintptr_t)aback[k].data(); }
+        assert(fma_k_launch_unpack(ad.data(), n_alt, &err, nullptr) == cudaSuccess);
+        DEVICE_SYNC();
+        assert(err == 0);
+        for (uint32_t k = 0; k < n_alt; ++k)
+            if (aback[k] != pages[src[k]]) { fprintf(stderr, "strided K5: page %u differs\n", k); return 1; }
+        const uint32_t items = n_alt * kParts, grid = pack_grid(items);
+        printf("K4/K5 strided launch: %u pages (RAW and coded alternate), %u items, grid %u, items/grid = %.2f\n", n_alt, items, grid, (double)items / grid);
+        if ((!kOnDevice || getenv("FMA_PACK_CTAS_PER_SM")) && items < 2 * grid) { fprintf(stderr, "the strided launch has fewer than 2 items per CTA\n"); return 1; }
     }
 
     // error counters: a page forced into the coded form although it overflows; a damaged header

@@ -17,9 +17,9 @@ fma_k_tma_cfg fma_k_default_tma_cfg() { return fma_k_tma_cfg{16u << 10, 3, 2, 1}
 cudaError_t fma_k_launch_page_copy(const uint64_t* src_tab, uint64_t src_base, const uint64_t* dst_tab, uint64_t dst_base, uint32_t n_pages,
                                    int variant, const fma_k_tma_cfg* cfg, cudaStream_t) {
     if (variant != FMA_K_VARIANT_TMA && variant != FMA_K_VARIANT_LDG) return cudaErrorInvalidValue;
-    if (variant == FMA_K_VARIANT_TMA && cfg) {
-        const size_t smem = (size_t)cfg->pipes * cfg->stages * cfg->tile_bytes + 128;
-        if (cfg->tile_bytes < 1024 || (FMA_K_PAGE_BYTES % cfg->tile_bytes) || smem > 227u * 1024u) return cudaErrorInvalidValue;
+    if (variant == FMA_K_VARIANT_TMA) {  // the real wrapper's clamps and rules, so both refuse the same shapes
+        fma_k_tma_cfg c = cfg ? *cfg : fma_k_default_tma_cfg();
+        if (!fma_k_tma_shape_fits(&c)) return cudaErrorInvalidValue;
     }
     for (uint32_t p = 0; p < n_pages; ++p) {
         const uint64_t s = src_tab ? src_tab[p] : src_base + (uint64_t)p * FMA_K_PAGE_BYTES;

@@ -3,7 +3,8 @@ fma_image.cu) are compiled with g++ against a host simulation of the CUDA runtim
 VMM driver calls (tests/cpp/hostsim/, test infrastructure: mmap-backed VMM with the real map/unmap semantics, eager
 streams) and host stand-ins for the kernel launch wrappers, then
 
-  1. the GPU parity suite (tests/test_gpu_parity.py, everything that does not need torch on a GPU) runs against that
+  1. the GPU parity suite (tests/test_gpu_parity.py, test_gpu_http.py and the engine-level tests of test_gpu_kernel_shapes.py:
+     everything that does not need torch or real kernels on a GPU) runs against that
      library in a subprocess — segment table, arenas, runs, ring, mapper/unmapper threads, modes, tiers incl. the
      peer tier, swap, cold load, error handling;
   2. a C++ scenario drives the C-ABI under ThreadSanitizer and under AddressSanitizer+UBSan+LeakSanitizer, including
@@ -59,7 +60,8 @@ def _xdist():
 
 def test_parity_suite_against_the_host_simulated_engine(hostsim_lib, oracle):
     env = dict(os.environ, FMA_B200_LIB=hostsim_lib, FMA_HOSTSIM="1", HOSTSIM_DEVICES="2")
-    r = subprocess.run([sys.executable, "-m", "pytest", os.path.join(ROOT, "tests", "test_gpu_parity.py"), os.path.join(ROOT, "tests", "test_gpu_http.py"), "-x", "-q", "-m", "gpu",
+    r = subprocess.run([sys.executable, "-m", "pytest", os.path.join(ROOT, "tests", "test_gpu_parity.py"), os.path.join(ROOT, "tests", "test_gpu_http.py"),
+                        os.path.join(ROOT, "tests", "test_gpu_kernel_shapes.py"), "-x", "-q", "-m", "gpu",
                         "-k", "not shim and not torch_pool and not full_size", "-p", "no:cacheprovider", *_xdist()],
                        env=env, cwd=ROOT, capture_output=True, text=True, timeout=900)
     tail = (r.stdout + r.stderr)[-3000:]

@@ -33,8 +33,8 @@ def _build_and_run(tmp_path, src, name, san, flags, marker):
 
 
 def test_kernel_sources_on_the_cpu_execution_model(tmp_path):
-    """Four builds side by side: {packed-image kernels (K4p, K4, K5: sub-page work items, a global exception counter per page, last-part header), hot-path kernels (K0, K1/K2 TMA in
-    five shapes + LDG, K3 — the source the GPU tests run on the H100; the emulation guards leave its nvcc SASS byte-identical)}
+    """Four builds side by side: {packed-image kernels (K4p, K4, K5: sub-page work items, a global exception counter per page, last-part header), hot-path kernels (K0, K1/K2 TMA over a
+    subset of the legal shapes, clamped and refused shapes + LDG, K3 — the source the GPU tests run on the H100; the emulation guards leave its nvcc SASS byte-identical)}
     x {plain, ThreadSanitizer}, each against the oracle."""
     if not os.path.exists("/usr/local/cuda/include/cuda_runtime.h"):
         pytest.skip("CUDA headers not installed")
