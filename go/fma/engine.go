@@ -145,6 +145,8 @@ func (e *Engine) LoadFile(path string, spans []LoadSpan) (seconds float64, err e
 	return float64(st.seconds), nil
 }
 
+// Stats returns the engine's fma_stats_t as cgo sees it, so every field of include/fma_engine.h is there without a Go copy of
+// the struct, resident_bytes (the HBM a sleeping image's resident share holds on this GPU) included.
 func (e *Engine) Stats() (C.fma_stats_t, error) {
 	var st C.fma_stats_t
 	if rc := C.fma_stats(e.h, &st); rc != 0 {

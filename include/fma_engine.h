@@ -146,10 +146,14 @@ typedef struct fma_stats {
     uint64_t hbm_aux_bytes;         /* staging ring + page tables + digest scratch on this GPU           */
     uint64_t parked_bytes;          /* parking buffer held in a peer's (or this GPU's) HBM               */
     uint64_t image_store_bytes;     /* bytes the last sleep's image takes in its store: == sleep_bytes_offloaded,
-                                       or less for a PACKED image (these are the bytes that cross PCIe)    */
+                                       or less for a PACKED image (these are the bytes that cross PCIe); with a
+                                       resident share only the host-store part                              */
     uint64_t sleep_bytes_copied;    /* bytes the last sleep actually moved into the store: image_store_bytes for a full
                                        sleep, 0 for a clean INCREMENTAL sleep, the changed segments for a partial one */
-    uint64_t reserved[3];
+    uint64_t resident_bytes;        /* HBM the resident part of a sleeping host-tier image holds on this GPU now
+                                       (option "resident_bytes"; its stored bytes, in one allocation rounded up to
+                                       2 MiB); 0 when there is none                                          */
+    uint64_t reserved[2];
 } fma_stats_t;
 
 /* ---- library ---------------------------------------------------------------------- */
@@ -375,7 +379,13 @@ FMA_API int  fma_load_file(fma_engine_t* e, const char* path, const fma_load_spa
 /* Change one knob of a live engine (between operations).  Keys: "mode", "kernel",
  * "copy_streams", "chunk_bytes", "ring_slots", "map_threads", "pack", "incremental" (1 = a host-tier sleep whose offloaded segments still have the K3 digests and image
  * offsets of the copy the host store kept from the last wake releases the device side without moving a byte; anything else
- * is a full sleep), "tma_tile_bytes",
+ * is a full sleep), "resident_bytes" (cap, rounded down to 2 MiB,
+ * on the HBM a sleeping host-tier image may keep on this GPU: walking the offloaded segments from the last in image order to the
+ * first, every segment whose stored size still fits the remaining cap stays here and is restored by an HBM-to-HBM copy at wake
+ * instead of crossing PCIe; 0 = off, also FMA_RESIDENT_MIB at engine creation.  Ignored by peer / local-tier sleeps and while
+ * helper paths are configured.  Resident segments report tier FMA_TIER_LOCAL and an offset in the resident part; their pages
+ * follow the host part's in fma_image_pages.  While an image keeps a resident part, fma_image_export, fma_image_describe and
+ * fma_host_store_share return FMA_ESTATE.  If the allocation fails the sleep is a plain host-tier sleep), "tma_tile_bytes",
  * "tma_stages", "tma_pipes", "tma_ctas_per_sm", "load_threads", "load_chunk_bytes", "load_slots". */
 FMA_API int  fma_set_option(fma_engine_t* e, const char* key, int64_t value);
 
@@ -386,7 +396,9 @@ FMA_API int  fma_stats(fma_engine_t* e, fma_stats_t* out);
  *   "<op>,<kind>,<idx>,<t0_ms>,<t1_ms>,<bytes>\n"   (times since the call's entry)
  * kinds: plan, map_ring / map_backed / map_remap (one cuMemCreate+Map+SetAccess each, mapper thread), gate_wait,
  * enqueue, copies_landed, wait_all_mapped, drain, unmap (sleep), kernel (K1/K2/K4/K5 launches, device-timed), total;
- * multi-path operations add path_chunks / path_local (idx = the path's GPU, bytes = what that path moved / moved NUMA-locally).
+ * multi-path operations add path_chunks / path_local (idx = the path's GPU, bytes = what that path moved / moved NUMA-locally);
+ * a resident share adds res_alloc (sleep) / res_free (wake) for the resident buffer's VMM calls, res_fallback (its allocation
+ * failed: plain sleep), and res_gather / res_restore rows for its K1 / K4 and K2 / K5 launches (device-timed, like kernel).
  * The reference has no tracing on this path (SURVEY.md section 5); this is what shows WHICH phase bounds a wake.
  * Returns the length of the full text (call with buf=NULL to size it), or a negative error. */
 FMA_API int  fma_timeline(fma_engine_t* e, char* buf, size_t cap);

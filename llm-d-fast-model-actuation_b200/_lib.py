@@ -60,7 +60,8 @@ class fma_stats_t(C.Structure):
         ("host_store_numa_node", C.c_int32), ("tier", C.c_int32), ("mode", C.c_int32), ("image_packed", C.c_int32),
         ("total_kernel_launches", C.c_uint64), ("total_copy_ops", C.c_uint64),
         ("hbm_mapped_bytes", C.c_uint64), ("hbm_aux_bytes", C.c_uint64), ("parked_bytes", C.c_uint64),
-        ("image_store_bytes", C.c_uint64), ("sleep_bytes_copied", C.c_uint64), ("reserved", C.c_uint64 * 3),
+        ("image_store_bytes", C.c_uint64), ("sleep_bytes_copied", C.c_uint64), ("resident_bytes", C.c_uint64),
+        ("reserved", C.c_uint64 * 2),
     ]
 
     def as_dict(self) -> dict:

@@ -544,36 +544,41 @@ void paths_release(fma_engine_t* e) {
     cudaGetLastError();
 }
 
+void park_store_free(ParkStore& p) {
+    if (!p.va) return;
+    g_drv.MemUnmap(p.va, p.cap);
+    g_drv.MemRelease(p.handle);
+    g_drv.MemAddressFree(p.va, p.cap);
+    p = ParkStore{};
+}
+
 int park_release(fma_engine_t* e) {
     if (!e->park.va) return FMA_OK;
     if (e->shadow_tier != FMA_TIER_HOST) invalidate_shadows(e);  // the parking buffer held the kept image
     cudaDeviceSynchronize();
-    g_drv.MemUnmap(e->park.va, e->park.cap);
-    g_drv.MemRelease(e->park.handle);
-    g_drv.MemAddressFree(e->park.va, e->park.cap);
-    e->park = ParkStore{};
+    park_store_free(e->park);
     return FMA_OK;
 }
 
-int park_reserve(fma_engine_t* e, int park_device, size_t bytes) {
+// One VMM allocation of `bytes` in `device`'s HBM, mapped at a VA of its own with access for the engine's GPU (and for `device`):
+// the peer / local parking buffer, and the resident part of a host-tier image.
+int park_store_create(fma_engine_t* e, int device, size_t bytes, ParkStore* out) {
     bytes = round_up(std::max<size_t>(bytes, FMA_PAGE_BYTES), e->gran);
-    if (e->park.va && e->park.device == park_device && e->park.cap >= bytes) return FMA_OK;
-    park_release(e);
     int ndev = 0;
     RT(cudaGetDeviceCount(&ndev));
-    if (park_device < 0 || park_device >= ndev) return fail(FMA_EINVAL, "parking device %d not visible (have %d)", park_device, ndev);
-    if (park_device != e->device) {
+    if (device < 0 || device >= ndev) return fail(FMA_EINVAL, "parking device %d not visible (have %d)", device, ndev);
+    if (device != e->device) {
         int can = 0;
-        RT(cudaDeviceCanAccessPeer(&can, e->device, park_device));
-        if (!can) return fail(FMA_ECUDA, "device %d cannot access peer %d (no NVLink/P2P path)", e->device, park_device);
+        RT(cudaDeviceCanAccessPeer(&can, e->device, device));
+        if (!can) return fail(FMA_ECUDA, "device %d cannot access peer %d (no NVLink/P2P path)", e->device, device);
         // make sure the peer's primary context exists (cuMemCreate needs the device initialised)
-        DeviceGuard g(park_device);
+        DeviceGuard g(device);
         RT(cudaFree(nullptr));
     }
     ParkStore p;
-    p.device = park_device;
+    p.device = device;
     p.cap = bytes;
-    CUmemAllocationProp prop = device_prop(park_device);
+    CUmemAllocationProp prop = device_prop(device);
     DRV(g_drv.MemCreate(&p.handle, bytes, &prop, 0));
     CUresult r = g_drv.MemAddressReserve(&p.va, bytes, FMA_PAGE_BYTES, 0, 0);
     if (r != CUDA_SUCCESS) {
@@ -592,16 +597,39 @@ int park_reserve(fma_engine_t* e, int park_device, size_t bytes) {
     acc[0].location.id = e->device;
     acc[0].flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;
     acc[1] = acc[0];
-    acc[1].location.id = park_device;
-    r = g_drv.MemSetAccess(p.va, bytes, acc, park_device != e->device ? 2 : 1);
+    acc[1].location.id = device;
+    r = g_drv.MemSetAccess(p.va, bytes, acc, device != e->device ? 2 : 1);
     if (r != CUDA_SUCCESS) {
         g_drv.MemUnmap(p.va, bytes);
         g_drv.MemAddressFree(p.va, bytes);
         g_drv.MemRelease(p.handle);
         return fail(FMA_ECUDA, "cuMemSetAccess(park, P2P) failed: %s", cu_err(r));
     }
-    e->park = p;
+    *out = p;
     return FMA_OK;
+}
+
+int park_reserve(fma_engine_t* e, int park_device, size_t bytes) {
+    bytes = round_up(std::max<size_t>(bytes, FMA_PAGE_BYTES), e->gran);
+    if (e->park.va && e->park.device == park_device && e->park.cap >= bytes) return FMA_OK;
+    park_release(e);
+    return park_store_create(e, park_device, bytes, &e->park);
+}
+
+void resident_release(fma_engine_t* e) {
+    park_store_free(e->res);
+    e->res_packed = false;
+    e->res_off.clear();
+    e->res_bytes.clear();
+    e->res_store_bytes = 0;
+}
+
+bool resident_asleep(fma_engine_t* e) {
+    if (!e->res.va) return false;
+    std::lock_guard<std::mutex> lk(e->mu);
+    for (const Segment& s : e->segs)
+        if (s.has_backup && !s.mapped && s.backup_tier == FMA_TIER_LOCAL) return true;
+    return false;
 }
 
 // ------------------------------------------------------------------------------------
@@ -693,7 +721,7 @@ int flush_kernel_times(fma_engine_t* e) {
         // device-side timeline: launch i/2 ran [ms0, ms0 + ms) after ev_start (recorded tl_dev_base after the entry)
         if (cudaEventElapsedTime(&ms0, e->ev_start, e->ev_pool[i]) == cudaSuccess) {
             const double t0 = e->tl_entry + e->tl_dev_base + ms0 * 1e-3;
-            e->tl_add("kernel", (int)(i / 2), t0, t0 + ms * 1e-3, i / 2 < e->tl_kbytes.size() ? e->tl_kbytes[i / 2] : 0);
+            e->tl_add(i / 2 < e->tl_kkind.size() ? e->tl_kkind[i / 2] : "kernel", (int)(i / 2), t0, t0 + ms * 1e-3, i / 2 < e->tl_kbytes.size() ? e->tl_kbytes[i / 2] : 0);
         } else {
             cudaGetLastError();
         }
@@ -814,6 +842,7 @@ int fma_engine_create(int device, const fma_config_t* cfg, fma_engine_t** out) {
     if (!e->cfg.map_threads) e->cfg.map_threads = env_int("FMA_MAP_THREADS", 0);
     if (!e->cfg.pack) e->cfg.pack = env_int("FMA_PACK", 0);
     e->incremental = env_int("FMA_INCREMENTAL", 0);
+    e->resident_cap = (uint64_t)std::max(env_int("FMA_RESIDENT_MIB", 0), 0) << 20 & ~(uint64_t)(FMA_PAGE_BYTES - 1);
     e->tma.tile_bytes = (uint32_t)env_int("FMA_TMA_TILE_KIB", (int)(e->tma.tile_bytes >> 10)) << 10;
     e->tma.stages = (uint32_t)env_int("FMA_TMA_STAGES", (int)e->tma.stages);
     e->tma.pipes = (uint32_t)env_int("FMA_TMA_PIPES", (int)e->tma.pipes);
@@ -855,6 +884,7 @@ int fma_engine_destroy(fma_engine_t* e) {
     e->segs.clear();
     host_store_free(e->host);
     park_release(e);
+    resident_release(e);
     paths_release(e);
     release_ring(e);
     for (int i = 0; i < kMaxRing; ++i) {
@@ -882,6 +912,7 @@ int fma_engine_destroy(fma_engine_t* e) {
     if (e->ks) cudaStreamDestroy(e->ks);
     if (e->ev_start) cudaEventDestroy(e->ev_start);
     if (e->ev_end) cudaEventDestroy(e->ev_end);
+    if (e->ev_res_done) cudaEventDestroy(e->ev_res_done);
     cudaGetLastError();
     delete e;
     return FMA_OK;
@@ -1491,7 +1522,13 @@ int fma_image_pages(fma_engine_t* e, uint64_t* out_offsets, uint32_t* out_bytes,
         if (out_offsets) out_offsets[p] = e->image_packed ? e->img_off[p] : (uint64_t)p * FMA_PAGE_BYTES;
         if (out_bytes) out_bytes[p] = e->image_packed ? e->img_bytes[p] : (uint32_t)FMA_PAGE_BYTES;
     }
-    return (int)n;
+    // RESIDENT share: the resident part's pages follow the host part's, with offsets in the resident buffer
+    const size_t nr = e->res.va ? (e->res_packed ? e->res_bytes.size() : e->res_store_bytes / FMA_PAGE_BYTES) : 0;
+    for (size_t q = 0; q < nr && n + q < cap; ++q) {
+        if (out_offsets) out_offsets[n + q] = e->res_packed ? e->res_off[q] : (uint64_t)q * FMA_PAGE_BYTES;
+        if (out_bytes) out_bytes[n + q] = e->res_packed ? e->res_bytes[q] : (uint32_t)FMA_PAGE_BYTES;
+    }
+    return (int)(n + nr);
 }
 
 int fma_op_pack_probe(fma_engine_t* e, const uint64_t* pages, uint64_t base, uint32_t n_pages, uint32_t* out_stored_bytes, float* out_ms) {
@@ -1613,6 +1650,9 @@ int fma_set_option(fma_engine_t* e, const char* key, int64_t value) {
     } else if (k == "incremental") {
         if (value != 0 && value != 1) return fail(FMA_EINVAL, "incremental must be 0 or 1");
         e->incremental = (int)value;
+    } else if (k == "resident_bytes") {
+        if (value < 0) return fail(FMA_EINVAL, "resident_bytes must be >= 0");
+        e->resident_cap = (uint64_t)value & ~(uint64_t)(FMA_PAGE_BYTES - 1);
     } else if (k == "tma_tile_bytes") {
         if (value < 1024 || (FMA_PAGE_BYTES % (size_t)value) != 0 || value % 16) return fail(FMA_EINVAL, "bad tma tile %lld", (long long)value);
         e->tma.tile_bytes = (uint32_t)value;
@@ -1661,6 +1701,7 @@ int fma_stats(fma_engine_t* e, fma_stats_t* out) {
     out->parked_bytes = e->park.cap;
     out->image_packed = e->image_packed ? 1 : 0;
     out->image_store_bytes = e->image_store_bytes;
+    out->resident_bytes = e->res.va ? e->res_store_bytes : 0;
     return FMA_OK;
 }
 

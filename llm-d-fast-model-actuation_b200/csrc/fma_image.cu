@@ -126,6 +126,7 @@ int fma_image_export(fma_engine_t* e, int* out_fd) {
     if (check_engine(e) != FMA_OK) return FMA_EINVAL;
     std::lock_guard<std::mutex> op(e->op_mu);
     if (!out_fd) return fail(FMA_EINVAL, "out_fd is NULL");
+    if (resident_asleep(e)) return fail(FMA_ESTATE, "part of the sleeping image is resident in this process's own HBM (option resident_bytes) and cannot be handed over: set it to 0 and sleep again");
     if (e->host.fd < 0 || !e->host.base) return fail(FMA_ESTATE, "the host store is not shareable (set FMA_HOST_STORE_SHM=1 before the first sleep)");
     if (e->image_tier != FMA_TIER_HOST) return fail(FMA_ESTATE, "no host-tier image");
     std::vector<char> desc;
@@ -243,6 +244,7 @@ int fma_image_adopt(fma_engine_t* e, int fd, uint64_t tag_mask, uint32_t flags) 
 int fma_image_describe(fma_engine_t* e, int tier, void* buf, size_t cap) {
     if (check_engine(e) != FMA_OK) return FMA_EINVAL;
     std::lock_guard<std::mutex> op(e->op_mu);
+    if (resident_asleep(e)) return fail(FMA_ESTATE, "part of the sleeping image is resident in this process's own HBM (option resident_bytes) and cannot be handed over: set it to 0 and sleep again");
     if (tier != e->image_tier) return fail(FMA_ESTATE, "no image sleeps in tier %d", tier);
     std::vector<char> desc;
     int rc = image_descriptor_build(e, tier, &desc);

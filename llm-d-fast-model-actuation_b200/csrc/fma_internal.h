@@ -237,6 +237,17 @@ struct fma_engine {
 
     HostStore host;
     ParkStore park;
+    // RESIDENT share (option "resident_bytes", FMA_RESIDENT_MIB): a host-tier sleep keeps the tail of its image in ONE VMM
+    // allocation on this GPU (`res`, device == the engine's).  Segments whose bytes live there have backup_tier == FMA_TIER_LOCAL
+    // and packed_off = their offset in the resident part (its own image space, laid out like the host part).
+    uint64_t resident_cap = 0;        // option: HBM the sleeping image may keep here (2 MiB multiple; 0 = off)
+    ParkStore res;
+    bool res_packed = false;          // the resident part holds stored pages of the PACKED form (res_off / res_bytes)
+    std::vector<uint64_t> res_off;
+    std::vector<uint32_t> res_bytes;
+    uint64_t res_store_bytes = 0;     // bytes the resident part occupies in `res`
+    cudaEvent_t ev_res_done = nullptr;  // wake: the resident part's last restore launch has completed
+    std::vector<uint64_t> res_seqs;   // Segment::seq of the segments the last sleep kept resident (INCREMENTAL: same split or full sleep)
     uint64_t image_bytes = 0;  // W of the current packed image
     int image_tier = FMA_TIER_HOST;
     // PACKED host image (option "pack", fma_codec.h): image page p (= packed_off / 2 MiB) is stored at
@@ -309,6 +320,7 @@ struct fma_engine {
     std::mutex tl_mu;
     std::vector<TimelineEv> tl;
     std::vector<uint64_t> tl_kbytes;   // algorithmic bytes of each pending kernel launch (pairs in ev_pool)
+    std::vector<const char*> tl_kkind; // timeline kind of each pending kernel launch ("kernel", "res_gather", "res_restore")
     char tl_op[8] = "";
     double tl_entry = 0;               // now_s() at the operation's entry
     double tl_dev_base = 0;            // host time (since entry) at which ev_start was recorded: origin of the device-side events
@@ -316,6 +328,7 @@ struct fma_engine {
         std::lock_guard<std::mutex> lk(tl_mu);
         tl.clear();
         tl_kbytes.clear();
+        tl_kkind.clear();
         snprintf(tl_op, sizeof(tl_op), "%s", op);
         tl_entry = t_entry;
         tl_dev_base = 0;
@@ -361,6 +374,10 @@ int host_store_reserve(fma_engine_t* e, size_t bytes);
 void paths_release(fma_engine_t* e);
 int park_release(fma_engine_t* e);
 int park_reserve(fma_engine_t* e, int park_device, size_t bytes);
+int park_store_create(fma_engine_t* e, int device, size_t bytes, ParkStore* out);   // one VMM allocation, mapped for e's GPU (+ device's)
+void park_store_free(ParkStore& p);
+void resident_release(fma_engine_t* e);              // drop the resident buffer (caller: nothing on the device still reads it)
+bool resident_asleep(fma_engine_t* e);               // a sleeping image keeps part of itself in the resident buffer
 CUmemAllocationProp device_prop(int device);
 // ---- image descriptor (fma_image.cu): what a sleeping image is made of, so another engine / process can adopt it ----
 int image_descriptor_build(fma_engine_t* e, int tier, std::vector<char>* out);
@@ -407,6 +424,7 @@ struct KernelTimes {  // event pairs around each K1/K2 launch on the kernel stre
     fma_engine_t* e;
     size_t used = 0;
     uint64_t bytes = 0;
+    const char* kind = "kernel";   // timeline kind of the launches that follow
     int launch(const uint64_t* src_tab, uint64_t src_base, const uint64_t* dst_tab, uint64_t dst_base, uint32_t n_pages) {
         return launch_on(e->ks, src_tab, src_base, dst_tab, dst_base, n_pages);
     }
@@ -420,6 +438,7 @@ struct KernelTimes {  // event pairs around each K1/K2 launch on the kernel stre
         used += 2;
         bytes += 2ull * n_pages * FMA_PAGE_BYTES;
         e->tl_kbytes.push_back(2ull * n_pages * FMA_PAGE_BYTES);
+        e->tl_kkind.push_back(kind);
         return FMA_OK;
     }
     // K4 / K5 (packed image): bracket a launch the caller makes itself; `b` = algorithmic bytes (read + write)
@@ -434,6 +453,7 @@ struct KernelTimes {  // event pairs around each K1/K2 launch on the kernel stre
         used += 2;
         bytes += b;
         e->tl_kbytes.push_back(b);
+        e->tl_kkind.push_back(kind);
         return FMA_OK;
     }
     // Called after the streams are synchronised.  Reading ~100s of event pairs costs ~1 ms, so it is

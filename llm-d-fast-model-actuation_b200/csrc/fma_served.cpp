@@ -188,7 +188,7 @@ std::string stats_json() {
         fma_stats(g_ranks[i].e, &st);
         o << (i ? "," : "") << "{\"device\":" << g_ranks[i].device << ",\"sleep_seconds\":" << st.sleep_seconds << ",\"wake_seconds\":" << st.wake_seconds
           << ",\"sleep_bytes_offloaded\":" << st.sleep_bytes_offloaded << ",\"wake_bytes_restored\":" << st.wake_bytes_restored
-          << ",\"image_store_bytes\":" << st.image_store_bytes << ",\"sleep_bytes_copied\":" << st.sleep_bytes_copied << ",\"image_packed\":" << st.image_packed << ",\"hbm_mapped_bytes\":" << st.hbm_mapped_bytes << "}";
+          << ",\"image_store_bytes\":" << st.image_store_bytes << ",\"sleep_bytes_copied\":" << st.sleep_bytes_copied << ",\"image_packed\":" << st.image_packed << ",\"hbm_mapped_bytes\":" << st.hbm_mapped_bytes << ",\"resident_bytes\":" << st.resident_bytes << "}";
     }
     o << "]}";
     return o.str();

@@ -201,6 +201,7 @@ struct SleepPipe {
     uint32_t& copy_ops;
     std::function<int(uint64_t, cudaStream_t)> publish_consumed;
     const std::vector<size_t>* subset = nullptr;  // INCREMENTAL + PACKED: only these image pages (ascending) are re-coded, in place
+    bool resident = false;  // the extents go to the resident buffer (e->res, its own page layout res_off / res_bytes), not the tier's store
     int publish_gathered(size_t pages_done) { return publish_consumed((uint64_t)pages_done * FMA_PAGE_BYTES, e->ks); }
     // page table of the image (device addresses of its pages, in order) -> e->h_tab / e->d_tab
     int upload_page_table(size_t* n_pages) {
@@ -263,12 +264,14 @@ int sleep_kernel_packed(SleepPipe& pipe) {
     // over NVLink and of the parking GPU's HBM), batches as below
     rc = ensure_pack_bufs(e, n_pages);
     if (rc != FMA_OK) return rc;
-    const uint64_t dbase = store_dev_base(e, tier);
+    const uint64_t dbase = pipe.resident ? (uint64_t)e->res.va : store_dev_base(e, tier);
+    const std::vector<uint64_t>& img_off = pipe.resident ? e->res_off : e->img_off;
+    const std::vector<uint32_t>& img_bytes = pipe.resident ? e->res_bytes : e->img_bytes;
     for (size_t p = 0; p < n_pages; ++p) {
         fma_k_pack_desc& d = e->h_pdesc[p];
         d.src = e->h_tab[p];
-        d.dst = dbase + e->img_off[p];
-        d.mode = e->img_bytes[p] == FMA_PAGE_BYTES ? FMA_K_PACK_RAW : FMA_K_PACK_BF16;
+        d.dst = dbase + img_off[p];
+        d.mode = img_bytes[p] == FMA_PAGE_BYTES ? FMA_K_PACK_RAW : FMA_K_PACK_BF16;
         d.state = 0;
     }
     uint32_t* d_err = e->d_psize + e->pdesc_cap;
@@ -278,7 +281,7 @@ int sleep_kernel_packed(SleepPipe& pipe) {
     for (size_t p0 = 0; p0 < n_pages; p0 += batch) {
         const size_t np = std::min(batch, n_pages - p0);
         uint64_t stored = 0;
-        for (size_t q = p0; q < p0 + np; ++q) stored += e->img_bytes[q];
+        for (size_t q = p0; q < p0 + np; ++q) stored += img_bytes[q];
         rc = kt.begin();
         if (rc != FMA_OK) return rc;
         RT(fma_k_launch_pack(e->d_pdesc + p0, (uint32_t)np, d_err, e->ks));
@@ -305,7 +308,7 @@ int sleep_kernel(SleepPipe& pipe) {
     // K1 writes the store itself: mapped pinned host memory (PCIe posted writes) or peer/local HBM;
     // launched in slot-sized batches so finished segments can be released while later ones still move
     const size_t batch = std::max<size_t>(staged_slot(e) / FMA_PAGE_BYTES, 1);
-    const uint64_t dbase = store_dev_base(e, tier);
+    const uint64_t dbase = pipe.resident ? (uint64_t)e->res.va : store_dev_base(e, tier);
     for (size_t p0 = 0; p0 < n_pages; p0 += batch) {
         const size_t np = std::min(batch, n_pages - p0);
         rc = kt.launch(e->d_tab + p0, 0, nullptr, dbase + p0 * FMA_PAGE_BYTES, (uint32_t)np);
@@ -556,6 +559,11 @@ int do_sleep(fma_engine_t* e, uint64_t offload_mask, int tier, uint32_t flags) {
     rc = check_tma_shape(e, tier);
     if (rc != FMA_OK) return rc;
     e->tl_begin("sleep", t_entry);
+    if (e->res.va) {  // a resident buffer kept by an FMA_FLAG_KEEP_BACKUP wake: this sleep gathers its resident part afresh
+        RT(cudaDeviceSynchronize());
+        GateHold hold(kGateUnmap, 0.1);
+        resident_release(e);
+    }
 
     // plan: offloaded segments -> packed image, in (arena, VA) order.  Arenas are bump-allocated per tag, so this is
     // allocation order (the reference's dict order, cumem.py:198) unless a freed hole was reused.
@@ -572,11 +580,13 @@ int do_sleep(fma_engine_t* e, uint64_t offload_mask, int tier, uint32_t flags) {
                                                   : (e->park.va != 0 && (tier == FMA_TIER_LOCAL ? e->park.device == e->device : e->park.device != e->device));
     bool shadows_match = e->incremental && tier == e->shadow_tier && !(flags & kFlagAdopt) && kept_store;
     std::vector<uint64_t> shadow_digest;  // digest of the copy the store holds, per extent
+    std::vector<uint64_t> shadow_at;      // where the store holds it (kNoOffset: no usable copy)
     for (size_t i : by_addr) {
         Segment& s = e->segs[i];
         if (tag_bit_set(offload_mask, s.tag)) {
             shadows_match = shadows_match && s.digest_valid && s.shadow_off == W;  // same bytes expected at the same image offset
             shadow_digest.push_back(s.digest);
+            shadow_at.push_back(s.digest_valid ? s.shadow_off : kNoOffset);
             ex.push_back(Extent{i, s.va, s.bytes, W});
             W += s.bytes;
         } else {
@@ -586,6 +596,98 @@ int do_sleep(fma_engine_t* e, uint64_t offload_mask, int tier, uint32_t flags) {
         s.packed_off = kNoOffset;
         s.digest_valid = false;
     }
+    // RESIDENT share (option "resident_bytes"): the tail of the image stays in one VMM allocation on this GPU.  Walking the
+    // offloaded segments from the last to the first, a segment stays if its stored size (2 MiB pages, or its pages' PACKED sizes)
+    // still fits what is left of the cap; the host store then holds only the other segments, back to back in image order.
+    std::vector<Extent> ex_res;       // resident extents, packed_off = offset in the resident part
+    uint64_t W_all = W;
+    std::vector<uint64_t> res_seqs;
+    bool pre_planned = false, pre_packed = false;  // the PACKED plan of the host part, made here already (K4p over the whole image)
+    std::vector<uint64_t> pre_off;
+    std::vector<uint32_t> pre_bytes;
+    uint64_t pre_total = 0;
+    if (e->resident_cap && tier == FMA_TIER_HOST && e->paths.empty() && !(flags & kFlagAdopt) && W) {
+        if (e->cfg.pack && resolve_mode(e, tier) == FMA_MODE_STAGED) {
+            rc = plan_packed_image(e, ex, W, &pre_off, &pre_bytes, &pre_total, &pre_packed);
+            if (rc != FMA_OK) return rc;
+            pre_planned = true;
+        }
+        std::vector<char> res(ex.size(), 0);
+        uint64_t left = e->resident_cap, res_stored = 0;
+        for (size_t k = ex.size(); k-- > 0;) {
+            uint64_t stored = ex[k].bytes;
+            if (pre_packed) {
+                stored = 0;
+                for (uint64_t o = 0; o < ex[k].bytes; o += FMA_PAGE_BYTES) stored += pre_bytes[(ex[k].packed_off + o) / FMA_PAGE_BYTES];
+            }
+            if (stored <= left) {
+                res[k] = 1;
+                left -= stored;
+                res_stored += stored;
+            }
+        }
+        if (res_stored) {
+            ParkStore buf;
+            const double a = now_s();
+            int arc;
+            {
+                GateHold hold(kGateUnmap, 0.1);   // an allocation of a sleep: as patient as the sleep's unmaps
+                arc = park_store_create(e, e->device, res_stored, &buf);
+            }
+            const double b = now_s();
+            if (arc != FMA_OK) {  // HBM too full: a plain host-tier sleep of everything
+                e->tl_add("res_fallback", 0, a, b, res_stored);
+                cudaGetLastError();
+            } else {
+                e->tl_add("res_alloc", 0, a, b, buf.cap);
+                std::vector<Extent> ex_host;
+                std::vector<uint64_t> h_off, r_off, h_digest;
+                std::vector<uint32_t> h_bytes, r_bytes;
+                uint64_t Wh = 0, Wr = 0, hs = 0, rs = 0;
+                bool host_shadows = true;
+                for (size_t k = 0; k < ex.size(); ++k) {
+                    Extent x = ex[k];
+                    const uint64_t p0 = x.packed_off / FMA_PAGE_BYTES;
+                    if (res[k]) {
+                        x.packed_off = Wr;
+                        Wr += x.bytes;
+                        ex_res.push_back(x);
+                        res_seqs.push_back(e->segs[x.seg_index].seq);
+                    } else {
+                        x.packed_off = Wh;
+                        Wh += x.bytes;
+                        ex_host.push_back(x);
+                        host_shadows = host_shadows && shadow_at[k] == x.packed_off;
+                        h_digest.push_back(shadow_digest[k]);
+                    }
+                    if (pre_packed)
+                        for (uint64_t p = p0; p < p0 + x.bytes / FMA_PAGE_BYTES; ++p) {
+                            (res[k] ? r_off : h_off).push_back(res[k] ? rs : hs);
+                            (res[k] ? r_bytes : h_bytes).push_back(pre_bytes[p]);
+                            (res[k] ? rs : hs) += pre_bytes[p];
+                        }
+                }
+                e->res = buf;
+                e->res_packed = pre_packed;
+                e->res_off = std::move(r_off);
+                e->res_bytes = std::move(r_bytes);
+                e->res_store_bytes = res_stored;
+                ex = std::move(ex_host);
+                W = Wh;
+                shadows_match = e->incremental && tier == e->shadow_tier && kept_store && host_shadows;
+                shadow_digest = std::move(h_digest);
+                if (pre_packed) {
+                    pre_off = std::move(h_off);
+                    pre_bytes = std::move(h_bytes);
+                    pre_total = hs;
+                } else {
+                    pre_total = Wh;
+                }
+            }
+        }
+    }
+    shadows_match = shadows_match && res_seqs == e->res_seqs;  // INCREMENTAL: a different split is a full sleep
+    e->res_seqs = res_seqs;
     // INCREMENTAL sleep: does the host store still hold exactly this image?  One K3 pass over the device copy decides.
     bool clean = false, partial = false, partial_packed = false, digests_known = false;
     std::vector<Extent> dirty;        // segments whose device bytes differ from the copy in the store
@@ -656,8 +758,15 @@ int do_sleep(fma_engine_t* e, uint64_t offload_mask, int tier, uint32_t flags) {
         // host tier: through the staging ring (STAGED); parking tiers (peer / local HBM): K4 writes the store itself (KERNEL)
         const bool pack_path = (tier == FMA_TIER_HOST && mode == FMA_MODE_STAGED) || (tier != FMA_TIER_HOST && mode == FMA_MODE_KERNEL);
         if (W && e->cfg.pack && !(flags & kFlagAdopt) && pack_path) {
-            rc = plan_packed_image(e, ex, W, &pk_off, &pk_bytes, &Wp, &packed);
-            if (rc != FMA_OK) return rc;
+            if (pre_planned) {
+                pk_off = std::move(pre_off);
+                pk_bytes = std::move(pre_bytes);
+                Wp = pre_total;
+                packed = pre_packed;
+            } else {
+                rc = plan_packed_image(e, ex, W, &pk_off, &pk_bytes, &Wp, &packed);
+                if (rc != FMA_OK) return rc;
+            }
         }
         e->image_packed = packed;
         e->image_store_bytes = Wp;
@@ -701,6 +810,47 @@ int do_sleep(fma_engine_t* e, uint64_t offload_mask, int tier, uint32_t flags) {
         for (size_t k = 0; k < idx.size(); ++k) {
             e->segs[idx[k]].digest = dg[k];
             e->segs[idx[k]].digest_valid = true;
+        }
+    }
+
+    // ---- RESIDENT share: K1 / K4 gather the resident segments into e->res (HBM only, a few ms), ahead of the host part's
+    // pipeline on the kernel stream.  Synchronised before the host part starts: it rewrites the page tables, and the units
+    // that hold only resident segments are unmapped right away below.
+    CopyTimer timer{e};
+    KernelTimes kt{e};
+    uint32_t copy_ops = 0;
+    double copy_s = 0;
+    if (!ex_res.empty()) {
+        if ((flags & FMA_FLAG_VERIFY) || e->incremental) {
+            std::vector<size_t> idx;
+            for (const Extent& x : ex_res) idx.push_back(x.seg_index);
+            std::vector<uint64_t> dg;
+            rc = digest_segments(e, idx, &dg);
+            if (rc != FMA_OK) return rc;
+            for (size_t k = 0; k < idx.size(); ++k) {
+                e->segs[idx[k]].digest = dg[k];
+                e->segs[idx[k]].digest_valid = true;
+            }
+        }
+        rc = timer.begin();
+        if (rc != FMA_OK) return rc;
+        uint32_t res_launches = 0;
+        SleepPipe rp{e, ex_res, W_all - W, FMA_TIER_LOCAL, nullptr, kt, res_launches, [](uint64_t, cudaStream_t) { return FMA_OK; }};
+        rp.resident = true;
+        kt.kind = "res_gather";
+        rc = e->res_packed ? sleep_kernel_packed(rp) : sleep_kernel(rp);
+        kt.kind = "kernel";
+        if (rc != FMA_OK) return rc;
+        if (e->res_packed) RT(cudaMemcpyAsync(e->h_psize + e->pdesc_cap, e->d_psize + e->pdesc_cap, sizeof(uint32_t), cudaMemcpyDeviceToHost, e->ks));
+        RT(cudaStreamSynchronize(e->ks));
+        if (e->res_packed && e->h_psize[e->pdesc_cap])
+            return fail(FMA_EINTEGRITY, "%u page(s) changed between the pack probe and the pack: weights were written during sleep", e->h_psize[e->pdesc_cap]);
+        std::lock_guard<std::mutex> lk(e->mu);
+        for (const Extent& x : ex_res) {
+            Segment& sg = e->segs[x.seg_index];
+            sg.has_backup = true;
+            sg.backup_tier = FMA_TIER_LOCAL;
+            sg.packed_off = x.packed_off;
         }
     }
 
@@ -760,10 +910,6 @@ int do_sleep(fma_engine_t* e, uint64_t offload_mask, int tier, uint32_t flags) {
     const bool overlap_unmap = env_int("FMA_OVERLAP_UNMAP", 1) != 0;
     if (overlap_unmap) un.th = std::thread([&un] { un.run(); });
 
-    CopyTimer timer{e};
-    KernelTimes kt{e};
-    uint32_t copy_ops = 0;
-    double copy_s = 0;
     if (W && adopt) {
         publish_consumed(W, e->ks);  // nothing to copy: every offloaded unit can go at once
         e->pending_events = 0;       // no kernel ran: the per-operation kernel statistics read zero
@@ -773,8 +919,10 @@ int do_sleep(fma_engine_t* e, uint64_t offload_mask, int tier, uint32_t flags) {
         if (!e->ring_attached && env_int("FMA_RING_PERSIST", 0) == 0) release_ring(e);  // a sleeping model holds no staging ring
     } else if (W) {
         char* store = static_cast<char*>(store_copy_base(e, tier));
-        rc = timer.begin();
-        if (rc != FMA_OK) return rc;
+        if (ex_res.empty()) {  // (else the resident gather opened the device-time bracket)
+            rc = timer.begin();
+            if (rc != FMA_OK) return rc;
+        }
         SleepPipe pipe{e, partial ? dirty : ex, W, tier, store, kt, copy_ops, publish_consumed};
         if (partial_packed) {  // only the changed segments' pages are re-coded, each into its old place
             pipe.subset = &dirty_pages;
@@ -803,6 +951,12 @@ int do_sleep(fma_engine_t* e, uint64_t offload_mask, int tier, uint32_t flags) {
                 return fail(FMA_EINTEGRITY, "%u page(s) changed between the pack probe and the pack: weights were written during sleep", e->h_psize[e->pdesc_cap]);
         }
         if (env_int("FMA_RING_PERSIST", 0) == 0 || e->ring_attached) release_ring(e);  // while the unmapper finishes its last ranges
+    }
+    if (!ex_res.empty() && (!W || adopt)) {  // only the resident gather ran: close its bracket
+        rc = timer.end(&copy_s);
+        if (rc != FMA_OK) return rc;
+        rc = kt.collect();
+        if (rc != FMA_OK) return rc;
     }
     un.finish();
     if (un.error != FMA_OK) return fail(un.error, "%s", un.msg);
@@ -834,11 +988,11 @@ int do_sleep(fma_engine_t* e, uint64_t offload_mask, int tier, uint32_t flags) {
     e->image_bytes = W;
     e->image_tier = tier;
 
-    e->tl_add("total", 0, t_entry, now_s(), W);
+    e->tl_add("total", 0, t_entry, now_s(), W_all);
     e->st.sleep_seconds = now_s() - t_entry;
     e->st.sleep_copy_seconds = copy_s;
     e->st.sleep_unmap_seconds = un.seconds;
-    e->st.sleep_bytes_offloaded = W;
+    e->st.sleep_bytes_offloaded = W_all;
     {
         uint64_t copied = 0;  // what this sleep moved into the store
         if (partial) for (const Extent& x : dirty) copied += x.bytes;
@@ -851,7 +1005,7 @@ int do_sleep(fma_engine_t* e, uint64_t offload_mask, int tier, uint32_t flags) {
     e->st.total_copy_ops += copy_ops;
     e->st.tier = tier;
     e->st.mode = mode;
-    if (!W) {
+    if (!W && ex_res.empty()) {
         e->pending_events = 0;
         e->st.kernel_seconds = 0;
         e->st.kernel_bytes = 0;

@@ -26,6 +26,9 @@ struct WakePipe {
     std::function<int(size_t)> wait_mapped;
     std::function<size_t()> mapped_now;
     const char* map_msg;
+    // called after each of the pipeline's K2 / K5 launches with (image pages launched so far, image pages): a RESIDENT share's
+    // restore launches one of its pieces there, so that a ring slot's hand-back waits for at most one such launch
+    std::function<int(size_t, size_t)> between = nullptr;
 };
 
 #define PIPE_CHECK(x)                 \
@@ -123,6 +126,7 @@ int wake_packed(WakePipe& pipe) {
             RT(fma_k_launch_unpack(e->d_pdesc + sl.p0, (uint32_t)sl.np, d_err, e->ks));
             PIPE_CHECK(kt.end((uint64_t)sl.np * FMA_PAGE_BYTES + sl.bytes));
             RT(cudaEventRecord(e->ev_ring_free[slot], e->ks));
+            if (pipe.between) PIPE_CHECK(pipe.between(sl.p0 + sl.np, n_pages));
         }
     } else {
         const uint64_t sbase = store_dev_base(e, tier);
@@ -151,6 +155,7 @@ int wake_packed(WakePipe& pipe) {
             if (!copy_ops) first_copy_delay = now_s() - t_entry;
             ++copy_ops;
             p0 += np;
+            if (pipe.between) PIPE_CHECK(pipe.between(p0, n_pages));
         }
     }
     return FMA_OK;
@@ -243,6 +248,7 @@ int wake_paged(WakePipe& pipe) {
             if (!copy_ops) first_copy_delay = now_s() - t_entry;
             ++copy_ops;
             p0 += np;
+            if (pipe.between) PIPE_CHECK(pipe.between(p0, n_pages));
         }
     } else {  // STAGED: copy engine H2D store -> ring slot (starts at t=0), K2 scatter once the targets are mapped
         if (ring_run) {  // the ring is run 0 (1 GiB, ~0.2 ms to map): wait for it before the first H2D
@@ -274,6 +280,7 @@ int wake_paged(WakePipe& pipe) {
             RT(cudaEventRecord(e->ev_ring_free[slot], e->ks));
             p0 += np;
             ++c;
+            if (pipe.between) PIPE_CHECK(pipe.between(p0, n_pages));
         }
     }
     return FMA_OK;
@@ -539,6 +546,7 @@ struct MapProgress {
 
 int do_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags) {
     DeviceGuard guard(e->device);
+    auto is_resident = [&](const Segment& s) { return s.has_backup && s.backup_tier == FMA_TIER_LOCAL && e->image_tier == FMA_TIER_HOST; };
     int rc = flush_kernel_times(e);
     if (rc != FMA_OK) return rc;
     const double t_entry = now_s();
@@ -569,7 +577,9 @@ int do_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags) {
         std::vector<fma_layout::SegView> view;
         for (size_t i : cand) {
             const Segment& s = e->segs[i];
-            view.push_back(fma_layout::SegView{i, s.arena, (uint64_t)s.va, s.bytes, s.has_backup, s.packed_off});
+            // a RESIDENT share's segments (their offsets are in the resident part) are mapped after the host part's
+            const uint64_t key = is_resident(s) ? (1ull << 62) + s.packed_off : s.packed_off;
+            view.push_back(fma_layout::SegView{i, s.arena, (uint64_t)s.va, s.bytes, s.has_backup, key});
         }
         // FMA_MAP_PIECE_MIB (default 2048; 0 = whole runs): backed-up runs are mapped in pieces of about that size, cut at segment
         // boundaries.  One 15 GiB mapping has only the ring's slack of a few milliseconds, and a shared host's driver calls
@@ -595,9 +605,11 @@ int do_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags) {
     // MULTI-PATH: idle peers' PCIe links are borrowed for a host-tier wake of a plain image (fma_paths_set)
     const bool multipath = !e->paths.empty() && tier == FMA_TIER_HOST && mode == FMA_MODE_STAGED && !packed;
     {
-        uint64_t w_bytes = 0;
+        uint64_t w_bytes = 0;   // what crosses the link (a resident share's segments do not)
         for (const Run& r : runs)
-            if (r.has_backup) w_bytes += r.bytes;
+            if (r.has_backup)
+                for (size_t i : r.segs)
+                    if (!is_resident(e->segs[i])) w_bytes += e->segs[i].bytes;
         if (w_bytes && mode == FMA_MODE_STAGED && multipath) {
             // every path brings its own staging slots: no ring
         } else if (w_bytes && mode == FMA_MODE_STAGED && no_ring()) {
@@ -631,6 +643,7 @@ int do_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags) {
     }
 
     std::vector<size_t> with_backup, remap_only;  // segment indices, image order
+    std::vector<size_t> with_host, with_res;      // with_backup split by store: the host part, the RESIDENT share
     std::vector<size_t> seg_run(e->segs.size(), 0);  // segment -> index of its run in `runs`
     size_t n_backup_runs = 0;
     for (size_t r = 0; r < runs.size(); ++r) {
@@ -638,6 +651,7 @@ int do_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags) {
         for (size_t i : runs[r].segs) {
             seg_run[i] = r;
             (runs[r].has_backup ? with_backup : remap_only).push_back(i);
+            if (runs[r].has_backup) (is_resident(e->segs[i]) ? with_res : with_host).push_back(i);
         }
     }
     const bool dbg_t = env_int("FMA_DEBUG_TIMING", 0) != 0;
@@ -645,7 +659,7 @@ int do_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags) {
     double remap_delay_s;
     {
         uint64_t w_bytes = 0;
-        for (size_t i : with_backup) w_bytes += e->segs[i].bytes;
+        for (size_t i : with_host) w_bytes += e->segs[i].bytes;
         // a fifth of the expected host-tier copy time (55 GB/s), half of the NVLink one (600 GB/s): far below the slack
         // (a multi-path wake has as many links as paths: its copy time, and with it the head start, shrinks accordingly)
         const double expected = (double)w_bytes / (tier == FMA_TIER_HOST ? 55e9 * (multipath ? (double)e->paths.size() : 1.0) : 600e9);
@@ -663,7 +677,7 @@ int do_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags) {
     int gate_first = n_backup_runs ? gate_announce(kGateFirst) : 0;
     const double expected_copy_s = [&] {
         uint64_t w = 0;
-        for (size_t i : with_backup) w += e->segs[i].bytes;
+        for (size_t i : with_host) w += e->segs[i].bytes;
         return (double)w / (tier == FMA_TIER_HOST ? 55e9 * (multipath ? (double)e->paths.size() : 1.0) : 600e9);
     }();
 
@@ -805,25 +819,110 @@ int do_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags) {
     } while (0)
 
     // ---- copy pipeline --------------------------------------------------------------------------
-    uint64_t W = 0;
-    for (size_t i : with_backup) W += e->segs[i].bytes;
+    uint64_t W = 0, W_res = 0;
+    for (size_t i : with_host) W += e->segs[i].bytes;
+    for (size_t i : with_res) W_res += e->segs[i].bytes;
     CopyTimer timer{e};
     KernelTimes kt{e};
     uint32_t copy_ops = 0;
     double copy_s = 0, first_copy_delay = 0;
-    if (W) {
+    // RESIDENT share: K2 / K5 copy the resident segments from e->res into their pages, on the kernel stream in pieces of at most
+    // one ring slot, each launched between two of the host part's launches once its destination is mapped (in the second half of
+    // the host part's launches the pipeline waits for that mapping); the tables sit behind the host part's in the same buffers.
+    struct ResPiece { size_t q0, np; size_t need; uint64_t stored; };
+    std::vector<ResPiece> res_pieces;
+    size_t res_next = 0;
+    const size_t n_host_pages = W / FMA_PAGE_BYTES;
+    const bool res_packed = W_res && e->res_packed;   // (the buffer may be released before the K5 error count is read)
+    auto res_setup = [&]() -> int {
+        if (!e->res.va) return fail(FMA_ESTATE, "the resident part of the image is gone");
+        const size_t n_res = W_res / FMA_PAGE_BYTES, n_all = n_host_pages + n_res;
+        int r = ensure_tables(e, n_all);
+        if (r == FMA_OK && e->res_packed) r = ensure_pack_bufs(e, n_all);
+        if (r == FMA_OK && !e->ev_res_done && cudaEventCreateWithFlags(&e->ev_res_done, cudaEventDisableTiming) != cudaSuccess)
+            r = fail(FMA_ECUDA, "cudaEventCreate(resident) failed");
+        if (r != FMA_OK) return r;
+        std::vector<size_t> order(with_res);
+        std::sort(order.begin(), order.end(), [&](size_t a, size_t b) { return e->segs[a].packed_off < e->segs[b].packed_off; });
+        uint64_t* dst_tab = e->h_tab + n_host_pages;
+        uint64_t* src_tab = e->h_tab + e->d_tab_cap + n_host_pages;
+        const size_t piece_pages = std::max<size_t>(staged_slot(e) / FMA_PAGE_BYTES, 1);
+        size_t q = 0;
+        for (size_t i : order) {
+            const Segment& s = e->segs[i];
+            for (size_t o = 0; o < s.bytes; o += FMA_PAGE_BYTES, ++q) {
+                const size_t lp = (size_t)((s.packed_off + o) / FMA_PAGE_BYTES);
+                if (e->res_packed && lp >= e->res_off.size()) return fail(FMA_ESTATE, "segment outside the resident part's page table");
+                const uint64_t soff = e->res_packed ? e->res_off[lp] : s.packed_off + o;
+                const uint32_t sb = e->res_packed ? e->res_bytes[lp] : (uint32_t)FMA_PAGE_BYTES;
+                if (e->res_packed) {
+                    fma_k_pack_desc& pd = e->h_pdesc[n_host_pages + q];
+                    pd.src = (uint64_t)e->res.va + soff;
+                    pd.dst = (uint64_t)s.va + o;
+                    pd.mode = sb == FMA_PAGE_BYTES ? FMA_K_PACK_RAW : FMA_K_PACK_BF16;
+                    pd.state = 0;
+                } else {
+                    dst_tab[q] = (uint64_t)s.va + o;
+                    src_tab[q] = (uint64_t)e->res.va + soff;
+                }
+                if (res_pieces.empty() || res_pieces.back().np == piece_pages) res_pieces.push_back(ResPiece{q, 0, 0, 0});
+                ResPiece& pc = res_pieces.back();
+                ++pc.np;
+                pc.need = std::max(pc.need, seg_run[i] + 1);
+                pc.stored += sb;
+            }
+        }
+        if (e->res_packed) {
+            RT(cudaMemcpyAsync(e->d_pdesc + n_host_pages, e->h_pdesc + n_host_pages, n_res * sizeof(fma_k_pack_desc), cudaMemcpyHostToDevice, e->ks));
+            if (!packed) RT(cudaMemsetAsync(e->d_psize + e->pdesc_cap, 0, sizeof(uint32_t), e->ks));   // (wake_packed clears it otherwise)
+        } else {
+            RT(cudaMemcpyAsync(e->d_tab + n_host_pages, dst_tab, n_res * sizeof(uint64_t), cudaMemcpyHostToDevice, e->ks));
+            RT(cudaMemcpyAsync(e->d_tab + e->d_tab_cap + n_host_pages, src_tab, n_res * sizeof(uint64_t), cudaMemcpyHostToDevice, e->ks));
+        }
+        return FMA_OK;
+    };
+    auto res_launch_next = [&]() -> int {
+        const ResPiece& pc = res_pieces[res_next];
+        int r = wait_mapped(pc.need);
+        if (r != FMA_OK) return fail(r, "%s", prog.msg);
+        kt.kind = "res_restore";
+        if (e->res_packed) {
+            r = kt.begin();
+            if (r == FMA_OK) {
+                cudaError_t ce = fma_k_launch_unpack(e->d_pdesc + n_host_pages + pc.q0, (uint32_t)pc.np, e->d_psize + e->pdesc_cap, e->ks);
+                r = ce == cudaSuccess ? kt.end((uint64_t)pc.np * FMA_PAGE_BYTES + pc.stored) : fail(FMA_ECUDA, "K5 (resident) launch failed: %s", cudaGetErrorString(ce));
+            }
+        } else {
+            r = kt.launch(e->d_tab + e->d_tab_cap + n_host_pages + pc.q0, 0, e->d_tab + n_host_pages + pc.q0, 0, (uint32_t)pc.np);
+        }
+        kt.kind = "kernel";
+        if (r != FMA_OK) return r;
+        if (++res_next == res_pieces.size()) RT(cudaEventRecord(e->ev_res_done, e->ks));
+        return FMA_OK;
+    };
+    auto res_pump = [&](size_t done, size_t total) -> int {
+        if (res_next >= res_pieces.size()) return FMA_OK;
+        if (2 * done < total && mapped_now() < res_pieces[res_next].need) return FMA_OK;
+        return res_launch_next();
+    };
+    if (W || W_res) {
         const char* store = static_cast<const char*>(store_copy_base(e, tier));
-        if (!store) WAKE_CHECK(fail(FMA_ESTATE, "backup store of tier %d is gone", tier));
-        if (tier == FMA_TIER_HOST && mode == FMA_MODE_KERNEL && !e->host.dev_alias)
+        if (W && !store) WAKE_CHECK(fail(FMA_ESTATE, "backup store of tier %d is gone", tier));
+        if (W && tier == FMA_TIER_HOST && mode == FMA_MODE_KERNEL && !e->host.dev_alias)
             WAKE_CHECK(fail(FMA_ECUDA, "host store has no device alias for zero-copy mode"));
         WAKE_CHECK(timer.begin());
-        WakePipe pipe{e, with_backup, seg_run, W, tier, mode, ring_run, store, kt, copy_ops, first_copy_delay, t_entry, wait_mapped, mapped_now, prog.msg};
-        const double t_enq0 = now_s();
-        if (packed) WAKE_CHECK(wake_packed(pipe));
-        else if (multipath) WAKE_CHECK(wake_multipath(pipe));
-        else if (mode == FMA_MODE_DIRECT) WAKE_CHECK(wake_direct(pipe));
-        else WAKE_CHECK(wake_paged(pipe));
-        e->tl_add("enqueue", (int)copy_ops, t_enq0, now_s(), W);
+        if (W_res) WAKE_CHECK(res_setup());
+        if (W) {
+            WakePipe pipe{e, with_host, seg_run, W, tier, mode, ring_run, store, kt, copy_ops, first_copy_delay, t_entry, wait_mapped, mapped_now, prog.msg};
+            if (W_res) pipe.between = res_pump;
+            const double t_enq0 = now_s();
+            if (packed) WAKE_CHECK(wake_packed(pipe));
+            else if (multipath) WAKE_CHECK(wake_multipath(pipe));
+            else if (mode == FMA_MODE_DIRECT) WAKE_CHECK(wake_direct(pipe));
+            else WAKE_CHECK(wake_paged(pipe));
+            e->tl_add("enqueue", (int)copy_ops, t_enq0, now_s(), W);
+        }
+        while (res_next < res_pieces.size()) WAKE_CHECK(res_launch_next());   // what the host part's launches left (or had no room for)
     }
     if (remap_after_copy && W) {  // let the DMA finish before the remap-only runs are touched
         const double t_w0 = now_s();
@@ -844,13 +943,30 @@ int do_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags) {
         gate_retract(gate_first);
         gate_first = 0;
     }
+    // RESIDENT share: the buffer goes once its restore has completed and every run is mapped (a wake that fails before that is
+    // rolled back and its retry needs the buffer), under the host part's copy; it stays while a resident segment still sleeps
+    // (tag-selective wake) and with FMA_FLAG_KEEP_BACKUP.
+    if (e->res.va && !(flags & FMA_FLAG_KEEP_BACKUP)) {
+        bool still_asleep = false;
+        for (const Segment& s : e->segs) still_asleep = still_asleep || (is_resident(s) && !s.mapped);
+        if (!still_asleep) {
+            if (res_next) WAKE_RT(cudaEventSynchronize(e->ev_res_done));
+            const double a = now_s();
+            const uint64_t cap = e->res.cap;
+            {
+                GateHold hold(kGateUnmap, 0.1);
+                resident_release(e);
+            }
+            e->tl_add("res_free", 0, a, now_s(), cap);
+        }
+    }
     const double t_joined = now_s();
     double t_copy_end = t_joined;
-    if (W) {
+    if (W || W_res) {
         WAKE_CHECK(timer.end(&copy_s));
         e->tl_add("drain", 0, t_joined, now_s(), W);
         WAKE_CHECK(kt.collect());
-        if (packed) {  // K5 counts stored pages it could not read (bad magic / count): the image is damaged
+        if (packed || res_packed) {  // K5 counts stored pages it could not read (bad magic / count): the image is damaged
             WAKE_RT(cudaMemcpyAsync(e->h_psize + e->pdesc_cap, e->d_psize + e->pdesc_cap, sizeof(uint32_t), cudaMemcpyDeviceToHost, e->ks));
             WAKE_RT(cudaStreamSynchronize(e->ks));
             if (e->h_psize[e->pdesc_cap]) WAKE_CHECK(fail(FMA_EINTEGRITY, "%u stored page(s) of the packed image are malformed", e->h_psize[e->pdesc_cap]));
@@ -867,7 +983,7 @@ int do_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags) {
     for (size_t i : remap_only) remapped_only += e->segs[i].bytes;
 
     int verify_rc = FMA_OK;
-    if ((flags & FMA_FLAG_VERIFY) && W) {
+    if ((flags & FMA_FLAG_VERIFY) && (W || W_res)) {
         std::vector<size_t> idx;
         for (size_t i : with_backup)
             if (e->segs[i].digest_valid) idx.push_back(i);
@@ -884,7 +1000,8 @@ int do_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags) {
         for (size_t i : with_backup) {  // data.cpu_backup_tensor = None (cumem.py:249)
             Segment& s = e->segs[i];
             // INCREMENTAL sleep: the host store keeps these bytes; remember where, together with their digest
-            s.shadow_off = (s.digest_valid && verify_rc == FMA_OK) ? s.packed_off : kNoOffset;   // host store or parking buffer: both outlive the wake
+            const bool kept = s.digest_valid && verify_rc == FMA_OK && !is_resident(s);   // (the resident buffer does not outlive the wake)
+            s.shadow_off = kept ? s.packed_off : kNoOffset;   // host store or parking buffer: both outlive the wake
             s.has_backup = false;
             s.packed_off = kNoOffset;
         }
@@ -896,18 +1013,18 @@ int do_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags) {
         }
     }
 
-    e->tl_add("total", 0, t_entry, now_s(), W);
+    e->tl_add("total", 0, t_entry, now_s(), W + W_res);
     e->st.wake_seconds = now_s() - t_entry;
     e->st.wake_copy_seconds = copy_s;
     e->st.wake_map_seconds = map_ns.load() * 1e-9;
     e->st.wake_first_copy_delay = first_copy_delay;
-    e->st.wake_bytes_restored = W;
+    e->st.wake_bytes_restored = W + W_res;
     e->st.wake_bytes_remapped_only = remapped_only;
     e->st.copy_ops = copy_ops;
     e->st.total_copy_ops += copy_ops;
     e->st.tier = tier;
     e->st.mode = mode;
-    if (!W) {
+    if (!W && !W_res) {
         e->pending_events = 0;
         e->st.kernel_seconds = 0;
         e->st.kernel_bytes = 0;

@@ -142,11 +142,17 @@ class CuMemAllocator:
                         raise
                     logger.warning("fma_b200: GPU %d cannot take %.2f GiB right now (%s): sleeping to the host tier instead", peer, nbytes / 1024**3, e.message)
                     tier = L.FMA_TIER_HOST
+        deposit_host = (tier == L.FMA_TIER_HOST and os.environ.get("FMA_DEPOSIT_HOST_IMAGE") == "1" and os.environ.get("FMA_NODE_AGENT_SOCK")
+                        and os.environ.get("FMA_HOST_STORE_SHM") == "1")
+        if deposit_host:
+            # a resident share lives in this process's HBM and cannot be handed over: the deposit wins
+            if int(os.environ.get("FMA_RESIDENT_MIB", "0") or 0) > 0:
+                logger.warning("fma_b200: FMA_DEPOSIT_HOST_IMAGE=1 takes precedence over FMA_RESIDENT_MIB: the whole image goes to the host store")
+            self.engine.set_option("resident_bytes", 0)
         self.engine.sleep(offload_tags, tier=tier)
         if owner is not None and self.engine.stats()["sleep_bytes_offloaded"]:
             owner.deposit(self.engine, _instance_id(), _rank(), tier)
-        elif (tier == L.FMA_TIER_HOST and os.environ.get("FMA_DEPOSIT_HOST_IMAGE") == "1" and os.environ.get("FMA_NODE_AGENT_SOCK")
-              and os.environ.get("FMA_HOST_STORE_SHM") == "1" and self.engine.stats()["sleep_bytes_offloaded"]):
+        elif deposit_host and self.engine.stats()["sleep_bytes_offloaded"]:
             # HOST tier, opt-in: hand the memfd behind the store to the node agent so the image outlives this process.  The exported
             # store is read-only from then on: this engine's NEXT sleep takes (and pins) a fresh private store — right for an instance
             # that is about to be deleted, wrong for one that sleeps and wakes all day, hence not the default.

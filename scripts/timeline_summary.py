@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Summarise the per-rank phase timelines bench.py --timeline wrote (fma_timeline) as markdown: for every rank the VMM calls of
 the wake's mapper thread (start, duration, bytes), when the enqueue finished, the cadence of the K2 launches (= arrival of the H2D
-ring slots: a gap longer than one slot's DMA time is a stall) and the total.
+ring slots: a gap longer than one slot's DMA time is a stall), for a resident share when its restore and the buffer's release
+ended against the last K2 (both should end before it: off the critical path), and the total.
 
     python scripts/timeline_summary.py gpurun_out/tl/A [label] >> profiles/wake_timeline_r2.md
 """
@@ -26,8 +27,8 @@ def main():
     if not files:
         sys.exit(f"no timelines under {d}")
     print(f"\n### {label}\n")
-    print("| rank | wake total ms | plan ms | ring map (start→dur) | backed maps: n, first start→last end, Σdur, max dur | remap maps (start→dur, GiB) | gate waits Σ ms | enqueue end ms | K2: n, first begin, last end, median gap ms, max gap ms (at) | drain ms |")
-    print("|---|---|---|---|---|---|---|---|---|---|")
+    print("| rank | wake total ms | plan ms | ring map (start→dur) | backed maps: n, first start→last end, Σdur, max dur | remap maps (start→dur, GiB) | gate waits Σ ms | enqueue end ms | K2: n, first begin, last end, median gap ms, max gap ms (at) | resident: restore end, release end ms | drain ms |")
+    print("|---|---|---|---|---|---|---|---|---|---|---|")
     for f in files:
         rows = [r for r in load(f) if r["op"] == "wake"]
         rank = os.path.basename(f).split("rank")[1].split(".")[0]
@@ -50,9 +51,11 @@ def main():
             k_s = f"{len(k)}, {k[0]['t0_ms']:.1f}, {k[-1]['t1_ms']:.1f}, {statistics.median(gaps):.2f}, {gaps[gi]:.1f} (@{k[gi]['t0_ms']:.0f})"
         else:
             k_s = f"{len(k)}"
+        rr, rf = by("res_restore"), by("res_free")
+        res_s = (f"{max(r['t1_ms'] for r in rr):.1f}, " + (f"{rf[0]['t1_ms']:.1f}" if rf else "–")) if rr else "–"
         dr = by("drain")
         dr_s = f"{dr[0]['t1_ms'] - dr[0]['t0_ms']:.1f}" if dr else "–"
-        print(f"| {rank} | {tot:.1f} | {plan:.2f} | {ring_s} | {mb_s} | {mr_s} | {gw:.1f} | {enq:.1f} | {k_s} | {dr_s} |")
+        print(f"| {rank} | {tot:.1f} | {plan:.2f} | {ring_s} | {mb_s} | {mr_s} | {gw:.1f} | {enq:.1f} | {k_s} | {res_s} | {dr_s} |")
 
 
 if __name__ == "__main__":
