@@ -12,6 +12,8 @@ import subprocess
 import numpy as np
 import pytest
 
+from tests.pagegen import stamp
+
 pytestmark = pytest.mark.gpu
 
 PAGE = 2 << 20
@@ -114,7 +116,8 @@ def test_zero_copy_packed_wake_reads_the_pinned_store(engine, oracle, monkeypatc
     store through its device alias (mode DIRECT); tag by tag, then everything; bytes and device addresses unchanged."""
     L = _L()
     uni, noise, cap = _pages_for_packing(oracle)
-    blobs = {"weights": np.concatenate([uni, noise, cap, uni]), "lora": np.concatenate([cap, noise, uni])}
+    blobs = {"weights": stamp(np.concatenate([uni, noise, cap, uni]), 23, 0),      # every page its own (tests/pagegen.py)
+             "lora": stamp(np.concatenate([cap, noise, uni]), 23, 4)}
     ptrs, idx = [], {}
     for tag in ("weights", "kv_cache", "lora"):
         ptrs.append(engine.alloc(blobs[tag].size if tag in blobs else 2 * PAGE, tag))

@@ -8,6 +8,8 @@ import os
 import numpy as np
 import pytest
 
+from tests.pagegen import all_distinct, pages_of, repeat_page, stamp
+
 pytestmark = pytest.mark.gpu
 
 PAGE = 2 << 20
@@ -901,7 +903,7 @@ def test_full_size_llama3_70b_tp8_shard_roundtrip_properties(engine, oracle):
     """Config[2] at full size: one rank's Llama-3-70B TP=8 shard (404 segments incl. kv_cache, 16.44 GiB of weights, the table of
     every N>1 bench line), through the plain, the PACKED (K4p / K4 / K5 on bf16-looking contents in a third of the segments) and the
     INCREMENTAL paths: every K3 digest, the checksum of checksums and every device address unchanged; spot-checked segments equal
-    the oracle's bytes; the packed image's host bytes of a spot-checked segment equal the oracle's stored pages."""
+    the oracle's bytes, and a seeded sample of coded pages (each one distinct) equal their own bytes."""
     from fma_b200 import workloads as W
 
     L = _L()
@@ -913,11 +915,16 @@ def test_full_size_llama3_70b_tp8_shard_roundtrip_properties(engine, oracle):
     weights = [i for i, s in enumerate(table) if s.tag == "weights"]
     for i in weights:
         engine.fill(i, 4321, first); firsts[i] = first; first += table[i].bytes // 8
-    # a third of the segments get bf16-looking contents (they code; the splitmix ones stay raw): one 2 MiB pattern page, repeated
+    # a third of the segments get bf16-looking contents (they code; the splitmix ones stay raw): one 2 MiB pattern page, repeated,
+    # every copy stamped with its own id (tests/pagegen.py) so that a page restored to another page's place changes the digest
     page = oracle.bf16_weights(1 << 20, 7).view(np.uint8)
     coded = weights[::3]
+    first_page = {}
     for i in coded:
-        engine.write(i, np.resize(page, table[i].bytes).tobytes())
+        first_page[i] = sum(table[j].bytes for j in coded if j < i) // PAGE
+        seg = repeat_page(page, table[i].bytes, seed=7, first_page=first_page[i])
+        engine.write_ptr(i, seg.ctypes.data, seg.size)
+        del seg
     before = engine.digest_all(["weights"])
     spot = [i for i in weights if i not in coded and table[i].bytes <= (32 << 20)][:3]
     for i in spot:
@@ -943,7 +950,12 @@ def test_full_size_llama3_70b_tp8_shard_roundtrip_properties(engine, oracle):
                 assert engine.stats()["wake_seconds"] < 3.0                 # north_star: host-tier wake of a 70B TP=8 shard <= 3.0 s
     for i in spot:
         assert engine.read(i, table[i].bytes) == oracle.fill(table[i].bytes, 4321, firsts[i]).tobytes()
-    assert engine.read(coded[0], 4 << 20) == np.resize(page, 4 << 20).tobytes()
+    rng = np.random.default_rng(70)                                 # a seeded sample of coded pages, read back whole
+    sample = [(i, k) for i in coded for k in range(table[i].bytes // PAGE)]
+    for n in sorted(rng.choice(len(sample), 8, replace=False)):
+        i, k = sample[n]
+        got = np.frombuffer(engine.read(i, PAGE, offset=k * PAGE), np.uint8)
+        assert np.array_equal(got, stamp(page, 7, first_page[i] + k)), (i, k)
 
 
 # ---- image hand-over between processes (memfd host store).
@@ -980,7 +992,8 @@ def test_image_handover_to_another_engine_and_process(engine, oracle, monkeypatc
         engine.set_option("mode", L.FMA_MODE_STAGED)
         engine.set_option("pack", 1)
         for k, i in enumerate(sorted(ref)):
-            ref[i] = np.resize(oracle.bf16_weights(1 << 20, 100 + k).view(np.uint8), table[i].bytes)
+            # every page distinct (tests/pagegen.py); page ids k * 64 on, as no segment of this table has more than 16 pages
+            ref[i] = repeat_page(oracle.bf16_weights(1 << 20, 100 + k), table[i].bytes, seed=100, first_page=k * 64)
             engine.write(i, ref[i].tobytes())
     want = engine.digest_all(["weights"])
     with pytest.raises(FmaError):
@@ -1031,7 +1044,7 @@ def test_image_saved_to_a_file_and_loaded_by_a_fresh_engine(engine, oracle, monk
         engine.set_option("mode", L.FMA_MODE_STAGED)
         engine.set_option("pack", 1)
         for k, i in enumerate(sorted(ref)):
-            ref[i] = np.resize(oracle.bf16_weights(1 << 20, 200 + k).view(np.uint8), table[i].bytes)
+            ref[i] = repeat_page(oracle.bf16_weights(1 << 20, 200 + k), table[i].bytes, seed=200, first_page=k * 64)
             engine.write(i, ref[i].tobytes())
     want = engine.digest_all(["weights"])
     engine.sleep(["weights"], flags=L.FMA_FLAG_VERIFY)
@@ -1264,13 +1277,17 @@ def test_packed_image_with_two_offloaded_tags_woken_separately(engine, oracle):
 def test_packed_random_tables_and_wake_orders(built, oracle, seed):
     """Seeded random tables (sizes, tags, page kinds), ring shapes and wake orders: whatever the plan, every offloaded byte
     comes back, discarded tags come back mapped, addresses do not move, and the stored size is what the oracle's per-page
-    decisions add up to (or the plain size when packing would save < 5 %)."""
+    decisions add up to (or the plain size when packing would save < 5 %).  Each use of a pool page is stamped with its
+    (segment, page) position (tests/pagegen.py), so no two pages of a table are alike and a page woken in another's place shows."""
     import fma_b200
 
     L = _L()
     rng = np.random.default_rng(seed)
     pool = _pack_pages(oracle)
     stored_size = [oracle.pack_page(p).size for p in pool]
+
+    def contents(i, kinds):                                             # segment i: at most 4 pages, ids 8 i .. 8 i + 3
+        return b"".join(stamp(pool[k], seed, 8 * i + j).tobytes() for j, k in enumerate(kinds))
     with fma_b200.Engine(0) as eng:
         segs, tags = [], ["weights", "adapters", "kv_cache", "scratch"]
         for _ in range(int(rng.integers(3, 9))):
@@ -1278,8 +1295,10 @@ def test_packed_random_tables_and_wake_orders(built, oracle, seed):
             kinds = [int(k) for k in rng.integers(0, len(pool), int(rng.integers(1, 5)))]
             ptr = eng.alloc(len(kinds) * PAGE, tag)
             segs.append((tag, kinds, ptr))
-        for i, (tag, kinds, _) in enumerate(segs):
-            eng.write(i, b"".join(pool[k].tobytes() for k in kinds))
+        data = [contents(i, kinds) for i, (_, kinds, _) in enumerate(segs)]
+        assert all_distinct(pages_of(np.frombuffer(b"".join(data), np.uint8)))
+        for i, d in enumerate(data):
+            eng.write(i, d)
         offload = [t for t in ("weights", "adapters") if rng.random() < 0.8] or ["weights"]
         eng.set_option("mode", L.FMA_MODE_STAGED)
         eng.set_option("pack", 1)
@@ -1310,15 +1329,16 @@ def test_packed_random_tables_and_wake_orders(built, oracle, seed):
             assert [s.va for s in info] == [p for _, _, p in segs]
             for i, (tag, kinds, _) in enumerate(segs):
                 if tag in offload:
-                    assert eng.read(i, len(kinds) * PAGE) == b"".join(pool[k].tobytes() for k in kinds), (seed, cycle, i)
+                    assert eng.read(i, len(kinds) * PAGE) == data[i], (seed, cycle, i)
                 else:                                                   # discarded: mapped again, contents undefined -> rewrite
-                    eng.write(i, b"".join(pool[k].tobytes() for k in kinds))
+                    eng.write(i, data[i])
             if rng.random() < 0.5:                                      # a segment gets new page kinds while awake (incremental: partial / full)
                 j = int(rng.integers(0, len(segs)))
                 tag, kinds, ptr = segs[j]
                 kinds = [int(k) for k in rng.integers(0, len(pool), len(kinds))]
                 segs[j] = (tag, kinds, ptr)
-                eng.write(j, b"".join(pool[k].tobytes() for k in kinds))
+                data[j] = contents(j, kinds)
+                eng.write(j, data[j])
 
 
 
@@ -1451,7 +1471,7 @@ def test_incremental_sleep_moves_nothing_when_the_weights_did_not_change(engine,
     ptrs, ref = _load(engine, oracle, table)
     if pack:
         for k, i in enumerate(sorted(ref)):
-            ref[i] = np.resize(oracle.bf16_weights(1 << 20, 300 + k).view(np.uint8), table[i].bytes)
+            ref[i] = repeat_page(oracle.bf16_weights(1 << 20, 300 + k), table[i].bytes, seed=300, first_page=k * 64)
             engine.write(i, ref[i].tobytes())
         engine.set_option("pack", 1)
     engine.set_option("mode", L.FMA_MODE_STAGED)

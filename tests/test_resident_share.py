@@ -10,6 +10,8 @@ import sys
 import numpy as np
 import pytest
 
+from tests.pagegen import pages_of, repeat_page
+
 PAGE = 2 << 20
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 gpu = pytest.mark.gpu
@@ -31,7 +33,7 @@ def _n_gpus():
 
 def _load(engine, oracle, bf16):
     """tiny-llama-test table: nine weight segments (2..32 MiB) and two kv_cache segments.  bf16=True: dummy bf16 weights that
-    the PACKED form codes (U(-1e-3, 1e-3)), else K0 fill."""
+    the PACKED form codes (U(-1e-3, 1e-3)), every page of them distinct (tests/pagegen.py), else K0 fill."""
     from fma_b200 import workloads as W
 
     table = W.allocation_table("tiny-llama-test", kv_cache_bytes=32 << 20, kv_tensors=2)
@@ -41,7 +43,8 @@ def _load(engine, oracle, bf16):
         if s.tag != "weights":
             continue
         if bf16:
-            ref[i] = np.resize(oracle.bf16_weights(1 << 20, 300 + i).view(np.uint8), s.bytes)
+            ref[i] = repeat_page(oracle.bf16_weights(1 << 20, 300 + i), s.bytes, seed=300, first_page=first)
+            first += s.bytes // PAGE
             engine.write(i, ref[i].tobytes())
         else:
             engine.fill(i, 1234, first)
@@ -62,10 +65,6 @@ def _resident_split(stored_sizes, budget):
             keep[k] = True
             left -= stored_sizes[k]
     return keep
-
-
-def _pages(buf):
-    return [buf[o:o + PAGE] for o in range(0, buf.size, PAGE)]
 
 
 def _host_image(engine):
@@ -106,7 +105,7 @@ def test_resident_share_roundtrip_matches_oracle(engine, oracle, monkeypatch, pa
     if mode == "noring":
         monkeypatch.setenv("FMA_NO_RING", "1")
     coded = pack and mode in ("staged", "noring")           # the stored sizes the split counts: the PACKED form's when this sleep codes
-    stored_pages = {i: [oracle.pack_page(p) if coded else p for p in _pages(ref[i])] for i in widx}
+    stored_pages = {i: [oracle.pack_page(p) if coded else p for p in pages_of(ref[i])] for i in widx}
     stored = [sum(p.size for p in stored_pages[i]) for i in widx]
     W = sum(ref[i].size for i in widx)
     cap = {"zero": 0, "below_smallest": (min(stored) - 1) // PAGE * PAGE, "one_segment": -(-stored[-1] // PAGE) * PAGE,
@@ -123,7 +122,7 @@ def test_resident_share_roundtrip_matches_oracle(engine, oracle, monkeypatch, pa
     host_packed = coded and mode == "staged"                  # without a ring the host part goes plain; the resident part stays coded
     assert st["resident_bytes"] == res_stored
     assert st["image_packed"] == (1 if host_packed and host else 0)
-    host_stored = [p for i in host for p in (stored_pages[i] if host_packed else _pages(ref[i]))]
+    host_stored = [p for i in host for p in (stored_pages[i] if host_packed else pages_of(ref[i]))]
     assert st["image_store_bytes"] == sum(p.size for p in host_stored)
     if budget == "zero" or (budget == "below_smallest" and not any(keep)):
         assert st["resident_bytes"] == 0 and all(s.tier == L.FMA_TIER_HOST for s in segs if s.has_backup)
