@@ -710,6 +710,12 @@ size_t build_page_table(const std::vector<Extent>& ex, uint64_t* tab) {
     return n;
 }
 
+int check_pack_errors(fma_engine_t* e, const char* fmt) {
+    RT(cudaMemcpyAsync(e->h_psize + e->pdesc_cap, e->d_psize + e->pdesc_cap, sizeof(uint32_t), cudaMemcpyDeviceToHost, e->ks));
+    RT(cudaStreamSynchronize(e->ks));
+    if (e->h_psize[e->pdesc_cap]) return fail(FMA_EINTEGRITY, fmt, e->h_psize[e->pdesc_cap]);
+    return FMA_OK;
+}
 
 int flush_kernel_times(fma_engine_t* e) {
     if (!e->pending_events) return FMA_OK;
@@ -1567,11 +1573,7 @@ static int run_pack_op(fma_engine_t* e, bool unpack, const uint64_t* dev_pages, 
         if (stored_bytes[p] != FMA_K_PACKED_PAGE_BYTES && stored_bytes[p] != FMA_PAGE_BYTES)
             return fail(FMA_EINVAL, "stored size %u of page %u is neither packed nor raw", stored_bytes[p], p);
         const uint64_t dev = dev_pages ? dev_pages[p] : dev_base + (uint64_t)p * FMA_PAGE_BYTES;
-        fma_k_pack_desc& d = e->h_pdesc[p];
-        d.src = unpack ? store_base + off : dev;
-        d.dst = unpack ? dev : store_base + off;
-        d.mode = stored_bytes[p] == FMA_PAGE_BYTES ? FMA_K_PACK_RAW : FMA_K_PACK_BF16;
-        d.state = 0;
+        set_pack_desc(e->h_pdesc[p], unpack ? store_base + off : dev, unpack ? dev : store_base + off, stored_bytes[p]);
         off += stored_bytes[p];
     }
     uint32_t* d_err = e->d_psize + e->pdesc_cap;
@@ -1581,13 +1583,11 @@ static int run_pack_op(fma_engine_t* e, bool unpack, const uint64_t* dev_pages, 
     if (unpack) RT(fma_k_launch_unpack(e->d_pdesc, n_pages, d_err, e->ks));
     else RT(fma_k_launch_pack(e->d_pdesc, n_pages, d_err, e->ks));
     RT(cudaEventRecord(e->ev_end, e->ks));
-    RT(cudaMemcpyAsync(e->h_psize + e->pdesc_cap, d_err, sizeof(uint32_t), cudaMemcpyDeviceToHost, e->ks));
-    RT(cudaStreamSynchronize(e->ks));
+    rc = check_pack_errors(e, unpack ? "%u page(s) could not be decoded (malformed stored page)"
+                                     : "%u page(s) could not be coded (more exceptions than the probe saw)");
     e->st.total_kernel_launches += 1;
     if (out_ms) RT(cudaEventElapsedTime(out_ms, e->ev_start, e->ev_end));
-    if (e->h_psize[e->pdesc_cap])
-        return fail(FMA_EINTEGRITY, "%u page(s) could not be %s", e->h_psize[e->pdesc_cap], unpack ? "decoded (malformed stored page)" : "coded (more exceptions than the probe saw)");
-    return FMA_OK;
+    return rc;
 }
 
 int fma_op_pack(fma_engine_t* e, const uint64_t* src_pages, uint64_t src_base, uint64_t dst_base, const uint32_t* stored_bytes,

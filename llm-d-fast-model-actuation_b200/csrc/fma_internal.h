@@ -153,7 +153,7 @@ struct HostStore {
     size_t map_bytes = 0;       // bytes mapped at base (cap + descriptor tail for memfd stores)
     // NUMA placement by byte range (MULTI-PATH wake: each path pulls the part of the image that lives on ITS GPU's node, so no
     // path drags its share across the socket interconnect); one range covering everything otherwise
-    struct NumaRange { size_t begin, end; int node; };
+    using NumaRange = fma_layout::NumaRange;
     std::vector<NumaRange> ranges;
     std::string placed_for;     // "node:paths,node:paths" the striping was computed for ("" = one node)
 };
@@ -473,6 +473,30 @@ int check_tma_shape(const fma_engine_t* e, int tier);
 uint64_t store_dev_base(const fma_engine_t* e, int tier);
 void* store_copy_base(const fma_engine_t* e, int tier);
 int digest_segments(fma_engine_t* e, const std::vector<size_t>& idx, std::vector<uint64_t>* out);
+
+static_assert(fma_layout::kPageBytes == FMA_PAGE_BYTES, "the layout planner's page is the engine's page");
+using fma_layout::Batch;
+using fma_layout::PagePlan;
+// pages per launch of K1 / K2 / K4 / K5 when they read or write the store in place, counted even when the pages are packed
+inline size_t slot_pages(const fma_engine_t* e) { return std::max<size_t>(staged_slot(e) / FMA_PAGE_BYTES, 1); }
+
+// K4 / K5 descriptor of one page: a stored size of a whole page means the page is stored verbatim
+inline void set_pack_desc(fma_k_pack_desc& d, uint64_t src, uint64_t dst, uint32_t stored_bytes) {
+    d.src = src;
+    d.dst = dst;
+    d.mode = stored_bytes == FMA_PAGE_BYTES ? FMA_K_PACK_RAW : FMA_K_PACK_BF16;
+    d.state = 0;
+}
+// Reads the K4 / K5 error counter d_psize[pdesc_cap] (synchronises the kernel stream); a non-zero count fails with
+// FMA_EINTEGRITY and `fmt`, which takes the count as its one %u.
+int check_pack_errors(fma_engine_t* e, const char* fmt);
+// No kernel ran in this operation: its kernel statistics read zero.
+inline void zero_kernel_stats(fma_engine_t* e) {
+    e->pending_events = 0;
+    e->st.kernel_seconds = 0;
+    e->st.kernel_bytes = 0;
+    e->st.kernel_launches = 0;
+}
 
 
 }  // namespace fma_impl

@@ -5,6 +5,42 @@
 
 namespace fma_impl {
 
+namespace {
+
+// K4p over the pages of `ex`: the stored size of each lands in e->h_psize[0, n_pages).  pack_pages: descriptors to provide for.
+int pack_probe(fma_engine_t* e, const std::vector<Extent>& ex, size_t n_pages, size_t pack_pages) {
+    int rc = ensure_tables(e, n_pages);
+    if (rc != FMA_OK) return rc;
+    rc = ensure_pack_bufs(e, pack_pages);
+    if (rc != FMA_OK) return rc;
+    build_page_table(ex, e->h_tab);
+    RT(cudaMemcpyAsync(e->d_tab, e->h_tab, n_pages * sizeof(uint64_t), cudaMemcpyHostToDevice, e->ks));
+    RT(fma_k_launch_pack_probe(e->d_tab, (uint32_t)n_pages, e->d_psize, e->ks));
+    RT(cudaMemcpyAsync(e->h_psize, e->d_psize, n_pages * sizeof(uint32_t), cudaMemcpyDeviceToHost, e->ks));
+    RT(cudaStreamSynchronize(e->ks));
+    e->st.total_kernel_launches += 1;
+    return FMA_OK;
+}
+
+// K3 digests of the segments of `ex` become their recorded digests; *out (if given) receives them too, in `ex` order.
+int digest_and_mark(fma_engine_t* e, const std::vector<Extent>& ex, std::vector<uint64_t>* out = nullptr) {
+    std::vector<size_t> idx;
+    for (const Extent& x : ex) idx.push_back(x.seg_index);
+    std::vector<uint64_t> dg;
+    int rc = digest_segments(e, idx, &dg);
+    if (rc != FMA_OK) return rc;
+    for (size_t k = 0; k < idx.size(); ++k) {
+        e->segs[idx[k]].digest = dg[k];
+        e->segs[idx[k]].digest_valid = true;
+    }
+    if (out) *out = std::move(dg);
+    return FMA_OK;
+}
+
+const char* const kPackChanged = "%u page(s) changed between the pack probe and the pack: weights were written during sleep";
+
+}  // namespace
+
 // ------------------------------------------------------------------------------------
 // PACKED host image: K4p over every page of the image, then the store layout on the host.
 // Stored pages are laid back to back (sizes are multiples of 16 KiB), so every ring slot's D2H / H2D is one
@@ -16,17 +52,9 @@ int plan_packed_image(fma_engine_t* e, const std::vector<Extent>& ex, uint64_t W
     *packed = false;
     *stored_total = W;
     const size_t n_pages = W / FMA_PAGE_BYTES;
-    int rc = ensure_tables(e, n_pages);
-    if (rc != FMA_OK) return rc;
-    rc = ensure_pack_bufs(e, n_pages);
-    if (rc != FMA_OK) return rc;
     RT(cudaDeviceSynchronize());  // the caller's streams may still be writing weights (same reason as in do_sleep)
-    build_page_table(ex, e->h_tab);
-    RT(cudaMemcpyAsync(e->d_tab, e->h_tab, n_pages * sizeof(uint64_t), cudaMemcpyHostToDevice, e->ks));
-    RT(fma_k_launch_pack_probe(e->d_tab, (uint32_t)n_pages, e->d_psize, e->ks));
-    RT(cudaMemcpyAsync(e->h_psize, e->d_psize, n_pages * sizeof(uint32_t), cudaMemcpyDeviceToHost, e->ks));
-    RT(cudaStreamSynchronize(e->ks));
-    e->st.total_kernel_launches += 1;
+    int rc = pack_probe(e, ex, n_pages, n_pages);
+    if (rc != FMA_OK) return rc;
     off->resize(n_pages);
     bytes->resize(n_pages);
     uint64_t total = 0;
@@ -203,24 +231,31 @@ struct SleepPipe {
     const std::vector<size_t>* subset = nullptr;  // INCREMENTAL + PACKED: only these image pages (ascending) are re-coded, in place
     bool resident = false;  // the extents go to the resident buffer (e->res, its own page layout res_off / res_bytes), not the tier's store
     int publish_gathered(size_t pages_done) { return publish_consumed((uint64_t)pages_done * FMA_PAGE_BYTES, e->ks); }
-    // page table of the image (device addresses of its pages, in order) -> e->h_tab / e->d_tab
-    int upload_page_table(size_t* n_pages) {
-        *n_pages = W / FMA_PAGE_BYTES;
-        int rc = ensure_tables(e, *n_pages);
+    // the image's pages, stored in the PACKED layout or verbatim; their device addresses in order -> e->h_tab / e->d_tab
+    int plan(bool packed, std::vector<PagePlan>* pages) {
+        std::vector<fma_layout::SegPages> segs;
+        for (const Extent& x : ex) segs.push_back(fma_layout::SegPages{(uint64_t)x.va, x.bytes, x.packed_off, 0});
+        const std::vector<uint64_t>& off = resident ? e->res_off : e->img_off;
+        const std::vector<uint32_t>& bytes = resident ? e->res_bytes : e->img_bytes;
+        uint64_t bad = 0;
+        if (!fma_layout::plan_pages(segs, packed ? &off : nullptr, &bytes, pages, &bad))
+            return fail(FMA_ESTATE, "image offset %llu is outside the packed image's page table", (unsigned long long)bad);
+        int rc = ensure_tables(e, pages->size());
         if (rc != FMA_OK) return rc;
         build_page_table(ex, e->h_tab);
-        RT(cudaMemcpyAsync(e->d_tab, e->h_tab, *n_pages * sizeof(uint64_t), cudaMemcpyHostToDevice, e->ks));
+        RT(cudaMemcpyAsync(e->d_tab, e->h_tab, pages->size() * sizeof(uint64_t), cudaMemcpyHostToDevice, e->ks));
         return FMA_OK;
     }
+    int direct();
+    int kernel_packed();
+    int kernel();
+    int staged_packed();
+    int staged();
+    int multipath();
 };
 
 // DIRECT: copy engines move each segment chunk straight into the packed image
-int sleep_direct(SleepPipe& pipe) {
-    fma_engine_t* e = pipe.e;
-    const std::vector<Extent>& ex = pipe.ex;
-    uint32_t& copy_ops = pipe.copy_ops;
-    char* store = pipe.store;
-    auto publish_consumed = [&](uint64_t done, cudaStream_t s) { return pipe.publish_consumed(done, s); };
+int SleepPipe::direct() {
     int rc = FMA_OK;
     const size_t chunk = direct_chunk(e);
     // copy engines straight from the segments into the packed image, chunks round-robin over the streams;
@@ -250,235 +285,154 @@ int sleep_direct(SleepPipe& pipe) {
 }
 
 // KERNEL + PACKED (parking tiers): K4 encodes straight into the peer / local HBM store
-int sleep_kernel_packed(SleepPipe& pipe) {
-    fma_engine_t* e = pipe.e;
-    KernelTimes& kt = pipe.kt;
-    uint32_t& copy_ops = pipe.copy_ops;
-    const int tier = pipe.tier;
-    auto publish_gathered = [&](size_t pages) { return pipe.publish_gathered(pages); };
-    int rc = FMA_OK;
-    size_t n_pages = 0;
-    rc = pipe.upload_page_table(&n_pages);
+int SleepPipe::kernel_packed() {
+    std::vector<PagePlan> pages;
+    int rc = plan(true, &pages);
     if (rc != FMA_OK) return rc;
     // PACKED image in a parking tier: K4 encodes straight into the peer / local HBM store (0.758 of the bytes
     // over NVLink and of the parking GPU's HBM), batches as below
-    rc = ensure_pack_bufs(e, n_pages);
+    rc = ensure_pack_bufs(e, pages.size());
     if (rc != FMA_OK) return rc;
-    const uint64_t dbase = pipe.resident ? (uint64_t)e->res.va : store_dev_base(e, tier);
-    const std::vector<uint64_t>& img_off = pipe.resident ? e->res_off : e->img_off;
-    const std::vector<uint32_t>& img_bytes = pipe.resident ? e->res_bytes : e->img_bytes;
-    for (size_t p = 0; p < n_pages; ++p) {
-        fma_k_pack_desc& d = e->h_pdesc[p];
-        d.src = e->h_tab[p];
-        d.dst = dbase + img_off[p];
-        d.mode = img_bytes[p] == FMA_PAGE_BYTES ? FMA_K_PACK_RAW : FMA_K_PACK_BF16;
-        d.state = 0;
-    }
+    const uint64_t dbase = resident ? (uint64_t)e->res.va : store_dev_base(e, tier);
+    for (size_t p = 0; p < pages.size(); ++p) set_pack_desc(e->h_pdesc[p], pages[p].va, dbase + pages[p].off, pages[p].bytes);
     uint32_t* d_err = e->d_psize + e->pdesc_cap;
-    RT(cudaMemcpyAsync(e->d_pdesc, e->h_pdesc, n_pages * sizeof(fma_k_pack_desc), cudaMemcpyHostToDevice, e->ks));
+    RT(cudaMemcpyAsync(e->d_pdesc, e->h_pdesc, pages.size() * sizeof(fma_k_pack_desc), cudaMemcpyHostToDevice, e->ks));
     RT(cudaMemsetAsync(d_err, 0, sizeof(uint32_t), e->ks));
-    const size_t batch = std::max<size_t>(staged_slot(e) / FMA_PAGE_BYTES, 1);
-    for (size_t p0 = 0; p0 < n_pages; p0 += batch) {
-        const size_t np = std::min(batch, n_pages - p0);
-        uint64_t stored = 0;
-        for (size_t q = p0; q < p0 + np; ++q) stored += img_bytes[q];
+    std::vector<Batch> batches;
+    fma_layout::plan_batches(pages, slot_pages(e), UINT64_MAX, false, &batches);
+    for (const Batch& b : batches) {
         rc = kt.begin();
         if (rc != FMA_OK) return rc;
-        RT(fma_k_launch_pack(e->d_pdesc + p0, (uint32_t)np, d_err, e->ks));
-        rc = kt.end((uint64_t)np * FMA_PAGE_BYTES + stored);
+        RT(fma_k_launch_pack(e->d_pdesc + b.p0, (uint32_t)b.np, d_err, e->ks));
+        rc = kt.end((uint64_t)b.np * FMA_PAGE_BYTES + b.stored);
         if (rc != FMA_OK) return rc;
         ++copy_ops;
-        rc = publish_gathered(p0 + np);
+        rc = publish_gathered(b.p0 + b.np);
         if (rc != FMA_OK) return rc;
     }
     return rc;
 }
 
 // KERNEL: K1 writes the store itself (mapped pinned host memory, peer or local HBM)
-int sleep_kernel(SleepPipe& pipe) {
-    fma_engine_t* e = pipe.e;
-    KernelTimes& kt = pipe.kt;
-    uint32_t& copy_ops = pipe.copy_ops;
-    const int tier = pipe.tier;
-    auto publish_gathered = [&](size_t pages) { return pipe.publish_gathered(pages); };
-    int rc = FMA_OK;
-    size_t n_pages = 0;
-    rc = pipe.upload_page_table(&n_pages);
+int SleepPipe::kernel() {
+    std::vector<PagePlan> pages;
+    int rc = plan(false, &pages);
     if (rc != FMA_OK) return rc;
     // K1 writes the store itself: mapped pinned host memory (PCIe posted writes) or peer/local HBM;
     // launched in slot-sized batches so finished segments can be released while later ones still move
-    const size_t batch = std::max<size_t>(staged_slot(e) / FMA_PAGE_BYTES, 1);
-    const uint64_t dbase = pipe.resident ? (uint64_t)e->res.va : store_dev_base(e, tier);
-    for (size_t p0 = 0; p0 < n_pages; p0 += batch) {
-        const size_t np = std::min(batch, n_pages - p0);
-        rc = kt.launch(e->d_tab + p0, 0, nullptr, dbase + p0 * FMA_PAGE_BYTES, (uint32_t)np);
+    const uint64_t dbase = resident ? (uint64_t)e->res.va : store_dev_base(e, tier);
+    std::vector<Batch> batches;
+    fma_layout::plan_batches(pages, slot_pages(e), UINT64_MAX, false, &batches);
+    for (const Batch& b : batches) {
+        rc = kt.launch(e->d_tab + b.p0, 0, nullptr, dbase + pages[b.p0].off, (uint32_t)b.np);
         if (rc != FMA_OK) return rc;
         ++copy_ops;
-        rc = publish_gathered(p0 + np);
+        rc = publish_gathered(b.p0 + b.np);
         if (rc != FMA_OK) return rc;
     }
     return rc;
 }
 
 // STAGED + PACKED: K4 gather + encode -> ring slot (stored pages back to back) -> one D2H per slot
-int sleep_staged_packed(SleepPipe& pipe) {
-    fma_engine_t* e = pipe.e;
-    KernelTimes& kt = pipe.kt;
-    uint32_t& copy_ops = pipe.copy_ops;
-    char* store = pipe.store;
-    const uint64_t W = pipe.W;
-    auto publish_consumed = [&](uint64_t done, cudaStream_t s) { return pipe.publish_consumed(done, s); };
-    int rc = FMA_OK;
-    size_t n_pages = 0;
-    rc = pipe.upload_page_table(&n_pages);
+int SleepPipe::staged_packed() {
+    std::vector<PagePlan> pages;
+    int rc = plan(true, &pages);
     if (rc != FMA_OK) return rc;
     rc = ensure_ring(e, W);
     if (rc != FMA_OK) return rc;
     // the image pages this sleep codes: all of them, or (incremental) the pages of the changed segments, whose stored size
     // is known not to change, so each goes back to its old place in the kept image
-    std::vector<size_t> all;
-    if (!pipe.subset) {
-        all.resize(n_pages);
-        for (size_t p = 0; p < n_pages; ++p) all[p] = p;
+    std::vector<size_t> img_page(pages.size());
+    for (size_t p = 0; p < pages.size(); ++p) img_page[p] = p;
+    if (subset) {
+        img_page = *subset;
+        std::vector<PagePlan> sel;
+        for (size_t p : img_page) sel.push_back(pages[p]);
+        pages = std::move(sel);
     }
-    const std::vector<size_t>& pages = pipe.subset ? *pipe.subset : all;
-    struct Slot { size_t k0, nk; uint64_t bytes; };  // pages[k0 .. k0+nk): adjacent in the store, together they fit a ring slot
-    std::vector<Slot> slots;
-    for (size_t k = 0; k < pages.size();) {
-        Slot sl{k, 0, 0};
-        while (k < pages.size() && sl.bytes + e->img_bytes[pages[k]] <= e->ring_slot_bytes &&
-               (sl.nk == 0 || e->img_off[pages[k]] == e->img_off[pages[k - 1]] + e->img_bytes[pages[k - 1]])) {
-            sl.bytes += e->img_bytes[pages[k]];
-            ++sl.nk;
-            ++k;
-        }
-        if (!sl.nk) return fail(FMA_EINVAL, "ring slot of %zu bytes cannot hold one page", e->ring_slot_bytes);
-        slots.push_back(sl);
-    }
+    std::vector<Batch> slots;  // pages adjacent in the store that together fit a ring slot
+    if (!fma_layout::plan_batches(pages, SIZE_MAX, e->ring_slot_bytes, true, &slots))
+        return fail(FMA_EINVAL, "ring slot of %zu bytes cannot hold one page", e->ring_slot_bytes);
     for (size_t c = 0; c < slots.size(); ++c)
-        for (size_t k = slots[c].k0; k < slots[c].k0 + slots[c].nk; ++k) {
-            const size_t p = pages[k];
-            fma_k_pack_desc& d = e->h_pdesc[k];
-            d.src = e->h_tab[p];
-            d.dst = (uint64_t)(uintptr_t)e->ring[c % e->n_ring] + (e->img_off[p] - e->img_off[pages[slots[c].k0]]);
-            d.mode = e->img_bytes[p] == FMA_PAGE_BYTES ? FMA_K_PACK_RAW : FMA_K_PACK_BF16;
-            d.state = 0;
-        }
+        for (size_t k = slots[c].p0; k < slots[c].p0 + slots[c].np; ++k)
+            set_pack_desc(e->h_pdesc[k], pages[k].va, (uint64_t)(uintptr_t)e->ring[c % e->n_ring] + (pages[k].off - pages[slots[c].p0].off), pages[k].bytes);
     uint32_t* d_err = e->d_psize + e->pdesc_cap;
     RT(cudaMemcpyAsync(e->d_pdesc, e->h_pdesc, pages.size() * sizeof(fma_k_pack_desc), cudaMemcpyHostToDevice, e->ks));
     RT(cudaMemsetAsync(d_err, 0, sizeof(uint32_t), e->ks));
     cudaStream_t last_stream = e->cs[0];
     for (size_t c = 0; c < slots.size(); ++c) {
-        const Slot& sl = slots[c];
+        const Batch& sl = slots[c];
         const int slot = (int)(c % e->n_ring);
         cudaStream_t cstream = e->cs[c % e->n_cs];
         if (c >= (size_t)e->n_ring) RT(cudaStreamWaitEvent(e->ks, e->ev_ring_free[slot], 0));
         rc = kt.begin();
         if (rc != FMA_OK) return rc;
-        RT(fma_k_launch_pack(e->d_pdesc + sl.k0, (uint32_t)sl.nk, d_err, e->ks));
-        rc = kt.end((uint64_t)sl.nk * FMA_PAGE_BYTES + sl.bytes);
+        RT(fma_k_launch_pack(e->d_pdesc + sl.p0, (uint32_t)sl.np, d_err, e->ks));
+        rc = kt.end((uint64_t)sl.np * FMA_PAGE_BYTES + sl.stored);
         if (rc != FMA_OK) return rc;
         RT(cudaEventRecord(e->ev_ring_full[slot], e->ks));
         RT(cudaStreamWaitEvent(cstream, e->ev_ring_full[slot], 0));
-        RT(cudaMemcpyAsync(store + e->img_off[pages[sl.k0]], e->ring[slot], sl.bytes, cudaMemcpyDefault, cstream));
+        RT(cudaMemcpyAsync(store + pages[sl.p0].off, e->ring[slot], sl.stored, cudaMemcpyDefault, cstream));
         if (c > 0) RT(cudaStreamWaitEvent(cstream, e->ev_ring_free[(c - 1) % e->n_ring], 0));  // same chaining as below
         RT(cudaEventRecord(e->ev_ring_free[slot], cstream));
         ++copy_ops;
         // every image byte below the last page of this slot is in the store: coded just now, or kept from the last wake
-        rc = publish_consumed((uint64_t)(pages[sl.k0 + sl.nk - 1] + 1) * FMA_PAGE_BYTES, cstream);
+        rc = publish_consumed((uint64_t)(img_page[sl.p0 + sl.np - 1] + 1) * FMA_PAGE_BYTES, cstream);
         if (rc != FMA_OK) return rc;
         last_stream = cstream;
     }
-    if (pipe.subset) rc = publish_consumed(W, last_stream);  // the clean tail of the image needs no copy
+    if (subset) rc = publish_consumed(W, last_stream);  // the clean tail of the image needs no copy
     return rc;
 }
 
 // STAGED: K1 gather -> HBM ring slot -> one large D2H per slot
-int sleep_staged(SleepPipe& pipe) {
-    fma_engine_t* e = pipe.e;
-    KernelTimes& kt = pipe.kt;
-    uint32_t& copy_ops = pipe.copy_ops;
-    char* store = pipe.store;
-    const uint64_t W = pipe.W;
-    auto publish_consumed = [&](uint64_t done, cudaStream_t s) { return pipe.publish_consumed(done, s); };
-    int rc = FMA_OK;
-    size_t n_pages = 0;
-    rc = pipe.upload_page_table(&n_pages);
+int SleepPipe::staged() {
+    std::vector<PagePlan> pages;
+    int rc = plan(false, &pages);
     if (rc != FMA_OK) return rc;
     rc = ensure_ring(e, W);
     if (rc != FMA_OK) return rc;
-    const size_t slot_pages = e->ring_slot_bytes / FMA_PAGE_BYTES;
-    size_t c = 0;
-    for (size_t p0 = 0; p0 < n_pages; p0 += slot_pages, ++c) {
+    std::vector<Batch> slots;
+    if (!fma_layout::plan_batches(pages, e->ring_slot_bytes / FMA_PAGE_BYTES, UINT64_MAX, true, &slots))
+        return fail(FMA_EINVAL, "ring slot of %zu bytes cannot hold one page", e->ring_slot_bytes);
+    for (size_t c = 0; c < slots.size(); ++c) {
+        const Batch& sl = slots[c];
         const int slot = (int)(c % e->n_ring);
-        const size_t np = std::min(slot_pages, n_pages - p0);
         cudaStream_t cstream = e->cs[c % e->n_cs];
         if (c >= (size_t)e->n_ring) RT(cudaStreamWaitEvent(e->ks, e->ev_ring_free[slot], 0));
-        rc = kt.launch(e->d_tab + p0, 0, nullptr, (uint64_t)(uintptr_t)e->ring[slot], (uint32_t)np);
+        rc = kt.launch(e->d_tab + sl.p0, 0, nullptr, (uint64_t)(uintptr_t)e->ring[slot], (uint32_t)sl.np);
         if (rc != FMA_OK) return rc;
         RT(cudaEventRecord(e->ev_ring_full[slot], e->ks));
         RT(cudaStreamWaitEvent(cstream, e->ev_ring_full[slot], 0));
-        RT(cudaMemcpyAsync(store + p0 * FMA_PAGE_BYTES, e->ring[slot], np * FMA_PAGE_BYTES, cudaMemcpyDefault, cstream));
+        RT(cudaMemcpyAsync(store + pages[sl.p0].off, e->ring[slot], sl.stored, cudaMemcpyDefault, cstream));
         // "slot free" also means "every earlier slot has reached the store" (chained through the previous
         // slot's event), so the unmapper below never releases device memory whose bytes are not yet on the host
         if (c > 0) RT(cudaStreamWaitEvent(cstream, e->ev_ring_free[(c - 1) % e->n_ring], 0));
         RT(cudaEventRecord(e->ev_ring_free[slot], cstream));
         ++copy_ops;
-        rc = publish_consumed((uint64_t)(p0 + np) * FMA_PAGE_BYTES, cstream);  // units fully in the store are dead
+        rc = publish_consumed((uint64_t)(sl.p0 + sl.np) * FMA_PAGE_BYTES, cstream);  // units fully in the store are dead
         if (rc != FMA_OK) return rc;
     }
     return rc;
 }
 
-// MULTI-PATH sleep (fma_paths_set): the mirror image of wake_multipath.  K1 on the sleeping GPU gathers a chunk of the image
+// MULTI-PATH sleep (fma_paths_set): the mirror image of the multi-path wake.  K1 on the sleeping GPU gathers a chunk of the image
 // into a staging slot of a PATH — its own HBM, or a helper GPU's HBM over NVLink — and THAT GPU's copy engine moves the slot into
 // the host store over THAT GPU's x16 link; chunk queues per NUMA node of the (striped) store, self-balancing.  Nothing is unmapped
 // before every byte has reached the store (one publish at the end), so a failure half way leaves the engine awake and intact.
-int sleep_multipath(SleepPipe& pipe) {
-    fma_engine_t* e = pipe.e;
-    KernelTimes& kt = pipe.kt;
-    char* store = pipe.store;
-    int rc = FMA_OK;
-    size_t n_pages = 0;
-    rc = pipe.upload_page_table(&n_pages);
+int SleepPipe::multipath() {
+    std::vector<PagePlan> pages;
+    int rc = plan(false, &pages);
     if (rc != FMA_OK) return rc;
     rc = ensure_ring_events(e, 1);
     if (rc != FMA_OK) return rc;
     cudaEvent_t ev_tab = e->ev_ring_full[0];
     RT(cudaEventRecord(ev_tab, e->ks));
-    struct Chunk { size_t p0, np; };
-    std::vector<Chunk> chunks;
-    const size_t chunk_pages = std::max<size_t>(e->path_slot_bytes / FMA_PAGE_BYTES, 1);
-    for (size_t q = 0; q < n_pages; q += chunk_pages) chunks.push_back(Chunk{q, std::min(chunk_pages, n_pages - q)});
-    std::vector<int> q_node;
-    std::vector<std::vector<size_t>> q_chunks;
-    for (size_t c = 0; c < chunks.size(); ++c) {
-        const uint64_t off = (uint64_t)chunks[c].p0 * FMA_PAGE_BYTES;
-        int node = -1;
-        for (const HostStore::NumaRange& r : e->host.ranges)
-            if (off >= r.begin && off < r.end) node = r.node;
-        size_t qi = 0;
-        while (qi < q_node.size() && q_node[qi] != node) ++qi;
-        if (qi == q_node.size()) {
-            q_node.push_back(node);
-            q_chunks.emplace_back();
-        }
-        q_chunks[qi].push_back(c);
-    }
-    std::vector<std::atomic<size_t>> q_next(q_node.size());
-    for (auto& a : q_next) a.store(0);
-    auto take_chunk = [&](int my_node, size_t* out) -> bool {
-        for (int pass = 0; pass < 2; ++pass)
-            for (size_t qi = 0; qi < q_node.size(); ++qi) {
-                if ((pass == 0) != (q_node[qi] == my_node)) continue;
-                const size_t k = q_next[qi].fetch_add(1);
-                if (k < q_chunks[qi].size()) {
-                    *out = q_chunks[qi][k];
-                    return true;
-                }
-            }
-        return false;
-    };
+    std::vector<Batch> chunks;
+    fma_layout::plan_batches(pages, std::max<size_t>(e->path_slot_bytes / FMA_PAGE_BYTES, 1), UINT64_MAX, true, &chunks);
+    std::vector<uint64_t> chunk_off;
+    for (const Batch& ch : chunks) chunk_off.push_back(pages[ch.p0].off);
+    fma_layout::ChunkQueues queues(chunk_off, e->host.ranges);
     std::atomic<int> error{FMA_OK};
     std::mutex kt_mu;
     char err_msg[512] = "";
@@ -496,8 +450,8 @@ int sleep_multipath(SleepPipe& pipe) {
         for (;;) {
             if (error.load() != FMA_OK) return;
             size_t c = 0;
-            if (!take_chunk(path.numa_node, &c)) break;
-            const Chunk& ch = chunks[c];
+            if (!queues.take(path.numa_node, &c)) break;
+            const Batch& ch = chunks[c];
             const int slot = (int)(mine % (uint32_t)e->path_slots);
             if (mine >= (uint32_t)e->path_slots) {   // the D2H that used this slot before has drained it (event on the path's GPU)
                 ce = cudaEventSynchronize(path.ev_full[slot]);
@@ -513,7 +467,7 @@ int sleep_multipath(SleepPipe& pipe) {
             if (ce != cudaSuccess) return failw(FMA_ECUDA, "cudaEventRecord(slot full)", ce);
             ce = cudaStreamWaitEvent(path.copy, path.ev_free[slot], 0);
             if (ce != cudaSuccess) return failw(FMA_ECUDA, "cudaStreamWaitEvent(slot full)", ce);
-            ce = cudaMemcpyAsync(store + (uint64_t)ch.p0 * FMA_PAGE_BYTES, slot_ptr, ch.np * FMA_PAGE_BYTES, cudaMemcpyDefault, path.copy);
+            ce = cudaMemcpyAsync(store + chunk_off[c], slot_ptr, ch.stored, cudaMemcpyDefault, path.copy);
             if (ce != cudaSuccess) return failw(FMA_ECUDA, "cudaMemcpyAsync(D2H)", ce);
             ce = cudaEventRecord(path.ev_full[slot], path.copy);           // (event on the path's GPU) the slot is drained
             if (ce != cudaSuccess) return failw(FMA_ECUDA, "cudaEventRecord(slot drained)", ce);
@@ -533,10 +487,10 @@ int sleep_multipath(SleepPipe& pipe) {
     }
     if (error.load() != FMA_OK) return fail(error.load(), "%s", err_msg);
     for (size_t pi = 0; pi < e->paths.size(); ++pi) {
-        pipe.copy_ops += per_path[pi];
+        copy_ops += per_path[pi];
         e->tl_add("path_chunks", e->paths[pi].device, e->tl_entry, now_s(), (uint64_t)per_path[pi] * e->path_slot_bytes);
     }
-    return pipe.publish_consumed(pipe.W, e->ks);   // all bytes are in the store: every offloaded unit may go
+    return publish_consumed(W, e->ks);   // all bytes are in the store: every offloaded unit may go
 }
 
 }  // namespace
@@ -612,20 +566,15 @@ int do_sleep(fma_engine_t* e, uint64_t offload_mask, int tier, uint32_t flags) {
             if (rc != FMA_OK) return rc;
             pre_planned = true;
         }
-        std::vector<char> res(ex.size(), 0);
-        uint64_t left = e->resident_cap, res_stored = 0;
-        for (size_t k = ex.size(); k-- > 0;) {
-            uint64_t stored = ex[k].bytes;
-            if (pre_packed) {
-                stored = 0;
-                for (uint64_t o = 0; o < ex[k].bytes; o += FMA_PAGE_BYTES) stored += pre_bytes[(ex[k].packed_off + o) / FMA_PAGE_BYTES];
-            }
-            if (stored <= left) {
-                res[k] = 1;
-                left -= stored;
-                res_stored += stored;
-            }
+        std::vector<uint64_t> stored(ex.size());
+        for (size_t k = 0; k < ex.size(); ++k) {
+            stored[k] = pre_packed ? 0 : ex[k].bytes;
+            if (pre_packed)
+                for (uint64_t o = 0; o < ex[k].bytes; o += FMA_PAGE_BYTES) stored[k] += pre_bytes[(ex[k].packed_off + o) / FMA_PAGE_BYTES];
         }
+        const std::vector<char> res = fma_layout::resident_split(stored, e->resident_cap);
+        uint64_t res_stored = 0;
+        for (size_t k = 0; k < ex.size(); ++k) res_stored += res[k] ? stored[k] : 0;
         if (res_stored) {
             ParkStore buf;
             const double a = now_s();
@@ -694,20 +643,15 @@ int do_sleep(fma_engine_t* e, uint64_t offload_mask, int tier, uint32_t flags) {
     std::vector<size_t> dirty_pages;  // their image pages (PACKED image)
     if (shadows_match && W && W == e->shadow_image_bytes && (tier == FMA_TIER_HOST ? e->host.cap : e->park.cap) >= e->shadow_store_bytes) {
         RT(cudaDeviceSynchronize());  // the caller's streams may still be writing weights
-        std::vector<size_t> idx;
-        for (const Extent& x : ex) idx.push_back(x.seg_index);
         std::vector<uint64_t> now;
-        rc = digest_segments(e, idx, &now);
+        rc = digest_and_mark(e, ex, &now);  // either way these are the digests of what sleeps now
         if (rc != FMA_OK) return rc;
         uint64_t dirty_bytes = 0;
-        for (size_t k = 0; k < idx.size(); ++k) {
+        for (size_t k = 0; k < ex.size(); ++k)
             if (now[k] != shadow_digest[k]) {
                 dirty.push_back(ex[k]);
                 dirty_bytes += ex[k].bytes;
             }
-            e->segs[idx[k]].digest = now[k];  // either way these are the digests of what sleeps now
-            e->segs[idx[k]].digest_valid = true;
-        }
         digests_known = true;
         clean = dirty.empty();
         // a few changed segments (an adapter, fp8 KV scales reset after wake, one synced layer): only they cross the link, into
@@ -718,20 +662,10 @@ int do_sleep(fma_engine_t* e, uint64_t offload_mask, int tier, uint32_t flags) {
         if (tier == FMA_TIER_HOST && !clean && e->shadow_packed && e->cfg.pack && 2 * dirty_bytes <= W && !e->host.shared && resolve_mode(e, tier) == FMA_MODE_STAGED) {
             for (const Extent& x : dirty)
                 for (size_t o = 0; o < x.bytes; o += FMA_PAGE_BYTES) dirty_pages.push_back((size_t)((x.packed_off + o) / FMA_PAGE_BYTES));
-            rc = ensure_tables(e, dirty_pages.size());
+            rc = pack_probe(e, dirty, dirty_pages.size(), std::max<size_t>(dirty_pages.size(), W / FMA_PAGE_BYTES));
             if (rc != FMA_OK) return rc;
-            rc = ensure_pack_bufs(e, std::max<size_t>(dirty_pages.size(), W / FMA_PAGE_BYTES));
-            if (rc != FMA_OK) return rc;
-            size_t k = 0;
-            for (const Extent& x : dirty)
-                for (size_t o = 0; o < x.bytes; o += FMA_PAGE_BYTES) e->h_tab[k++] = (uint64_t)x.va + o;
-            RT(cudaMemcpyAsync(e->d_tab, e->h_tab, k * sizeof(uint64_t), cudaMemcpyHostToDevice, e->ks));
-            RT(fma_k_launch_pack_probe(e->d_tab, (uint32_t)k, e->d_psize, e->ks));
-            RT(cudaMemcpyAsync(e->h_psize, e->d_psize, k * sizeof(uint32_t), cudaMemcpyDeviceToHost, e->ks));
-            RT(cudaStreamSynchronize(e->ks));
-            e->st.total_kernel_launches += 1;
             partial_packed = dirty_pages.size() <= e->img_bytes.size();
-            for (size_t q = 0; q < k && partial_packed; ++q)
+            for (size_t q = 0; q < dirty_pages.size() && partial_packed; ++q)
                 partial_packed = dirty_pages[q] < e->img_bytes.size() && e->h_psize[q] == e->img_bytes[dirty_pages[q]];
             if (partial_packed && (no_ring() || ensure_ring(e, W) != FMA_OK)) partial_packed = false;  // no HBM for a ring: full sleep through the plain path
         }
@@ -802,15 +736,8 @@ int do_sleep(fma_engine_t* e, uint64_t offload_mask, int tier, uint32_t flags) {
 
     const bool adopt = (flags & kFlagAdopt) != 0;  // the store already holds the image: release the device side only
     if (((flags & FMA_FLAG_VERIFY) || e->incremental) && W && !adopt && !digests_known) {  // incremental: digests seed the next sleep's check
-        std::vector<size_t> idx;
-        for (const Extent& x : ex) idx.push_back(x.seg_index);
-        std::vector<uint64_t> dg;
-        rc = digest_segments(e, idx, &dg);
+        rc = digest_and_mark(e, ex);
         if (rc != FMA_OK) return rc;
-        for (size_t k = 0; k < idx.size(); ++k) {
-            e->segs[idx[k]].digest = dg[k];
-            e->segs[idx[k]].digest_valid = true;
-        }
     }
 
     // ---- RESIDENT share: K1 / K4 gather the resident segments into e->res (HBM only, a few ms), ahead of the host part's
@@ -822,15 +749,8 @@ int do_sleep(fma_engine_t* e, uint64_t offload_mask, int tier, uint32_t flags) {
     double copy_s = 0;
     if (!ex_res.empty()) {
         if ((flags & FMA_FLAG_VERIFY) || e->incremental) {
-            std::vector<size_t> idx;
-            for (const Extent& x : ex_res) idx.push_back(x.seg_index);
-            std::vector<uint64_t> dg;
-            rc = digest_segments(e, idx, &dg);
+            rc = digest_and_mark(e, ex_res);
             if (rc != FMA_OK) return rc;
-            for (size_t k = 0; k < idx.size(); ++k) {
-                e->segs[idx[k]].digest = dg[k];
-                e->segs[idx[k]].digest_valid = true;
-            }
         }
         rc = timer.begin();
         if (rc != FMA_OK) return rc;
@@ -838,13 +758,12 @@ int do_sleep(fma_engine_t* e, uint64_t offload_mask, int tier, uint32_t flags) {
         SleepPipe rp{e, ex_res, W_all - W, FMA_TIER_LOCAL, nullptr, kt, res_launches, [](uint64_t, cudaStream_t) { return FMA_OK; }};
         rp.resident = true;
         kt.kind = "res_gather";
-        rc = e->res_packed ? sleep_kernel_packed(rp) : sleep_kernel(rp);
+        rc = e->res_packed ? rp.kernel_packed() : rp.kernel();
         kt.kind = "kernel";
         if (rc != FMA_OK) return rc;
-        if (e->res_packed) RT(cudaMemcpyAsync(e->h_psize + e->pdesc_cap, e->d_psize + e->pdesc_cap, sizeof(uint32_t), cudaMemcpyDeviceToHost, e->ks));
-        RT(cudaStreamSynchronize(e->ks));
-        if (e->res_packed && e->h_psize[e->pdesc_cap])
-            return fail(FMA_EINTEGRITY, "%u page(s) changed between the pack probe and the pack: weights were written during sleep", e->h_psize[e->pdesc_cap]);
+        if (e->res_packed) rc = check_pack_errors(e, kPackChanged);
+        else RT(cudaStreamSynchronize(e->ks));
+        if (rc != FMA_OK) return rc;
         std::lock_guard<std::mutex> lk(e->mu);
         for (const Extent& x : ex_res) {
             Segment& sg = e->segs[x.seg_index];
@@ -912,10 +831,7 @@ int do_sleep(fma_engine_t* e, uint64_t offload_mask, int tier, uint32_t flags) {
 
     if (W && adopt) {
         publish_consumed(W, e->ks);  // nothing to copy: every offloaded unit can go at once
-        e->pending_events = 0;       // no kernel ran: the per-operation kernel statistics read zero
-        e->st.kernel_seconds = 0;
-        e->st.kernel_bytes = 0;
-        e->st.kernel_launches = 0;
+        zero_kernel_stats(e);
         if (!e->ring_attached && env_int("FMA_RING_PERSIST", 0) == 0) release_ring(e);  // a sleeping model holds no staging ring
     } else if (W) {
         char* store = static_cast<char*>(store_copy_base(e, tier));
@@ -926,14 +842,14 @@ int do_sleep(fma_engine_t* e, uint64_t offload_mask, int tier, uint32_t flags) {
         SleepPipe pipe{e, partial ? dirty : ex, W, tier, store, kt, copy_ops, publish_consumed};
         if (partial_packed) {  // only the changed segments' pages are re-coded, each into its old place
             pipe.subset = &dirty_pages;
-            rc = sleep_staged_packed(pipe);
+            rc = pipe.staged_packed();
         } else if (partial) {  // only the changed segments move; everything below each of them is in the store already
-            rc = sleep_direct(pipe);
+            rc = pipe.direct();
             if (rc == FMA_OK) rc = publish_consumed(W, e->cs[0]);  // cs[0] has joined the other streams after the last extent
-        } else if (mode == FMA_MODE_DIRECT) rc = sleep_direct(pipe);
-        else if (mode == FMA_MODE_KERNEL) rc = packed ? sleep_kernel_packed(pipe) : sleep_kernel(pipe);
-        else if (multipath && !packed) rc = sleep_multipath(pipe);
-        else rc = packed ? sleep_staged_packed(pipe) : sleep_staged(pipe);
+        } else if (mode == FMA_MODE_DIRECT) rc = pipe.direct();
+        else if (mode == FMA_MODE_KERNEL) rc = packed ? pipe.kernel_packed() : pipe.kernel();
+        else if (multipath && !packed) rc = pipe.multipath();
+        else rc = packed ? pipe.staged_packed() : pipe.staged();
         if (rc != FMA_OK) return rc;
         {
             std::lock_guard<std::mutex> lk(un.mu);
@@ -945,10 +861,8 @@ int do_sleep(fma_engine_t* e, uint64_t offload_mask, int tier, uint32_t flags) {
         rc = kt.collect();
         if (rc != FMA_OK) return rc;
         if (packed) {  // K4 counts pages that no longer fit the form the probe chose (weights written during the sleep)
-            RT(cudaMemcpyAsync(e->h_psize + e->pdesc_cap, e->d_psize + e->pdesc_cap, sizeof(uint32_t), cudaMemcpyDeviceToHost, e->ks));
-            RT(cudaStreamSynchronize(e->ks));
-            if (e->h_psize[e->pdesc_cap])
-                return fail(FMA_EINTEGRITY, "%u page(s) changed between the pack probe and the pack: weights were written during sleep", e->h_psize[e->pdesc_cap]);
+            rc = check_pack_errors(e, kPackChanged);
+            if (rc != FMA_OK) return rc;
         }
         if (env_int("FMA_RING_PERSIST", 0) == 0 || e->ring_attached) release_ring(e);  // while the unmapper finishes its last ranges
     }
@@ -1005,12 +919,7 @@ int do_sleep(fma_engine_t* e, uint64_t offload_mask, int tier, uint32_t flags) {
     e->st.total_copy_ops += copy_ops;
     e->st.tier = tier;
     e->st.mode = mode;
-    if (!W && ex_res.empty()) {
-        e->pending_events = 0;
-        e->st.kernel_seconds = 0;
-        e->st.kernel_bytes = 0;
-        e->st.kernel_launches = 0;
-    }
+    if (!W && ex_res.empty()) zero_kernel_stats(e);
     return FMA_OK;
 }
 

@@ -29,7 +29,26 @@ struct WakePipe {
     // called after each of the pipeline's K2 / K5 launches with (image pages launched so far, image pages): a RESIDENT share's
     // restore launches one of its pieces there, so that a ring slot's hand-back waits for at most one such launch
     std::function<int(size_t, size_t)> between = nullptr;
+    int wait(size_t upto) {
+        const int mrc = wait_mapped(upto);
+        return mrc == FMA_OK ? FMA_OK : fail(mrc, "%s", map_msg);
+    }
+    void copied() {
+        if (!copy_ops) first_copy_delay = now_s() - t_entry;
+        ++copy_ops;
+    }
+    int packed();
+    int direct();
+    int paged();
+    int multipath();
 };
+
+// The segments `idx` as the page planner sees them: each waits for the mapper work item of its run.
+std::vector<fma_layout::SegPages> wake_segs(const fma_engine_t* e, const std::vector<size_t>& idx, const std::vector<size_t>& seg_run) {
+    std::vector<fma_layout::SegPages> v;
+    for (size_t i : idx) v.push_back(fma_layout::SegPages{(uint64_t)e->segs[i].va, e->segs[i].bytes, e->segs[i].packed_off, seg_run[i] + 1});
+    return v;
+}
 
 #define PIPE_CHECK(x)                 \
     do {                              \
@@ -38,193 +57,95 @@ struct WakePipe {
     } while (0)
 
 // PACKED image: H2D of the stored pages (0.758 of the bytes) -> ring slot -> K5 decode + scatter; or K5 reads the store itself
-int wake_packed(WakePipe& pipe) {
-    fma_engine_t* e = pipe.e;
-    const std::vector<size_t>& with_backup = pipe.with_backup;
-    const std::vector<size_t>& seg_run = pipe.seg_run;
-    KernelTimes& kt = pipe.kt;
-    uint32_t& copy_ops = pipe.copy_ops;
-    double& first_copy_delay = pipe.first_copy_delay;
-    const double t_entry = pipe.t_entry;
-    const int tier = pipe.tier;
-    const int mode = pipe.mode;
-    const bool ring_run = pipe.ring_run;
-    const char* store = pipe.store;
-    const uint64_t W = pipe.W;
-    auto wait_mapped = [&](size_t upto) { return pipe.wait_mapped(upto); };
-    // ---- PACKED image: H2D of the stored pages (0.758 of the bytes) -> ring slot -> K5 decode + scatter ----
+int WakePipe::packed() {
     // K5 reads the store itself when it is peer / local HBM, or when no ring could be had (then over PCIe)
     const bool zero_copy = mode != FMA_MODE_STAGED;
     if (zero_copy && tier == FMA_TIER_HOST && !e->host.dev_alias)
-        PIPE_CHECK(fail(FMA_ENOMEM, "no HBM for a staging ring and the host store has no device alias: a packed image cannot be woken"));
-    struct Dst { uint64_t packed_off; size_t w; };
-    std::vector<Dst> d;
-    for (size_t w = 0; w < with_backup.size(); ++w) d.push_back(Dst{e->segs[with_backup[w]].packed_off, w});
-    std::sort(d.begin(), d.end(), [](const Dst& a, const Dst& b) { return a.packed_off < b.packed_off; });
-    const size_t n_pages = W / FMA_PAGE_BYTES;
+        return fail(FMA_ENOMEM, "no HBM for a staging ring and the host store has no device alias: a packed image cannot be woken");
+    std::vector<PagePlan> pages;
+    uint64_t bad = 0;
+    if (!fma_layout::plan_pages(wake_segs(e, with_backup, seg_run), &e->img_off, &e->img_bytes, &pages, &bad))
+        return fail(FMA_ESTATE, "segment at image offset %llu is outside the packed image's page table", (unsigned long long)bad);
+    const size_t n_pages = pages.size();
     PIPE_CHECK(ensure_pack_bufs(e, n_pages));
-    std::vector<size_t> need_item(n_pages);
-    std::vector<uint64_t> soff(n_pages), dsts(n_pages);
-    std::vector<uint32_t> sbytes(n_pages);
-    size_t p = 0;
-    for (const Dst& x : d) {
-        const Segment& s = e->segs[with_backup[x.w]];
-        for (size_t o = 0; o < s.bytes; o += FMA_PAGE_BYTES, ++p) {
-            const size_t lp = (size_t)((s.packed_off + o) / FMA_PAGE_BYTES);
-            if (lp >= e->img_off.size()) PIPE_CHECK(fail(FMA_ESTATE, "segment at image offset %llu is outside the packed image's page table", (unsigned long long)(s.packed_off + o)));
-            soff[p] = e->img_off[lp];
-            sbytes[p] = e->img_bytes[lp];
-            dsts[p] = (uint64_t)s.va + o;
-            need_item[p] = seg_run[with_backup[x.w]] + 1;
-        }
-    }
     uint32_t* d_err = e->d_psize + e->pdesc_cap;
     RT(cudaMemsetAsync(d_err, 0, sizeof(uint32_t), e->ks));
     if (!zero_copy) {
-        if (ring_run) {
-            int mrc0 = wait_mapped(1);
-            if (mrc0 != FMA_OK) PIPE_CHECK(fail(mrc0, "%s", pipe.map_msg));
-        } else {
-            PIPE_CHECK(ensure_ring(e, W));
-        }
-        struct Slot { size_t p0, np; uint64_t bytes; };
-        std::vector<Slot> slots;  // pages that are adjacent in the store and fit one ring slot
-        for (size_t q = 0; q < n_pages;) {
-            Slot sl{q, 0, 0};
-            while (q < n_pages && sl.bytes + sbytes[q] <= e->ring_slot_bytes && (sl.np == 0 || soff[q] == soff[q - 1] + sbytes[q - 1])) {
-                sl.bytes += sbytes[q];
-                ++sl.np;
-                ++q;
-            }
-            if (!sl.np) PIPE_CHECK(fail(FMA_EINVAL, "ring slot of %zu bytes cannot hold one page", e->ring_slot_bytes));
-            slots.push_back(sl);
-        }
+        if (ring_run) PIPE_CHECK(wait(1));
+        else PIPE_CHECK(ensure_ring(e, W));
+        std::vector<Batch> slots;  // pages that are adjacent in the store and fit one ring slot
+        if (!fma_layout::plan_batches(pages, SIZE_MAX, e->ring_slot_bytes, true, &slots))
+            return fail(FMA_EINVAL, "ring slot of %zu bytes cannot hold one page", e->ring_slot_bytes);
         for (size_t c = 0; c < slots.size(); ++c)
-            for (size_t q = slots[c].p0; q < slots[c].p0 + slots[c].np; ++q) {
-                fma_k_pack_desc& pd = e->h_pdesc[q];
-                pd.src = (uint64_t)(uintptr_t)e->ring[c % e->n_ring] + (soff[q] - soff[slots[c].p0]);
-                pd.dst = dsts[q];
-                pd.mode = sbytes[q] == FMA_PAGE_BYTES ? FMA_K_PACK_RAW : FMA_K_PACK_BF16;
-                pd.state = 0;
-            }
+            for (size_t q = slots[c].p0; q < slots[c].p0 + slots[c].np; ++q)
+                set_pack_desc(e->h_pdesc[q], (uint64_t)(uintptr_t)e->ring[c % e->n_ring] + (pages[q].off - pages[slots[c].p0].off), pages[q].va, pages[q].bytes);
         RT(cudaMemcpyAsync(e->d_pdesc, e->h_pdesc, n_pages * sizeof(fma_k_pack_desc), cudaMemcpyHostToDevice, e->ks));
         for (size_t c = 0; c < slots.size(); ++c) {
-            const Slot& sl = slots[c];
+            const Batch& sl = slots[c];
             const int slot = (int)(c % e->n_ring);
             cudaStream_t cstream = e->cs[c % e->n_cs];
             if (c >= (size_t)e->n_ring) RT(cudaStreamWaitEvent(cstream, e->ev_ring_free[slot], 0));
-            RT(cudaMemcpyAsync(e->ring[slot], store + soff[sl.p0], sl.bytes, cudaMemcpyDefault, cstream));
-            if (!copy_ops) first_copy_delay = now_s() - t_entry;
-            ++copy_ops;
+            RT(cudaMemcpyAsync(e->ring[slot], store + pages[sl.p0].off, sl.stored, cudaMemcpyDefault, cstream));
+            copied();
             RT(cudaEventRecord(e->ev_ring_full[slot], cstream));
-            size_t need = 0;
-            for (size_t q = sl.p0; q < sl.p0 + sl.np; ++q) need = std::max(need, need_item[q]);
-            int mrc = wait_mapped(need);
-            if (mrc != FMA_OK) PIPE_CHECK(fail(mrc, "%s", pipe.map_msg));
+            PIPE_CHECK(wait(sl.need));
             RT(cudaStreamWaitEvent(e->ks, e->ev_ring_full[slot], 0));
             PIPE_CHECK(kt.begin());
             RT(fma_k_launch_unpack(e->d_pdesc + sl.p0, (uint32_t)sl.np, d_err, e->ks));
-            PIPE_CHECK(kt.end((uint64_t)sl.np * FMA_PAGE_BYTES + sl.bytes));
+            PIPE_CHECK(kt.end((uint64_t)sl.np * FMA_PAGE_BYTES + sl.stored));
             RT(cudaEventRecord(e->ev_ring_free[slot], e->ks));
-            if (pipe.between) PIPE_CHECK(pipe.between(sl.p0 + sl.np, n_pages));
+            if (between) PIPE_CHECK(between(sl.p0 + sl.np, n_pages));
         }
     } else {
         const uint64_t sbase = store_dev_base(e, tier);
-        for (size_t q = 0; q < n_pages; ++q) {
-            fma_k_pack_desc& pd = e->h_pdesc[q];
-            pd.src = sbase + soff[q];
-            pd.dst = dsts[q];
-            pd.mode = sbytes[q] == FMA_PAGE_BYTES ? FMA_K_PACK_RAW : FMA_K_PACK_BF16;
-            pd.state = 0;
-        }
+        for (size_t q = 0; q < n_pages; ++q) set_pack_desc(e->h_pdesc[q], sbase + pages[q].off, pages[q].va, pages[q].bytes);
         RT(cudaMemcpyAsync(e->d_pdesc, e->h_pdesc, n_pages * sizeof(fma_k_pack_desc), cudaMemcpyHostToDevice, e->ks));
-        const size_t batch_pages = std::max<size_t>(staged_slot(e) / FMA_PAGE_BYTES, 1);
-        for (size_t p0 = 0; p0 < n_pages;) {
-            const size_t np = std::min(batch_pages, n_pages - p0);
-            size_t need = 0;
-            uint64_t stored = 0;
-            for (size_t q = p0; q < p0 + np; ++q) {
-                need = std::max(need, need_item[q]);
-                stored += sbytes[q];
-            }
-            int mrc = wait_mapped(need);
-            if (mrc != FMA_OK) PIPE_CHECK(fail(mrc, "%s", pipe.map_msg));
+        std::vector<Batch> batches;
+        fma_layout::plan_batches(pages, slot_pages(e), UINT64_MAX, false, &batches);
+        for (const Batch& b : batches) {
+            PIPE_CHECK(wait(b.need));
             PIPE_CHECK(kt.begin());
-            RT(fma_k_launch_unpack(e->d_pdesc + p0, (uint32_t)np, d_err, e->ks));
-            PIPE_CHECK(kt.end((uint64_t)np * FMA_PAGE_BYTES + stored));
-            if (!copy_ops) first_copy_delay = now_s() - t_entry;
-            ++copy_ops;
-            p0 += np;
-            if (pipe.between) PIPE_CHECK(pipe.between(p0, n_pages));
+            RT(fma_k_launch_unpack(e->d_pdesc + b.p0, (uint32_t)b.np, d_err, e->ks));
+            PIPE_CHECK(kt.end((uint64_t)b.np * FMA_PAGE_BYTES + b.stored));
+            copied();
+            if (between) PIPE_CHECK(between(b.p0 + b.np, n_pages));
         }
     }
     return FMA_OK;
 }
 
 // DIRECT: copy engines move each chunk of the image straight into its segment as soon as the segment is mapped
-int wake_direct(WakePipe& pipe) {
-    fma_engine_t* e = pipe.e;
-    const std::vector<size_t>& with_backup = pipe.with_backup;
-    const std::vector<size_t>& seg_run = pipe.seg_run;
-    uint32_t& copy_ops = pipe.copy_ops;
-    double& first_copy_delay = pipe.first_copy_delay;
-    const double t_entry = pipe.t_entry;
-    const char* store = pipe.store;
-    auto wait_mapped = [&](size_t upto) { return pipe.wait_mapped(upto); };
+int WakePipe::direct() {
     const size_t chunk = direct_chunk(e);
     int k = 0;
-    for (size_t w = 0; w < with_backup.size(); ++w) {
-        int mrc = wait_mapped(seg_run[with_backup[w]] + 1);
-        if (mrc != FMA_OK) PIPE_CHECK(fail(mrc, "%s", pipe.map_msg));
-        const Segment& s = e->segs[with_backup[w]];
+    for (size_t i : with_backup) {
+        PIPE_CHECK(wait(seg_run[i] + 1));
+        const Segment& s = e->segs[i];
         for (size_t o = 0; o < s.bytes; o += chunk, ++k) {
             const size_t n = std::min(chunk, s.bytes - o);
             RT(cudaMemcpyAsync(reinterpret_cast<void*>(s.va + o), store + s.packed_off + o, n, cudaMemcpyDefault,
                                     e->cs[k % e->n_cs]));
-            if (!copy_ops) first_copy_delay = now_s() - t_entry;
-            ++copy_ops;
+            copied();
         }
     }
     return FMA_OK;
 }
 
 // KERNEL / STAGED: page-table driven — K2 reads the store itself, or H2D -> ring slot -> K2 scatter
-int wake_paged(WakePipe& pipe) {
-    fma_engine_t* e = pipe.e;
-    const std::vector<size_t>& with_backup = pipe.with_backup;
-    const std::vector<size_t>& seg_run = pipe.seg_run;
-    KernelTimes& kt = pipe.kt;
-    uint32_t& copy_ops = pipe.copy_ops;
-    double& first_copy_delay = pipe.first_copy_delay;
-    const double t_entry = pipe.t_entry;
-    const int tier = pipe.tier;
-    const int mode = pipe.mode;
-    const bool ring_run = pipe.ring_run;
-    const char* store = pipe.store;
-    const uint64_t W = pipe.W;
-    auto wait_mapped = [&](size_t upto) { return pipe.wait_mapped(upto); };
-    auto mapped_now = [&]() { return pipe.mapped_now(); };
-    // page table of the DESTINATIONS, ordered by packed offset (== with_backup order by construction
-    // only if every backed-up segment is woken; build explicitly from packed offsets to stay general)
-    struct Dst { uint64_t packed_off; size_t w; };
-    std::vector<Dst> d;
-    for (size_t w = 0; w < with_backup.size(); ++w) d.push_back(Dst{e->segs[with_backup[w]].packed_off, w});
-    std::sort(d.begin(), d.end(), [](const Dst& a, const Dst& b) { return a.packed_off < b.packed_off; });
-    // runs of pages: (image page index, destination address), plus the latest work item each page needs
-    size_t n_pages = W / FMA_PAGE_BYTES;
+int WakePipe::paged() {
+    // page table of the DESTINATIONS in image order (== with_backup order only if every backed-up segment is woken), with the
+    // latest work item each page needs
+    std::vector<PagePlan> pages;
+    uint64_t bad = 0;
+    fma_layout::plan_pages(wake_segs(e, with_backup, seg_run), nullptr, nullptr, &pages, &bad);
+    const size_t n_pages = pages.size();
     PIPE_CHECK(ensure_tables(e, n_pages));
     uint64_t* dst_tab = e->h_tab;                 // destination page addresses
     uint64_t* src_tab = e->h_tab + e->d_tab_cap;  // source page addresses inside the store (may be sparse)
-    std::vector<size_t> need_item(n_pages);
     const uint64_t sbase = store_dev_base(e, tier);
-    size_t p = 0;
-    for (const Dst& x : d) {
-        const Segment& s = e->segs[with_backup[x.w]];
-        for (size_t o = 0; o < s.bytes; o += FMA_PAGE_BYTES, ++p) {
-            dst_tab[p] = (uint64_t)s.va + o;
-            src_tab[p] = sbase + s.packed_off + o;
-            need_item[p] = seg_run[with_backup[x.w]] + 1;
-        }
+    for (size_t p = 0; p < n_pages; ++p) {
+        dst_tab[p] = pages[p].va;
+        src_tab[p] = sbase + pages[p].off;
     }
     RT(cudaMemcpyAsync(e->d_tab, dst_tab, n_pages * sizeof(uint64_t), cudaMemcpyHostToDevice, e->ks));
     RT(cudaMemcpyAsync(e->d_tab + e->d_tab_cap, src_tab, n_pages * sizeof(uint64_t), cudaMemcpyHostToDevice, e->ks));
@@ -233,54 +154,37 @@ int wake_paged(WakePipe& pipe) {
     if (mode == FMA_MODE_KERNEL) {
         // K2 reads the store itself (zero-copy PCIe reads, or NVLink/HBM loads); launch batches as the
         // mapper makes progress so the scatter overlaps cuMemCreate/Map of later segments
-        const size_t batch_pages = std::max<size_t>(staged_slot(e) / FMA_PAGE_BYTES, 1);
-        size_t p0 = 0;
-        while (p0 < n_pages) {
-            size_t np = std::min(batch_pages, n_pages - p0);
-            size_t need = 0;
-            for (size_t q = p0; q < p0 + np; ++q) need = std::max(need, need_item[q]);
-            int mrc = wait_mapped(need);
-            if (mrc != FMA_OK) PIPE_CHECK(fail(mrc, "%s", pipe.map_msg));
+        for (size_t p0 = 0; p0 < n_pages;) {
+            Batch b = fma_layout::next_batch(pages, p0, slot_pages(e), UINT64_MAX, false);
+            PIPE_CHECK(wait(b.need));
             // opportunistically extend the batch over everything already mapped
             const size_t have = mapped_now();
-            while (p0 + np < n_pages && need_item[p0 + np] <= have) ++np;
-            PIPE_CHECK(kt.launch(d_src + p0, 0, d_dst + p0, 0, (uint32_t)np));
-            if (!copy_ops) first_copy_delay = now_s() - t_entry;
-            ++copy_ops;
-            p0 += np;
-            if (pipe.between) PIPE_CHECK(pipe.between(p0, n_pages));
+            while (p0 + b.np < n_pages && pages[p0 + b.np].need <= have) ++b.np;
+            PIPE_CHECK(kt.launch(d_src + p0, 0, d_dst + p0, 0, (uint32_t)b.np));
+            copied();
+            p0 += b.np;
+            if (between) PIPE_CHECK(between(p0, n_pages));
         }
     } else {  // STAGED: copy engine H2D store -> ring slot (starts at t=0), K2 scatter once the targets are mapped
-        if (ring_run) {  // the ring is run 0 (1 GiB, ~0.2 ms to map): wait for it before the first H2D
-            int mrc0 = wait_mapped(1);
-            if (mrc0 != FMA_OK) PIPE_CHECK(fail(mrc0, "%s", pipe.map_msg));
-        } else {
-            PIPE_CHECK(ensure_ring(e, W));
-        }
-        const size_t slot_pages = e->ring_slot_bytes / FMA_PAGE_BYTES;
+        if (ring_run) PIPE_CHECK(wait(1));  // the ring is run 0 (1 GiB, ~0.2 ms to map): wait for it before the first H2D
+        else PIPE_CHECK(ensure_ring(e, W));
         // the store image may be only partially woken; H2D works on runs that are contiguous in the store
-        size_t c = 0;
-        size_t p0 = 0;
-        while (p0 < n_pages) {
-            size_t np = 1;
-            while (np < slot_pages && p0 + np < n_pages && src_tab[p0 + np] == src_tab[p0 + np - 1] + FMA_PAGE_BYTES) ++np;
+        std::vector<Batch> slots;
+        if (!fma_layout::plan_batches(pages, e->ring_slot_bytes / FMA_PAGE_BYTES, UINT64_MAX, true, &slots))
+            return fail(FMA_EINVAL, "ring slot of %zu bytes cannot hold one page", e->ring_slot_bytes);
+        for (size_t c = 0; c < slots.size(); ++c) {
+            const Batch& sl = slots[c];
             const int slot = (int)(c % e->n_ring);
             cudaStream_t cstream = e->cs[c % e->n_cs];
             if (c >= (size_t)e->n_ring) RT(cudaStreamWaitEvent(cstream, e->ev_ring_free[slot], 0));
-            RT(cudaMemcpyAsync(e->ring[slot], store + (src_tab[p0] - sbase), np * FMA_PAGE_BYTES, cudaMemcpyDefault, cstream));
-            if (!copy_ops) first_copy_delay = now_s() - t_entry;
-            ++copy_ops;
+            RT(cudaMemcpyAsync(e->ring[slot], store + pages[sl.p0].off, sl.stored, cudaMemcpyDefault, cstream));
+            copied();
             RT(cudaEventRecord(e->ev_ring_full[slot], cstream));
-            size_t need = 0;
-            for (size_t q = p0; q < p0 + np; ++q) need = std::max(need, need_item[q]);
-            int mrc = wait_mapped(need);
-            if (mrc != FMA_OK) PIPE_CHECK(fail(mrc, "%s", pipe.map_msg));
+            PIPE_CHECK(wait(sl.need));
             RT(cudaStreamWaitEvent(e->ks, e->ev_ring_full[slot], 0));
-            PIPE_CHECK(kt.launch(nullptr, (uint64_t)(uintptr_t)e->ring[slot], d_dst + p0, 0, (uint32_t)np));
+            PIPE_CHECK(kt.launch(nullptr, (uint64_t)(uintptr_t)e->ring[slot], d_dst + sl.p0, 0, (uint32_t)sl.np));
             RT(cudaEventRecord(e->ev_ring_free[slot], e->ks));
-            p0 += np;
-            ++c;
-            if (pipe.between) PIPE_CHECK(pipe.between(p0, n_pages));
+            if (between) PIPE_CHECK(between(sl.p0 + sl.np, n_pages));
         }
     }
     return FMA_OK;
@@ -290,73 +194,30 @@ int wake_paged(WakePipe& pipe) {
 // GPU — pulls the next chunk whenever one of its staging slots is free (H2D by THAT GPU's copy engine over THAT GPU's x16
 // link), and K2 on the waking GPU gathers the chunk from the path's staging slot (own HBM, or the peer's HBM over NVLink) into
 // the destination pages.  Self-balancing: a slower path (other NUMA node, busy link) simply takes fewer chunks.
-int wake_multipath(WakePipe& pipe) {
-    fma_engine_t* e = pipe.e;
-    const std::vector<size_t>& with_backup = pipe.with_backup;
-    const std::vector<size_t>& seg_run = pipe.seg_run;
-    KernelTimes& kt = pipe.kt;
-    const char* store = pipe.store;
-    const uint64_t W = pipe.W;
-    struct Dst { uint64_t packed_off; size_t w; };
-    std::vector<Dst> d;
-    for (size_t w = 0; w < with_backup.size(); ++w) d.push_back(Dst{e->segs[with_backup[w]].packed_off, w});
-    std::sort(d.begin(), d.end(), [](const Dst& a, const Dst& b) { return a.packed_off < b.packed_off; });
-    const size_t n_pages = W / FMA_PAGE_BYTES;
+int WakePipe::multipath() {
+    std::vector<PagePlan> pages;
+    uint64_t bad = 0;
+    fma_layout::plan_pages(wake_segs(e, with_backup, seg_run), nullptr, nullptr, &pages, &bad);
+    const size_t n_pages = pages.size();
     PIPE_CHECK(ensure_tables(e, n_pages));
-    uint64_t* dst_tab = e->h_tab;
-    std::vector<uint64_t> src_off(n_pages);
-    std::vector<size_t> need_item(n_pages);
-    size_t p = 0;
-    for (const Dst& x : d) {
-        const Segment& s = e->segs[with_backup[x.w]];
-        for (size_t o = 0; o < s.bytes; o += FMA_PAGE_BYTES, ++p) {
-            dst_tab[p] = (uint64_t)s.va + o;
-            src_off[p] = s.packed_off + o;
-            need_item[p] = seg_run[with_backup[x.w]] + 1;
-        }
-    }
-    RT(cudaMemcpyAsync(e->d_tab, dst_tab, n_pages * sizeof(uint64_t), cudaMemcpyHostToDevice, e->ks));
+    for (size_t p = 0; p < n_pages; ++p) e->h_tab[p] = pages[p].va;
+    RT(cudaMemcpyAsync(e->d_tab, e->h_tab, n_pages * sizeof(uint64_t), cudaMemcpyHostToDevice, e->ks));
     cudaEvent_t ev_tab = nullptr;   // the page table must be on the device before any path's K2 reads it
     PIPE_CHECK(ensure_ring_events(e, 1));
     ev_tab = e->ev_ring_full[0];
     RT(cudaEventRecord(ev_tab, e->ks));
-    struct Chunk { size_t p0, np, need; };
-    std::vector<Chunk> chunks;
-    const size_t chunk_pages = std::max<size_t>(e->path_slot_bytes / FMA_PAGE_BYTES, 1);
-    for (size_t q = 0; q < n_pages;) {
-        Chunk c{q, 1, need_item[q]};
-        while (c.np < chunk_pages && q + c.np < n_pages && src_off[q + c.np] == src_off[q + c.np - 1] + FMA_PAGE_BYTES) {
-            c.need = std::max(c.need, need_item[q + c.np]);
-            ++c.np;
-        }
-        chunks.push_back(c);
-        q += c.np;
-    }
-    // chunk queues by NUMA node of the store range the chunk lives in (HostStore::ranges): a path drains the queue of ITS GPU's
-    // node first and then helps with the others, so bytes cross the socket interconnect only to balance the tail
-    std::vector<int> q_node;                       // queue -> node
-    std::vector<std::vector<size_t>> q_chunks;     // queue -> chunk indices, image order
-    for (size_t c = 0; c < chunks.size(); ++c) {
-        const uint64_t off = src_off[chunks[c].p0];
-        int node = -1;
-        for (const HostStore::NumaRange& r : e->host.ranges)
-            if (off >= r.begin && off < r.end) node = r.node;
-        size_t qi = 0;
-        while (qi < q_node.size() && q_node[qi] != node) ++qi;
-        if (qi == q_node.size()) {
-            q_node.push_back(node);
-            q_chunks.emplace_back();
-        }
-        q_chunks[qi].push_back(c);
-    }
-    std::vector<std::atomic<size_t>> q_next(q_node.size());
-    for (auto& a : q_next) a.store(0);
+    std::vector<Batch> chunks;
+    fma_layout::plan_batches(pages, std::max<size_t>(e->path_slot_bytes / FMA_PAGE_BYTES, 1), UINT64_MAX, true, &chunks);
+    std::vector<uint64_t> chunk_off;
+    for (const Batch& ch : chunks) chunk_off.push_back(pages[ch.p0].off);
+    // a path drains the chunk queue of ITS GPU's NUMA node first and then helps with the others (HostStore::ranges)
+    fma_layout::ChunkQueues queues(chunk_off, e->host.ranges);
     // REMOTE paths (fma_paths_attach): helpers in the node-level owner's process pull from the SAME work counter, which therefore
     // lives in the shared mailbox together with the chunk table of this wake (fma_pull.h); published with the generation bump.
     PullMailbox* mb = e->mbox;
     if (mb) {
         if (chunks.size() > kPullMaxChunks) PIPE_CHECK(fail(FMA_EINVAL, "%zu chunks exceed the mailbox's table (use larger path slots)", chunks.size()));
-        for (size_t c = 0; c < chunks.size(); ++c) mb->chunks[c] = PullChunk{src_off[chunks[c].p0], (uint32_t)(chunks[c].np * FMA_PAGE_BYTES), 0};
+        for (size_t c = 0; c < chunks.size(); ++c) mb->chunks[c] = PullChunk{chunk_off[c], (uint32_t)chunks[c].stored, 0};
         for (uint32_t pi = 0; pi < kPullMaxPaths; ++pi) {
             mb->helper_error[pi].store(0);
             mb->helper_seen[pi].store(0);
@@ -374,16 +235,7 @@ int wake_multipath(WakePipe& pipe) {
             *out = k;
             return true;
         }
-        for (int pass = 0; pass < 2; ++pass)
-            for (size_t qi = 0; qi < q_node.size(); ++qi) {
-                if ((pass == 0) != (q_node[qi] == my_node)) continue;   // own node's queue first
-                const size_t k = q_next[qi].fetch_add(1);
-                if (k < q_chunks[qi].size()) {
-                    *out = q_chunks[qi][k];
-                    return true;
-                }
-            }
-        return false;
+        return queues.take(my_node, out);
     };
     std::atomic<int> error{FMA_OK};
     std::atomic<bool> first_copy_seen{false};
@@ -395,7 +247,7 @@ int wake_multipath(WakePipe& pipe) {
         cudaSetDevice(e->device);
         auto failw = [&](int code, const char* what, cudaError_t ce) {
             int expect = FMA_OK;
-            if (error.compare_exchange_strong(expect, code)) snprintf(err_msg, sizeof(err_msg), "%s failed on path %zu (device %d): %s", what, pi, path.device, ce == cudaSuccess ? (code == FMA_ESTATE || code == FMA_EINTEGRITY ? what : pipe.map_msg) : cudaGetErrorString(ce));
+            if (error.compare_exchange_strong(expect, code)) snprintf(err_msg, sizeof(err_msg), "%s failed on path %zu (device %d): %s", what, pi, path.device, ce == cudaSuccess ? (code == FMA_ESTATE || code == FMA_EINTEGRITY ? what : map_msg) : cudaGetErrorString(ce));
         };
         cudaError_t ce = cudaStreamWaitEvent(path.kern, ev_tab, 0);
         if (ce != cudaSuccess) return failw(FMA_ECUDA, "cudaStreamWaitEvent(table)", ce);
@@ -444,8 +296,8 @@ int wake_multipath(WakePipe& pipe) {
                 if (st != 0) {
                     const size_t c = st - 1;
                     if (c >= chunks.size()) return failw(FMA_EINTEGRITY, "the mailbox names a chunk that does not exist", cudaSuccess);
-                    const Chunk& ch = chunks[c];
-                    const int mrc = pipe.wait_mapped(ch.need);
+                    const Batch& ch = chunks[c];
+                    const int mrc = wait_mapped(ch.need);
                     if (mrc != FMA_OK) return failw(mrc, "mapping", cudaSuccess);
                     char* slot_ptr = reinterpret_cast<char*>(path.va) + (size_t)slot * e->path_slot_bytes;
                     {
@@ -456,7 +308,7 @@ int wake_multipath(WakePipe& pipe) {
                     ce = cudaEventRecord(path.ev_free[slot], path.kern);
                     if (ce != cudaSuccess) return failw(FMA_ECUDA, "cudaEventRecord(slot drained)", ce);
                     busy[slot] = true;
-                    if (!first_copy_seen.exchange(true)) pipe.first_copy_delay = now_s() - pipe.t_entry;
+                    if (!first_copy_seen.exchange(true)) first_copy_delay = now_s() - t_entry;
                     ++mine;
                     progressed = true;
                 }
@@ -476,9 +328,9 @@ int wake_multipath(WakePipe& pipe) {
             if (error.load() != FMA_OK) return;
             size_t c = 0;
             if (!take_chunk(path.numa_node, &c)) break;
-            const Chunk& ch = chunks[c];
+            const Batch& ch = chunks[c];
             {
-                const uint64_t off = src_off[ch.p0];
+                const uint64_t off = chunk_off[c];
                 for (const HostStore::NumaRange& r : e->host.ranges)
                     if (off >= r.begin && off < r.end && r.node == path.numa_node) ++per_path_local[pi];
             }
@@ -488,12 +340,12 @@ int wake_multipath(WakePipe& pipe) {
                 if (ce != cudaSuccess) return failw(FMA_ECUDA, "cudaEventSynchronize(slot free)", ce);
             }
             char* slot_ptr = reinterpret_cast<char*>(path.va) + (size_t)slot * e->path_slot_bytes;
-            ce = cudaMemcpyAsync(slot_ptr, store + src_off[ch.p0], ch.np * FMA_PAGE_BYTES, cudaMemcpyDefault, path.copy);
+            ce = cudaMemcpyAsync(slot_ptr, store + chunk_off[c], ch.stored, cudaMemcpyDefault, path.copy);
             if (ce != cudaSuccess) return failw(FMA_ECUDA, "cudaMemcpyAsync(H2D)", ce);
-            if (!first_copy_seen.exchange(true)) pipe.first_copy_delay = now_s() - pipe.t_entry;
+            if (!first_copy_seen.exchange(true)) first_copy_delay = now_s() - t_entry;
             ce = cudaEventRecord(path.ev_full[slot], path.copy);
             if (ce != cudaSuccess) return failw(FMA_ECUDA, "cudaEventRecord(slot full)", ce);
-            const int mrc = pipe.wait_mapped(ch.need);
+            const int mrc = wait_mapped(ch.need);
             if (mrc != FMA_OK) return failw(mrc, "mapping", cudaSuccess);
             ce = cudaStreamWaitEvent(path.kern, path.ev_full[slot], 0);
             if (ce != cudaSuccess) return failw(FMA_ECUDA, "cudaStreamWaitEvent(slot full)", ce);
@@ -521,10 +373,10 @@ int wake_multipath(WakePipe& pipe) {
     }
     for (size_t pi = 0; pi < e->paths.size(); ++pi) {
         RT(cudaStreamWaitEvent(e->ks, e->paths[pi].ev_done, 0));   // the wake's device-time bracket and the final sync cover every path
-        pipe.copy_ops += per_path[pi];
+        copy_ops += per_path[pi];
         const int idx = e->paths[pi].remote ? -(int)pi : e->paths[pi].device;   // remote paths: -(path index), their GPU is not visible here
-        e->tl_add("path_chunks", idx, pipe.t_entry, now_s(), (uint64_t)per_path[pi] * e->path_slot_bytes);
-        e->tl_add("path_local", idx, pipe.t_entry, now_s(), (uint64_t)per_path_local[pi] * e->path_slot_bytes);
+        e->tl_add("path_chunks", idx, t_entry, now_s(), (uint64_t)per_path[pi] * e->path_slot_bytes);
+        e->tl_add("path_local", idx, t_entry, now_s(), (uint64_t)per_path_local[pi] * e->path_slot_bytes);
     }
     return FMA_OK;
 }
@@ -656,16 +508,15 @@ int do_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags) {
     }
     const bool dbg_t = env_int("FMA_DEBUG_TIMING", 0) != 0;
     const double t_ring = now_s();
-    double remap_delay_s;
-    {
-        uint64_t w_bytes = 0;
-        for (size_t i : with_host) w_bytes += e->segs[i].bytes;
-        // a fifth of the expected host-tier copy time (55 GB/s), half of the NVLink one (600 GB/s): far below the slack
-        // (a multi-path wake has as many links as paths: its copy time, and with it the head start, shrinks accordingly)
-        const double expected = (double)w_bytes / (tier == FMA_TIER_HOST ? 55e9 * (multipath ? (double)e->paths.size() : 1.0) : 600e9);
-        const int forced = env_int("FMA_REMAP_DELAY_MS", -1);
-        remap_delay_s = forced >= 0 ? forced * 1e-3 : expected * (tier == FMA_TIER_HOST ? 0.2 : 0.5);
-    }
+    // expected copy time of the host part: 55 GB/s per host-tier link (a multi-path wake has as many links as paths), 600 GB/s
+    // over NVLink.  Remap-only runs wait a fifth of it (host tier) or half of it (NVLink): far below the slack.
+    const double expected_copy_s = [&] {
+        uint64_t w = 0;
+        for (size_t i : with_host) w += e->segs[i].bytes;
+        return (double)w / (tier == FMA_TIER_HOST ? 55e9 * (multipath ? (double)e->paths.size() : 1.0) : 600e9);
+    }();
+    const int forced_delay_ms = env_int("FMA_REMAP_DELAY_MS", -1);
+    const double remap_delay_s = forced_delay_ms >= 0 ? forced_delay_ms * 1e-3 : expected_copy_s * (tier == FMA_TIER_HOST ? 0.2 : 0.5);
 
     // FMA_REMAP_AFTER_COPY=1: remap-only runs (kv_cache) are mapped only after this rank's last copy has LANDED — a 32 GiB
     // cuMemCreate/Map/SetAccess then never runs beside this rank's DMA (its cost, a few ms, is added to the wake instead of
@@ -675,11 +526,6 @@ int do_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags) {
     e->tl_add("plan", (int)runs.size(), t_entry, t_ring, 0);
     // Cross-process VMM gate (fma_gate.h): tell the other engines on this host that a call which gates a first copy is coming
     int gate_first = n_backup_runs ? gate_announce(kGateFirst) : 0;
-    const double expected_copy_s = [&] {
-        uint64_t w = 0;
-        for (size_t i : with_host) w += e->segs[i].bytes;
-        return (double)w / (tier == FMA_TIER_HOST ? 55e9 * (multipath ? (double)e->paths.size() : 1.0) : 600e9);
-    }();
 
     // ---- mapper thread(s): one create + map + set-access per run, in `runs` order ----------------------
     MapProgress prog;
@@ -829,8 +675,7 @@ int do_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags) {
     // RESIDENT share: K2 / K5 copy the resident segments from e->res into their pages, on the kernel stream in pieces of at most
     // one ring slot, each launched between two of the host part's launches once its destination is mapped (in the second half of
     // the host part's launches the pipeline waits for that mapping); the tables sit behind the host part's in the same buffers.
-    struct ResPiece { size_t q0, np; size_t need; uint64_t stored; };
-    std::vector<ResPiece> res_pieces;
+    std::vector<Batch> res_pieces;
     size_t res_next = 0;
     const size_t n_host_pages = W / FMA_PAGE_BYTES;
     const bool res_packed = W_res && e->res_packed;   // (the buffer may be released before the K5 error count is read)
@@ -842,39 +687,24 @@ int do_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags) {
         if (r == FMA_OK && !e->ev_res_done && cudaEventCreateWithFlags(&e->ev_res_done, cudaEventDisableTiming) != cudaSuccess)
             r = fail(FMA_ECUDA, "cudaEventCreate(resident) failed");
         if (r != FMA_OK) return r;
-        std::vector<size_t> order(with_res);
-        std::sort(order.begin(), order.end(), [&](size_t a, size_t b) { return e->segs[a].packed_off < e->segs[b].packed_off; });
+        std::vector<PagePlan> pages;
+        uint64_t bad = 0;
+        if (!fma_layout::plan_pages(wake_segs(e, with_res, seg_run), e->res_packed ? &e->res_off : nullptr, &e->res_bytes, &pages, &bad))
+            return fail(FMA_ESTATE, "segment outside the resident part's page table");
         uint64_t* dst_tab = e->h_tab + n_host_pages;
         uint64_t* src_tab = e->h_tab + e->d_tab_cap + n_host_pages;
-        const size_t piece_pages = std::max<size_t>(staged_slot(e) / FMA_PAGE_BYTES, 1);
-        size_t q = 0;
-        for (size_t i : order) {
-            const Segment& s = e->segs[i];
-            for (size_t o = 0; o < s.bytes; o += FMA_PAGE_BYTES, ++q) {
-                const size_t lp = (size_t)((s.packed_off + o) / FMA_PAGE_BYTES);
-                if (e->res_packed && lp >= e->res_off.size()) return fail(FMA_ESTATE, "segment outside the resident part's page table");
-                const uint64_t soff = e->res_packed ? e->res_off[lp] : s.packed_off + o;
-                const uint32_t sb = e->res_packed ? e->res_bytes[lp] : (uint32_t)FMA_PAGE_BYTES;
-                if (e->res_packed) {
-                    fma_k_pack_desc& pd = e->h_pdesc[n_host_pages + q];
-                    pd.src = (uint64_t)e->res.va + soff;
-                    pd.dst = (uint64_t)s.va + o;
-                    pd.mode = sb == FMA_PAGE_BYTES ? FMA_K_PACK_RAW : FMA_K_PACK_BF16;
-                    pd.state = 0;
-                } else {
-                    dst_tab[q] = (uint64_t)s.va + o;
-                    src_tab[q] = (uint64_t)e->res.va + soff;
-                }
-                if (res_pieces.empty() || res_pieces.back().np == piece_pages) res_pieces.push_back(ResPiece{q, 0, 0, 0});
-                ResPiece& pc = res_pieces.back();
-                ++pc.np;
-                pc.need = std::max(pc.need, seg_run[i] + 1);
-                pc.stored += sb;
+        for (size_t q = 0; q < pages.size(); ++q) {
+            if (e->res_packed) {
+                set_pack_desc(e->h_pdesc[n_host_pages + q], (uint64_t)e->res.va + pages[q].off, pages[q].va, pages[q].bytes);
+            } else {
+                dst_tab[q] = pages[q].va;
+                src_tab[q] = (uint64_t)e->res.va + pages[q].off;
             }
         }
+        fma_layout::plan_batches(pages, slot_pages(e), UINT64_MAX, false, &res_pieces);
         if (e->res_packed) {
             RT(cudaMemcpyAsync(e->d_pdesc + n_host_pages, e->h_pdesc + n_host_pages, n_res * sizeof(fma_k_pack_desc), cudaMemcpyHostToDevice, e->ks));
-            if (!packed) RT(cudaMemsetAsync(e->d_psize + e->pdesc_cap, 0, sizeof(uint32_t), e->ks));   // (wake_packed clears it otherwise)
+            if (!packed) RT(cudaMemsetAsync(e->d_psize + e->pdesc_cap, 0, sizeof(uint32_t), e->ks));   // (WakePipe::packed clears it otherwise)
         } else {
             RT(cudaMemcpyAsync(e->d_tab + n_host_pages, dst_tab, n_res * sizeof(uint64_t), cudaMemcpyHostToDevice, e->ks));
             RT(cudaMemcpyAsync(e->d_tab + e->d_tab_cap + n_host_pages, src_tab, n_res * sizeof(uint64_t), cudaMemcpyHostToDevice, e->ks));
@@ -882,18 +712,18 @@ int do_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags) {
         return FMA_OK;
     };
     auto res_launch_next = [&]() -> int {
-        const ResPiece& pc = res_pieces[res_next];
+        const Batch& pc = res_pieces[res_next];
         int r = wait_mapped(pc.need);
         if (r != FMA_OK) return fail(r, "%s", prog.msg);
         kt.kind = "res_restore";
         if (e->res_packed) {
             r = kt.begin();
             if (r == FMA_OK) {
-                cudaError_t ce = fma_k_launch_unpack(e->d_pdesc + n_host_pages + pc.q0, (uint32_t)pc.np, e->d_psize + e->pdesc_cap, e->ks);
+                cudaError_t ce = fma_k_launch_unpack(e->d_pdesc + n_host_pages + pc.p0, (uint32_t)pc.np, e->d_psize + e->pdesc_cap, e->ks);
                 r = ce == cudaSuccess ? kt.end((uint64_t)pc.np * FMA_PAGE_BYTES + pc.stored) : fail(FMA_ECUDA, "K5 (resident) launch failed: %s", cudaGetErrorString(ce));
             }
         } else {
-            r = kt.launch(e->d_tab + e->d_tab_cap + n_host_pages + pc.q0, 0, e->d_tab + n_host_pages + pc.q0, 0, (uint32_t)pc.np);
+            r = kt.launch(e->d_tab + e->d_tab_cap + n_host_pages + pc.p0, 0, e->d_tab + n_host_pages + pc.p0, 0, (uint32_t)pc.np);
         }
         kt.kind = "kernel";
         if (r != FMA_OK) return r;
@@ -916,10 +746,10 @@ int do_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags) {
             WakePipe pipe{e, with_host, seg_run, W, tier, mode, ring_run, store, kt, copy_ops, first_copy_delay, t_entry, wait_mapped, mapped_now, prog.msg};
             if (W_res) pipe.between = res_pump;
             const double t_enq0 = now_s();
-            if (packed) WAKE_CHECK(wake_packed(pipe));
-            else if (multipath) WAKE_CHECK(wake_multipath(pipe));
-            else if (mode == FMA_MODE_DIRECT) WAKE_CHECK(wake_direct(pipe));
-            else WAKE_CHECK(wake_paged(pipe));
+            if (packed) WAKE_CHECK(pipe.packed());
+            else if (multipath) WAKE_CHECK(pipe.multipath());
+            else if (mode == FMA_MODE_DIRECT) WAKE_CHECK(pipe.direct());
+            else WAKE_CHECK(pipe.paged());
             e->tl_add("enqueue", (int)copy_ops, t_enq0, now_s(), W);
         }
         while (res_next < res_pieces.size()) WAKE_CHECK(res_launch_next());   // what the host part's launches left (or had no room for)
@@ -966,11 +796,8 @@ int do_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags) {
         WAKE_CHECK(timer.end(&copy_s));
         e->tl_add("drain", 0, t_joined, now_s(), W);
         WAKE_CHECK(kt.collect());
-        if (packed || res_packed) {  // K5 counts stored pages it could not read (bad magic / count): the image is damaged
-            WAKE_RT(cudaMemcpyAsync(e->h_psize + e->pdesc_cap, e->d_psize + e->pdesc_cap, sizeof(uint32_t), cudaMemcpyDeviceToHost, e->ks));
-            WAKE_RT(cudaStreamSynchronize(e->ks));
-            if (e->h_psize[e->pdesc_cap]) WAKE_CHECK(fail(FMA_EINTEGRITY, "%u stored page(s) of the packed image are malformed", e->h_psize[e->pdesc_cap]));
-        }
+        if (packed || res_packed)  // K5 counts stored pages it could not read (bad magic / count): the image is damaged
+            WAKE_CHECK(check_pack_errors(e, "%u stored page(s) of the packed image are malformed"));
         t_copy_end = now_s();
     }
     if (dbg_t)
@@ -1024,12 +851,7 @@ int do_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags) {
     e->st.total_copy_ops += copy_ops;
     e->st.tier = tier;
     e->st.mode = mode;
-    if (!W && !W_res) {
-        e->pending_events = 0;
-        e->st.kernel_seconds = 0;
-        e->st.kernel_bytes = 0;
-        e->st.kernel_launches = 0;
-    }
+    if (!W && !W_res) zero_kernel_stats(e);
     return verify_rc;
 }
 

@@ -2,6 +2,7 @@
 #include <cassert>
 #include <cstdio>
 #include <random>
+#include <thread>
 
 #include "fma_layout.h"
 
@@ -95,11 +96,157 @@ static void test_plan_runs() {
     assert(plan_runs(y, true, 0).size() == 2);
 }
 
+static const uint32_t C = 1589248;  // a coded page's stored size
+
+static std::vector<PagePlan> pages_with(const std::vector<uint64_t>& off, const std::vector<uint32_t>& bytes, size_t need = 0) {
+    std::vector<PagePlan> v;
+    for (size_t p = 0; p < off.size(); ++p) v.push_back(PagePlan{0x100000000ull + p * P, off[p], bytes[p], need});
+    return v;
+}
+
+static bool same(const std::vector<Batch>& b, const std::vector<Batch>& want) {
+    if (b.size() != want.size()) return false;
+    for (size_t i = 0; i < b.size(); ++i)
+        if (b[i].p0 != want[i].p0 || b[i].np != want[i].np || b[i].stored != want[i].stored || b[i].need != want[i].need) return false;
+    return true;
+}
+
+static void test_plan_pages() {
+    // given out of image order: a (2 pages at image page 3), b (3 pages at image page 0), c (1 page at image page 5)
+    std::vector<SegPages> segs = {{900 * P, 2 * P, 3 * P, 7}, {100 * P, 3 * P, 0, 2}, {500 * P, P, 5 * P, 4}};
+    std::vector<PagePlan> pg;
+    uint64_t bad = 0;
+    assert(plan_pages(segs, nullptr, nullptr, &pg, &bad) && pg.size() == 6);   // plain image: stored verbatim at its image offset
+    const uint64_t va[] = {100 * P, 101 * P, 102 * P, 900 * P, 901 * P, 500 * P};
+    const size_t need[] = {2, 2, 2, 7, 7, 4};
+    for (size_t p = 0; p < 6; ++p) assert(pg[p].va == va[p] && pg[p].off == p * P && pg[p].bytes == P && pg[p].need == need[p]);
+    // PACKED layout, indexed by image page
+    const std::vector<uint64_t> off = {0, C, 2 * C, 3 * C, 3 * C + P, 4 * C + P};
+    const std::vector<uint32_t> bytes = {C, C, C, (uint32_t)P, C, C};
+    assert(plan_pages(segs, &off, &bytes, &pg, &bad) && pg.size() == 6);
+    for (size_t p = 0; p < 6; ++p) assert(pg[p].va == va[p] && pg[p].off == off[p] && pg[p].bytes == bytes[p] && pg[p].need == need[p]);
+    // a tag-selective wake: only some segments, same image pages and layout entries
+    assert(plan_pages({segs[0]}, &off, &bytes, &pg, &bad) && pg.size() == 2 && pg[0].off == 3 * C && pg[1].off == 3 * C + P && pg[1].bytes == C);
+    // a page outside the layout
+    const std::vector<uint64_t> short_off(off.begin(), off.begin() + 4);
+    assert(!plan_pages(segs, &short_off, &bytes, &pg, &bad) && bad == 4 * P);
+    assert(plan_pages({}, nullptr, nullptr, &pg, &bad) && pg.empty());
+}
+
+static void test_batches_by_stored_bytes() {
+    // STAGED + PACKED: stored bytes <= one ring slot, adjacent in the store.  Pages 0-3 coded, 4 raw, 5-6 coded; a gap before page 5.
+    const std::vector<uint64_t> off = {0, C, 2 * C, 3 * C, 4 * C, 5 * C + P, 6 * C + P};
+    const std::vector<uint32_t> bytes = {C, C, C, C, (uint32_t)P, C, C};
+    std::vector<Batch> b;
+    assert(plan_batches(pages_with(off, bytes), SIZE_MAX, 3 * P, true, &b));   // 3 coded pages fit 6 MiB, the 4th does not
+    assert(same(b, {{0, 3, 3 * C, 0}, {3, 2, C + P, 0}, {5, 2, 2 * C, 0}}));
+    assert(!plan_batches(pages_with(off, bytes), SIZE_MAX, P - 1, true, &b));  // a raw page larger than the slot
+    assert(!plan_batches(pages_with(off, bytes), SIZE_MAX, C - 1, true, &b));
+    // INCREMENTAL: the changed pages only (holes between them), each in its old place
+    std::vector<PagePlan> all = pages_with(off, bytes), sub;
+    for (size_t p : {1, 2, 4, 6}) sub.push_back(all[p]);
+    assert(plan_batches(sub, SIZE_MAX, 3 * P, true, &b) && same(b, {{0, 2, 2 * C, 0}, {2, 1, P, 0}, {3, 1, C, 0}}));
+    // a byte cap that ends a batch inside a segment: the cap, not the segment, decides
+    assert(plan_batches(pages_with({0, C, 2 * C, 3 * C}, {C, C, C, C}), SIZE_MAX, 2 * C, true, &b) && same(b, {{0, 2, 2 * C, 0}, {2, 2, 2 * C, 0}}));
+}
+
+static void test_batches_by_pages() {
+    // STAGED / MULTI-PATH of a plain image: a page count per slot, adjacent in the store; `need` = the largest in the batch
+    std::vector<PagePlan> pg = pages_with({0, P, 2 * P, 3 * P, 9 * P, 10 * P, 11 * P}, std::vector<uint32_t>(7, (uint32_t)P));
+    const size_t need[] = {1, 1, 3, 2, 5, 4, 4};
+    for (size_t p = 0; p < pg.size(); ++p) pg[p].need = need[p];
+    std::vector<Batch> b;
+    assert(plan_batches(pg, 3, UINT64_MAX, true, &b));   // the gap after page 3 (a segment that is not woken) ends a batch
+    assert(same(b, {{0, 3, 3 * P, 3}, {3, 1, P, 2}, {4, 3, 3 * P, 5}}));
+    assert(!plan_batches(pg, 0, UINT64_MAX, true, &b));  // a slot smaller than a page
+    // K1 / K2 / K4 / K5 in place: by count, not adjacent, even when the pages are packed
+    assert(plan_batches(pg, 3, UINT64_MAX, false, &b) && same(b, {{0, 3, 3 * P, 3}, {3, 3, 3 * P, 5}, {6, 1, P, 4}}));
+    std::vector<PagePlan> packed = pages_with({0, C, 5 * P, 5 * P + C, 9 * P}, {C, C, C, (uint32_t)P, C}, 6);
+    assert(plan_batches(packed, 2, UINT64_MAX, false, &b) && same(b, {{0, 2, 2 * C, 6}, {2, 2, C + P, 6}, {4, 1, C, 6}}));
+    // next_batch alone: the first cut of a launch the wake may then extend over pages already mapped
+    const Batch first = next_batch(pg, 4, 2, UINT64_MAX, false);
+    assert(first.p0 == 4 && first.np == 2 && first.need == 5 && first.stored == 2 * P);
+    assert(plan_batches({}, 3, UINT64_MAX, true, &b) && b.empty());
+}
+
+static void test_chunk_queues() {
+    const std::vector<NumaRange> ranges = {{0, 10 * P, 0}, {10 * P, 20 * P, 1}};
+    const std::vector<uint64_t> off = {0, 4 * P, 8 * P, 12 * P, 16 * P, 19 * P};   // chunks 0-2 on node 0, 3-5 on node 1
+    {
+        ChunkQueues q(off, ranges);
+        size_t c, got[6];
+        for (size_t i = 0; i < 6; ++i) assert(q.take(1, &got[i]));   // own node's queue first, in image order, then the other
+        const size_t want[] = {3, 4, 5, 0, 1, 2};
+        for (size_t i = 0; i < 6; ++i) assert(got[i] == want[i]);
+        assert(!q.take(1, &c) && !q.take(0, &c));
+    }
+    {
+        ChunkQueues q(off, ranges);
+        size_t c;
+        assert(q.take(7, &c) && c == 0);   // a path on no node of the store: the queues in order
+        assert(q.take(0, &c) && c == 1);
+        assert(q.take(1, &c) && c == 3);
+    }
+    {
+        ChunkQueues q(off, {});   // no NUMA placement: one queue, image order
+        size_t c;
+        for (size_t i = 0; i < 6; ++i) assert(q.take(1, &c) && c == i);
+        assert(!q.take(0, &c));
+    }
+    // several threads: every chunk is taken exactly once
+    std::vector<uint64_t> many;
+    for (size_t i = 0; i < 5000; ++i) many.push_back((i * 7919 % 20) * P);
+    ChunkQueues q(many, ranges);
+    std::vector<std::atomic<int>> taken(many.size());
+    for (auto& t : taken) t.store(0);
+    std::vector<std::thread> th;
+    for (int t = 0; t < 6; ++t)
+        th.emplace_back([&, t] {
+            size_t c;
+            while (q.take(t % 3, &c)) taken[c].fetch_add(1);
+        });
+    for (auto& t : th) t.join();
+    for (auto& t : taken) assert(t.load() == 1);
+}
+
+static void test_resident_split() {
+    const uint64_t M = P;
+    auto split = [](std::vector<uint64_t> s, uint64_t cap) { return resident_split(s, cap); };
+    using K = std::vector<char>;
+    assert(split({4 * M, 2 * M, 6 * M}, 0) == K({0, 0, 0}));
+    assert(split({4 * M, 2 * M, 6 * M}, 6 * M) == K({0, 0, 1}));
+    assert(split({4 * M, 2 * M, 6 * M}, 7 * M) == K({0, 0, 1}));        // what is left fits nothing
+    assert(split({4 * M, 2 * M, 6 * M}, 9 * M) == K({0, 1, 1}));        // 4 pages do not fit the last 3: skipped
+    assert(split({4 * M, 2 * M, 6 * M}, 12 * M + M - 1) == K({1, 1, 1}));
+    assert(split({3 << 20, 3 << 20}, 6 << 20) == K({1, 1}));            // (the engine rounds the cap down to 2 MiB first)
+    assert(split({3 << 20, 3 << 20}, 5 << 20) == K({0, 1}));
+    assert(split({}, 8 * M).empty());
+    // against a brute-force restatement: from the last extent back, keep one when the kept ones after it leave room for it
+    std::mt19937 rng(11);
+    for (int it = 0; it < 2000; ++it) {
+        std::vector<uint64_t> s(rng() % 9);
+        for (auto& x : s) x = (rng() % 3 == 0) ? (1 + rng() % 6) * P : (1 + rng() % 6) * (uint64_t)C;
+        const uint64_t cap = rng() % 40 * P;
+        const K keep = resident_split(s, cap);
+        assert(keep.size() == s.size());
+        for (size_t k = 0; k < s.size(); ++k) {
+            uint64_t after = 0;
+            for (size_t j = k + 1; j < s.size(); ++j) after += keep[j] ? s[j] : 0;
+            assert(keep[k] == (after + s[k] <= cap));
+        }
+    }
+}
+
 int main() {
     test_bump_and_first_fit();
     test_coalescing_and_top_lowering();
     test_random_alloc_free_never_overlaps();
     test_plan_runs();
+    test_plan_pages();
+    test_batches_by_stored_bytes();
+    test_batches_by_pages();
+    test_chunk_queues();
+    test_resident_split();
     std::puts("layout ok");
     return 0;
 }

@@ -1,6 +1,6 @@
-"""The engine's address-space layout logic (VA arenas with first-fit reuse, run planning) is plain C++ in
-csrc/fma_layout.h and is what the engine (csrc/fma_engine.cu, fma_wake.cu) compiles in; exercised here on CPU with g++ (incl. a 20k-step randomised
-alloc/free invariant check)."""
+"""The engine's layout logic (VA arenas with first-fit reuse, run planning, and the pages, batches, chunk queues and resident
+split of the sleep / wake copy pipelines) is plain C++ in csrc/fma_layout.h and is what the engine (csrc/fma_engine.cu,
+fma_sleep.cu, fma_wake.cu) compiles in; exercised here on CPU with g++ (incl. a 20k-step randomised alloc/free invariant check)."""
 import os
 import subprocess
 
@@ -9,7 +9,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 def test_layout_logic(tmp_path):
     exe = str(tmp_path / "layout_test")
-    subprocess.check_call(["g++", "-std=c++17", "-O1", "-Wall", "-Wextra", "-Werror", "-I",
+    subprocess.check_call(["g++", "-std=c++17", "-O1", "-pthread", "-Wall", "-Wextra", "-Werror", "-I",
                            os.path.join(ROOT, "llm-d-fast-model-actuation_b200", "csrc"),
                            os.path.join(ROOT, "tests", "cpp", "layout_test.cpp"), "-o", exe])
     out = subprocess.check_output([exe], text=True)
@@ -18,5 +18,13 @@ def test_layout_logic(tmp_path):
 
 def test_engine_uses_the_tested_header():
     csrc = os.path.join(ROOT, "llm-d-fast-model-actuation_b200", "csrc")
-    src = "".join(open(os.path.join(csrc, f)).read() for f in ("fma_internal.h", "fma_engine.cu", "fma_wake.cu"))
+    read = {f: open(os.path.join(csrc, f)).read() for f in ("fma_internal.h", "fma_engine.cu", "fma_sleep.cu", "fma_wake.cu")}
+    src = "".join(read.values())
     assert '#include "fma_layout.h"' in src and "fma_layout::plan_runs(" in src and "fma_layout::arena_take(" in src
+    for f in ("fma_sleep.cu", "fma_wake.cu"):   # every copy pipeline takes its pages, batches and chunk queues from the header
+        for fn in ("fma_layout::plan_pages(", "fma_layout::plan_batches(", "fma_layout::ChunkQueues "):
+            assert fn in read[f], (f, fn)
+    assert "fma_layout::next_batch(" in read["fma_wake.cu"] and "fma_layout::resident_split(" in read["fma_sleep.cu"]
+    for f in ("fma_sleep.cu", "fma_wake.cu"):   # no pipeline plans by hand any more
+        for local in ("struct Dst", "struct Slot", "struct Chunk", "struct ResPiece", "need_item"):
+            assert local not in read[f], (f, local)
