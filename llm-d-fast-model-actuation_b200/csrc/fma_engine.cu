@@ -178,23 +178,31 @@ int arena_take(fma_engine_t* e, int tag, size_t bytes, int* out_arena, CUdevicep
     return FMA_OK;
 }
 
-// Unmap one unit (or, for `span_bytes` > unit.bytes, a VA-contiguous group of units in one driver call) and return
-// the VA of its zombies to their arena.  Caller has made sure nothing on the device still touches the range.
+// Unmap one unit (or, for `span_bytes` > unit.bytes, a VA-contiguous group of units in one driver call) and forget it.
+// Caller has made sure nothing on the device still touches the range.
 int unmap_units(fma_engine_t* e, CUdeviceptr va, size_t span_bytes) {
     DRV(g_drv.MemUnmap(va, span_bytes));
-    if (e->ring_attached && e->ring_unit_va >= va && e->ring_unit_va < va + span_bytes) {  // the ring went with its unit
-        for (int i = 0; i < kMaxRing; ++i) e->ring[i] = nullptr;
-        e->n_ring = 0;
-        e->ring_slot_bytes = 0;
-        e->ring_attached = false;
-        e->ring_unit_va = 0;
-    }
-    auto it = e->units.find(va);
-    while (it != e->units.end() && it->first < va + span_bytes) {
-        for (auto& z : it->second.zombies) arena_give_back(e->arenas[it->second.arena], z.first - e->arenas[it->second.arena].base, z.second);
+    forget_units(e, va, span_bytes);
+    return FMA_OK;
+}
+
+// The ring's fields once its memory is gone (freed, or unmapped with the unit that carried it).
+static void detach_ring(fma_engine_t* e) {
+    e->ring_attached = false;
+    e->ring_unit_va = 0;
+    for (int i = 0; i < kMaxRing; ++i) e->ring[i] = nullptr;
+    e->n_ring = 0;
+    e->ring_slot_bytes = 0;
+}
+
+void forget_units(fma_engine_t* e, CUdeviceptr va, size_t bytes) {
+    auto it = e->units.lower_bound(va);
+    while (it != e->units.end() && it->first < va + bytes) {
+        Arena& a = e->arenas[it->second.arena];
+        for (auto& z : it->second.zombies) arena_give_back(a, z.first - a.base, z.second);
         it = e->units.erase(it);
     }
-    return FMA_OK;
+    if (e->ring_attached && e->ring_unit_va >= va && e->ring_unit_va < va + bytes) detach_ring(e);  // the ring went with its unit
 }
 
 // ------------------------------------------------------------------------------------
@@ -276,11 +284,7 @@ size_t staged_slot(const fma_engine_t* e) {
 
 void release_ring(fma_engine_t* e) {
     if (e->n_ring && e->ring[0] && !e->ring_attached) cudaFree(e->ring[0]);  // one allocation backs every slot
-    e->ring_attached = false;           // an attached ring goes away with its unit's cuMemUnmap
-    e->ring_unit_va = 0;
-    for (int i = 0; i < kMaxRing; ++i) e->ring[i] = nullptr;
-    e->n_ring = 0;
-    e->ring_slot_bytes = 0;
+    detach_ring(e);                     // an attached ring goes away with its unit's cuMemUnmap
     cudaGetLastError();
 }
 
@@ -320,11 +324,8 @@ int ensure_ring(fma_engine_t* e, size_t image_bytes) {
         cudaGetLastError();
         return fail(FMA_ENOMEM, "cannot allocate %d x %zu byte HBM staging ring: %s", n, slot, cudaGetErrorString(r));
     }
-    for (int i = 0; i < n; ++i) {
-        e->ring[i] = static_cast<char*>(base) + (size_t)i * slot;
-        if (!e->ev_ring_full[i]) RT(cudaEventCreateWithFlags(&e->ev_ring_full[i], cudaEventDisableTiming));
-        if (!e->ev_ring_free[i]) RT(cudaEventCreateWithFlags(&e->ev_ring_free[i], cudaEventDisableTiming));
-    }
+    for (int i = 0; i < n; ++i) e->ring[i] = static_cast<char*>(base) + (size_t)i * slot;
+    RC(ensure_ring_events(e, n));
     e->n_ring = n;
     e->ring_slot_bytes = slot;
     return FMA_OK;
@@ -641,9 +642,8 @@ int engine_alloc(fma_engine_t* e, size_t bytes, int tag, void** out) {
     std::lock_guard<std::mutex> lk(e->mu);
     int arena = -1;
     CUdeviceptr va = 0;
-    int rc = arena_take(e, tag, sz, &arena, &va);
-    if (rc != FMA_OK) return rc;
-    rc = vmm_create_and_map(e->device, va, sz);
+    RC(arena_take(e, tag, sz, &arena, &va));
+    const int rc = vmm_create_and_map(e->device, va, sz);
     if (rc != FMA_OK) {
         arena_give_back(e->arenas[arena], va - e->arenas[arena].base, sz);
         return rc;
@@ -739,19 +739,12 @@ int flush_kernel_times(fma_engine_t* e) {
     return FMA_OK;
 }
 
-int resolve_mode(const fma_engine_t* e, int tier) {
-    int m = e->cfg.mode;
-    if (m == FMA_MODE_AUTO) m = (tier == FMA_TIER_HOST) ? FMA_MODE_STAGED : FMA_MODE_KERNEL;
-    if (tier != FMA_TIER_HOST && m == FMA_MODE_STAGED) m = FMA_MODE_KERNEL;  // staging only helps across PCIe
-    return m;
-}
-
 // A sleep or wake that may launch K1 / K2 checks the engine's TMA shape before it unmaps, maps or copies anything: the
 // launch wrapper refuses a shape that cannot run, and by the time of the first launch a sleep has already discarded
 // segments while others are still mapped.  set_option checks one key at a time (a shape is set key by key, through
 // combinations that do not fit), and FMA_TMA_* only seeds the same fields, so both are checked here.
 int check_tma_shape(const fma_engine_t* e, int tier) {
-    if (e->cfg.kernel != FMA_KERNEL_TMA || resolve_mode(e, tier) == FMA_MODE_DIRECT) return FMA_OK;
+    if (e->cfg.kernel != FMA_KERNEL_TMA || fma_layout::resolve_mode(e->cfg.mode, tier) == FMA_MODE_DIRECT) return FMA_OK;
     fma_k_tma_cfg c = e->tma;
     if (fma_k_tma_shape_fits(&c)) return FMA_OK;
     return fail(FMA_EINVAL, "TMA shape does not fit (tile %u B, %u stages, %u pipes): the tile must be >= 1 KiB, a multiple of 16 dividing "
@@ -773,10 +766,8 @@ int digest_segments(fma_engine_t* e, const std::vector<size_t>& idx, std::vector
     for (size_t i : idx) n_pages += e->segs[i].bytes / FMA_PAGE_BYTES;
     out->assign(idx.size(), 0);
     if (!n_pages) return FMA_OK;
-    int rc = ensure_streams(e);
-    if (rc != FMA_OK) return rc;
-    rc = ensure_desc(e, n_pages);
-    if (rc != FMA_OK) return rc;
+    RC(ensure_streams(e));
+    RC(ensure_desc(e, n_pages));
     size_t p = 0;
     for (size_t i : idx) {
         const Segment& s = e->segs[i];
@@ -1069,8 +1060,7 @@ int fma_timeline(fma_engine_t* e, char* buf, size_t cap) {
     if (check_engine(e) != FMA_OK) return FMA_EINVAL;
     {
         DeviceGuard guard(e->device);
-        int rc = flush_kernel_times(e);
-        if (rc != FMA_OK) return rc;
+        RC(flush_kernel_times(e));
     }
     std::lock_guard<std::mutex> lk(e->tl_mu);
     std::string out;
@@ -1266,8 +1256,7 @@ int fma_peer_attach(fma_engine_t* e, int fd, size_t bytes) {
             if (s.has_backup && s.backup_tier != FMA_TIER_HOST) return fail(FMA_ESTATE, "parking buffer holds a sleeping image");
     }
     DeviceGuard guard(e->device);
-    int rc = park_release(e);
-    if (rc != FMA_OK) return rc;
+    RC(park_release(e));
     ParkStore p;
     p.device = kForeignDevice;
     p.cap = bytes;
@@ -1312,8 +1301,7 @@ static int replace_store_for_paths(fma_engine_t* e) {
         const size_t cap = e->host.cap;
         if (e->shadow_tier == FMA_TIER_HOST) invalidate_shadows(e);
         host_store_free(e->host);
-        int rc = host_store_reserve(e, cap);
-        if (rc != FMA_OK) return rc;
+        RC(host_store_reserve(e, cap));
     }
     return FMA_OK;
 }
@@ -1413,8 +1401,7 @@ int fma_digest_all(fma_engine_t* e, uint64_t tag_mask, uint64_t* out, int n) {
         if (s.mapped && (!tag_mask || tag_bit_set(tag_mask, s.tag))) idx.push_back(i);
     }
     std::vector<uint64_t> dg;
-    int rc = digest_segments(e, idx, &dg);
-    if (rc != FMA_OK) return rc;
+    RC(digest_segments(e, idx, &dg));
     for (size_t k = 0; k < idx.size(); ++k) out[idx[k]] = dg[k];
     return FMA_OK;
 }
@@ -1426,8 +1413,7 @@ int fma_fill_segment(fma_engine_t* e, int index, uint64_t seed, uint64_t first_w
     if (!s.mapped) return fail(FMA_ESTATE, "segment %d is not mapped", index);
     DeviceGuard guard(e->device);
     const size_t n_pages = s.bytes / FMA_PAGE_BYTES;
-    int rc = ensure_desc(e, n_pages);
-    if (rc != FMA_OK) return rc;
+    RC(ensure_desc(e, n_pages));
     for (size_t p = 0; p < n_pages; ++p) {
         e->h_desc[p].addr = (uint64_t)s.va + p * FMA_PAGE_BYTES;
         e->h_desc[p].first_word = first_word + p * (FMA_PAGE_BYTES / 8);
@@ -1468,8 +1454,7 @@ int fma_op_page_copy(fma_engine_t* e, const uint64_t* src_pages, uint64_t src_ba
     if (check_engine(e) != FMA_OK) return FMA_EINVAL;
     if (!n_pages) return FMA_OK;
     DeviceGuard guard(e->device);
-    int rc = ensure_tables(e, n_pages);
-    if (rc != FMA_OK) return rc;
+    RC(ensure_tables(e, n_pages));
     const uint64_t* d_src = nullptr;
     const uint64_t* d_dst = nullptr;
     if (src_pages) {
@@ -1497,8 +1482,7 @@ int fma_op_page_digest(fma_engine_t* e, const uint64_t* pages, uint64_t base, co
     if (!n_pages) return FMA_OK;
     if (!out_page_digests) return fail(FMA_EINVAL, "out is NULL");
     DeviceGuard guard(e->device);
-    int rc = ensure_desc(e, n_pages);
-    if (rc != FMA_OK) return rc;
+    RC(ensure_desc(e, n_pages));
     for (uint32_t p = 0; p < n_pages; ++p) {
         e->h_desc[p].addr = pages ? pages[p] : base + (uint64_t)p * FMA_PAGE_BYTES;
         e->h_desc[p].first_word = first_word ? first_word[p] : (uint64_t)p * (FMA_PAGE_BYTES / 8);
@@ -1542,10 +1526,8 @@ int fma_op_pack_probe(fma_engine_t* e, const uint64_t* pages, uint64_t base, uin
     if (!n_pages) return FMA_OK;
     if (!out_stored_bytes) return fail(FMA_EINVAL, "out is NULL");
     DeviceGuard guard(e->device);
-    int rc = ensure_tables(e, n_pages);
-    if (rc != FMA_OK) return rc;
-    rc = ensure_pack_bufs(e, n_pages);
-    if (rc != FMA_OK) return rc;
+    RC(ensure_tables(e, n_pages));
+    RC(ensure_pack_bufs(e, n_pages));
     for (uint32_t p = 0; p < n_pages; ++p) e->h_tab[p] = pages ? pages[p] : base + (uint64_t)p * FMA_PAGE_BYTES;
     RT(cudaMemcpyAsync(e->d_tab, e->h_tab, n_pages * sizeof(uint64_t), cudaMemcpyHostToDevice, e->ks));
     RT(cudaEventRecord(e->ev_start, e->ks));
@@ -1566,8 +1548,7 @@ static int run_pack_op(fma_engine_t* e, bool unpack, const uint64_t* dev_pages, 
     if (!n_pages) return FMA_OK;
     if (!stored_bytes) return fail(FMA_EINVAL, "stored_bytes is NULL");
     DeviceGuard guard(e->device);
-    int rc = ensure_pack_bufs(e, n_pages);
-    if (rc != FMA_OK) return rc;
+    RC(ensure_pack_bufs(e, n_pages));
     uint64_t off = 0;
     for (uint32_t p = 0; p < n_pages; ++p) {
         if (stored_bytes[p] != FMA_K_PACKED_PAGE_BYTES && stored_bytes[p] != FMA_PAGE_BYTES)
@@ -1583,8 +1564,8 @@ static int run_pack_op(fma_engine_t* e, bool unpack, const uint64_t* dev_pages, 
     if (unpack) RT(fma_k_launch_unpack(e->d_pdesc, n_pages, d_err, e->ks));
     else RT(fma_k_launch_pack(e->d_pdesc, n_pages, d_err, e->ks));
     RT(cudaEventRecord(e->ev_end, e->ks));
-    rc = check_pack_errors(e, unpack ? "%u page(s) could not be decoded (malformed stored page)"
-                                     : "%u page(s) could not be coded (more exceptions than the probe saw)");
+    const int rc = check_pack_errors(e, unpack ? "%u page(s) could not be decoded (malformed stored page)"
+                                           : "%u page(s) could not be coded (more exceptions than the probe saw)");
     e->st.total_kernel_launches += 1;
     if (out_ms) RT(cudaEventElapsedTime(out_ms, e->ev_start, e->ev_end));
     return rc;
@@ -1682,8 +1663,7 @@ int fma_stats(fma_engine_t* e, fma_stats_t* out) {
     if (!out) return fail(FMA_EINVAL, "out is NULL");
     {
         DeviceGuard guard(e->device);
-        int rc = flush_kernel_times(e);
-        if (rc != FMA_OK) return rc;
+        RC(flush_kernel_times(e));
     }
     *out = e->st;
     {

@@ -231,8 +231,7 @@ int fma_image_adopt(fma_engine_t* e, int fd, uint64_t tag_mask, uint32_t flags) 
     e->st.host_store_bytes = cap;
     e->st.host_store_pin_seconds = h.pin_seconds;
     // release the device side exactly as a sleep would, without copying anything out
-    int rc = do_sleep(e, tag_mask, FMA_TIER_HOST, (flags & ~FMA_FLAG_VERIFY) | kFlagAdopt);
-    if (rc != FMA_OK) return rc;
+    RC(do_sleep(e, tag_mask, FMA_TIER_HOST, (flags & ~FMA_FLAG_VERIFY) | kFlagAdopt));
     (void)hd;
     image_apply(e, pi);
     return FMA_OK;
@@ -247,8 +246,7 @@ int fma_image_describe(fma_engine_t* e, int tier, void* buf, size_t cap) {
     if (resident_asleep(e)) return fail(FMA_ESTATE, "part of the sleeping image is resident in this process's own HBM (option resident_bytes) and cannot be handed over: set it to 0 and sleep again");
     if (tier != e->image_tier) return fail(FMA_ESTATE, "no image sleeps in tier %d", tier);
     std::vector<char> desc;
-    int rc = image_descriptor_build(e, tier, &desc);
-    if (rc != FMA_OK) return rc;
+    RC(image_descriptor_build(e, tier, &desc));
     if (buf && cap >= desc.size()) memcpy(buf, desc.data(), desc.size());
     return (int)desc.size();
 }
@@ -264,21 +262,18 @@ int fma_image_adopt_parked(fma_engine_t* e, const void* desc, size_t desc_bytes,
             if (!s.mapped) return fail(FMA_ESTATE, "adopt needs a fully awake engine");
     }
     ParsedImage pi;
-    int rc = image_descriptor_parse(e, static_cast<const char*>(desc), desc_bytes, e->park.cap, tag_mask, &pi);
-    if (rc != FMA_OK) return rc;
+    RC(image_descriptor_parse(e, static_cast<const char*>(desc), desc_bytes, e->park.cap, tag_mask, &pi));
     DeviceGuard guard(e->device);
     cudaDeviceSynchronize();
     if (flags & FMA_FLAG_VERIFY) {  // "sleep by adoption" (see fma_image_adopt): only if this engine's bytes ARE the image's
         std::vector<uint64_t> now;
-        rc = digest_segments(e, pi.order, &now);
-        if (rc != FMA_OK) return rc;
+        RC(digest_segments(e, pi.order, &now));
         for (size_t i = 0; i < pi.ds.size(); ++i)
             if (!pi.ds[i].digest_valid || pi.ds[i].digest != now[i])
                 return fail(FMA_EINTEGRITY, pi.ds[i].digest_valid ? "the image holds different bytes than this engine's segments" : "the image carries no digests to compare with");
     }
     if (e->shadow_tier != FMA_TIER_HOST) invalidate_shadows(e);
-    rc = do_sleep(e, tag_mask, FMA_TIER_PEER, (flags & ~FMA_FLAG_VERIFY) | kFlagAdopt);
-    if (rc != FMA_OK) return rc;
+    RC(do_sleep(e, tag_mask, FMA_TIER_PEER, (flags & ~FMA_FLAG_VERIFY) | kFlagAdopt));
     image_apply(e, pi);
     return FMA_OK;
 }

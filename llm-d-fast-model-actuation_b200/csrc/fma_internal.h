@@ -21,7 +21,6 @@
 #include <cstdlib>
 #include <cerrno>
 #include <cstring>
-#include <functional>
 #include <iterator>
 #include <map>
 #include <mutex>
@@ -57,6 +56,8 @@ int env_int(const char* name, int dflt);
         if (_e != cudaSuccess)                                                                            \
             return fail(FMA_ECUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(_e), __FILE__, __LINE__); \
     } while (0)
+
+#define RC(expr) do { int _rc = (expr); if (_rc != FMA_OK) return _rc; } while (0)   // an FMA_* error code goes back to the caller
 
 // ------------------------------------------------------------------------------------
 // driver API, resolved lazily through the (static) runtime: no link-time libcuda dependency
@@ -353,6 +354,8 @@ int check_engine(fma_engine_t* e);
 // ---- VMM primitives, arenas (fma_engine.cu) ----
 int vmm_create_and_map(int device, CUdeviceptr va, size_t bytes);
 int unmap_units(fma_engine_t* e, CUdeviceptr va, size_t span_bytes);
+// drop the (unmapped) units in [va, va + bytes) from the table: zombies' VA back to their arenas, an attached ring detached
+void forget_units(fma_engine_t* e, CUdeviceptr va, size_t bytes);
 // ---- engine resources (fma_engine.cu) ----
 int ensure_streams(fma_engine_t* e);
 int ensure_tables(fma_engine_t* e, size_t n_pages);
@@ -468,7 +471,6 @@ struct KernelTimes {  // event pairs around each K1/K2 launch on the kernel stre
 };
 
 int flush_kernel_times(fma_engine_t* e);
-int resolve_mode(const fma_engine_t* e, int tier);
 int check_tma_shape(const fma_engine_t* e, int tier);
 uint64_t store_dev_base(const fma_engine_t* e, int tier);
 void* store_copy_base(const fma_engine_t* e, int tier);

@@ -12,6 +12,8 @@
 #include <map>
 #include <vector>
 
+#include "../../include/fma_engine.h"
+
 namespace fma_layout {
 
 // One VA arena per tag: segments of a tag are bump-allocated next to each other, so that after a sleep the whole tag
@@ -242,6 +244,81 @@ inline std::vector<char> resident_split(const std::vector<uint64_t>& stored, uin
             cap -= stored[k];
         }
     return keep;
+}
+
+// ---- which pipeline a sleep / wake runs ----
+// The configured mode as a tier runs it: AUTO is STAGED on the host tier, KERNEL on the parking tiers (staging helps over PCIe).
+inline int resolve_mode(int cfg_mode, int tier) {
+    int m = cfg_mode;
+    if (m == FMA_MODE_AUTO) m = (tier == FMA_TIER_HOST) ? FMA_MODE_STAGED : FMA_MODE_KERNEL;
+    if (tier != FMA_TIER_HOST && m == FMA_MODE_STAGED) m = FMA_MODE_KERNEL;
+    return m;
+}
+
+enum class SleepPipeKind { Adopt, PartialDirect, PartialPacked, Direct, Kernel, KernelPacked, Staged, StagedPacked, Multipath };
+
+// What a sleep knows when it picks its pipeline.  `ring` and `worth_packing` are answers of calls with side effects (a ring
+// allocation, the K4p probe): ask with both true, make the calls the route wants, then ask again with the answers.
+struct SleepFacts {
+    int tier, mode;            // mode: resolve_mode of the configured mode
+    bool pack, paths, mbox;    // option "pack"; MULTI-PATH configured; ... with remote paths
+    bool adopt;                // nothing moves: an adopted image, or no bytes to offload
+    // INCREMENTAL: the store holds exactly this image; only the changed segments move (plain image); only the changed pages
+    // are re-coded in place (PACKED image: their stored sizes held, and a staging ring was had for them)
+    bool clean, partial, partial_packed;
+    bool multipath_env, ring = true, worth_packing = true;  // FMA_MULTIPATH_SLEEP; a staging ring is available; K4p found it worth packing
+};
+struct SleepRoute {
+    SleepPipeKind pipe;
+    int mode;                  // what fma_stats_t.mode reports
+    bool wants_ring, wants_probe;  // `ring` / `worth_packing` decide the pipe
+};
+
+inline SleepRoute sleep_route(const SleepFacts& f) {
+    if (f.adopt || f.clean) return SleepRoute{SleepPipeKind::Adopt, f.mode, false, false};
+    if (f.partial_packed) return SleepRoute{SleepPipeKind::PartialPacked, f.mode, false, false};
+    if (f.partial) return SleepRoute{SleepPipeKind::PartialDirect, FMA_MODE_DIRECT, false, false};
+    SleepRoute r{SleepPipeKind::Staged, f.mode, false, false};
+    // MULTI-PATH: a full, plain host-tier sleep is striped over the paths' links, each with its own staging slots
+    const bool multipath = f.paths && !f.mbox && f.tier == FMA_TIER_HOST && f.mode == FMA_MODE_STAGED && !f.pack && f.multipath_env;
+    r.wants_ring = f.mode == FMA_MODE_STAGED && !multipath;
+    if (r.wants_ring && !f.ring) r.mode = FMA_MODE_DIRECT;  // HBM too full for a ring
+    // PACKED: through the staging ring on the host tier; K4 writes the store itself on the parking tiers
+    r.wants_probe = f.pack && ((f.tier == FMA_TIER_HOST && r.mode == FMA_MODE_STAGED) || (f.tier != FMA_TIER_HOST && r.mode == FMA_MODE_KERNEL));
+    const bool packed = r.wants_probe && f.worth_packing;
+    if (r.mode == FMA_MODE_DIRECT) r.pipe = SleepPipeKind::Direct;
+    else if (r.mode == FMA_MODE_KERNEL) r.pipe = packed ? SleepPipeKind::KernelPacked : SleepPipeKind::Kernel;
+    else if (multipath) r.pipe = SleepPipeKind::Multipath;
+    else r.pipe = packed ? SleepPipeKind::StagedPacked : SleepPipeKind::Staged;
+    return r;
+}
+
+enum class WakePipeKind { PackedRing, PackedZeroCopy, Direct, Kernel, Staged, Multipath };
+
+// What a wake knows when it picks its pipeline; `ring` as in SleepFacts (a ring attached to the first run, or allocated).
+struct WakeFacts {
+    int tier, mode;            // mode: resolve_mode of the configured mode
+    bool image_packed, paths;  // the sleeping image is PACKED; MULTI-PATH configured
+    bool moves;                // bytes cross the link (a resident share's do not)
+    bool no_ring, ring = true; // FMA_NO_RING; a staging ring is available
+};
+struct WakeRoute {
+    WakePipeKind pipe;
+    int mode;                  // what fma_stats_t.mode reports
+    bool wants_ring;           // `ring` decides the pipe
+};
+
+inline WakeRoute wake_route(const WakeFacts& f) {
+    // a PACKED image can only be read by K5: through the staging ring, or straight from the store
+    WakeRoute r{WakePipeKind::Staged, f.image_packed && f.tier == FMA_TIER_HOST ? FMA_MODE_STAGED : f.mode, false};
+    const bool multipath = f.paths && f.tier == FMA_TIER_HOST && r.mode == FMA_MODE_STAGED && !f.image_packed;
+    r.wants_ring = f.moves && r.mode == FMA_MODE_STAGED && !multipath && !f.no_ring;
+    if (f.moves && r.mode == FMA_MODE_STAGED && !multipath && (f.no_ring || !f.ring)) r.mode = FMA_MODE_DIRECT;
+    if (f.image_packed) r.pipe = r.mode == FMA_MODE_STAGED ? WakePipeKind::PackedRing : WakePipeKind::PackedZeroCopy;
+    else if (multipath) r.pipe = WakePipeKind::Multipath;
+    else if (r.mode == FMA_MODE_DIRECT) r.pipe = WakePipeKind::Direct;
+    else if (r.mode == FMA_MODE_KERNEL) r.pipe = WakePipeKind::Kernel;
+    return r;
 }
 
 }  // namespace fma_layout

@@ -12,8 +12,7 @@ int fma_load_file(fma_engine_t* e, const char* path, const fma_load_span_t* span
     if (!path || (!spans && n_spans)) return fail(FMA_EINVAL, "NULL path or spans");
     const double t_entry = now_s();
     DeviceGuard guard(e->device);
-    int rc = ensure_streams(e);
-    if (rc != FMA_OK) return rc;
+    RC(ensure_streams(e));
     const bool direct = (flags & FMA_LOAD_O_DIRECT) != 0;
     int fd = open(path, O_RDONLY | (direct ? O_DIRECT : 0));
     if (fd < 0) return fail(FMA_EINVAL, "cannot open %s: %s", path, strerror(errno));

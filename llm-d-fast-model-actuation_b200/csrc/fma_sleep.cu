@@ -9,10 +9,8 @@ namespace {
 
 // K4p over the pages of `ex`: the stored size of each lands in e->h_psize[0, n_pages).  pack_pages: descriptors to provide for.
 int pack_probe(fma_engine_t* e, const std::vector<Extent>& ex, size_t n_pages, size_t pack_pages) {
-    int rc = ensure_tables(e, n_pages);
-    if (rc != FMA_OK) return rc;
-    rc = ensure_pack_bufs(e, pack_pages);
-    if (rc != FMA_OK) return rc;
+    RC(ensure_tables(e, n_pages));
+    RC(ensure_pack_bufs(e, pack_pages));
     build_page_table(ex, e->h_tab);
     RT(cudaMemcpyAsync(e->d_tab, e->h_tab, n_pages * sizeof(uint64_t), cudaMemcpyHostToDevice, e->ks));
     RT(fma_k_launch_pack_probe(e->d_tab, (uint32_t)n_pages, e->d_psize, e->ks));
@@ -27,14 +25,21 @@ int digest_and_mark(fma_engine_t* e, const std::vector<Extent>& ex, std::vector<
     std::vector<size_t> idx;
     for (const Extent& x : ex) idx.push_back(x.seg_index);
     std::vector<uint64_t> dg;
-    int rc = digest_segments(e, idx, &dg);
-    if (rc != FMA_OK) return rc;
+    RC(digest_segments(e, idx, &dg));
     for (size_t k = 0; k < idx.size(); ++k) {
         e->segs[idx[k]].digest = dg[k];
         e->segs[idx[k]].digest_valid = true;
     }
     if (out) *out = std::move(dg);
     return FMA_OK;
+}
+
+// x's bytes are in the store of `tier`, at x.packed_off
+void mark_backed_up(fma_engine_t* e, const Extent& x, int tier) {
+    Segment& s = e->segs[x.seg_index];
+    s.has_backup = true;
+    s.backup_tier = tier;
+    s.packed_off = x.packed_off;
 }
 
 const char* const kPackChanged = "%u page(s) changed between the pack probe and the pack: weights were written during sleep";
@@ -53,8 +58,7 @@ int plan_packed_image(fma_engine_t* e, const std::vector<Extent>& ex, uint64_t W
     *stored_total = W;
     const size_t n_pages = W / FMA_PAGE_BYTES;
     RT(cudaDeviceSynchronize());  // the caller's streams may still be writing weights (same reason as in do_sleep)
-    int rc = pack_probe(e, ex, n_pages, n_pages);
-    if (rc != FMA_OK) return rc;
+    RC(pack_probe(e, ex, n_pages, n_pages));
     off->resize(n_pages);
     bytes->resize(n_pages);
     uint64_t total = 0;
@@ -85,6 +89,14 @@ struct Stage {
     cudaEvent_t ev;
     std::vector<Range> ranges;
 };
+// Units in VA order, split into "discarded" (release now) and "offloaded" (release once the image has their
+// bytes).  image_end = packed offset just past the unit's last live segment.
+struct PlannedUnit {
+    CUdeviceptr va;
+    size_t bytes;
+    uint64_t image_end;
+};
+
 struct Unmapper {
     fma_engine_t* e;
     std::mutex mu;
@@ -96,7 +108,60 @@ struct Unmapper {
     double seconds = 0;
     std::vector<Range> first;  // ranges with nothing to wait for (discarded tags)
     std::vector<Range> done;   // ranges actually unmapped
+    std::vector<PlannedUnit> off_units;  // offloaded units, same order as the image
+    size_t next_unit = 0;                // first offloaded unit not yet handed to the thread
+    size_t stage_events_used = 0;
     std::thread th;
+    explicit Unmapper(fma_engine_t* eng) : e(eng) {}
+    static void add_range(std::vector<Range>& v, CUdeviceptr va, size_t bytes) {
+        if (!v.empty() && v.back().va + v.back().bytes == va) v.back().bytes += bytes;  // VA-adjacent: one driver call
+        else v.push_back(Range{va, bytes});
+    }
+    // every unit: discarded (unmapped first) or offloaded (once the image has its bytes); keep_ring: the unit that holds the
+    // ring is unmapped after the last D2H
+    void plan(const std::vector<Extent>& ex, bool keep_ring) {
+        std::map<CUdeviceptr, uint64_t> unit_end;  // unit -> image_end (offloaded units only)
+        for (const Extent& x : ex) {
+            uint64_t& end = unit_end[e->segs[x.seg_index].unit_va];
+            end = std::max<uint64_t>(end, x.packed_off + x.bytes);
+        }
+        // arenas in index order, units by VA inside: identical to the image order
+        std::vector<const Unit*> ordered;
+        for (auto& kv : e->units) ordered.push_back(&kv.second);
+        std::sort(ordered.begin(), ordered.end(), [](const Unit* a, const Unit* b) { return a->arena != b->arena ? a->arena < b->arena : a->va < b->va; });
+        for (const Unit* u : ordered) {
+            auto it = unit_end.find(u->va);
+            if (e->ring_attached && u->va == e->ring_unit_va && keep_ring) continue;
+            if (it == unit_end.end()) add_range(first, u->va, u->bytes);
+            else off_units.push_back(PlannedUnit{u->va, u->bytes, it->second});
+        }
+    }
+    int stage_event(cudaStream_t stream, cudaEvent_t* out) {
+        if (stage_events_used == e->ev_stage.size()) {
+            cudaEvent_t ev;
+            RT(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+            e->ev_stage.push_back(ev);
+        }
+        *out = e->ev_stage[stage_events_used++];
+        RT(cudaEventRecord(*out, stream));
+        return FMA_OK;
+    }
+    // everything whose bytes are inside image[0, image_done) and has been read by work enqueued on `stream` so far
+    int publish_consumed(uint64_t image_done, cudaStream_t stream) {
+        Stage st;
+        while (next_unit < off_units.size() && off_units[next_unit].image_end <= image_done) {
+            add_range(st.ranges, off_units[next_unit].va, off_units[next_unit].bytes);
+            ++next_unit;
+        }
+        if (st.ranges.empty()) return FMA_OK;
+        RC(stage_event(stream, &st.ev));
+        {
+            std::lock_guard<std::mutex> lk(mu);
+            stages.push_back(std::move(st));
+        }
+        cv.notify_all();
+        return FMA_OK;
+    }
     void unmap_range(const Range& r, bool dbg) {
         double a;
         CUresult r1;
@@ -146,19 +211,15 @@ struct Unmapper {
             ++k;
         }
     }
-    void publish(Stage&& st) {
-        {
-            std::lock_guard<std::mutex> lk(mu);
-            stages.push_back(std::move(st));
-        }
-        cv.notify_all();
-    }
-    void finish() {
+    void close() {  // nothing more to come: the thread ends after the last published stage
         {
             std::lock_guard<std::mutex> lk(mu);
             closed = true;
         }
         cv.notify_all();
+    }
+    void finish() {
+        close();
         if (th.joinable()) th.join();
     }
     ~Unmapper() { finish(); }
@@ -176,45 +237,21 @@ struct ApplyUnmapped {
         std::lock_guard<std::mutex> lk(e->mu);
         for (; applied < un->done.size(); ++applied) {
             const Range& r = un->done[applied];
-            auto it = e->units.lower_bound(r.va);
-            while (it != e->units.end() && it->first < r.va + r.bytes) {
-                Arena& a = e->arenas[it->second.arena];
-                for (auto& z : it->second.zombies) arena_give_back(a, z.first - a.base, z.second);
-                it = e->units.erase(it);
-            }
-            if (e->ring_attached && e->ring_unit_va >= r.va && e->ring_unit_va < r.va + r.bytes) {
-                for (int i = 0; i < kMaxRing; ++i) e->ring[i] = nullptr;
-                e->n_ring = 0; e->ring_slot_bytes = 0; e->ring_attached = false; e->ring_unit_va = 0;
-            }
+            forget_units(e, r.va, r.bytes);
             for (Segment& sg : e->segs)
                 if (sg.va >= r.va && sg.va < r.va + r.bytes) {
                     sg.mapped = false;
                     sg.unit_va = 0;
                 }
             for (const Extent& x : *ex)
-                if (x.va >= r.va && x.va < r.va + r.bytes) {
-                    Segment& sg = e->segs[x.seg_index];
-                    sg.has_backup = true;
-                    sg.backup_tier = tier;
-                    sg.packed_off = x.packed_off;
-                }
+                if (x.va >= r.va && x.va < r.va + r.bytes) mark_backed_up(e, x, tier);
         }
-        if (!un->done.empty()) {  // even a failed sleep leaves an image a later wake can restore from
-            e->image_tier = tier;
-        }
+        if (!un->done.empty()) e->image_tier = tier;  // even a failed sleep leaves an image a later wake can restore from
     }
     ~ApplyUnmapped() {
         un->finish();
         run();
     }
-};
-
-// Units in VA order, split into "discarded" (release now) and "offloaded" (release once the image has their
-// bytes).  image_end = packed offset just past the unit's last live segment.
-struct PlannedUnit {
-    CUdeviceptr va;
-    size_t bytes;
-    uint64_t image_end;
 };
 
 // What the copy pipelines of one sleep share.  Each pipeline enqueues the work that moves image[0, W) into the store
@@ -227,9 +264,10 @@ struct SleepPipe {
     char* store;           // host pointer of the store (copy-engine target), or the parking buffer
     KernelTimes& kt;
     uint32_t& copy_ops;
-    std::function<int(uint64_t, cudaStream_t)> publish_consumed;
+    Unmapper* un;          // releases units behind the pipeline; null: nothing is released (the resident gather)
     const std::vector<size_t>* subset = nullptr;  // INCREMENTAL + PACKED: only these image pages (ascending) are re-coded, in place
     bool resident = false;  // the extents go to the resident buffer (e->res, its own page layout res_off / res_bytes), not the tier's store
+    int publish_consumed(uint64_t image_done, cudaStream_t stream) { return un ? un->publish_consumed(image_done, stream) : FMA_OK; }
     int publish_gathered(size_t pages_done) { return publish_consumed((uint64_t)pages_done * FMA_PAGE_BYTES, e->ks); }
     // the image's pages, stored in the PACKED layout or verbatim; their device addresses in order -> e->h_tab / e->d_tab
     int plan(bool packed, std::vector<PagePlan>* pages) {
@@ -240,8 +278,7 @@ struct SleepPipe {
         uint64_t bad = 0;
         if (!fma_layout::plan_pages(segs, packed ? &off : nullptr, &bytes, pages, &bad))
             return fail(FMA_ESTATE, "image offset %llu is outside the packed image's page table", (unsigned long long)bad);
-        int rc = ensure_tables(e, pages->size());
-        if (rc != FMA_OK) return rc;
+        RC(ensure_tables(e, pages->size()));
         build_page_table(ex, e->h_tab);
         RT(cudaMemcpyAsync(e->d_tab, e->h_tab, pages->size() * sizeof(uint64_t), cudaMemcpyHostToDevice, e->ks));
         return FMA_OK;
@@ -256,7 +293,6 @@ struct SleepPipe {
 
 // DIRECT: copy engines move each segment chunk straight into the packed image
 int SleepPipe::direct() {
-    int rc = FMA_OK;
     const size_t chunk = direct_chunk(e);
     // copy engines straight from the segments into the packed image, chunks round-robin over the streams;
     // every `slot` bytes of image the streams are joined so that one event marks the units behind it dead
@@ -276,23 +312,20 @@ int SleepPipe::direct() {
                 RT(cudaEventRecord(e->ev_cs[i], e->cs[i]));
                 RT(cudaStreamWaitEvent(e->cs[0], e->ev_cs[i], 0));
             }
-            rc = publish_consumed(image_done, e->cs[0]);
-            if (rc != FMA_OK) return rc;
+            RC(publish_consumed(image_done, e->cs[0]));
             next_join = image_done + slot;
         }
     }
-    return rc;
+    return FMA_OK;
 }
 
 // KERNEL + PACKED (parking tiers): K4 encodes straight into the peer / local HBM store
 int SleepPipe::kernel_packed() {
     std::vector<PagePlan> pages;
-    int rc = plan(true, &pages);
-    if (rc != FMA_OK) return rc;
+    RC(plan(true, &pages));
     // PACKED image in a parking tier: K4 encodes straight into the peer / local HBM store (0.758 of the bytes
     // over NVLink and of the parking GPU's HBM), batches as below
-    rc = ensure_pack_bufs(e, pages.size());
-    if (rc != FMA_OK) return rc;
+    RC(ensure_pack_bufs(e, pages.size()));
     const uint64_t dbase = resident ? (uint64_t)e->res.va : store_dev_base(e, tier);
     for (size_t p = 0; p < pages.size(); ++p) set_pack_desc(e->h_pdesc[p], pages[p].va, dbase + pages[p].off, pages[p].bytes);
     uint32_t* d_err = e->d_psize + e->pdesc_cap;
@@ -301,45 +334,36 @@ int SleepPipe::kernel_packed() {
     std::vector<Batch> batches;
     fma_layout::plan_batches(pages, slot_pages(e), UINT64_MAX, false, &batches);
     for (const Batch& b : batches) {
-        rc = kt.begin();
-        if (rc != FMA_OK) return rc;
+        RC(kt.begin());
         RT(fma_k_launch_pack(e->d_pdesc + b.p0, (uint32_t)b.np, d_err, e->ks));
-        rc = kt.end((uint64_t)b.np * FMA_PAGE_BYTES + b.stored);
-        if (rc != FMA_OK) return rc;
+        RC(kt.end((uint64_t)b.np * FMA_PAGE_BYTES + b.stored));
         ++copy_ops;
-        rc = publish_gathered(b.p0 + b.np);
-        if (rc != FMA_OK) return rc;
+        RC(publish_gathered(b.p0 + b.np));
     }
-    return rc;
+    return FMA_OK;
 }
 
 // KERNEL: K1 writes the store itself (mapped pinned host memory, peer or local HBM)
 int SleepPipe::kernel() {
     std::vector<PagePlan> pages;
-    int rc = plan(false, &pages);
-    if (rc != FMA_OK) return rc;
+    RC(plan(false, &pages));
     // K1 writes the store itself: mapped pinned host memory (PCIe posted writes) or peer/local HBM;
     // launched in slot-sized batches so finished segments can be released while later ones still move
     const uint64_t dbase = resident ? (uint64_t)e->res.va : store_dev_base(e, tier);
     std::vector<Batch> batches;
     fma_layout::plan_batches(pages, slot_pages(e), UINT64_MAX, false, &batches);
     for (const Batch& b : batches) {
-        rc = kt.launch(e->d_tab + b.p0, 0, nullptr, dbase + pages[b.p0].off, (uint32_t)b.np);
-        if (rc != FMA_OK) return rc;
+        RC(kt.launch(e->d_tab + b.p0, 0, nullptr, dbase + pages[b.p0].off, (uint32_t)b.np));
         ++copy_ops;
-        rc = publish_gathered(b.p0 + b.np);
-        if (rc != FMA_OK) return rc;
+        RC(publish_gathered(b.p0 + b.np));
     }
-    return rc;
+    return FMA_OK;
 }
 
 // STAGED + PACKED: K4 gather + encode -> ring slot (stored pages back to back) -> one D2H per slot
 int SleepPipe::staged_packed() {
     std::vector<PagePlan> pages;
-    int rc = plan(true, &pages);
-    if (rc != FMA_OK) return rc;
-    rc = ensure_ring(e, W);
-    if (rc != FMA_OK) return rc;
+    RC(plan(true, &pages));   // (the route has the ring)
     // the image pages this sleep codes: all of them, or (incremental) the pages of the changed segments, whose stored size
     // is known not to change, so each goes back to its old place in the kept image
     std::vector<size_t> img_page(pages.size());
@@ -365,11 +389,9 @@ int SleepPipe::staged_packed() {
         const int slot = (int)(c % e->n_ring);
         cudaStream_t cstream = e->cs[c % e->n_cs];
         if (c >= (size_t)e->n_ring) RT(cudaStreamWaitEvent(e->ks, e->ev_ring_free[slot], 0));
-        rc = kt.begin();
-        if (rc != FMA_OK) return rc;
+        RC(kt.begin());
         RT(fma_k_launch_pack(e->d_pdesc + sl.p0, (uint32_t)sl.np, d_err, e->ks));
-        rc = kt.end((uint64_t)sl.np * FMA_PAGE_BYTES + sl.stored);
-        if (rc != FMA_OK) return rc;
+        RC(kt.end((uint64_t)sl.np * FMA_PAGE_BYTES + sl.stored));
         RT(cudaEventRecord(e->ev_ring_full[slot], e->ks));
         RT(cudaStreamWaitEvent(cstream, e->ev_ring_full[slot], 0));
         RT(cudaMemcpyAsync(store + pages[sl.p0].off, e->ring[slot], sl.stored, cudaMemcpyDefault, cstream));
@@ -377,21 +399,16 @@ int SleepPipe::staged_packed() {
         RT(cudaEventRecord(e->ev_ring_free[slot], cstream));
         ++copy_ops;
         // every image byte below the last page of this slot is in the store: coded just now, or kept from the last wake
-        rc = publish_consumed((uint64_t)(img_page[sl.p0 + sl.np - 1] + 1) * FMA_PAGE_BYTES, cstream);
-        if (rc != FMA_OK) return rc;
+        RC(publish_consumed((uint64_t)(img_page[sl.p0 + sl.np - 1] + 1) * FMA_PAGE_BYTES, cstream));
         last_stream = cstream;
     }
-    if (subset) rc = publish_consumed(W, last_stream);  // the clean tail of the image needs no copy
-    return rc;
+    return subset ? publish_consumed(W, last_stream) : FMA_OK;  // the clean tail of the image needs no copy
 }
 
 // STAGED: K1 gather -> HBM ring slot -> one large D2H per slot
 int SleepPipe::staged() {
     std::vector<PagePlan> pages;
-    int rc = plan(false, &pages);
-    if (rc != FMA_OK) return rc;
-    rc = ensure_ring(e, W);
-    if (rc != FMA_OK) return rc;
+    RC(plan(false, &pages));   // (the route has the ring)
     std::vector<Batch> slots;
     if (!fma_layout::plan_batches(pages, e->ring_slot_bytes / FMA_PAGE_BYTES, UINT64_MAX, true, &slots))
         return fail(FMA_EINVAL, "ring slot of %zu bytes cannot hold one page", e->ring_slot_bytes);
@@ -400,8 +417,7 @@ int SleepPipe::staged() {
         const int slot = (int)(c % e->n_ring);
         cudaStream_t cstream = e->cs[c % e->n_cs];
         if (c >= (size_t)e->n_ring) RT(cudaStreamWaitEvent(e->ks, e->ev_ring_free[slot], 0));
-        rc = kt.launch(e->d_tab + sl.p0, 0, nullptr, (uint64_t)(uintptr_t)e->ring[slot], (uint32_t)sl.np);
-        if (rc != FMA_OK) return rc;
+        RC(kt.launch(e->d_tab + sl.p0, 0, nullptr, (uint64_t)(uintptr_t)e->ring[slot], (uint32_t)sl.np));
         RT(cudaEventRecord(e->ev_ring_full[slot], e->ks));
         RT(cudaStreamWaitEvent(cstream, e->ev_ring_full[slot], 0));
         RT(cudaMemcpyAsync(store + pages[sl.p0].off, e->ring[slot], sl.stored, cudaMemcpyDefault, cstream));
@@ -410,10 +426,9 @@ int SleepPipe::staged() {
         if (c > 0) RT(cudaStreamWaitEvent(cstream, e->ev_ring_free[(c - 1) % e->n_ring], 0));
         RT(cudaEventRecord(e->ev_ring_free[slot], cstream));
         ++copy_ops;
-        rc = publish_consumed((uint64_t)(sl.p0 + sl.np) * FMA_PAGE_BYTES, cstream);  // units fully in the store are dead
-        if (rc != FMA_OK) return rc;
+        RC(publish_consumed((uint64_t)(sl.p0 + sl.np) * FMA_PAGE_BYTES, cstream));  // units fully in the store are dead
     }
-    return rc;
+    return FMA_OK;
 }
 
 // MULTI-PATH sleep (fma_paths_set): the mirror image of the multi-path wake.  K1 on the sleeping GPU gathers a chunk of the image
@@ -422,10 +437,8 @@ int SleepPipe::staged() {
 // before every byte has reached the store (one publish at the end), so a failure half way leaves the engine awake and intact.
 int SleepPipe::multipath() {
     std::vector<PagePlan> pages;
-    int rc = plan(false, &pages);
-    if (rc != FMA_OK) return rc;
-    rc = ensure_ring_events(e, 1);
-    if (rc != FMA_OK) return rc;
+    RC(plan(false, &pages));
+    RC(ensure_ring_events(e, 1));
     cudaEvent_t ev_tab = e->ev_ring_full[0];
     RT(cudaEventRecord(ev_tab, e->ks));
     std::vector<Batch> chunks;
@@ -493,6 +506,340 @@ int SleepPipe::multipath() {
     return publish_consumed(W, e->ks);   // all bytes are in the store: every offloaded unit may go
 }
 
+// What one sleep moves and how, filled in phase by phase by do_sleep.
+struct SleepPlan {
+    int tier;
+    uint32_t flags;
+    std::vector<Extent> ex;       // offloaded extents the tier's store receives, image order
+    std::vector<Extent> ex_res;   // RESIDENT share: extents kept in e->res, packed_off = offset in the resident part
+    uint64_t W = 0, W_all = 0, discarded = 0;   // bytes of ex, of everything offloaded, of the discarded tags
+    // the store that would hold the kept image exists; INCREMENTAL: it may still hold exactly this image
+    bool kept_store = false, shadows_match = false;
+    // per extent: digest of the copy the store holds, and where it holds it (kNoOffset: no usable copy)
+    std::vector<uint64_t> shadow_digest, shadow_at, res_seqs;
+    // the image in the store: PACKED or not, its page table and its bytes; planned by the resident split (pre_planned: K4p over
+    // the whole image before the ring is known) or by route_sleep
+    bool pre_planned = false, packed = false;
+    std::vector<uint64_t> pk_off;
+    std::vector<uint32_t> pk_bytes;
+    uint64_t Wp = 0;
+    bool clean = false, partial = false, partial_packed = false, digests_known = false;   // INCREMENTAL outcome
+    std::vector<Extent> dirty;        // segments whose device bytes differ from the copy in the store
+    std::vector<size_t> dirty_pages;  // their image pages (PACKED image)
+    fma_layout::SleepRoute route{};
+    CopyTimer timer;                  // device-time bookkeeping of the copies
+    KernelTimes kt;
+    uint32_t copy_ops = 0;
+    double copy_s = 0;
+    SleepPlan(fma_engine_t* e, int t, uint32_t f) : tier(t), flags(f), timer{e}, kt{e} {}
+    bool adopt() const { return (flags & kFlagAdopt) || clean || !W; }  // not a byte moves (the route is then Adopt)
+};
+
+fma_layout::SleepFacts sleep_facts(const fma_engine_t* e, const SleepPlan& p) {
+    return fma_layout::SleepFacts{p.tier, fma_layout::resolve_mode(e->cfg.mode, p.tier), e->cfg.pack != 0, !e->paths.empty(), e->mbox != nullptr,
+                                  (p.flags & kFlagAdopt) || !p.W, p.clean, p.partial, p.partial_packed, env_int("FMA_MULTIPATH_SLEEP", 1) != 0};
+}
+
+// 1. offloaded segments -> packed image, in (arena, VA) order.  Arenas are bump-allocated per tag, so this is allocation order
+// (the reference's dict order, cumem.py:198) unless a freed hole was reused.
+void plan_image(fma_engine_t* e, uint64_t offload_mask, SleepPlan& p) {
+    std::vector<size_t> by_addr(e->segs.size());
+    for (size_t i = 0; i < by_addr.size(); ++i) by_addr[i] = i;
+    std::sort(by_addr.begin(), by_addr.end(), [&](size_t a, size_t b) {
+        const Segment &x = e->segs[a], &y = e->segs[b];
+        return x.arena != y.arena ? x.arena < y.arena : x.va < y.va;
+    });
+    // the store that would hold the kept image: the host store, or the parking buffer of the same (peer / local) tier
+    p.kept_store = p.tier == FMA_TIER_HOST ? e->host.base != nullptr
+                                           : (e->park.va != 0 && (p.tier == FMA_TIER_LOCAL ? e->park.device == e->device : e->park.device != e->device));
+    p.shadows_match = e->incremental && p.tier == e->shadow_tier && !(p.flags & kFlagAdopt) && p.kept_store;
+    for (size_t i : by_addr) {
+        Segment& s = e->segs[i];
+        if (tag_bit_set(offload_mask, s.tag)) {
+            p.shadows_match = p.shadows_match && s.digest_valid && s.shadow_off == p.W;  // same bytes expected at the same image offset
+            p.shadow_digest.push_back(s.digest);
+            p.shadow_at.push_back(s.digest_valid ? s.shadow_off : kNoOffset);
+            p.ex.push_back(Extent{i, s.va, s.bytes, p.W});
+            p.W += s.bytes;
+        } else {
+            p.discarded += s.bytes;
+        }
+        s.has_backup = false;
+        s.packed_off = kNoOffset;
+        s.digest_valid = false;
+    }
+    p.W_all = p.W;
+}
+
+// 2. RESIDENT share (option "resident_bytes"): the tail of the image stays in one VMM allocation on this GPU.  Walking the
+// offloaded segments from the last to the first, a segment stays if its stored size (2 MiB pages, or its pages' PACKED sizes)
+// still fits what is left of the cap; the host store then holds only the other segments, back to back in image order.
+int split_resident(fma_engine_t* e, SleepPlan& p) {
+    if (!e->resident_cap || p.tier != FMA_TIER_HOST || !e->paths.empty() || (p.flags & kFlagAdopt) || !p.W) return FMA_OK;
+    if (fma_layout::sleep_route(sleep_facts(e, p)).wants_probe) {  // asked before the ring is known
+        RC(plan_packed_image(e, p.ex, p.W, &p.pk_off, &p.pk_bytes, &p.Wp, &p.packed));
+        p.pre_planned = true;
+    }
+    std::vector<uint64_t> stored(p.ex.size());
+    for (size_t k = 0; k < p.ex.size(); ++k) {
+        stored[k] = p.packed ? 0 : p.ex[k].bytes;
+        if (p.packed)
+            for (uint64_t o = 0; o < p.ex[k].bytes; o += FMA_PAGE_BYTES) stored[k] += p.pk_bytes[(p.ex[k].packed_off + o) / FMA_PAGE_BYTES];
+    }
+    const std::vector<char> res = fma_layout::resident_split(stored, e->resident_cap);
+    uint64_t res_stored = 0;
+    for (size_t k = 0; k < p.ex.size(); ++k) res_stored += res[k] ? stored[k] : 0;
+    if (!res_stored) return FMA_OK;
+    ParkStore buf;
+    const double a = now_s();
+    int arc;
+    {
+        GateHold hold(kGateUnmap, 0.1);   // an allocation of a sleep: as patient as the sleep's unmaps
+        arc = park_store_create(e, e->device, res_stored, &buf);
+    }
+    const double b = now_s();
+    if (arc != FMA_OK) {  // HBM too full: a plain host-tier sleep of everything
+        e->tl_add("res_fallback", 0, a, b, res_stored);
+        cudaGetLastError();
+        return FMA_OK;
+    }
+    e->tl_add("res_alloc", 0, a, b, buf.cap);
+    // the two parts, each laid out back to back in image order: [0] the host store, [1] the resident buffer
+    struct Part {
+        std::vector<Extent> ex;
+        std::vector<uint64_t> off;     // PACKED: stored offset and size of each image page
+        std::vector<uint32_t> bytes;
+        uint64_t W = 0, stored = 0;
+    } part[2];
+    std::vector<uint64_t> h_digest;
+    bool host_shadows = true;
+    for (size_t k = 0; k < p.ex.size(); ++k) {
+        Part& d = part[(int)res[k]];
+        Extent x = p.ex[k];
+        const uint64_t p0 = x.packed_off / FMA_PAGE_BYTES;
+        x.packed_off = d.W;
+        d.W += x.bytes;
+        d.ex.push_back(x);
+        if (res[k]) {
+            p.res_seqs.push_back(e->segs[x.seg_index].seq);
+        } else {
+            host_shadows = host_shadows && p.shadow_at[k] == x.packed_off;
+            h_digest.push_back(p.shadow_digest[k]);
+        }
+        if (p.packed)
+            for (uint64_t q = p0; q < p0 + x.bytes / FMA_PAGE_BYTES; ++q) {
+                d.off.push_back(d.stored);
+                d.bytes.push_back(p.pk_bytes[q]);
+                d.stored += p.pk_bytes[q];
+            }
+    }
+    e->res = buf;
+    e->res_packed = p.packed;
+    e->res_off = std::move(part[1].off);
+    e->res_bytes = std::move(part[1].bytes);
+    e->res_store_bytes = res_stored;
+    p.ex = std::move(part[0].ex);
+    p.ex_res = std::move(part[1].ex);
+    p.W = part[0].W;
+    p.shadows_match = e->incremental && p.tier == e->shadow_tier && p.kept_store && host_shadows;
+    p.shadow_digest = std::move(h_digest);
+    p.Wp = p.packed ? part[0].stored : part[0].W;
+    if (p.packed) {
+        p.pk_off = std::move(part[0].off);
+        p.pk_bytes = std::move(part[0].bytes);
+    }
+    return FMA_OK;
+}
+
+// 3. INCREMENTAL sleep: does the store still hold exactly this image?  One K3 pass over the device copy decides.
+int check_incremental(fma_engine_t* e, SleepPlan& p) {
+    p.shadows_match = p.shadows_match && p.res_seqs == e->res_seqs;  // a different split is a full sleep
+    e->res_seqs = p.res_seqs;
+    const uint64_t W = p.W;
+    if (!p.shadows_match || !W || W != e->shadow_image_bytes || (p.tier == FMA_TIER_HOST ? e->host.cap : e->park.cap) < e->shadow_store_bytes) return FMA_OK;
+    RT(cudaDeviceSynchronize());  // the caller's streams may still be writing weights
+    std::vector<uint64_t> now;
+    RC(digest_and_mark(e, p.ex, &now));  // either way these are the digests of what sleeps now
+    uint64_t dirty_bytes = 0;
+    for (size_t k = 0; k < p.ex.size(); ++k)
+        if (now[k] != p.shadow_digest[k]) {
+            p.dirty.push_back(p.ex[k]);
+            dirty_bytes += p.ex[k].bytes;
+        }
+    p.digests_known = true;
+    p.clean = p.dirty.empty();
+    // a few changed segments (an adapter, fp8 KV scales reset after wake, one synced layer): only they cross the link, into
+    // their old place in the kept image (partial sleeps are a host-tier refinement; in a parking tier a changed image is
+    // simply parked again)
+    const bool few = p.tier == FMA_TIER_HOST && !p.clean && 2 * dirty_bytes <= W && !e->host.shared;  // a shared image is read-only
+    p.partial = few && !e->shadow_packed;
+    // PACKED image: a changed page can go back to its old place only if its stored size stays what it was (K4p on those pages)
+    if (few && e->shadow_packed && fma_layout::sleep_route(sleep_facts(e, p)).wants_probe) {
+        for (const Extent& x : p.dirty)
+            for (size_t o = 0; o < x.bytes; o += FMA_PAGE_BYTES) p.dirty_pages.push_back((size_t)((x.packed_off + o) / FMA_PAGE_BYTES));
+        RC(pack_probe(e, p.dirty, p.dirty_pages.size(), std::max<size_t>(p.dirty_pages.size(), W / FMA_PAGE_BYTES)));
+        bool fits = p.dirty_pages.size() <= e->img_bytes.size();
+        for (size_t q = 0; q < p.dirty_pages.size() && fits; ++q)
+            fits = p.dirty_pages[q] < e->img_bytes.size() && e->h_psize[q] == e->img_bytes[p.dirty_pages[q]];
+        p.partial_packed = fits && !no_ring() && ensure_ring(e, W) == FMA_OK;  // no HBM for a ring: full sleep through the plain path
+    }
+    return FMA_OK;
+}
+
+// 4. the pipeline (fma_layout::sleep_route), with the staging ring and the PACKED plan it needs, BEFORE the store is sized
+int route_sleep(fma_engine_t* e, SleepPlan& p) {
+    if (!p.clean && !p.partial && !p.partial_packed) invalidate_shadows(e);  // this sleep rewrites the store (or leaves the host tier alone: be conservative)
+    fma_layout::SleepFacts f = sleep_facts(e, p);
+    if (fma_layout::sleep_route(f).wants_ring) f.ring = !no_ring() && ensure_ring(e, p.W) == FMA_OK;
+    p.route = fma_layout::sleep_route(f);
+    const bool kept = p.clean || p.partial_packed;  // the image in the store, its form and its page table stay as they are
+    if (kept) {
+        p.packed = e->shadow_packed;
+        p.Wp = e->shadow_store_bytes;
+    } else if (p.route.wants_probe) {
+        if (!p.pre_planned) RC(plan_packed_image(e, p.ex, p.W, &p.pk_off, &p.pk_bytes, &p.Wp, &p.packed));
+        f.worth_packing = p.packed;
+        p.route = fma_layout::sleep_route(f);
+    } else {  // (a plan of the resident split is dropped)
+        p.packed = false;
+        p.Wp = p.W;
+    }
+    e->image_packed = p.packed;
+    e->image_store_bytes = p.Wp;
+    if (!kept) {
+        e->img_off = p.packed ? std::move(p.pk_off) : std::vector<uint64_t>();
+        e->img_bytes = p.packed ? std::move(p.pk_bytes) : std::vector<uint32_t>();
+    }
+    if (kept || p.packed) e->image_bytes = p.W;  // the layout is indexed by image page: valid from here on, also if the sleep fails
+    return FMA_OK;
+}
+
+// 5. a store of the tier that holds Wp bytes
+int size_store(fma_engine_t* e, const SleepPlan& p) {
+    if (!p.W) return FMA_OK;
+    if (p.tier == FMA_TIER_HOST && p.adopt()) {
+        if (!e->host.base) return fail(FMA_ESTATE, "adopt without a store");  // the adopted store IS the image: never re-sized
+    } else if (p.tier == FMA_TIER_HOST) {
+        if (e->host.shared) {  // this sleep writes: leave the shared image to its other holders and take a private store
+            invalidate_shadows(e);
+            host_store_free(e->host);
+        }
+        RC(host_store_reserve(e, p.Wp));
+        if (p.route.mode == FMA_MODE_KERNEL && !e->host.dev_alias) return fail(FMA_ECUDA, "host store has no device alias for zero-copy mode");
+    } else if (p.tier == FMA_TIER_PEER) {
+        if (!e->park.va || e->park.cap < p.Wp || e->park.device == e->device)
+            return fail(FMA_ESTATE, "peer tier needs fma_peer_reserve(peer_device, >= %llu bytes) first", (unsigned long long)p.Wp);
+    } else if (p.tier == FMA_TIER_LOCAL) {
+        return park_reserve(e, e->device, p.Wp);
+    } else {
+        return fail(FMA_EINVAL, "unknown tier %d", p.tier);
+    }
+    return FMA_OK;
+}
+
+// 6. RESIDENT share: K1 / K4 gather the resident segments into e->res (HBM only, a few ms), ahead of the host part's pipeline on
+// the kernel stream.  Synchronised before the host part starts: it rewrites the page tables, and the units that hold only
+// resident segments are unmapped right away after it.
+int gather_resident(fma_engine_t* e, SleepPlan& p) {
+    if (p.ex_res.empty()) return FMA_OK;
+    if ((p.flags & FMA_FLAG_VERIFY) || e->incremental) RC(digest_and_mark(e, p.ex_res));
+    RC(p.timer.begin());
+    uint32_t res_launches = 0;
+    SleepPipe rp{e, p.ex_res, p.W_all - p.W, FMA_TIER_LOCAL, nullptr, p.kt, res_launches, nullptr};  // units go with the host part
+    rp.resident = true;
+    p.kt.kind = "res_gather";
+    const int rc = e->res_packed ? rp.kernel_packed() : rp.kernel();
+    p.kt.kind = "kernel";
+    if (rc != FMA_OK) return rc;
+    if (e->res_packed) RC(check_pack_errors(e, kPackChanged));
+    else RT(cudaStreamSynchronize(e->ks));
+    std::lock_guard<std::mutex> lk(e->mu);
+    for (const Extent& x : p.ex_res) mark_backed_up(e, x, FMA_TIER_LOCAL);
+    return FMA_OK;
+}
+
+// 7. the copy pipeline of the route, with the unmapper releasing units behind it
+int run_pipeline(fma_engine_t* e, SleepPlan& p, Unmapper& un) {
+    using fma_layout::SleepPipeKind;
+    if (p.W && p.adopt()) {
+        un.publish_consumed(p.W, e->ks);  // nothing to copy: every offloaded unit can go at once
+        zero_kernel_stats(e);
+        if (!e->ring_attached && env_int("FMA_RING_PERSIST", 0) == 0) release_ring(e);  // a sleeping model holds no staging ring
+    } else if (p.W) {
+        char* store = static_cast<char*>(store_copy_base(e, p.tier));
+        if (p.ex_res.empty()) RC(p.timer.begin());  // (else the resident gather opened the device-time bracket)
+        SleepPipe pipe{e, p.partial ? p.dirty : p.ex, p.W, p.tier, store, p.kt, p.copy_ops, &un};
+        switch (p.route.pipe) {
+        case SleepPipeKind::PartialPacked:  // only the changed segments' pages are re-coded, each into its old place
+            pipe.subset = &p.dirty_pages;
+            RC(pipe.staged_packed());
+            break;
+        case SleepPipeKind::PartialDirect:  // only the changed segments move; everything below each of them is in the store already
+            RC(pipe.direct());
+            RC(un.publish_consumed(p.W, e->cs[0]));  // cs[0] has joined the other streams after the last extent
+            break;
+        case SleepPipeKind::Direct: RC(pipe.direct()); break;
+        case SleepPipeKind::Kernel: RC(pipe.kernel()); break;
+        case SleepPipeKind::KernelPacked: RC(pipe.kernel_packed()); break;
+        case SleepPipeKind::Multipath: RC(pipe.multipath()); break;
+        case SleepPipeKind::StagedPacked: RC(pipe.staged_packed()); break;
+        case SleepPipeKind::Staged: RC(pipe.staged()); break;
+        case SleepPipeKind::Adopt: return fail(FMA_ESTATE, "an adopted image has no copy pipeline");  // (handled above)
+        }
+        un.close();
+        RC(p.timer.end(&p.copy_s));
+        RC(p.kt.collect());
+        if (p.packed) RC(check_pack_errors(e, kPackChanged));  // K4 counts pages that no longer fit the form the probe chose (weights written during the sleep)
+        if (env_int("FMA_RING_PERSIST", 0) == 0 || e->ring_attached) release_ring(e);  // while the unmapper finishes its last ranges
+    }
+    if (!p.ex_res.empty() && (!p.W || p.adopt())) {  // only the resident gather ran: close its bracket
+        RC(p.timer.end(&p.copy_s));
+        RC(p.kt.collect());
+    }
+    return FMA_OK;
+}
+
+// 8. apply what the unmapper did to the table, then unmap whatever is left (FMA_OVERLAP_UNMAP=0, nothing offloaded, ...) —
+// every unit goes (cumem.py:213), VAs stay reserved; then the stats
+int finish_sleep(fma_engine_t* e, const SleepPlan& p, Unmapper& un, ApplyUnmapped& apply_unmapped, double t_entry) {
+    un.finish();
+    if (un.error != FMA_OK) return fail(un.error, "%s", un.msg);
+    for (const Extent& x : p.ex) mark_backed_up(e, x, p.tier);
+    apply_unmapped.run();
+    {
+        std::lock_guard<std::mutex> lk(e->mu);
+        std::vector<Range> rest;
+        for (auto& kv : e->units) Unmapper::add_range(rest, kv.second.va, kv.second.bytes);
+        const double a0 = now_s();
+        for (const Range& r : rest) RC(unmap_units(e, r.va, r.bytes));
+        un.seconds += now_s() - a0;
+        for (Segment& s : e->segs) {
+            s.mapped = false;
+            s.unit_va = 0;
+        }
+    }
+    e->image_bytes = p.W;
+    e->image_tier = p.tier;
+
+    e->tl_add("total", 0, t_entry, now_s(), p.W_all);
+    e->st.sleep_seconds = now_s() - t_entry;
+    e->st.sleep_copy_seconds = p.copy_s;
+    e->st.sleep_unmap_seconds = un.seconds;
+    e->st.sleep_bytes_offloaded = p.W_all;
+    uint64_t copied = 0;  // what this sleep moved into the store
+    if (p.partial) for (const Extent& x : p.dirty) copied += x.bytes;
+    else if (p.partial_packed) for (size_t q : p.dirty_pages) copied += e->img_bytes[q];
+    else if (!p.adopt()) copied = p.Wp;
+    e->st.sleep_bytes_copied = copied;
+    e->st.sleep_bytes_discarded = p.discarded;
+    e->st.copy_ops = p.copy_ops;
+    e->st.total_copy_ops += p.copy_ops;
+    e->st.tier = p.tier;
+    e->st.mode = p.route.mode;
+    if (!p.W && p.ex_res.empty()) zero_kernel_stats(e);
+    return FMA_OK;
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------------------------
@@ -500,18 +847,15 @@ int SleepPipe::multipath() {
 // ------------------------------------------------------------------------------------
 int do_sleep(fma_engine_t* e, uint64_t offload_mask, int tier, uint32_t flags) {
     DeviceGuard guard(e->device);
-    int rc = flush_kernel_times(e);
-    if (rc != FMA_OK) return rc;
+    RC(flush_kernel_times(e));
     const double t_entry = now_s();
-    rc = ensure_streams(e);
-    if (rc != FMA_OK) return rc;
+    RC(ensure_streams(e));
 
     // Executor.sleep is a no-op while sleeping (abstract.py:323-325)
     bool any_unmapped = false, any_mapped = false;
     for (const Segment& s : e->segs) (s.mapped ? any_mapped : any_unmapped) = true;
     if (any_unmapped || !any_mapped) return FMA_OK;
-    rc = check_tma_shape(e, tier);
-    if (rc != FMA_OK) return rc;
+    RC(check_tma_shape(e, tier));
     e->tl_begin("sleep", t_entry);
     if (e->res.va) {  // a resident buffer kept by an FMA_FLAG_KEEP_BACKUP wake: this sleep gathers its resident part afresh
         RT(cudaDeviceSynchronize());
@@ -519,408 +863,28 @@ int do_sleep(fma_engine_t* e, uint64_t offload_mask, int tier, uint32_t flags) {
         resident_release(e);
     }
 
-    // plan: offloaded segments -> packed image, in (arena, VA) order.  Arenas are bump-allocated per tag, so this is
-    // allocation order (the reference's dict order, cumem.py:198) unless a freed hole was reused.
-    std::vector<size_t> by_addr(e->segs.size());
-    for (size_t i = 0; i < by_addr.size(); ++i) by_addr[i] = i;
-    std::sort(by_addr.begin(), by_addr.end(), [&](size_t a, size_t b) {
-        const Segment &x = e->segs[a], &y = e->segs[b];
-        return x.arena != y.arena ? x.arena < y.arena : x.va < y.va;
-    });
-    std::vector<Extent> ex;
-    uint64_t W = 0, discarded = 0;
-    // the store that would hold the kept image: the host store, or the parking buffer of the same (peer / local) tier
-    const bool kept_store = tier == FMA_TIER_HOST ? e->host.base != nullptr
-                                                  : (e->park.va != 0 && (tier == FMA_TIER_LOCAL ? e->park.device == e->device : e->park.device != e->device));
-    bool shadows_match = e->incremental && tier == e->shadow_tier && !(flags & kFlagAdopt) && kept_store;
-    std::vector<uint64_t> shadow_digest;  // digest of the copy the store holds, per extent
-    std::vector<uint64_t> shadow_at;      // where the store holds it (kNoOffset: no usable copy)
-    for (size_t i : by_addr) {
-        Segment& s = e->segs[i];
-        if (tag_bit_set(offload_mask, s.tag)) {
-            shadows_match = shadows_match && s.digest_valid && s.shadow_off == W;  // same bytes expected at the same image offset
-            shadow_digest.push_back(s.digest);
-            shadow_at.push_back(s.digest_valid ? s.shadow_off : kNoOffset);
-            ex.push_back(Extent{i, s.va, s.bytes, W});
-            W += s.bytes;
-        } else {
-            discarded += s.bytes;
-        }
-        s.has_backup = false;
-        s.packed_off = kNoOffset;
-        s.digest_valid = false;
-    }
-    // RESIDENT share (option "resident_bytes"): the tail of the image stays in one VMM allocation on this GPU.  Walking the
-    // offloaded segments from the last to the first, a segment stays if its stored size (2 MiB pages, or its pages' PACKED sizes)
-    // still fits what is left of the cap; the host store then holds only the other segments, back to back in image order.
-    std::vector<Extent> ex_res;       // resident extents, packed_off = offset in the resident part
-    uint64_t W_all = W;
-    std::vector<uint64_t> res_seqs;
-    bool pre_planned = false, pre_packed = false;  // the PACKED plan of the host part, made here already (K4p over the whole image)
-    std::vector<uint64_t> pre_off;
-    std::vector<uint32_t> pre_bytes;
-    uint64_t pre_total = 0;
-    if (e->resident_cap && tier == FMA_TIER_HOST && e->paths.empty() && !(flags & kFlagAdopt) && W) {
-        if (e->cfg.pack && resolve_mode(e, tier) == FMA_MODE_STAGED) {
-            rc = plan_packed_image(e, ex, W, &pre_off, &pre_bytes, &pre_total, &pre_packed);
-            if (rc != FMA_OK) return rc;
-            pre_planned = true;
-        }
-        std::vector<uint64_t> stored(ex.size());
-        for (size_t k = 0; k < ex.size(); ++k) {
-            stored[k] = pre_packed ? 0 : ex[k].bytes;
-            if (pre_packed)
-                for (uint64_t o = 0; o < ex[k].bytes; o += FMA_PAGE_BYTES) stored[k] += pre_bytes[(ex[k].packed_off + o) / FMA_PAGE_BYTES];
-        }
-        const std::vector<char> res = fma_layout::resident_split(stored, e->resident_cap);
-        uint64_t res_stored = 0;
-        for (size_t k = 0; k < ex.size(); ++k) res_stored += res[k] ? stored[k] : 0;
-        if (res_stored) {
-            ParkStore buf;
-            const double a = now_s();
-            int arc;
-            {
-                GateHold hold(kGateUnmap, 0.1);   // an allocation of a sleep: as patient as the sleep's unmaps
-                arc = park_store_create(e, e->device, res_stored, &buf);
-            }
-            const double b = now_s();
-            if (arc != FMA_OK) {  // HBM too full: a plain host-tier sleep of everything
-                e->tl_add("res_fallback", 0, a, b, res_stored);
-                cudaGetLastError();
-            } else {
-                e->tl_add("res_alloc", 0, a, b, buf.cap);
-                std::vector<Extent> ex_host;
-                std::vector<uint64_t> h_off, r_off, h_digest;
-                std::vector<uint32_t> h_bytes, r_bytes;
-                uint64_t Wh = 0, Wr = 0, hs = 0, rs = 0;
-                bool host_shadows = true;
-                for (size_t k = 0; k < ex.size(); ++k) {
-                    Extent x = ex[k];
-                    const uint64_t p0 = x.packed_off / FMA_PAGE_BYTES;
-                    if (res[k]) {
-                        x.packed_off = Wr;
-                        Wr += x.bytes;
-                        ex_res.push_back(x);
-                        res_seqs.push_back(e->segs[x.seg_index].seq);
-                    } else {
-                        x.packed_off = Wh;
-                        Wh += x.bytes;
-                        ex_host.push_back(x);
-                        host_shadows = host_shadows && shadow_at[k] == x.packed_off;
-                        h_digest.push_back(shadow_digest[k]);
-                    }
-                    if (pre_packed)
-                        for (uint64_t p = p0; p < p0 + x.bytes / FMA_PAGE_BYTES; ++p) {
-                            (res[k] ? r_off : h_off).push_back(res[k] ? rs : hs);
-                            (res[k] ? r_bytes : h_bytes).push_back(pre_bytes[p]);
-                            (res[k] ? rs : hs) += pre_bytes[p];
-                        }
-                }
-                e->res = buf;
-                e->res_packed = pre_packed;
-                e->res_off = std::move(r_off);
-                e->res_bytes = std::move(r_bytes);
-                e->res_store_bytes = res_stored;
-                ex = std::move(ex_host);
-                W = Wh;
-                shadows_match = e->incremental && tier == e->shadow_tier && kept_store && host_shadows;
-                shadow_digest = std::move(h_digest);
-                if (pre_packed) {
-                    pre_off = std::move(h_off);
-                    pre_bytes = std::move(h_bytes);
-                    pre_total = hs;
-                } else {
-                    pre_total = Wh;
-                }
-            }
-        }
-    }
-    shadows_match = shadows_match && res_seqs == e->res_seqs;  // INCREMENTAL: a different split is a full sleep
-    e->res_seqs = res_seqs;
-    // INCREMENTAL sleep: does the host store still hold exactly this image?  One K3 pass over the device copy decides.
-    bool clean = false, partial = false, partial_packed = false, digests_known = false;
-    std::vector<Extent> dirty;        // segments whose device bytes differ from the copy in the store
-    std::vector<size_t> dirty_pages;  // their image pages (PACKED image)
-    if (shadows_match && W && W == e->shadow_image_bytes && (tier == FMA_TIER_HOST ? e->host.cap : e->park.cap) >= e->shadow_store_bytes) {
-        RT(cudaDeviceSynchronize());  // the caller's streams may still be writing weights
-        std::vector<uint64_t> now;
-        rc = digest_and_mark(e, ex, &now);  // either way these are the digests of what sleeps now
-        if (rc != FMA_OK) return rc;
-        uint64_t dirty_bytes = 0;
-        for (size_t k = 0; k < ex.size(); ++k)
-            if (now[k] != shadow_digest[k]) {
-                dirty.push_back(ex[k]);
-                dirty_bytes += ex[k].bytes;
-            }
-        digests_known = true;
-        clean = dirty.empty();
-        // a few changed segments (an adapter, fp8 KV scales reset after wake, one synced layer): only they cross the link, into
-        // their old place in the kept image (partial sleeps are a host-tier refinement; in a parking tier a changed image is
-        // simply parked again)
-        partial = tier == FMA_TIER_HOST && !clean && !e->shadow_packed && 2 * dirty_bytes <= W && !e->host.shared;  // a shared image is read-only
-        // PACKED image: a changed page can go back to its old place only if its stored size stays what it was (K4p on those pages)
-        if (tier == FMA_TIER_HOST && !clean && e->shadow_packed && e->cfg.pack && 2 * dirty_bytes <= W && !e->host.shared && resolve_mode(e, tier) == FMA_MODE_STAGED) {
-            for (const Extent& x : dirty)
-                for (size_t o = 0; o < x.bytes; o += FMA_PAGE_BYTES) dirty_pages.push_back((size_t)((x.packed_off + o) / FMA_PAGE_BYTES));
-            rc = pack_probe(e, dirty, dirty_pages.size(), std::max<size_t>(dirty_pages.size(), W / FMA_PAGE_BYTES));
-            if (rc != FMA_OK) return rc;
-            partial_packed = dirty_pages.size() <= e->img_bytes.size();
-            for (size_t q = 0; q < dirty_pages.size() && partial_packed; ++q)
-                partial_packed = dirty_pages[q] < e->img_bytes.size() && e->h_psize[q] == e->img_bytes[dirty_pages[q]];
-            if (partial_packed && (no_ring() || ensure_ring(e, W) != FMA_OK)) partial_packed = false;  // no HBM for a ring: full sleep through the plain path
-        }
-    }
-    if (clean) flags |= kFlagAdopt;                  // release the device side only: not a byte moves
-    else if (!partial && !partial_packed) invalidate_shadows(e);  // this sleep rewrites the store (or leaves the host tier alone: be conservative)
-    int mode = partial ? FMA_MODE_DIRECT : resolve_mode(e, tier);
-    // MULTI-PATH (fma_paths_set): a full, plain host-tier sleep is striped over the paths' links; every path has its own staging slots
-    const bool multipath = !e->paths.empty() && !e->mbox && tier == FMA_TIER_HOST && mode == FMA_MODE_STAGED && !partial && !partial_packed && !clean &&
-                           !(flags & kFlagAdopt) && !e->cfg.pack && env_int("FMA_MULTIPATH_SLEEP", 1) != 0;
-    if (W && !(flags & kFlagAdopt) && mode == FMA_MODE_STAGED && !multipath && (no_ring() || ensure_ring(e, W) != FMA_OK)) mode = FMA_MODE_DIRECT;  // HBM too full for a ring
-    // PACKED image (config.pack): decide per page what its stored form is BEFORE the store is sized
-    bool packed = false;
-    uint64_t Wp = W;
-    if (clean || partial_packed) {  // the image in the store, its form and its page table stay as they are
-        packed = e->shadow_packed;
-        Wp = e->shadow_store_bytes;
-        e->image_packed = packed;
-        e->image_store_bytes = Wp;
-        e->image_bytes = W;
-    } else {
-        std::vector<uint64_t> pk_off;
-        std::vector<uint32_t> pk_bytes;
-        // host tier: through the staging ring (STAGED); parking tiers (peer / local HBM): K4 writes the store itself (KERNEL)
-        const bool pack_path = (tier == FMA_TIER_HOST && mode == FMA_MODE_STAGED) || (tier != FMA_TIER_HOST && mode == FMA_MODE_KERNEL);
-        if (W && e->cfg.pack && !(flags & kFlagAdopt) && pack_path) {
-            if (pre_planned) {
-                pk_off = std::move(pre_off);
-                pk_bytes = std::move(pre_bytes);
-                Wp = pre_total;
-                packed = pre_packed;
-            } else {
-                rc = plan_packed_image(e, ex, W, &pk_off, &pk_bytes, &Wp, &packed);
-                if (rc != FMA_OK) return rc;
-            }
-        }
-        e->image_packed = packed;
-        e->image_store_bytes = Wp;
-        e->img_off = packed ? std::move(pk_off) : std::vector<uint64_t>();
-        e->img_bytes = packed ? std::move(pk_bytes) : std::vector<uint32_t>();
-        if (packed) e->image_bytes = W;  // the layout above is indexed by image page: valid from here on, also if the sleep fails
-    }
-    if (W) {
-        if (tier == FMA_TIER_HOST && (flags & kFlagAdopt)) {
-            if (!e->host.base) return fail(FMA_ESTATE, "adopt without a store");  // the adopted store IS the image: never re-sized
-        } else if (tier == FMA_TIER_HOST) {
-            if (e->host.shared) {  // this sleep writes: leave the shared image to its other holders and take a private store
-                invalidate_shadows(e);
-                host_store_free(e->host);
-            }
-            rc = host_store_reserve(e, Wp);
-            if (rc != FMA_OK) return rc;
-            if (mode == FMA_MODE_KERNEL && !e->host.dev_alias) return fail(FMA_ECUDA, "host store has no device alias for zero-copy mode");
-        } else if (tier == FMA_TIER_PEER) {
-            if (!e->park.va || e->park.cap < Wp || e->park.device == e->device)
-                return fail(FMA_ESTATE, "peer tier needs fma_peer_reserve(peer_device, >= %llu bytes) first", (unsigned long long)Wp);
-        } else if (tier == FMA_TIER_LOCAL) {
-            rc = park_reserve(e, e->device, Wp);
-            if (rc != FMA_OK) return rc;
-        } else {
-            return fail(FMA_EINVAL, "unknown tier %d", tier);
-        }
-    }
+    SleepPlan p(e, tier, flags);
+    plan_image(e, offload_mask, p);
+    RC(split_resident(e, p));
+    RC(check_incremental(e, p));
+    RC(route_sleep(e, p));
+    RC(size_store(e, p));
 
     // The caller's own streams may still be writing weights: drain the device once, as the
     // reference's blocking cudaMemcpy on the legacy stream implicitly does (before anything reads the segments).
     RT(cudaDeviceSynchronize());
-
-    const bool adopt = (flags & kFlagAdopt) != 0;  // the store already holds the image: release the device side only
-    if (((flags & FMA_FLAG_VERIFY) || e->incremental) && W && !adopt && !digests_known) {  // incremental: digests seed the next sleep's check
-        rc = digest_and_mark(e, ex);
-        if (rc != FMA_OK) return rc;
+    if (((flags & FMA_FLAG_VERIFY) || e->incremental) && p.W && !p.adopt() && !p.digests_known) {  // incremental: digests seed the next sleep's check
+        RC(digest_and_mark(e, p.ex));
     }
-
-    // ---- RESIDENT share: K1 / K4 gather the resident segments into e->res (HBM only, a few ms), ahead of the host part's
-    // pipeline on the kernel stream.  Synchronised before the host part starts: it rewrites the page tables, and the units
-    // that hold only resident segments are unmapped right away below.
-    CopyTimer timer{e};
-    KernelTimes kt{e};
-    uint32_t copy_ops = 0;
-    double copy_s = 0;
-    if (!ex_res.empty()) {
-        if ((flags & FMA_FLAG_VERIFY) || e->incremental) {
-            rc = digest_and_mark(e, ex_res);
-            if (rc != FMA_OK) return rc;
-        }
-        rc = timer.begin();
-        if (rc != FMA_OK) return rc;
-        uint32_t res_launches = 0;
-        SleepPipe rp{e, ex_res, W_all - W, FMA_TIER_LOCAL, nullptr, kt, res_launches, [](uint64_t, cudaStream_t) { return FMA_OK; }};
-        rp.resident = true;
-        kt.kind = "res_gather";
-        rc = e->res_packed ? rp.kernel_packed() : rp.kernel();
-        kt.kind = "kernel";
-        if (rc != FMA_OK) return rc;
-        if (e->res_packed) rc = check_pack_errors(e, kPackChanged);
-        else RT(cudaStreamSynchronize(e->ks));
-        if (rc != FMA_OK) return rc;
-        std::lock_guard<std::mutex> lk(e->mu);
-        for (const Extent& x : ex_res) {
-            Segment& sg = e->segs[x.seg_index];
-            sg.has_backup = true;
-            sg.backup_tier = FMA_TIER_LOCAL;
-            sg.packed_off = x.packed_off;
-        }
-    }
+    RC(gather_resident(e, p));
 
     // ---- unmapper thread (types above): cuMemUnmap runs UNDER the copy pipeline instead of after it ----
-    Unmapper un;
-    un.e = e;
-    ApplyUnmapped apply_unmapped{&un, e, &ex, tier};
-
-    std::vector<PlannedUnit> off_units;  // same order as the image
-    auto add_range = [](std::vector<Range>& v, CUdeviceptr va, size_t bytes) {
-        if (!v.empty() && v.back().va + v.back().bytes == va) v.back().bytes += bytes;  // VA-adjacent: one driver call
-        else v.push_back(Range{va, bytes});
-    };
-    {
-        std::map<CUdeviceptr, uint64_t> unit_end;  // unit -> image_end (offloaded units only)
-        for (const Extent& x : ex) {
-            const CUdeviceptr key = e->segs[x.seg_index].unit_va;
-            uint64_t& end = unit_end[key];
-            end = std::max<uint64_t>(end, x.packed_off + x.bytes);
-        }
-        // arenas in index order, units by VA inside: identical to the image order
-        std::vector<const Unit*> ordered;
-        for (auto& kv : e->units) ordered.push_back(&kv.second);
-        std::sort(ordered.begin(), ordered.end(), [](const Unit* a, const Unit* b) { return a->arena != b->arena ? a->arena < b->arena : a->va < b->va; });
-        for (const Unit* u : ordered) {
-            auto it = unit_end.find(u->va);
-            if (e->ring_attached && u->va == e->ring_unit_va && mode == FMA_MODE_STAGED) continue;  // holds the ring: unmapped after the last D2H
-            if (it == unit_end.end()) add_range(un.first, u->va, u->bytes);
-            else off_units.push_back(PlannedUnit{u->va, u->bytes, it->second});
-        }
-    }
-    size_t next_unit = 0;  // first offloaded unit not yet handed to the unmapper
-    size_t stage_events_used = 0;
-    auto stage_event = [&](cudaStream_t stream, cudaEvent_t* out) -> int {
-        if (stage_events_used == e->ev_stage.size()) {
-            cudaEvent_t ev;
-            RT(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-            e->ev_stage.push_back(ev);
-        }
-        *out = e->ev_stage[stage_events_used++];
-        RT(cudaEventRecord(*out, stream));
-        return FMA_OK;
-    };
-    // everything whose bytes are inside image[0, image_done) and has been read by work enqueued on `stream` so far
-    auto publish_consumed = [&](uint64_t image_done, cudaStream_t stream) -> int {
-        Stage st;
-        while (next_unit < off_units.size() && off_units[next_unit].image_end <= image_done) {
-            add_range(st.ranges, off_units[next_unit].va, off_units[next_unit].bytes);
-            ++next_unit;
-        }
-        if (st.ranges.empty()) return FMA_OK;
-        int r = stage_event(stream, &st.ev);
-        if (r != FMA_OK) return r;
-        un.publish(std::move(st));
-        return FMA_OK;
-    };
-    const bool overlap_unmap = env_int("FMA_OVERLAP_UNMAP", 1) != 0;
-    if (overlap_unmap) un.th = std::thread([&un] { un.run(); });
-
-    if (W && adopt) {
-        publish_consumed(W, e->ks);  // nothing to copy: every offloaded unit can go at once
-        zero_kernel_stats(e);
-        if (!e->ring_attached && env_int("FMA_RING_PERSIST", 0) == 0) release_ring(e);  // a sleeping model holds no staging ring
-    } else if (W) {
-        char* store = static_cast<char*>(store_copy_base(e, tier));
-        if (ex_res.empty()) {  // (else the resident gather opened the device-time bracket)
-            rc = timer.begin();
-            if (rc != FMA_OK) return rc;
-        }
-        SleepPipe pipe{e, partial ? dirty : ex, W, tier, store, kt, copy_ops, publish_consumed};
-        if (partial_packed) {  // only the changed segments' pages are re-coded, each into its old place
-            pipe.subset = &dirty_pages;
-            rc = pipe.staged_packed();
-        } else if (partial) {  // only the changed segments move; everything below each of them is in the store already
-            rc = pipe.direct();
-            if (rc == FMA_OK) rc = publish_consumed(W, e->cs[0]);  // cs[0] has joined the other streams after the last extent
-        } else if (mode == FMA_MODE_DIRECT) rc = pipe.direct();
-        else if (mode == FMA_MODE_KERNEL) rc = packed ? pipe.kernel_packed() : pipe.kernel();
-        else if (multipath && !packed) rc = pipe.multipath();
-        else rc = packed ? pipe.staged_packed() : pipe.staged();
-        if (rc != FMA_OK) return rc;
-        {
-            std::lock_guard<std::mutex> lk(un.mu);
-            un.closed = true;
-        }
-        un.cv.notify_all();
-        rc = timer.end(&copy_s);
-        if (rc != FMA_OK) return rc;
-        rc = kt.collect();
-        if (rc != FMA_OK) return rc;
-        if (packed) {  // K4 counts pages that no longer fit the form the probe chose (weights written during the sleep)
-            rc = check_pack_errors(e, kPackChanged);
-            if (rc != FMA_OK) return rc;
-        }
-        if (env_int("FMA_RING_PERSIST", 0) == 0 || e->ring_attached) release_ring(e);  // while the unmapper finishes its last ranges
-    }
-    if (!ex_res.empty() && (!W || adopt)) {  // only the resident gather ran: close its bracket
-        rc = timer.end(&copy_s);
-        if (rc != FMA_OK) return rc;
-        rc = kt.collect();
-        if (rc != FMA_OK) return rc;
-    }
-    un.finish();
-    if (un.error != FMA_OK) return fail(un.error, "%s", un.msg);
-
-    // apply what the unmapper did to the table, then unmap whatever is left (FMA_OVERLAP_UNMAP=0, nothing
-    // offloaded, ...) — every unit goes (cumem.py:213), VAs stay reserved
-    for (const Extent& x : ex) {
-        Segment& s = e->segs[x.seg_index];
-        s.has_backup = true;
-        s.backup_tier = tier;
-        s.packed_off = x.packed_off;
-    }
-    apply_unmapped.run();
-    {
-        std::lock_guard<std::mutex> lk(e->mu);
-        std::vector<Range> rest;
-        for (auto& kv : e->units) add_range(rest, kv.second.va, kv.second.bytes);
-        const double a0 = now_s();
-        for (const Range& r : rest) {
-            rc = unmap_units(e, r.va, r.bytes);
-            if (rc != FMA_OK) return rc;
-        }
-        un.seconds += now_s() - a0;
-        for (Segment& s : e->segs) {
-            s.mapped = false;
-            s.unit_va = 0;
-        }
-    }
-    e->image_bytes = W;
-    e->image_tier = tier;
-
-    e->tl_add("total", 0, t_entry, now_s(), W_all);
-    e->st.sleep_seconds = now_s() - t_entry;
-    e->st.sleep_copy_seconds = copy_s;
-    e->st.sleep_unmap_seconds = un.seconds;
-    e->st.sleep_bytes_offloaded = W_all;
-    {
-        uint64_t copied = 0;  // what this sleep moved into the store
-        if (partial) for (const Extent& x : dirty) copied += x.bytes;
-        else if (partial_packed) for (size_t p : dirty_pages) copied += e->img_bytes[p];
-        else if (!adopt) copied = Wp;
-        e->st.sleep_bytes_copied = copied;
-    }
-    e->st.sleep_bytes_discarded = discarded;
-    e->st.copy_ops = copy_ops;
-    e->st.total_copy_ops += copy_ops;
-    e->st.tier = tier;
-    e->st.mode = mode;
-    if (!W && ex_res.empty()) zero_kernel_stats(e);
-    return FMA_OK;
+    Unmapper un(e);
+    ApplyUnmapped apply_unmapped{&un, e, &p.ex, tier};
+    un.plan(p.ex, p.route.mode == FMA_MODE_STAGED);
+    if (env_int("FMA_OVERLAP_UNMAP", 1) != 0) un.th = std::thread([&un] { un.run(); });
+    RC(run_pipeline(e, p, un));
+    return finish_sleep(e, p, un, apply_unmapped, t_entry);
 }
 
 }  // namespace fma_impl

@@ -7,9 +7,190 @@ namespace fma_impl {
 
 namespace {
 
+using fma_layout::Run;
+
+// ---- mapper thread(s): one create + map + set-access per run, in `runs` order ----------------------
+// A wake that fails is rolled back (the destructor, unless committed): every run THIS call mapped is unmapped again (its segments still have their
+// backup), so the table is what it was at entry and the controller's retry (inference-server.go:477-480) redoes the whole wake.
+// Leaving the mapped prefix in place would make the retry skip it (`mapped` == already awake) and report success over
+// weights that were never copied back — vLLM's allocator raises in that situation (cumem.py:237-249).
+struct Mapper {
+    fma_engine_t* e;
+    const std::vector<Run>& runs;
+    bool ring_run;                 // the staging ring is work item 0
+    double t_entry;
+    size_t n_backup_runs = 0;
+    double expected_copy_s = 0, remap_delay_s = 0;   // of the host part; remap-only runs start no earlier than this after entry
+    bool remap_after_copy = false; // ... nor before copies_landed
+    int gate_first = 0;            // cross-process VMM gate: announced for the call that gates the first copy
+    std::mutex mu{};
+    std::condition_variable cv{};
+    std::atomic<size_t> done{0};   // number of work items fully mapped (prefix; written under mu)
+    int error = FMA_OK;
+    char msg[512] = "";
+    std::vector<char> item_done{};
+    std::atomic<size_t> next_item{0};
+    std::atomic<uint64_t> map_ns{0};
+    std::atomic<bool> copies_landed{false};
+    std::vector<std::thread> threads{};
+    bool committed = false;        // the wake has succeeded: nothing to roll back
+
+    void start(int tier, double copy_s) {
+        for (const Run& r : runs) n_backup_runs += r.has_backup;
+        expected_copy_s = copy_s;
+        // Remap-only runs wait a fifth of the expected copy time (host tier) or half of it (NVLink): far below the slack.
+        const int forced_delay_ms = env_int("FMA_REMAP_DELAY_MS", -1);
+        remap_delay_s = forced_delay_ms >= 0 ? forced_delay_ms * 1e-3 : expected_copy_s * (tier == FMA_TIER_HOST ? 0.2 : 0.5);
+        // FMA_REMAP_AFTER_COPY=1: remap-only runs (kv_cache) are mapped only after this rank's last copy has LANDED — a 32 GiB
+        // cuMemCreate/Map/SetAccess then never runs beside this rank's DMA (its cost, a few ms, is added to the wake instead of
+        // hidden under it).  A/B knob for the question "does a large VMM call slow a running H2D stream down?".
+        remap_after_copy = env_int("FMA_REMAP_AFTER_COPY", 0) != 0 && n_backup_runs > 0;
+        // Cross-process VMM gate (fma_gate.h): tell the other engines on this host that a call which gates a first copy is coming
+        gate_first = n_backup_runs ? gate_announce(kGateFirst) : 0;
+        item_done.assign(runs.size(), 0);
+        const int n_threads = std::max(1, std::min(e->cfg.map_threads > 0 ? e->cfg.map_threads : 1, 8));
+        for (int t = 0; t < n_threads; ++t) threads.emplace_back([this] { run(); });
+    }
+    void run() {
+        cudaSetDevice(e->device);
+        for (;;) {
+            const size_t k = next_item.fetch_add(1);
+            if (k >= runs.size()) break;
+            {
+                std::lock_guard<std::mutex> lk(mu);
+                if (error != FMA_OK) break;
+            }
+            const Run& run = runs[k];
+            if (!run.has_backup && n_backup_runs && remap_delay_s > 0) {
+                // Remap-only runs (kv_cache) have the whole copy time as slack, the weights run only the ring's worth
+                // (~19 ms).  Driver VMM calls of ALL processes on the host serialise, so a rank that maps its kv early
+                // delays another rank's weights mapping: give every rank's weights a head start.
+                const double wait = t_entry + remap_delay_s - now_s();
+                if (wait > 0) std::this_thread::sleep_for(std::chrono::duration<double>(wait));
+            }
+            if (!run.has_backup && remap_after_copy) {
+                while (!copies_landed.load(std::memory_order_acquire)) {
+                    {
+                        std::lock_guard<std::mutex> lk(mu);
+                        if (error != FMA_OK) break;
+                    }
+                    std::this_thread::sleep_for(std::chrono::microseconds(200));
+                }
+            }
+            const bool is_ring = ring_run && k == 0;
+            // gate class: whatever gates the first copy (ring, or the first backed-up item when there is no ring run) goes
+            // first on the whole host; the other backed-up items have one ring's worth of slack; remap-only runs have what is
+            // left of the copy time.
+            const bool first_item = run.has_backup && k == 0;
+            const int cls = first_item ? kGateFirst : run.has_backup ? std::min(kGateWeights + (int)k - (ring_run ? 1 : 0), kGateWeightsLast) : kGateRemap;
+            const double left = std::max(0.0, t_entry + expected_copy_s * 0.8 - now_s());
+            const double t_ask = now_s();
+            int r;
+            double t0;
+            {
+                GateHold hold(cls, cls >= kGateRemap ? left : std::min(left, 0.05));
+                if (first_item) retract_gate();
+                t0 = now_s();
+                r = vmm_create_and_map(e->device, run.va, run.bytes);
+            }
+            const double t1 = now_s();
+            map_ns.fetch_add((uint64_t)((t1 - t0) * 1e9));
+            if (t0 - t_ask > 1e-4) e->tl_add("gate_wait", (int)k, t_ask, t0, 0);
+            e->tl_add(is_ring ? "map_ring" : run.has_backup ? "map_backed" : "map_remap", (int)k, t0, t1, run.bytes);
+            std::lock_guard<std::mutex> lk(mu);
+            if (r != FMA_OK) {
+                error = r;
+                snprintf(msg, sizeof(msg), "%s", tl_err);
+                if (is_ring) {  // the ring never came to exist
+                    arena_give_back(e->arenas[run.arena], run.va - e->arenas[run.arena].base, run.bytes);
+                    release_ring(e);
+                }
+            } else {
+                Unit u;
+                u.va = run.va; u.bytes = run.bytes; u.arena = run.arena;
+                if (is_ring) u.zombies.emplace_back(run.va, run.bytes);  // ring VA returns to the arena when the unit is unmapped
+                for (size_t i : run.segs) {
+                    u.live_bytes += e->segs[i].bytes;
+                    e->segs[i].mapped = true;
+                    e->segs[i].unit_va = run.va;
+                }
+                // holes inside a run cannot exist (runs are VA-contiguous live segments), so bytes == live_bytes
+                e->units[run.va] = u;
+                item_done[k] = 1;
+                while (done < runs.size() && item_done[done]) ++done;
+            }
+            cv.notify_all();
+        }
+    }
+    int wait_mapped(size_t upto) {  // wait until items [0, upto) are mapped; the error code of a failed mapping (text in msg)
+        std::unique_lock<std::mutex> lk(mu);
+        cv.wait(lk, [&] { return done >= upto || error != FMA_OK; });
+        return error;
+    }
+    int wait(size_t upto) {  // the same, failing with the mapping's message
+        const int mrc = wait_mapped(upto);
+        return mrc == FMA_OK ? FMA_OK : fail(mrc, "%s", msg);
+    }
+    void retract_gate() {
+        if (gate_first) gate_retract(gate_first);
+        gate_first = 0;
+    }
+    void join() {
+        for (auto& t : threads)
+            if (t.joinable()) t.join();
+    }
+    ~Mapper() {  // the rollback of a failed wake
+        if (committed) return;
+        char keep[512];
+        snprintf(keep, sizeof(keep), "%s", tl_err);
+        {
+            std::lock_guard<std::mutex> lk(mu);
+            if (error == FMA_OK) error = FMA_ESTATE;   // the mapper threads stop
+        }
+        copies_landed.store(true, std::memory_order_release);
+        join();
+        retract_gate();
+        cudaDeviceSynchronize();
+        cudaGetLastError();
+        for (size_t k = 0; k < runs.size(); ++k) {
+            if (!item_done[k]) continue;
+            for (size_t i : runs[k].segs) {
+                e->segs[i].mapped = false;
+                e->segs[i].unit_va = 0;
+            }
+            unmap_units(e, runs[k].va, runs[k].bytes);  // the ring run gives its VA back to the arena through its zombie entry
+        }
+        e->pending_events = 0;
+        snprintf(tl_err, sizeof(tl_err), "%s", keep);
+    }
+};
+
+// RESIDENT share: K2 / K5 copy the resident segments from e->res into their pages, on the kernel stream in pieces of at most one
+// ring slot, each launched between two of the host part's launches once its destination is mapped (in the second half of the
+// host part's launches the pipeline waits for that mapping); the tables sit behind the host part's in the same buffers.
+struct ResidentRestore {
+    fma_engine_t* e;
+    Mapper& mapper;
+    KernelTimes& kt;
+    const std::vector<size_t>& with_res;
+    const std::vector<size_t>& seg_run;
+    uint64_t W_res;
+    size_t n_host_pages;
+    bool image_packed;             // WakePipe::packed clears the K5 error counter
+    std::vector<Batch> pieces{};
+    size_t next = 0;
+    int setup();
+    int launch_next();
+    // after (host part's pages launched so far, host part's pages): launch the next piece if due
+    int pump(size_t launched, size_t total) {
+        if (next >= pieces.size()) return FMA_OK;
+        if (2 * launched < total && mapper.done.load() < pieces[next].need) return FMA_OK;
+        return launch_next();
+    }
+};
+
 // What the copy pipelines of one wake share.  A pipeline enqueues the work that brings the backed-up segments'
-// bytes from the store into their (re-)mapped runs; wait_mapped(n) blocks until the mapper thread has mapped work
-// items [0, n) (or failed: the error code comes back, its text is in map_msg).
+// bytes from the store into their (re-)mapped runs; wait(n) blocks until the mapper has mapped work items [0, n).
 struct WakePipe {
     fma_engine_t* e;
     const std::vector<size_t>& with_backup;   // segment indices that have a backup, image order
@@ -23,16 +204,9 @@ struct WakePipe {
     uint32_t& copy_ops;
     double& first_copy_delay;
     double t_entry;
-    std::function<int(size_t)> wait_mapped;
-    std::function<size_t()> mapped_now;
-    const char* map_msg;
-    // called after each of the pipeline's K2 / K5 launches with (image pages launched so far, image pages): a RESIDENT share's
-    // restore launches one of its pieces there, so that a ring slot's hand-back waits for at most one such launch
-    std::function<int(size_t, size_t)> between = nullptr;
-    int wait(size_t upto) {
-        const int mrc = wait_mapped(upto);
-        return mrc == FMA_OK ? FMA_OK : fail(mrc, "%s", map_msg);
-    }
+    Mapper& mapper;
+    // pumped after each K2 / K5 launch: a RESIDENT share's restore launches a piece there (a slot's hand-back waits for one at most)
+    ResidentRestore* between = nullptr;
     void copied() {
         if (!copy_ops) first_copy_delay = now_s() - t_entry;
         ++copy_ops;
@@ -50,11 +224,57 @@ std::vector<fma_layout::SegPages> wake_segs(const fma_engine_t* e, const std::ve
     return v;
 }
 
-#define PIPE_CHECK(x)                 \
-    do {                              \
-        int _rc = (x);                \
-        if (_rc != FMA_OK) return _rc; \
-    } while (0)
+int ResidentRestore::setup() {
+    if (!e->res.va) return fail(FMA_ESTATE, "the resident part of the image is gone");
+    const size_t n_res = W_res / FMA_PAGE_BYTES, n_all = n_host_pages + n_res;
+    RC(ensure_tables(e, n_all));
+    if (e->res_packed) RC(ensure_pack_bufs(e, n_all));
+    if (!e->ev_res_done && cudaEventCreateWithFlags(&e->ev_res_done, cudaEventDisableTiming) != cudaSuccess)
+        return fail(FMA_ECUDA, "cudaEventCreate(resident) failed");
+    std::vector<PagePlan> pages;
+    uint64_t bad = 0;
+    if (!fma_layout::plan_pages(wake_segs(e, with_res, seg_run), e->res_packed ? &e->res_off : nullptr, &e->res_bytes, &pages, &bad))
+        return fail(FMA_ESTATE, "segment outside the resident part's page table");
+    uint64_t* dst_tab = e->h_tab + n_host_pages;
+    uint64_t* src_tab = e->h_tab + e->d_tab_cap + n_host_pages;
+    for (size_t q = 0; q < pages.size(); ++q) {
+        if (e->res_packed) {
+            set_pack_desc(e->h_pdesc[n_host_pages + q], (uint64_t)e->res.va + pages[q].off, pages[q].va, pages[q].bytes);
+        } else {
+            dst_tab[q] = pages[q].va;
+            src_tab[q] = (uint64_t)e->res.va + pages[q].off;
+        }
+    }
+    fma_layout::plan_batches(pages, slot_pages(e), UINT64_MAX, false, &pieces);
+    if (e->res_packed) {
+        RT(cudaMemcpyAsync(e->d_pdesc + n_host_pages, e->h_pdesc + n_host_pages, n_res * sizeof(fma_k_pack_desc), cudaMemcpyHostToDevice, e->ks));
+        if (!image_packed) RT(cudaMemsetAsync(e->d_psize + e->pdesc_cap, 0, sizeof(uint32_t), e->ks));   // (WakePipe::packed clears it otherwise)
+    } else {
+        RT(cudaMemcpyAsync(e->d_tab + n_host_pages, dst_tab, n_res * sizeof(uint64_t), cudaMemcpyHostToDevice, e->ks));
+        RT(cudaMemcpyAsync(e->d_tab + e->d_tab_cap + n_host_pages, src_tab, n_res * sizeof(uint64_t), cudaMemcpyHostToDevice, e->ks));
+    }
+    return FMA_OK;
+}
+
+int ResidentRestore::launch_next() {
+    const Batch& pc = pieces[next];
+    RC(mapper.wait(pc.need));
+    int r;
+    kt.kind = "res_restore";
+    if (e->res_packed) {
+        r = kt.begin();
+        if (r == FMA_OK) {
+            cudaError_t ce = fma_k_launch_unpack(e->d_pdesc + n_host_pages + pc.p0, (uint32_t)pc.np, e->d_psize + e->pdesc_cap, e->ks);
+            r = ce == cudaSuccess ? kt.end((uint64_t)pc.np * FMA_PAGE_BYTES + pc.stored) : fail(FMA_ECUDA, "K5 (resident) launch failed: %s", cudaGetErrorString(ce));
+        }
+    } else {
+        r = kt.launch(e->d_tab + e->d_tab_cap + n_host_pages + pc.p0, 0, e->d_tab + n_host_pages + pc.p0, 0, (uint32_t)pc.np);
+    }
+    kt.kind = "kernel";
+    if (r != FMA_OK) return r;
+    if (++next == pieces.size()) RT(cudaEventRecord(e->ev_res_done, e->ks));
+    return FMA_OK;
+}
 
 // PACKED image: H2D of the stored pages (0.758 of the bytes) -> ring slot -> K5 decode + scatter; or K5 reads the store itself
 int WakePipe::packed() {
@@ -67,12 +287,11 @@ int WakePipe::packed() {
     if (!fma_layout::plan_pages(wake_segs(e, with_backup, seg_run), &e->img_off, &e->img_bytes, &pages, &bad))
         return fail(FMA_ESTATE, "segment at image offset %llu is outside the packed image's page table", (unsigned long long)bad);
     const size_t n_pages = pages.size();
-    PIPE_CHECK(ensure_pack_bufs(e, n_pages));
+    RC(ensure_pack_bufs(e, n_pages));
     uint32_t* d_err = e->d_psize + e->pdesc_cap;
     RT(cudaMemsetAsync(d_err, 0, sizeof(uint32_t), e->ks));
     if (!zero_copy) {
-        if (ring_run) PIPE_CHECK(wait(1));
-        else PIPE_CHECK(ensure_ring(e, W));
+        if (ring_run) RC(mapper.wait(1));   // (else the route has the ring)
         std::vector<Batch> slots;  // pages that are adjacent in the store and fit one ring slot
         if (!fma_layout::plan_batches(pages, SIZE_MAX, e->ring_slot_bytes, true, &slots))
             return fail(FMA_EINVAL, "ring slot of %zu bytes cannot hold one page", e->ring_slot_bytes);
@@ -88,13 +307,13 @@ int WakePipe::packed() {
             RT(cudaMemcpyAsync(e->ring[slot], store + pages[sl.p0].off, sl.stored, cudaMemcpyDefault, cstream));
             copied();
             RT(cudaEventRecord(e->ev_ring_full[slot], cstream));
-            PIPE_CHECK(wait(sl.need));
+            RC(mapper.wait(sl.need));
             RT(cudaStreamWaitEvent(e->ks, e->ev_ring_full[slot], 0));
-            PIPE_CHECK(kt.begin());
+            RC(kt.begin());
             RT(fma_k_launch_unpack(e->d_pdesc + sl.p0, (uint32_t)sl.np, d_err, e->ks));
-            PIPE_CHECK(kt.end((uint64_t)sl.np * FMA_PAGE_BYTES + sl.stored));
+            RC(kt.end((uint64_t)sl.np * FMA_PAGE_BYTES + sl.stored));
             RT(cudaEventRecord(e->ev_ring_free[slot], e->ks));
-            if (between) PIPE_CHECK(between(sl.p0 + sl.np, n_pages));
+            if (between) RC(between->pump(sl.p0 + sl.np, n_pages));
         }
     } else {
         const uint64_t sbase = store_dev_base(e, tier);
@@ -103,12 +322,12 @@ int WakePipe::packed() {
         std::vector<Batch> batches;
         fma_layout::plan_batches(pages, slot_pages(e), UINT64_MAX, false, &batches);
         for (const Batch& b : batches) {
-            PIPE_CHECK(wait(b.need));
-            PIPE_CHECK(kt.begin());
+            RC(mapper.wait(b.need));
+            RC(kt.begin());
             RT(fma_k_launch_unpack(e->d_pdesc + b.p0, (uint32_t)b.np, d_err, e->ks));
-            PIPE_CHECK(kt.end((uint64_t)b.np * FMA_PAGE_BYTES + b.stored));
+            RC(kt.end((uint64_t)b.np * FMA_PAGE_BYTES + b.stored));
             copied();
-            if (between) PIPE_CHECK(between(b.p0 + b.np, n_pages));
+            if (between) RC(between->pump(b.p0 + b.np, n_pages));
         }
     }
     return FMA_OK;
@@ -119,7 +338,7 @@ int WakePipe::direct() {
     const size_t chunk = direct_chunk(e);
     int k = 0;
     for (size_t i : with_backup) {
-        PIPE_CHECK(wait(seg_run[i] + 1));
+        RC(mapper.wait(seg_run[i] + 1));
         const Segment& s = e->segs[i];
         for (size_t o = 0; o < s.bytes; o += chunk, ++k) {
             const size_t n = std::min(chunk, s.bytes - o);
@@ -139,7 +358,7 @@ int WakePipe::paged() {
     uint64_t bad = 0;
     fma_layout::plan_pages(wake_segs(e, with_backup, seg_run), nullptr, nullptr, &pages, &bad);
     const size_t n_pages = pages.size();
-    PIPE_CHECK(ensure_tables(e, n_pages));
+    RC(ensure_tables(e, n_pages));
     uint64_t* dst_tab = e->h_tab;                 // destination page addresses
     uint64_t* src_tab = e->h_tab + e->d_tab_cap;  // source page addresses inside the store (may be sparse)
     const uint64_t sbase = store_dev_base(e, tier);
@@ -156,18 +375,17 @@ int WakePipe::paged() {
         // mapper makes progress so the scatter overlaps cuMemCreate/Map of later segments
         for (size_t p0 = 0; p0 < n_pages;) {
             Batch b = fma_layout::next_batch(pages, p0, slot_pages(e), UINT64_MAX, false);
-            PIPE_CHECK(wait(b.need));
+            RC(mapper.wait(b.need));
             // opportunistically extend the batch over everything already mapped
-            const size_t have = mapped_now();
+            const size_t have = mapper.done.load();
             while (p0 + b.np < n_pages && pages[p0 + b.np].need <= have) ++b.np;
-            PIPE_CHECK(kt.launch(d_src + p0, 0, d_dst + p0, 0, (uint32_t)b.np));
+            RC(kt.launch(d_src + p0, 0, d_dst + p0, 0, (uint32_t)b.np));
             copied();
             p0 += b.np;
-            if (between) PIPE_CHECK(between(p0, n_pages));
+            if (between) RC(between->pump(p0, n_pages));
         }
     } else {  // STAGED: copy engine H2D store -> ring slot (starts at t=0), K2 scatter once the targets are mapped
-        if (ring_run) PIPE_CHECK(wait(1));  // the ring is run 0 (1 GiB, ~0.2 ms to map): wait for it before the first H2D
-        else PIPE_CHECK(ensure_ring(e, W));
+        if (ring_run) RC(mapper.wait(1));  // the ring is run 0 (1 GiB, ~0.2 ms to map): wait for it before the first H2D
         // the store image may be only partially woken; H2D works on runs that are contiguous in the store
         std::vector<Batch> slots;
         if (!fma_layout::plan_batches(pages, e->ring_slot_bytes / FMA_PAGE_BYTES, UINT64_MAX, true, &slots))
@@ -180,11 +398,11 @@ int WakePipe::paged() {
             RT(cudaMemcpyAsync(e->ring[slot], store + pages[sl.p0].off, sl.stored, cudaMemcpyDefault, cstream));
             copied();
             RT(cudaEventRecord(e->ev_ring_full[slot], cstream));
-            PIPE_CHECK(wait(sl.need));
+            RC(mapper.wait(sl.need));
             RT(cudaStreamWaitEvent(e->ks, e->ev_ring_full[slot], 0));
-            PIPE_CHECK(kt.launch(nullptr, (uint64_t)(uintptr_t)e->ring[slot], d_dst + sl.p0, 0, (uint32_t)sl.np));
+            RC(kt.launch(nullptr, (uint64_t)(uintptr_t)e->ring[slot], d_dst + sl.p0, 0, (uint32_t)sl.np));
             RT(cudaEventRecord(e->ev_ring_free[slot], e->ks));
-            if (between) PIPE_CHECK(between(sl.p0 + sl.np, n_pages));
+            if (between) RC(between->pump(sl.p0 + sl.np, n_pages));
         }
     }
     return FMA_OK;
@@ -199,12 +417,11 @@ int WakePipe::multipath() {
     uint64_t bad = 0;
     fma_layout::plan_pages(wake_segs(e, with_backup, seg_run), nullptr, nullptr, &pages, &bad);
     const size_t n_pages = pages.size();
-    PIPE_CHECK(ensure_tables(e, n_pages));
+    RC(ensure_tables(e, n_pages));
     for (size_t p = 0; p < n_pages; ++p) e->h_tab[p] = pages[p].va;
     RT(cudaMemcpyAsync(e->d_tab, e->h_tab, n_pages * sizeof(uint64_t), cudaMemcpyHostToDevice, e->ks));
-    cudaEvent_t ev_tab = nullptr;   // the page table must be on the device before any path's K2 reads it
-    PIPE_CHECK(ensure_ring_events(e, 1));
-    ev_tab = e->ev_ring_full[0];
+    RC(ensure_ring_events(e, 1));
+    cudaEvent_t ev_tab = e->ev_ring_full[0];   // the page table must be on the device before any path's K2 reads it
     RT(cudaEventRecord(ev_tab, e->ks));
     std::vector<Batch> chunks;
     fma_layout::plan_batches(pages, std::max<size_t>(e->path_slot_bytes / FMA_PAGE_BYTES, 1), UINT64_MAX, true, &chunks);
@@ -216,7 +433,7 @@ int WakePipe::multipath() {
     // lives in the shared mailbox together with the chunk table of this wake (fma_pull.h); published with the generation bump.
     PullMailbox* mb = e->mbox;
     if (mb) {
-        if (chunks.size() > kPullMaxChunks) PIPE_CHECK(fail(FMA_EINVAL, "%zu chunks exceed the mailbox's table (use larger path slots)", chunks.size()));
+        if (chunks.size() > kPullMaxChunks) RC(fail(FMA_EINVAL, "%zu chunks exceed the mailbox's table (use larger path slots)", chunks.size()));
         for (size_t c = 0; c < chunks.size(); ++c) mb->chunks[c] = PullChunk{chunk_off[c], (uint32_t)chunks[c].stored, 0};
         for (uint32_t pi = 0; pi < kPullMaxPaths; ++pi) {
             mb->helper_error[pi].store(0);
@@ -247,7 +464,7 @@ int WakePipe::multipath() {
         cudaSetDevice(e->device);
         auto failw = [&](int code, const char* what, cudaError_t ce) {
             int expect = FMA_OK;
-            if (error.compare_exchange_strong(expect, code)) snprintf(err_msg, sizeof(err_msg), "%s failed on path %zu (device %d): %s", what, pi, path.device, ce == cudaSuccess ? (code == FMA_ESTATE || code == FMA_EINTEGRITY ? what : map_msg) : cudaGetErrorString(ce));
+            if (error.compare_exchange_strong(expect, code)) snprintf(err_msg, sizeof(err_msg), "%s failed on path %zu (device %d): %s", what, pi, path.device, ce == cudaSuccess ? (code == FMA_ESTATE || code == FMA_EINTEGRITY ? what : mapper.msg) : cudaGetErrorString(ce));
         };
         cudaError_t ce = cudaStreamWaitEvent(path.kern, ev_tab, 0);
         if (ce != cudaSuccess) return failw(FMA_ECUDA, "cudaStreamWaitEvent(table)", ce);
@@ -297,7 +514,7 @@ int WakePipe::multipath() {
                     const size_t c = st - 1;
                     if (c >= chunks.size()) return failw(FMA_EINTEGRITY, "the mailbox names a chunk that does not exist", cudaSuccess);
                     const Batch& ch = chunks[c];
-                    const int mrc = wait_mapped(ch.need);
+                    const int mrc = mapper.wait_mapped(ch.need);
                     if (mrc != FMA_OK) return failw(mrc, "mapping", cudaSuccess);
                     char* slot_ptr = reinterpret_cast<char*>(path.va) + (size_t)slot * e->path_slot_bytes;
                     {
@@ -345,7 +562,7 @@ int WakePipe::multipath() {
             if (!first_copy_seen.exchange(true)) first_copy_delay = now_s() - t_entry;
             ce = cudaEventRecord(path.ev_full[slot], path.copy);
             if (ce != cudaSuccess) return failw(FMA_ECUDA, "cudaEventRecord(slot full)", ce);
-            const int mrc = wait_mapped(ch.need);
+            const int mrc = mapper.wait_mapped(ch.need);
             if (mrc != FMA_OK) return failw(mrc, "mapping", cudaSuccess);
             ce = cudaStreamWaitEvent(path.kern, path.ev_full[slot], 0);
             if (ce != cudaSuccess) return failw(FMA_ECUDA, "cudaStreamWaitEvent(slot full)", ce);
@@ -381,406 +598,202 @@ int WakePipe::multipath() {
     return FMA_OK;
 }
 
-#undef PIPE_CHECK
+// A RESIDENT share's segments: their bytes are in e->res, their offsets in the resident part.
+bool is_resident(const fma_engine_t* e, const Segment& s) { return s.has_backup && s.backup_tier == FMA_TIER_LOCAL && e->image_tier == FMA_TIER_HOST; }
+
+// Work list: RUNS — maximal VA-contiguous groups of sleeping segments of one arena — so a whole tag is re-created with one
+// cuMemCreate + cuMemMap + cuMemSetAccess.  Runs that have a backup come first, in image order (they gate the copy pipeline);
+// remap-only runs (e.g. kv_cache) are mapped after them.  No runs: nothing to wake.
+int plan_wake_runs(fma_engine_t* e, uint64_t tag_mask, double t_entry, std::vector<Run>* runs) {
+    std::vector<size_t> cand;
+    for (size_t i = 0; i < e->segs.size(); ++i) {
+        const Segment& s = e->segs[i];
+        if (s.mapped) continue;                                  // idempotent: already awake
+        if (tag_mask && !tag_bit_set(tag_mask, s.tag)) continue;  // tags is None or data.tag in tags (cumem.py:238)
+        cand.push_back(i);
+    }
+    if (cand.empty()) return FMA_OK;
+    RC(check_tma_shape(e, e->image_tier));
+    e->tl_begin("wake", t_entry);
+    std::sort(cand.begin(), cand.end(), [&](size_t a, size_t b) {
+        const Segment &x = e->segs[a], &y = e->segs[b];
+        return x.arena != y.arena ? x.arena < y.arena : x.va < y.va;
+    });
+    std::vector<fma_layout::SegView> view;
+    for (size_t i : cand) {
+        const Segment& s = e->segs[i];
+        // a RESIDENT share's segments (their offsets are in the resident part) are mapped after the host part's
+        const uint64_t key = is_resident(e, s) ? (1ull << 62) + s.packed_off : s.packed_off;
+        view.push_back(fma_layout::SegView{i, s.arena, (uint64_t)s.va, s.bytes, s.has_backup, key});
+    }
+    // FMA_MAP_PIECE_MIB (default 2048; 0 = whole runs): backed-up runs are mapped in pieces of about that size, cut at segment
+    // boundaries.  One 15 GiB mapping has only the ring's slack of a few milliseconds, and a shared host's driver calls
+    // sometimes stall for tens of milliseconds; with pieces K2 starts on the first piece and every later call has the copy
+    // time of the pieces before it as slack.
+    *runs = fma_layout::plan_runs(view, env_int("FMA_MERGE_RUNS", 1) != 0, (size_t)std::max(env_int("FMA_MAP_PIECE_MIB", 2048), 0) << 20);
+    return FMA_OK;
+}
+
+// Staging ring.  Steady state: the ring is its OWN small run (2 x 512 MiB) placed right after the first backed-up
+// run at the arena's bump pointer and mapped FIRST — a 1 GiB cuMemCreate/Map/SetAccess costs ~0.2 ms, the H2D
+// stream starts as soon as it exists, and the big weights run (whose mapping takes 1.4 ms alone but tens of ms
+// when 8 ranks wake at once) keeps the ring's ~19 ms of slack.  At the next sleep the ring goes with a cuMemUnmap
+// like every other unit: no cudaMalloc / cudaFree anywhere (a cudaFree of 1 GiB stalls 0.8-300 ms on these hosts).
+// Needs the run to end at its arena's bump pointer; otherwise (or FMA_RING_ATTACH=0) one cudaMalloc provides it.
+// Either way the ring must exist BEFORE the other runs start taking HBM.  false: HBM too full for a ring.
+bool ring_for_wake(fma_engine_t* e, std::vector<Run>& runs, uint64_t w_bytes, bool* ring_run) {
+    if (!e->n_ring) {
+        const Run& r0 = runs[0];
+        Arena& a = e->arenas[r0.arena];
+        const size_t slot = ring_slot_for(e, w_bytes);
+        const size_t total = slot * ring_slots_for(e);
+        // end of the VA-contiguous chain of backed-up runs that starts with the first one (one run, or its pieces)
+        uint64_t chain_end = r0.va + r0.bytes;
+        for (size_t k = 1; k < runs.size() && runs[k].has_backup && runs[k].arena == r0.arena && runs[k].va == chain_end; ++k) chain_end += runs[k].bytes;
+        const bool at_top = r0.has_backup && (chain_end == a.base + a.top) && a.top + total <= a.cap;
+        if (at_top && env_int("FMA_RING_ATTACH", 1) != 0 && ensure_ring_events(e, ring_slots_for(e)) == FMA_OK) {
+            Run rr;
+            rr.va = chain_end; rr.bytes = total; rr.arena = r0.arena; rr.has_backup = true; rr.first_off = 0;  // no segments
+            a.top += total;  // later allocations of this tag land after the ring; the range returns at unmap
+            e->n_ring = ring_slots_for(e);
+            e->ring_slot_bytes = slot;
+            e->ring_attached = true;
+            e->ring_unit_va = rr.va;
+            for (int i = 0; i < e->n_ring; ++i) e->ring[i] = reinterpret_cast<void*>(rr.va + (size_t)i * slot);
+            runs.insert(runs.begin(), std::move(rr));
+            *ring_run = true;
+            return true;
+        }
+    }
+    return ensure_ring(e, w_bytes) == FMA_OK;  // (else copy engines go straight into the runs)
+}
+
+// FMA_FLAG_VERIFY: every restored segment against its digest from before the sleep
+int verify_wake(fma_engine_t* e, const std::vector<size_t>& with_backup, int* verify_rc) {
+    std::vector<size_t> idx;
+    for (size_t i : with_backup)
+        if (e->segs[i].digest_valid) idx.push_back(i);
+    std::vector<uint64_t> dg;
+    RC(digest_segments(e, idx, &dg));
+    for (size_t k = 0; k < idx.size(); ++k)
+        if (dg[k] != e->segs[idx[k]].digest)
+            *verify_rc = fail(FMA_EINTEGRITY, "segment %zu (va 0x%llx): digest %016llx after wake != %016llx before sleep", idx[k],
+                              (unsigned long long)e->segs[idx[k]].va, (unsigned long long)dg[k], (unsigned long long)e->segs[idx[k]].digest);
+    return FMA_OK;
+}
+
+// data.cpu_backup_tensor = None (cumem.py:249), unless FMA_FLAG_KEEP_BACKUP
+void drop_backups(fma_engine_t* e, const std::vector<size_t>& with_backup, uint64_t W, int tier, bool verified) {
+    for (size_t i : with_backup) {
+        Segment& s = e->segs[i];
+        // INCREMENTAL sleep: the host store keeps these bytes; remember where, together with their digest
+        const bool kept = s.digest_valid && verified && !is_resident(e, s);   // (the resident buffer does not outlive the wake)
+        s.shadow_off = kept ? s.packed_off : kNoOffset;   // host store or parking buffer: both outlive the wake
+        s.has_backup = false;
+        s.packed_off = kNoOffset;
+    }
+    if (W) {
+        e->shadow_tier = tier;
+        e->shadow_packed = e->image_packed;
+        e->shadow_store_bytes = e->image_store_bytes;
+        e->shadow_image_bytes = e->image_bytes;
+    }
+}
 
 }  // namespace
 
 // ------------------------------------------------------------------------------------
 // WAKE
 // ------------------------------------------------------------------------------------
-struct MapProgress {
-    std::mutex mu;
-    std::condition_variable cv;
-    size_t done = 0;      // number of work items fully mapped (prefix)
-    int error = FMA_OK;
-    char msg[512] = "";
-};
-
 int do_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags) {
     DeviceGuard guard(e->device);
-    auto is_resident = [&](const Segment& s) { return s.has_backup && s.backup_tier == FMA_TIER_LOCAL && e->image_tier == FMA_TIER_HOST; };
-    int rc = flush_kernel_times(e);
-    if (rc != FMA_OK) return rc;
+    RC(flush_kernel_times(e));
     const double t_entry = now_s();
-    rc = ensure_streams(e);
-    if (rc != FMA_OK) return rc;
-
-    // Work list: RUNS — maximal VA-contiguous groups of sleeping segments of one arena — so a whole tag is
-    // re-created with one cuMemCreate + cuMemMap + cuMemSetAccess.  Runs that have a backup come first, in image
-    // order (they gate the copy pipeline); remap-only runs (e.g. kv_cache) are mapped after them.
-    using Run = fma_layout::Run;
+    RC(ensure_streams(e));
     std::vector<Run> runs;
-    {
-        std::vector<size_t> cand;
-        for (size_t i = 0; i < e->segs.size(); ++i) {
-            const Segment& s = e->segs[i];
-            if (s.mapped) continue;                                  // idempotent: already awake
-            if (tag_mask && !tag_bit_set(tag_mask, s.tag)) continue;  // tags is None or data.tag in tags (cumem.py:238)
-            cand.push_back(i);
-        }
-        if (cand.empty()) return FMA_OK;
-        rc = check_tma_shape(e, e->image_tier);
-        if (rc != FMA_OK) return rc;
-        e->tl_begin("wake", t_entry);
-        std::sort(cand.begin(), cand.end(), [&](size_t a, size_t b) {
-            const Segment &x = e->segs[a], &y = e->segs[b];
-            return x.arena != y.arena ? x.arena < y.arena : x.va < y.va;
-        });
-        std::vector<fma_layout::SegView> view;
-        for (size_t i : cand) {
-            const Segment& s = e->segs[i];
-            // a RESIDENT share's segments (their offsets are in the resident part) are mapped after the host part's
-            const uint64_t key = is_resident(s) ? (1ull << 62) + s.packed_off : s.packed_off;
-            view.push_back(fma_layout::SegView{i, s.arena, (uint64_t)s.va, s.bytes, s.has_backup, key});
-        }
-        // FMA_MAP_PIECE_MIB (default 2048; 0 = whole runs): backed-up runs are mapped in pieces of about that size, cut at segment
-        // boundaries.  One 15 GiB mapping has only the ring's slack of a few milliseconds, and a shared host's driver calls
-        // sometimes stall for tens of milliseconds; with pieces K2 starts on the first piece and every later call has the copy
-        // time of the pieces before it as slack.
-        runs = fma_layout::plan_runs(view, env_int("FMA_MERGE_RUNS", 1) != 0, (size_t)std::max(env_int("FMA_MAP_PIECE_MIB", 2048), 0) << 20);
-    }
+    RC(plan_wake_runs(e, tag_mask, t_entry, &runs));
+    if (runs.empty()) return FMA_OK;
     const int tier = e->image_tier;
-    int mode = resolve_mode(e, tier);
-    // A PACKED image can only be read by K5: through the staging ring, or (no HBM for a ring) straight from the
-    // mapped pinned store.
-    const bool packed = e->image_packed;
-    if (packed && tier == FMA_TIER_HOST) mode = FMA_MODE_STAGED;
 
-    // Staging ring.  Steady state: the ring is its OWN small run (2 x 512 MiB) placed right after the first backed-up
-    // run at the arena's bump pointer and mapped FIRST — a 1 GiB cuMemCreate/Map/SetAccess costs ~0.2 ms, the H2D
-    // stream starts as soon as it exists, and the big weights run (whose mapping takes 1.4 ms alone but tens of ms
-    // when 8 ranks wake at once) keeps the ring's ~19 ms of slack.  At the next sleep the ring goes with a cuMemUnmap
-    // like every other unit: no cudaMalloc / cudaFree anywhere (a cudaFree of 1 GiB stalls 0.8-300 ms on these hosts).
-    // Needs the run to end at its arena's bump pointer; otherwise (or FMA_RING_ATTACH=0) one cudaMalloc provides it.
-    // Either way the ring must exist BEFORE the other runs start taking HBM.
-    bool ring_run = false;
-    // MULTI-PATH: idle peers' PCIe links are borrowed for a host-tier wake of a plain image (fma_paths_set)
-    const bool multipath = !e->paths.empty() && tier == FMA_TIER_HOST && mode == FMA_MODE_STAGED && !packed;
-    {
-        uint64_t w_bytes = 0;   // what crosses the link (a resident share's segments do not)
-        for (const Run& r : runs)
-            if (r.has_backup)
-                for (size_t i : r.segs)
-                    if (!is_resident(e->segs[i])) w_bytes += e->segs[i].bytes;
-        if (w_bytes && mode == FMA_MODE_STAGED && multipath) {
-            // every path brings its own staging slots: no ring
-        } else if (w_bytes && mode == FMA_MODE_STAGED && no_ring()) {
-            mode = FMA_MODE_DIRECT;  // as when HBM is too full for a ring
-        } else if (w_bytes && mode == FMA_MODE_STAGED && !e->n_ring) {
-            const Run& r0 = runs[0];
-            Arena& a = e->arenas[r0.arena];
-            const size_t slot = ring_slot_for(e, w_bytes);
-            const size_t total = slot * ring_slots_for(e);
-            // end of the VA-contiguous chain of backed-up runs that starts with the first one (one run, or its pieces)
-            uint64_t chain_end = r0.va + r0.bytes;
-            for (size_t k = 1; k < runs.size() && runs[k].has_backup && runs[k].arena == r0.arena && runs[k].va == chain_end; ++k) chain_end += runs[k].bytes;
-            const bool at_top = r0.has_backup && (chain_end == a.base + a.top) && a.top + total <= a.cap;
-            if (at_top && env_int("FMA_RING_ATTACH", 1) != 0 && ensure_ring_events(e, ring_slots_for(e)) == FMA_OK) {
-                Run rr;
-                rr.va = chain_end; rr.bytes = total; rr.arena = r0.arena; rr.has_backup = true; rr.first_off = 0;  // no segments
-                a.top += total;  // later allocations of this tag land after the ring; the range returns at unmap
-                e->n_ring = ring_slots_for(e);
-                e->ring_slot_bytes = slot;
-                e->ring_attached = true;
-                e->ring_unit_va = rr.va;
-                for (int i = 0; i < e->n_ring; ++i) e->ring[i] = reinterpret_cast<void*>(rr.va + (size_t)i * slot);
-                runs.insert(runs.begin(), std::move(rr));
-                ring_run = true;
-            } else if (ensure_ring(e, w_bytes) != FMA_OK) {
-                mode = FMA_MODE_DIRECT;  // HBM too full for a ring: copy engines go straight into the runs
-            }
-        } else if (w_bytes && mode == FMA_MODE_STAGED && ensure_ring(e, w_bytes) != FMA_OK) {
-            mode = FMA_MODE_DIRECT;
-        }
-    }
-
-    std::vector<size_t> with_backup, remap_only;  // segment indices, image order
-    std::vector<size_t> with_host, with_res;      // with_backup split by store: the host part, the RESIDENT share
-    std::vector<size_t> seg_run(e->segs.size(), 0);  // segment -> index of its run in `runs`
-    size_t n_backup_runs = 0;
+    std::vector<size_t> with_backup, with_host, with_res;  // segment indices, image order; with_backup by store: host part, RESIDENT share
+    std::vector<size_t> seg_run(e->segs.size(), 0);       // segment -> index of its run in `runs`
+    uint64_t W = 0, W_res = 0, remapped_only = 0;         // W: what crosses the link (a resident share's segments do not)
     for (size_t r = 0; r < runs.size(); ++r) {
-        if (runs[r].has_backup) ++n_backup_runs;
         for (size_t i : runs[r].segs) {
             seg_run[i] = r;
-            (runs[r].has_backup ? with_backup : remap_only).push_back(i);
-            if (runs[r].has_backup) (is_resident(e->segs[i]) ? with_res : with_host).push_back(i);
+            if (!runs[r].has_backup) {
+                remapped_only += e->segs[i].bytes;
+                continue;
+            }
+            with_backup.push_back(i);
+            const bool res = is_resident(e, e->segs[i]);
+            (res ? with_res : with_host).push_back(i);
+            (res ? W_res : W) += e->segs[i].bytes;
         }
     }
+    fma_layout::WakeFacts facts{tier, fma_layout::resolve_mode(e->cfg.mode, tier), e->image_packed, !e->paths.empty(), W != 0, no_ring()};
+    bool ring_run = false;
+    if (fma_layout::wake_route(facts).wants_ring) facts.ring = ring_for_wake(e, runs, W, &ring_run);
+    if (ring_run)  // the ring became run 0
+        for (size_t& r : seg_run) ++r;
+    const fma_layout::WakeRoute route = fma_layout::wake_route(facts);
     const bool dbg_t = env_int("FMA_DEBUG_TIMING", 0) != 0;
     const double t_ring = now_s();
-    // expected copy time of the host part: 55 GB/s per host-tier link (a multi-path wake has as many links as paths), 600 GB/s
-    // over NVLink.  Remap-only runs wait a fifth of it (host tier) or half of it (NVLink): far below the slack.
-    const double expected_copy_s = [&] {
-        uint64_t w = 0;
-        for (size_t i : with_host) w += e->segs[i].bytes;
-        return (double)w / (tier == FMA_TIER_HOST ? 55e9 * (multipath ? (double)e->paths.size() : 1.0) : 600e9);
-    }();
-    const int forced_delay_ms = env_int("FMA_REMAP_DELAY_MS", -1);
-    const double remap_delay_s = forced_delay_ms >= 0 ? forced_delay_ms * 1e-3 : expected_copy_s * (tier == FMA_TIER_HOST ? 0.2 : 0.5);
-
-    // FMA_REMAP_AFTER_COPY=1: remap-only runs (kv_cache) are mapped only after this rank's last copy has LANDED — a 32 GiB
-    // cuMemCreate/Map/SetAccess then never runs beside this rank's DMA (its cost, a few ms, is added to the wake instead of
-    // hidden under it).  A/B knob for the question "does a large VMM call slow a running H2D stream down?".
-    const bool remap_after_copy = env_int("FMA_REMAP_AFTER_COPY", 0) != 0 && n_backup_runs > 0;
-    std::atomic<bool> copies_landed{false};
     e->tl_add("plan", (int)runs.size(), t_entry, t_ring, 0);
-    // Cross-process VMM gate (fma_gate.h): tell the other engines on this host that a call which gates a first copy is coming
-    int gate_first = n_backup_runs ? gate_announce(kGateFirst) : 0;
-
-    // ---- mapper thread(s): one create + map + set-access per run, in `runs` order ----------------------
-    MapProgress prog;
-    std::vector<char> item_done(runs.size(), 0);
-    std::atomic<size_t> next_item{0};
-    std::atomic<uint64_t> map_ns{0};
-    const int n_map = std::max(1, std::min(e->cfg.map_threads > 0 ? e->cfg.map_threads : 1, 8));
-    auto mapper = [&]() {
-        cudaSetDevice(e->device);
-        for (;;) {
-            const size_t k = next_item.fetch_add(1);
-            if (k >= runs.size()) break;
-            {
-                std::lock_guard<std::mutex> lk(prog.mu);
-                if (prog.error != FMA_OK) break;
-            }
-            const Run& run = runs[k];
-            if (!run.has_backup && n_backup_runs && remap_delay_s > 0) {
-                // Remap-only runs (kv_cache) have the whole copy time as slack, the weights run only the ring's worth
-                // (~19 ms).  Driver VMM calls of ALL processes on the host serialise, so a rank that maps its kv early
-                // delays another rank's weights mapping: give every rank's weights a head start.
-                const double wait = t_entry + remap_delay_s - now_s();
-                if (wait > 0) std::this_thread::sleep_for(std::chrono::duration<double>(wait));
-            }
-            if (!run.has_backup && remap_after_copy) {
-                while (!copies_landed.load(std::memory_order_acquire)) {
-                    {
-                        std::lock_guard<std::mutex> lk(prog.mu);
-                        if (prog.error != FMA_OK) break;
-                    }
-                    std::this_thread::sleep_for(std::chrono::microseconds(200));
-                }
-            }
-            const bool is_ring = ring_run && k == 0;
-            // gate class: whatever gates the first copy (ring, or the first backed-up item when there is no ring run) goes
-            // first on the whole host; the other backed-up items have one ring's worth of slack; remap-only runs have what is
-            // left of the copy time.
-            const bool first_item = run.has_backup && k == 0;
-            const int cls = first_item ? kGateFirst : run.has_backup ? std::min(kGateWeights + (int)k - (ring_run ? 1 : 0), kGateWeightsLast) : kGateRemap;
-            const double left = std::max(0.0, t_entry + expected_copy_s * 0.8 - now_s());
-            const double t_ask = now_s();
-            int r;
-            double t0;
-            {
-                GateHold hold(cls, cls >= kGateRemap ? left : std::min(left, 0.05));
-                if (first_item && gate_first) {
-                    gate_retract(gate_first);
-                    gate_first = 0;
-                }
-                t0 = now_s();
-                r = vmm_create_and_map(e->device, run.va, run.bytes);
-            }
-            const double t1 = now_s();
-            map_ns.fetch_add((uint64_t)((t1 - t0) * 1e9));
-            if (t0 - t_ask > 1e-4) e->tl_add("gate_wait", (int)k, t_ask, t0, 0);
-            e->tl_add(is_ring ? "map_ring" : run.has_backup ? "map_backed" : "map_remap", (int)k, t0, t1, run.bytes);
-            std::lock_guard<std::mutex> lk(prog.mu);
-            if (r != FMA_OK) {
-                prog.error = r;
-                snprintf(prog.msg, sizeof(prog.msg), "%s", tl_err);
-                if (is_ring) {  // the ring never came to exist
-                    arena_give_back(e->arenas[run.arena], run.va - e->arenas[run.arena].base, run.bytes);
-                    release_ring(e);
-                }
-            } else {
-                Unit u;
-                u.va = run.va; u.bytes = run.bytes; u.arena = run.arena;
-                if (is_ring) u.zombies.emplace_back(run.va, run.bytes);  // ring VA returns to the arena when the unit is unmapped
-                for (size_t i : run.segs) {
-                    u.live_bytes += e->segs[i].bytes;
-                    e->segs[i].mapped = true;
-                    e->segs[i].unit_va = run.va;
-                }
-                // holes inside a run cannot exist (runs are VA-contiguous live segments), so bytes == live_bytes
-                e->units[run.va] = u;
-                item_done[k] = 1;
-                while (prog.done < runs.size() && item_done[prog.done]) ++prog.done;
-            }
-            prog.cv.notify_all();
-        }
-    };
-    std::vector<std::thread> mappers;
-    for (int t = 0; t < n_map; ++t) mappers.emplace_back(mapper);
-    auto join_mappers = [&]() {
-        for (auto& t : mappers)
-            if (t.joinable()) t.join();
-    };
-    auto wait_mapped = [&](size_t upto) -> int {  // wait until items [0, upto) are mapped
-        std::unique_lock<std::mutex> lk(prog.mu);
-        prog.cv.wait(lk, [&] { return prog.done >= upto || prog.error != FMA_OK; });
-        return prog.error;
-    };
-    auto mapped_now = [&]() -> size_t {
-        std::lock_guard<std::mutex> lk(prog.mu);
-        return prog.done;
-    };
-    // A wake that fails is rolled back: every run THIS call mapped is unmapped again (its segments still have their backup),
-    // so the table is what it was at entry and the controller's retry (inference-server.go:477-480) redoes the whole wake.
-    // Leaving the mapped prefix in place would make the retry skip it (`mapped` == already awake) and report success over
-    // weights that were never copied back — vLLM's allocator raises in that situation (cumem.py:237-249).
-    auto abort_wake = [&](int code) -> int {
-        char keep[512];
-        snprintf(keep, sizeof(keep), "%s", tl_err);
-        {
-            std::lock_guard<std::mutex> lk(prog.mu);
-            if (prog.error == FMA_OK) prog.error = code;
-        }
-        copies_landed.store(true, std::memory_order_release);
-        join_mappers();
-        if (gate_first) {
-            gate_retract(gate_first);
-            gate_first = 0;
-        }
-        cudaDeviceSynchronize();
-        cudaGetLastError();
-        for (size_t k = 0; k < runs.size(); ++k) {
-            if (!item_done[k]) continue;
-            for (size_t i : runs[k].segs) {
-                e->segs[i].mapped = false;
-                e->segs[i].unit_va = 0;
-            }
-            unmap_units(e, runs[k].va, runs[k].bytes);  // the ring run gives its VA back to the arena through its zombie entry
-        }
-        e->pending_events = 0;
-        snprintf(tl_err, sizeof(tl_err), "%s", keep);
-        return code;
-    };
-#define WAKE_CHECK(x)                     \
-    do {                                  \
-        int _rc = (x);                    \
-        if (_rc != FMA_OK) return abort_wake(_rc); \
-    } while (0)
-#define WAKE_RT(call)                                                                              \
-    do {                                                                                           \
-        cudaError_t _e = (call);                                                                   \
-        if (_e != cudaSuccess) WAKE_CHECK(fail(FMA_ECUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(_e), __FILE__, __LINE__)); \
-    } while (0)
+    Mapper mapper{e, runs, ring_run, t_entry};
+    // expected copy time of the host part: 55 GB/s per host-tier link (a multi-path wake has as many links as paths), 600 GB/s over NVLink
+    mapper.start(tier, (double)W / (tier == FMA_TIER_HOST ? 55e9 * (route.pipe == fma_layout::WakePipeKind::Multipath ? (double)e->paths.size() : 1.0) : 600e9));
 
     // ---- copy pipeline --------------------------------------------------------------------------
-    uint64_t W = 0, W_res = 0;
-    for (size_t i : with_host) W += e->segs[i].bytes;
-    for (size_t i : with_res) W_res += e->segs[i].bytes;
     CopyTimer timer{e};
     KernelTimes kt{e};
     uint32_t copy_ops = 0;
     double copy_s = 0, first_copy_delay = 0;
-    // RESIDENT share: K2 / K5 copy the resident segments from e->res into their pages, on the kernel stream in pieces of at most
-    // one ring slot, each launched between two of the host part's launches once its destination is mapped (in the second half of
-    // the host part's launches the pipeline waits for that mapping); the tables sit behind the host part's in the same buffers.
-    std::vector<Batch> res_pieces;
-    size_t res_next = 0;
-    const size_t n_host_pages = W / FMA_PAGE_BYTES;
+    ResidentRestore res{e, mapper, kt, with_res, seg_run, W_res, W / FMA_PAGE_BYTES, facts.image_packed};
     const bool res_packed = W_res && e->res_packed;   // (the buffer may be released before the K5 error count is read)
-    auto res_setup = [&]() -> int {
-        if (!e->res.va) return fail(FMA_ESTATE, "the resident part of the image is gone");
-        const size_t n_res = W_res / FMA_PAGE_BYTES, n_all = n_host_pages + n_res;
-        int r = ensure_tables(e, n_all);
-        if (r == FMA_OK && e->res_packed) r = ensure_pack_bufs(e, n_all);
-        if (r == FMA_OK && !e->ev_res_done && cudaEventCreateWithFlags(&e->ev_res_done, cudaEventDisableTiming) != cudaSuccess)
-            r = fail(FMA_ECUDA, "cudaEventCreate(resident) failed");
-        if (r != FMA_OK) return r;
-        std::vector<PagePlan> pages;
-        uint64_t bad = 0;
-        if (!fma_layout::plan_pages(wake_segs(e, with_res, seg_run), e->res_packed ? &e->res_off : nullptr, &e->res_bytes, &pages, &bad))
-            return fail(FMA_ESTATE, "segment outside the resident part's page table");
-        uint64_t* dst_tab = e->h_tab + n_host_pages;
-        uint64_t* src_tab = e->h_tab + e->d_tab_cap + n_host_pages;
-        for (size_t q = 0; q < pages.size(); ++q) {
-            if (e->res_packed) {
-                set_pack_desc(e->h_pdesc[n_host_pages + q], (uint64_t)e->res.va + pages[q].off, pages[q].va, pages[q].bytes);
-            } else {
-                dst_tab[q] = pages[q].va;
-                src_tab[q] = (uint64_t)e->res.va + pages[q].off;
-            }
-        }
-        fma_layout::plan_batches(pages, slot_pages(e), UINT64_MAX, false, &res_pieces);
-        if (e->res_packed) {
-            RT(cudaMemcpyAsync(e->d_pdesc + n_host_pages, e->h_pdesc + n_host_pages, n_res * sizeof(fma_k_pack_desc), cudaMemcpyHostToDevice, e->ks));
-            if (!packed) RT(cudaMemsetAsync(e->d_psize + e->pdesc_cap, 0, sizeof(uint32_t), e->ks));   // (WakePipe::packed clears it otherwise)
-        } else {
-            RT(cudaMemcpyAsync(e->d_tab + n_host_pages, dst_tab, n_res * sizeof(uint64_t), cudaMemcpyHostToDevice, e->ks));
-            RT(cudaMemcpyAsync(e->d_tab + e->d_tab_cap + n_host_pages, src_tab, n_res * sizeof(uint64_t), cudaMemcpyHostToDevice, e->ks));
-        }
-        return FMA_OK;
-    };
-    auto res_launch_next = [&]() -> int {
-        const Batch& pc = res_pieces[res_next];
-        int r = wait_mapped(pc.need);
-        if (r != FMA_OK) return fail(r, "%s", prog.msg);
-        kt.kind = "res_restore";
-        if (e->res_packed) {
-            r = kt.begin();
-            if (r == FMA_OK) {
-                cudaError_t ce = fma_k_launch_unpack(e->d_pdesc + n_host_pages + pc.p0, (uint32_t)pc.np, e->d_psize + e->pdesc_cap, e->ks);
-                r = ce == cudaSuccess ? kt.end((uint64_t)pc.np * FMA_PAGE_BYTES + pc.stored) : fail(FMA_ECUDA, "K5 (resident) launch failed: %s", cudaGetErrorString(ce));
-            }
-        } else {
-            r = kt.launch(e->d_tab + e->d_tab_cap + n_host_pages + pc.p0, 0, e->d_tab + n_host_pages + pc.p0, 0, (uint32_t)pc.np);
-        }
-        kt.kind = "kernel";
-        if (r != FMA_OK) return r;
-        if (++res_next == res_pieces.size()) RT(cudaEventRecord(e->ev_res_done, e->ks));
-        return FMA_OK;
-    };
-    auto res_pump = [&](size_t done, size_t total) -> int {
-        if (res_next >= res_pieces.size()) return FMA_OK;
-        if (2 * done < total && mapped_now() < res_pieces[res_next].need) return FMA_OK;
-        return res_launch_next();
-    };
     if (W || W_res) {
         const char* store = static_cast<const char*>(store_copy_base(e, tier));
-        if (W && !store) WAKE_CHECK(fail(FMA_ESTATE, "backup store of tier %d is gone", tier));
-        if (W && tier == FMA_TIER_HOST && mode == FMA_MODE_KERNEL && !e->host.dev_alias)
-            WAKE_CHECK(fail(FMA_ECUDA, "host store has no device alias for zero-copy mode"));
-        WAKE_CHECK(timer.begin());
-        if (W_res) WAKE_CHECK(res_setup());
+        if (W && !store) return fail(FMA_ESTATE, "backup store of tier %d is gone", tier);
+        if (W && tier == FMA_TIER_HOST && route.mode == FMA_MODE_KERNEL && !e->host.dev_alias)
+            return fail(FMA_ECUDA, "host store has no device alias for zero-copy mode");
+        RC(timer.begin());
+        if (W_res) RC(res.setup());
         if (W) {
-            WakePipe pipe{e, with_host, seg_run, W, tier, mode, ring_run, store, kt, copy_ops, first_copy_delay, t_entry, wait_mapped, mapped_now, prog.msg};
-            if (W_res) pipe.between = res_pump;
+            WakePipe pipe{e, with_host, seg_run, W, tier, route.mode, ring_run, store, kt, copy_ops, first_copy_delay, t_entry, mapper, W_res ? &res : nullptr};
             const double t_enq0 = now_s();
-            if (packed) WAKE_CHECK(pipe.packed());
-            else if (multipath) WAKE_CHECK(pipe.multipath());
-            else if (mode == FMA_MODE_DIRECT) WAKE_CHECK(pipe.direct());
-            else WAKE_CHECK(pipe.paged());
+            switch (route.pipe) {
+            case fma_layout::WakePipeKind::PackedRing: case fma_layout::WakePipeKind::PackedZeroCopy: RC(pipe.packed()); break;
+            case fma_layout::WakePipeKind::Multipath: RC(pipe.multipath()); break;
+            case fma_layout::WakePipeKind::Direct: RC(pipe.direct()); break;
+            case fma_layout::WakePipeKind::Kernel: case fma_layout::WakePipeKind::Staged: RC(pipe.paged()); break;
+            }
             e->tl_add("enqueue", (int)copy_ops, t_enq0, now_s(), W);
         }
-        while (res_next < res_pieces.size()) WAKE_CHECK(res_launch_next());   // what the host part's launches left (or had no room for)
+        while (res.next < res.pieces.size()) RC(res.launch_next());   // what the host part's launches left (or had no room for)
     }
-    if (remap_after_copy && W) {  // let the DMA finish before the remap-only runs are touched
+    if (mapper.remap_after_copy && W) {  // let the DMA finish before the remap-only runs are touched
         const double t_w0 = now_s();
-        for (int i = 0; i < e->n_cs; ++i) WAKE_RT(cudaStreamSynchronize(e->cs[i]));
-        WAKE_RT(cudaStreamSynchronize(e->ks));
+        for (int i = 0; i < e->n_cs; ++i) RT(cudaStreamSynchronize(e->cs[i]));
+        RT(cudaStreamSynchronize(e->ks));
         e->tl_add("copies_landed", 0, t_w0, now_s(), W);
     }
-    copies_landed.store(true, std::memory_order_release);
+    mapper.copies_landed.store(true, std::memory_order_release);
     // every requested segment must be mapped before wake returns (cumem.py:237-240)
     {
         const double t_w0 = now_s();
-        int mrc = wait_mapped(runs.size());
-        if (mrc != FMA_OK) WAKE_CHECK(fail(mrc, "%s", prog.msg));
+        RC(mapper.wait(runs.size()));
         e->tl_add("wait_all_mapped", (int)runs.size(), t_w0, now_s(), 0);
     }
-    join_mappers();
-    if (gate_first) {
-        gate_retract(gate_first);
-        gate_first = 0;
-    }
+    mapper.join();
+    mapper.retract_gate();
     // RESIDENT share: the buffer goes once its restore has completed and every run is mapped (a wake that fails before that is
     // rolled back and its retry needs the buffer), under the host part's copy; it stays while a resident segment still sleeps
     // (tag-selective wake) and with FMA_FLAG_KEEP_BACKUP.
     if (e->res.va && !(flags & FMA_FLAG_KEEP_BACKUP)) {
         bool still_asleep = false;
-        for (const Segment& s : e->segs) still_asleep = still_asleep || (is_resident(s) && !s.mapped);
+        for (const Segment& s : e->segs) still_asleep = still_asleep || (is_resident(e, s) && !s.mapped);
         if (!still_asleep) {
-            if (res_next) WAKE_RT(cudaEventSynchronize(e->ev_res_done));
+            if (res.next) RT(cudaEventSynchronize(e->ev_res_done));
             const double a = now_s();
             const uint64_t cap = e->res.cap;
             {
@@ -793,64 +806,33 @@ int do_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags) {
     const double t_joined = now_s();
     double t_copy_end = t_joined;
     if (W || W_res) {
-        WAKE_CHECK(timer.end(&copy_s));
+        RC(timer.end(&copy_s));
         e->tl_add("drain", 0, t_joined, now_s(), W);
-        WAKE_CHECK(kt.collect());
-        if (packed || res_packed)  // K5 counts stored pages it could not read (bad magic / count): the image is damaged
-            WAKE_CHECK(check_pack_errors(e, "%u stored page(s) of the packed image are malformed"));
+        RC(kt.collect());
+        if (facts.image_packed || res_packed)  // K5 counts stored pages it could not read (bad magic / count): the image is damaged
+            RC(check_pack_errors(e, "%u stored page(s) of the packed image are malformed"));
         t_copy_end = now_s();
     }
     if (dbg_t)
         fprintf(stderr, "[fma] wake phases: plan+ring %.1f ms | enqueue+map-wait %.1f ms | drain %.1f ms | ring free %.1f ms | runs %zu\n",
                 (t_ring - t_entry) * 1e3, (t_joined - t_ring) * 1e3, (t_copy_end - t_joined) * 1e3, (now_s() - t_copy_end) * 1e3, runs.size());
-#undef WAKE_CHECK
-#undef WAKE_RT
-
-    uint64_t remapped_only = 0;
-    for (size_t i : remap_only) remapped_only += e->segs[i].bytes;
+    mapper.committed = true;
 
     int verify_rc = FMA_OK;
-    if ((flags & FMA_FLAG_VERIFY) && (W || W_res)) {
-        std::vector<size_t> idx;
-        for (size_t i : with_backup)
-            if (e->segs[i].digest_valid) idx.push_back(i);
-        std::vector<uint64_t> dg;
-        rc = digest_segments(e, idx, &dg);
-        if (rc != FMA_OK) return rc;
-        for (size_t k = 0; k < idx.size(); ++k)
-            if (dg[k] != e->segs[idx[k]].digest)
-                verify_rc = fail(FMA_EINTEGRITY, "segment %zu (va 0x%llx): digest %016llx after wake != %016llx before sleep", idx[k],
-                                 (unsigned long long)e->segs[idx[k]].va, (unsigned long long)dg[k],
-                                 (unsigned long long)e->segs[idx[k]].digest);
-    }
-    if (!(flags & FMA_FLAG_KEEP_BACKUP)) {
-        for (size_t i : with_backup) {  // data.cpu_backup_tensor = None (cumem.py:249)
-            Segment& s = e->segs[i];
-            // INCREMENTAL sleep: the host store keeps these bytes; remember where, together with their digest
-            const bool kept = s.digest_valid && verify_rc == FMA_OK && !is_resident(s);   // (the resident buffer does not outlive the wake)
-            s.shadow_off = kept ? s.packed_off : kNoOffset;   // host store or parking buffer: both outlive the wake
-            s.has_backup = false;
-            s.packed_off = kNoOffset;
-        }
-        if (W) {
-            e->shadow_tier = tier;
-            e->shadow_packed = e->image_packed;
-            e->shadow_store_bytes = e->image_store_bytes;
-            e->shadow_image_bytes = e->image_bytes;
-        }
-    }
+    if ((flags & FMA_FLAG_VERIFY) && (W || W_res)) RC(verify_wake(e, with_backup, &verify_rc));
+    if (!(flags & FMA_FLAG_KEEP_BACKUP)) drop_backups(e, with_backup, W, tier, verify_rc == FMA_OK);
 
     e->tl_add("total", 0, t_entry, now_s(), W + W_res);
     e->st.wake_seconds = now_s() - t_entry;
     e->st.wake_copy_seconds = copy_s;
-    e->st.wake_map_seconds = map_ns.load() * 1e-9;
+    e->st.wake_map_seconds = mapper.map_ns.load() * 1e-9;
     e->st.wake_first_copy_delay = first_copy_delay;
     e->st.wake_bytes_restored = W + W_res;
     e->st.wake_bytes_remapped_only = remapped_only;
     e->st.copy_ops = copy_ops;
     e->st.total_copy_ops += copy_ops;
     e->st.tier = tier;
-    e->st.mode = mode;
+    e->st.mode = route.mode;
     if (!W && !W_res) zero_kernel_stats(e);
     return verify_rc;
 }

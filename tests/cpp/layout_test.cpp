@@ -237,6 +237,146 @@ static void test_resident_split() {
     }
 }
 
+// ---- routes: the sleep and wake restated the way do_sleep / do_wake spelled them out before the routes were made functions.
+// One deliberate difference: a partial-packed sleep wants no ring here.  do_sleep used to call ensure_ring(e, W) for it a second
+// time, after the partial check had got the ring; that call returned at once (ring count and slot size already matched).
+static const int H = FMA_TIER_HOST, DIR = FMA_MODE_DIRECT, STG = FMA_MODE_STAGED, KRN = FMA_MODE_KERNEL;
+
+static SleepRoute sleep_restated(const SleepFacts& f) {
+    const bool adopt = f.adopt || f.clean;
+    int mode = f.partial ? DIR : f.mode;
+    const bool multipath = f.paths && !f.mbox && f.tier == H && mode == STG && !f.partial && !f.partial_packed && !adopt && !f.pack && f.multipath_env;
+    const bool wants_ring = !adopt && mode == STG && !multipath && !f.partial_packed;  // (a partial-packed sleep has its ring already)
+    if (wants_ring && !f.ring) mode = DIR;
+    const bool pack_path = (f.tier == H && mode == STG) || (f.tier != H && mode == KRN);
+    const bool wants_probe = !adopt && !f.partial_packed && f.pack && pack_path;
+    const bool packed = wants_probe && f.worth_packing;
+    using K = SleepPipeKind;
+    const K pipe = adopt ? K::Adopt : f.partial_packed ? K::PartialPacked : f.partial ? K::PartialDirect : mode == DIR ? K::Direct
+                 : mode == KRN ? (packed ? K::KernelPacked : K::Kernel) : multipath && !packed ? K::Multipath : packed ? K::StagedPacked : K::Staged;
+    return SleepRoute{pipe, mode, wants_ring, wants_probe};
+}
+
+static WakeRoute wake_restated(const WakeFacts& f) {
+    int mode = f.mode;
+    if (f.image_packed && f.tier == H) mode = STG;
+    const bool multipath = f.paths && f.tier == H && mode == STG && !f.image_packed;
+    bool wants_ring = false;
+    if (f.moves && mode == STG && multipath) {
+    } else if (f.moves && mode == STG && f.no_ring) {
+        mode = DIR;
+    } else if (f.moves && mode == STG) {
+        wants_ring = true;
+        if (!f.ring) mode = DIR;
+    }
+    using K = WakePipeKind;
+    const K pipe = f.image_packed ? (mode == STG ? K::PackedRing : K::PackedZeroCopy) : multipath ? K::Multipath : mode == DIR ? K::Direct
+                 : mode == KRN ? K::Kernel : K::Staged;
+    return WakeRoute{pipe, mode, wants_ring};
+}
+
+static bool same(const SleepRoute& a, const SleepRoute& b) {
+    return a.pipe == b.pipe && a.mode == b.mode && a.wants_ring == b.wants_ring && a.wants_probe == b.wants_probe;
+}
+static bool same(const WakeRoute& a, const WakeRoute& b) { return a.pipe == b.pipe && a.mode == b.mode && a.wants_ring == b.wants_ring; }
+
+static void test_resolve_mode() {
+    assert(resolve_mode(FMA_MODE_AUTO, H) == STG && resolve_mode(FMA_MODE_AUTO, FMA_TIER_PEER) == KRN);
+    assert(resolve_mode(STG, FMA_TIER_LOCAL) == KRN && resolve_mode(DIR, FMA_TIER_PEER) == DIR && resolve_mode(KRN, H) == KRN);
+}
+
+static SleepFacts sleep_facts(int tier, int mode, bool pack) { return SleepFacts{tier, mode, pack, false, false, false, false, false, false, true}; }
+
+static void test_sleep_route_quirks() {
+    using K = SleepPipeKind;
+    // a partial sleep reports DIRECT, whatever the configured mode
+    SleepFacts f = sleep_facts(H, STG, false);
+    f.partial = true;
+    assert(same(sleep_route(f), SleepRoute{K::PartialDirect, DIR, false, false}));
+    // a clean (adopt) sleep reports the resolved mode and asks for no ring and no probe
+    f = sleep_facts(H, KRN, true);
+    f.clean = true;
+    assert(same(sleep_route(f), SleepRoute{K::Adopt, KRN, false, false}));
+    // the resident split probes on the route asked before the ring is known, and a ring that then fails drops the probe's verdict
+    f = sleep_facts(H, STG, true);
+    assert(sleep_route(f).wants_probe && sleep_route(f).pipe == K::StagedPacked);
+    f.ring = false;
+    assert(same(sleep_route(f), SleepRoute{K::Direct, DIR, true, false}));
+    // a partial-packed sleep has its ring already and keeps the image's form
+    f = sleep_facts(H, STG, true);
+    f.partial_packed = true;
+    assert(same(sleep_route(f), SleepRoute{K::PartialPacked, STG, false, false}));
+    // the parking tiers pack through K4 straight into the store
+    assert(sleep_route(sleep_facts(FMA_TIER_PEER, KRN, true)).pipe == K::KernelPacked);
+    f = sleep_facts(FMA_TIER_LOCAL, KRN, true);
+    f.worth_packing = false;
+    assert(sleep_route(f).pipe == K::Kernel);
+    // multi-path: plain images only, local paths only, and FMA_MULTIPATH_SLEEP=0 turns it off; it needs no ring
+    f = sleep_facts(H, STG, false);
+    f.paths = true;
+    assert(same(sleep_route(f), SleepRoute{K::Multipath, STG, false, false}));
+    f.multipath_env = false;
+    assert(sleep_route(f).pipe == K::Staged && sleep_route(f).wants_ring);
+    f.multipath_env = true;
+    f.mbox = true;
+    assert(sleep_route(f).pipe == K::Staged);
+}
+
+static void test_wake_route_quirks() {
+    using K = WakePipeKind;
+    // a packed host-tier image without a ring: K5 reads the store itself, and the wake reports DIRECT
+    WakeFacts f{H, DIR, true, false, true, false};
+    assert(same(wake_route(f), WakeRoute{K::PackedRing, STG, true}));   // a packed host-tier image wants a ring whatever the mode
+    f.ring = false;
+    assert(same(wake_route(f), WakeRoute{K::PackedZeroCopy, DIR, true}));
+    f = WakeFacts{H, STG, true, false, true, true};                     // FMA_NO_RING: not even asked
+    assert(same(wake_route(f), WakeRoute{K::PackedZeroCopy, DIR, false}));
+    // parking tiers: K5 / K2 read the store itself
+    assert(same(wake_route(WakeFacts{FMA_TIER_PEER, KRN, true, false, true, false}), WakeRoute{K::PackedZeroCopy, KRN, false}));
+    assert(same(wake_route(WakeFacts{FMA_TIER_LOCAL, KRN, false, true, true, false}), WakeRoute{K::Kernel, KRN, false}));
+    // multi-path: a plain host-tier image, no ring; nothing that crosses the link asks for no ring either
+    assert(same(wake_route(WakeFacts{H, STG, false, true, true, false}), WakeRoute{K::Multipath, STG, false}));
+    assert(same(wake_route(WakeFacts{H, STG, false, false, false, false}), WakeRoute{K::Staged, STG, false}));
+    assert(same(wake_route(WakeFacts{H, STG, false, false, true, true}), WakeRoute{K::Direct, DIR, false}));
+}
+
+// every input the engine can present, against the restatement; an answer the route does not want does not change it
+static void test_routes_exhaustive() {
+    size_t n_sleep = 0, n_wake = 0;
+    for (int tier : {FMA_TIER_HOST, FMA_TIER_PEER, FMA_TIER_LOCAL})
+        for (int cfg : {FMA_MODE_AUTO, FMA_MODE_DIRECT, FMA_MODE_STAGED, FMA_MODE_KERNEL})
+            for (int bits = 0; bits < 1 << 7; ++bits)
+                for (int outcome = 0; outcome < 4; ++outcome) {   // none, clean, partial, partial-packed
+                    const int mode = resolve_mode(cfg, tier);
+                    SleepFacts f{tier, mode, (bits & 1) != 0, (bits & 2) != 0, (bits & 4) != 0, (bits & 8) != 0,
+                                 outcome == 1, outcome == 2, outcome == 3, (bits & 16) != 0, (bits & 32) != 0, (bits & 64) != 0};
+                    if ((f.mbox && !f.paths) || (f.adopt && outcome)) continue;   // (adopt: no INCREMENTAL check)
+                    if ((f.partial || f.partial_packed) && tier != H) continue;                   // partial sleeps are host-tier only
+                    if (f.partial_packed && !(f.pack && mode == STG)) continue;
+                    const SleepRoute r = sleep_route(f);
+                    assert(same(r, sleep_restated(f)));
+                    SleepFacts g = f;
+                    g.ring = !f.ring;
+                    if (!r.wants_ring) assert(same(sleep_route(g), r));
+                    g = f;
+                    g.worth_packing = !f.worth_packing;
+                    if (!r.wants_probe) assert(same(sleep_route(g), r));
+                    ++n_sleep;
+                }
+    for (int tier : {FMA_TIER_HOST, FMA_TIER_PEER, FMA_TIER_LOCAL})
+        for (int cfg : {FMA_MODE_AUTO, FMA_MODE_DIRECT, FMA_MODE_STAGED, FMA_MODE_KERNEL})
+            for (int bits = 0; bits < 1 << 5; ++bits) {
+                const WakeFacts f{tier, resolve_mode(cfg, tier), (bits & 1) != 0, (bits & 2) != 0, (bits & 4) != 0, (bits & 8) != 0, (bits & 16) != 0};
+                const WakeRoute r = wake_route(f);
+                assert(same(r, wake_restated(f)));
+                WakeFacts g = f;
+                g.ring = !f.ring;
+                if (!r.wants_ring) assert(same(wake_route(g), r));
+                ++n_wake;
+            }
+    assert(n_sleep == 1968 && n_wake == 384);   // the feasible inputs
+}
+
 int main() {
     test_bump_and_first_fit();
     test_coalescing_and_top_lowering();
@@ -247,6 +387,10 @@ int main() {
     test_batches_by_pages();
     test_chunk_queues();
     test_resident_split();
+    test_resolve_mode();
+    test_sleep_route_quirks();
+    test_wake_route_quirks();
+    test_routes_exhaustive();
     std::puts("layout ok");
     return 0;
 }

@@ -28,3 +28,12 @@ def test_engine_uses_the_tested_header():
     for f in ("fma_sleep.cu", "fma_wake.cu"):   # no pipeline plans by hand any more
         for local in ("struct Dst", "struct Slot", "struct Chunk", "struct ResPiece", "need_item"):
             assert local not in read[f], (f, local)
+    # the pipeline each sleep / wake runs is chosen by the header's routes, and the two functions are short orchestrators
+    assert "fma_layout::sleep_route(" in read["fma_sleep.cu"] and "fma_layout::wake_route(" in read["fma_wake.cu"]
+    assert "int resolve_mode(" not in read["fma_engine.cu"] + read["fma_internal.h"]
+    wake_pipe = read["fma_wake.cu"].split("struct WakePipe {", 1)[1].split("\n};", 1)[0]
+    assert "std::function" not in wake_pipe
+    for f, fn in (("fma_sleep.cu", "int do_sleep("), ("fma_wake.cu", "int do_wake(")):
+        body = read[f].split(fn, 1)[1].split("\n}\n", 1)[0]
+        for local in ("MapProgress", "partial_packed", "pre_planned"):
+            assert local not in body, (fn, local)
