@@ -122,30 +122,83 @@ CUmemAllocationProp device_prop(int device) {
     return prop;
 }
 
+// Maps `h` at `va` and grants each of `devices` read/write access (once per device).  On failure nothing stays mapped, *call
+// names the call that failed, and the caller still owns `h`.
+static CUresult map_with_access(CUdeviceptr va, size_t bytes, CUmemGenericAllocationHandle h, std::initializer_list<int> devices, const char** call) {
+    CUmemAccessDesc acc[2];
+    size_t n = 0;
+    for (int d : devices) {
+        if (n == 2 || (n == 1 && acc[0].location.id == d)) continue;
+        memset(&acc[n], 0, sizeof(acc[n]));
+        acc[n].location.type = CU_MEM_LOCATION_TYPE_DEVICE;
+        acc[n].location.id = d;
+        acc[n++].flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;
+    }
+    *call = "cuMemMap";
+    CUresult r = g_drv.MemMap(va, bytes, 0, h, 0);
+    if (r != CUDA_SUCCESS) return r;
+    *call = "cuMemSetAccess";
+    r = g_drv.MemSetAccess(va, bytes, acc, n);
+    if (r != CUDA_SUCCESS) g_drv.MemUnmap(va, bytes);
+    return r;
+}
+
 // create + map + set access, then drop the handle: the physical memory stays alive until cuMemUnmap
 // (scripts/vmm_span_probe.py checks this), which makes teardown a single driver call per range.
 int vmm_create_and_map(int device, CUdeviceptr va, size_t bytes) {
     CUmemAllocationProp prop = device_prop(device);
     CUmemGenericAllocationHandle h = 0;
     DRV(g_drv.MemCreate(&h, bytes, &prop, 0));
-    CUresult r = g_drv.MemMap(va, bytes, 0, h, 0);
+    const char* call = nullptr;
+    const CUresult r = map_with_access(va, bytes, h, {device}, &call);
     if (r != CUDA_SUCCESS) {
         g_drv.MemRelease(h);
-        return fail(FMA_ECUDA, "cuMemMap failed: %s", cu_err(r));
-    }
-    CUmemAccessDesc acc;
-    memset(&acc, 0, sizeof(acc));
-    acc.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
-    acc.location.id = device;
-    acc.flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;
-    r = g_drv.MemSetAccess(va, bytes, &acc, 1);
-    if (r != CUDA_SUCCESS) {
-        g_drv.MemUnmap(va, bytes);
-        g_drv.MemRelease(h);
-        return fail(FMA_ECUDA, "cuMemSetAccess failed: %s", cu_err(r));
+        return fail(FMA_ECUDA, "%s failed: %s", call, cu_err(r));
     }
     DRV(g_drv.MemRelease(h));
     return FMA_OK;
+}
+
+int vmm_create(int device, size_t bytes, bool exportable, CUmemGenericAllocationHandle* out) {
+    CUmemAllocationProp prop = device_prop(device);
+    if (exportable) prop.requestedHandleTypes = CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR;
+    const CUresult r = g_drv.MemCreate(out, bytes, &prop, 0);
+    if (r != CUDA_SUCCESS)
+        return fail(r == CUDA_ERROR_OUT_OF_MEMORY ? FMA_ENOMEM : FMA_ECUDA, "cuMemCreate(%zu bytes on device %d) failed: %s", bytes, device, cu_err(r));
+    return FMA_OK;
+}
+
+int vmm_import(int fd, CUmemGenericAllocationHandle* out) {
+    const CUresult r = g_drv.MemImportFromShareableHandle(out, reinterpret_cast<void*>(static_cast<uintptr_t>(fd)), CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR);
+    if (r != CUDA_SUCCESS)
+        return fail(r == CUDA_ERROR_OUT_OF_MEMORY ? FMA_ENOMEM : FMA_ECUDA, "cuMemImportFromShareableHandle(fd %d) failed: %s", fd, cu_err(r));
+    return FMA_OK;
+}
+
+int vmm_buffer_map(CUmemGenericAllocationHandle h, size_t bytes, std::initializer_list<int> access_devices, const char* what, VmmBuffer* out) {
+    VmmBuffer b;
+    b.bytes = bytes;
+    b.handle = h;
+    const char* call = "cuMemAddressReserve";
+    CUresult r = g_drv.MemAddressReserve(&b.va, bytes, FMA_PAGE_BYTES, 0, 0);
+    if (r == CUDA_SUCCESS) {
+        r = map_with_access(b.va, bytes, h, access_devices, &call);
+        if (r != CUDA_SUCCESS) g_drv.MemAddressFree(b.va, bytes);
+    }
+    if (r != CUDA_SUCCESS) {
+        g_drv.MemRelease(h);
+        return fail(FMA_ECUDA, "%s(%s) failed: %s", call, what, cu_err(r));
+    }
+    *out = b;
+    return FMA_OK;
+}
+
+void vmm_buffer_free(VmmBuffer& b) {
+    if (!b.va) return;
+    g_drv.MemUnmap(b.va, b.bytes);
+    g_drv.MemAddressFree(b.va, b.bytes);
+    g_drv.MemRelease(b.handle);
+    b = VmmBuffer{};
 }
 
 // ---- arenas ----------------------------------------------------------------------------------------
@@ -511,6 +564,35 @@ int host_store_reserve(fma_engine_t* e, size_t bytes) {
     return FMA_OK;
 }
 
+int open_path(WakePath& p, int slots) {
+    if (!p.remote) {
+        DeviceGuard g(p.device);
+        RT(cudaStreamCreateWithFlags(&p.copy, cudaStreamNonBlocking));
+        for (int i = 0; i < slots; ++i) RT(cudaEventCreateWithFlags(&p.ev_full[i], cudaEventDisableTiming));
+    }
+    RT(cudaStreamCreateWithFlags(&p.kern, cudaStreamNonBlocking));
+    for (int i = 0; i < slots; ++i) RT(cudaEventCreateWithFlags(&p.ev_free[i], cudaEventDisableTiming));
+    RT(cudaEventCreateWithFlags(&p.ev_done, cudaEventDisableTiming));
+    return FMA_OK;
+}
+
+void close_path(fma_engine_t* e, WakePath& p) {
+    if (!p.remote) {
+        DeviceGuard g(p.device);
+        if (p.copy) cudaStreamSynchronize(p.copy);
+        if (p.copy) cudaStreamDestroy(p.copy);
+        for (cudaEvent_t ev : p.ev_full)
+            if (ev) cudaEventDestroy(ev);
+    }
+    DeviceGuard g(e->device);
+    if (p.kern) cudaStreamSynchronize(p.kern);
+    if (p.kern) cudaStreamDestroy(p.kern);
+    for (cudaEvent_t ev : p.ev_free)
+        if (ev) cudaEventDestroy(ev);
+    if (p.ev_done) cudaEventDestroy(p.ev_done);
+    vmm_buffer_free(p.staging);
+}
+
 void paths_release(fma_engine_t* e) {
     if (e->mbox) {   // tell a helper that may still be pulling to stop, then let go of the mailbox
         e->mbox->abort.store(1);
@@ -519,45 +601,25 @@ void paths_release(fma_engine_t* e) {
     }
     if (e->mbox_fd >= 0) close(e->mbox_fd);
     e->mbox_fd = -1;
-    for (WakePath& p : e->paths) {
-        if (!p.remote) {
-            DeviceGuard g(p.device);
-            if (p.copy) cudaStreamSynchronize(p.copy);
-            if (p.copy) cudaStreamDestroy(p.copy);
-            for (int i = 0; i < kMaxRing; ++i)
-                if (p.ev_full[i]) cudaEventDestroy(p.ev_full[i]);
-        }
-        DeviceGuard g(e->device);
-        if (p.kern) cudaStreamSynchronize(p.kern);
-        if (p.kern) cudaStreamDestroy(p.kern);
-        for (int i = 0; i < kMaxRing; ++i)
-            if (p.ev_free[i]) cudaEventDestroy(p.ev_free[i]);
-        if (p.ev_done) cudaEventDestroy(p.ev_done);
-        if (p.va) {
-            g_drv.MemUnmap(p.va, p.bytes);
-            g_drv.MemAddressFree(p.va, p.bytes);
-        }
-        if (p.remote && p.handle) g_drv.MemRelease(p.handle);
-    }
+    for (WakePath& p : e->paths) close_path(e, p);
     e->paths.clear();
     e->path_slot_bytes = 0;
     e->path_slots = 0;
     cudaGetLastError();
 }
 
-void park_store_free(ParkStore& p) {
-    if (!p.va) return;
-    g_drv.MemUnmap(p.va, p.cap);
-    g_drv.MemRelease(p.handle);
-    g_drv.MemAddressFree(p.va, p.cap);
-    p = ParkStore{};
+int paths_fail(fma_engine_t* e, int rc) {
+    char keep[512];
+    snprintf(keep, sizeof(keep), "%s", tl_err);
+    paths_release(e);
+    return fail(rc, "%s", keep);
 }
 
 int park_release(fma_engine_t* e) {
     if (!e->park.va) return FMA_OK;
     if (e->shadow_tier != FMA_TIER_HOST) invalidate_shadows(e);  // the parking buffer held the kept image
     cudaDeviceSynchronize();
-    park_store_free(e->park);
+    vmm_buffer_free(e->park);
     return FMA_OK;
 }
 
@@ -576,60 +638,39 @@ int park_store_create(fma_engine_t* e, int device, size_t bytes, ParkStore* out)
         DeviceGuard g(device);
         RT(cudaFree(nullptr));
     }
-    ParkStore p;
-    p.device = device;
-    p.cap = bytes;
-    CUmemAllocationProp prop = device_prop(device);
-    DRV(g_drv.MemCreate(&p.handle, bytes, &prop, 0));
-    CUresult r = g_drv.MemAddressReserve(&p.va, bytes, FMA_PAGE_BYTES, 0, 0);
-    if (r != CUDA_SUCCESS) {
-        g_drv.MemRelease(p.handle);
-        return fail(FMA_ECUDA, "cuMemAddressReserve(park) failed: %s", cu_err(r));
-    }
-    r = g_drv.MemMap(p.va, bytes, 0, p.handle, 0);
-    if (r != CUDA_SUCCESS) {
-        g_drv.MemAddressFree(p.va, bytes);
-        g_drv.MemRelease(p.handle);
-        return fail(FMA_ECUDA, "cuMemMap(park) failed: %s", cu_err(r));
-    }
-    CUmemAccessDesc acc[2];
-    memset(acc, 0, sizeof(acc));
-    acc[0].location.type = CU_MEM_LOCATION_TYPE_DEVICE;
-    acc[0].location.id = e->device;
-    acc[0].flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;
-    acc[1] = acc[0];
-    acc[1].location.id = device;
-    r = g_drv.MemSetAccess(p.va, bytes, acc, device != e->device ? 2 : 1);
-    if (r != CUDA_SUCCESS) {
-        g_drv.MemUnmap(p.va, bytes);
-        g_drv.MemAddressFree(p.va, bytes);
-        g_drv.MemRelease(p.handle);
-        return fail(FMA_ECUDA, "cuMemSetAccess(park, P2P) failed: %s", cu_err(r));
-    }
-    *out = p;
+    CUmemGenericAllocationHandle h = 0;
+    RC(vmm_create(device, bytes, false, &h));
+    RC(vmm_buffer_map(h, bytes, {e->device, device}, "park", out));
+    out->device = device;
     return FMA_OK;
 }
 
 int park_reserve(fma_engine_t* e, int park_device, size_t bytes) {
     bytes = round_up(std::max<size_t>(bytes, FMA_PAGE_BYTES), e->gran);
-    if (e->park.va && e->park.device == park_device && e->park.cap >= bytes) return FMA_OK;
+    if (e->park.va && e->park.device == park_device && e->park.bytes >= bytes) return FMA_OK;
     park_release(e);
     return park_store_create(e, park_device, bytes, &e->park);
 }
 
 void resident_release(fma_engine_t* e) {
-    park_store_free(e->res);
+    vmm_buffer_free(e->res);
     e->res_packed = false;
     e->res_off.clear();
     e->res_bytes.clear();
     e->res_store_bytes = 0;
 }
 
-bool resident_asleep(fma_engine_t* e) {
-    if (!e->res.va) return false;
+bool image_in(fma_engine_t* e, ImageIn where) {
     std::lock_guard<std::mutex> lk(e->mu);
-    for (const Segment& s : e->segs)
-        if (s.has_backup && !s.mapped && s.backup_tier == FMA_TIER_LOCAL) return true;
+    for (const Segment& s : e->segs) {
+        if (!s.has_backup) continue;
+        switch (where) {
+            case ImageIn::Host: if (s.backup_tier == FMA_TIER_HOST) return true; break;
+            case ImageIn::NotHost: if (s.backup_tier != FMA_TIER_HOST) return true; break;
+            case ImageIn::Local: if (!s.mapped && s.backup_tier == FMA_TIER_LOCAL) return true; break;
+            case ImageIn::AnyAsleep: if (!s.mapped) return true; break;
+        }
+    }
     return false;
 }
 
@@ -1118,12 +1159,7 @@ int fma_swap(fma_engine_t* out_e, uint64_t offload_tag_mask, int tier, fma_engin
 int fma_host_reserve(fma_engine_t* e, size_t bytes) {
     if (check_engine(e) != FMA_OK) return FMA_EINVAL;
     std::lock_guard<std::mutex> op(e->op_mu);
-    {
-        std::lock_guard<std::mutex> lk(e->mu);
-        for (const Segment& s : e->segs)
-            if (s.has_backup && s.backup_tier == FMA_TIER_HOST && e->host.cap < bytes)
-                return fail(FMA_ESTATE, "cannot regrow the host store while it holds a sleeping image");
-    }
+    if (e->host.cap < bytes && image_in(e, ImageIn::Host)) return fail(FMA_ESTATE, "cannot regrow the host store while it holds a sleeping image");
     DeviceGuard guard(e->device);
     return host_store_reserve(e, bytes);
 }
@@ -1131,11 +1167,7 @@ int fma_host_reserve(fma_engine_t* e, size_t bytes) {
 int fma_host_release(fma_engine_t* e) {
     if (check_engine(e) != FMA_OK) return FMA_EINVAL;
     std::lock_guard<std::mutex> op(e->op_mu);
-    {
-        std::lock_guard<std::mutex> lk(e->mu);
-        for (const Segment& s : e->segs)
-            if (s.has_backup && s.backup_tier == FMA_TIER_HOST) return fail(FMA_ESTATE, "host store holds a sleeping image");
-    }
+    if (image_in(e, ImageIn::Host)) return fail(FMA_ESTATE, "host store holds a sleeping image");
     DeviceGuard guard(e->device);
     cudaDeviceSynchronize();
     invalidate_shadows(e);
@@ -1156,11 +1188,7 @@ int fma_host_store_view(fma_engine_t* e, const void** base, uint64_t* bytes) {
 int fma_peer_reserve(fma_engine_t* e, int peer_device, size_t bytes) {
     if (check_engine(e) != FMA_OK) return FMA_EINVAL;
     std::lock_guard<std::mutex> op(e->op_mu);
-    {
-        std::lock_guard<std::mutex> lk(e->mu);
-        for (const Segment& s : e->segs)
-            if (s.has_backup && s.backup_tier != FMA_TIER_HOST) return fail(FMA_ESTATE, "parking buffer holds a sleeping image");
-    }
+    if (image_in(e, ImageIn::NotHost)) return fail(FMA_ESTATE, "parking buffer holds a sleeping image");
     DeviceGuard guard(e->device);
     return park_reserve(e, peer_device, bytes);
 }
@@ -1168,11 +1196,7 @@ int fma_peer_reserve(fma_engine_t* e, int peer_device, size_t bytes) {
 int fma_peer_release(fma_engine_t* e) {
     if (check_engine(e) != FMA_OK) return FMA_EINVAL;
     std::lock_guard<std::mutex> op(e->op_mu);
-    {
-        std::lock_guard<std::mutex> lk(e->mu);
-        for (const Segment& s : e->segs)
-            if (s.has_backup && s.backup_tier != FMA_TIER_HOST) return fail(FMA_ESTATE, "parking buffer holds a sleeping image");
-    }
+    if (image_in(e, ImageIn::NotHost)) return fail(FMA_ESTATE, "parking buffer holds a sleeping image");
     DeviceGuard guard(e->device);
     return park_release(e);
 }
@@ -1211,7 +1235,7 @@ int fma_parking_create(int device, size_t bytes, uint64_t* out_handle, int* out_
     Parking p;
     p.bytes = bytes;
     p.device = device;
-    DRV(g_drv.MemCreate(&p.handle, bytes, &prop, 0));
+    RC(vmm_create(device, bytes, true, &p.handle));
     int fd = -1;
     CUresult r = g_drv.MemExportToShareableHandle(&fd, p.handle, CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR, 0);
     if (r != CUDA_SUCCESS) {
@@ -1250,41 +1274,15 @@ int fma_peer_attach(fma_engine_t* e, int fd, size_t bytes) {
     if (check_engine(e) != FMA_OK) return FMA_EINVAL;
     if (fd < 0 || bytes == 0 || bytes % FMA_PAGE_BYTES) return fail(FMA_EINVAL, "attach needs the owner's fd and the buffer's size (a multiple of 2 MiB)");
     std::lock_guard<std::mutex> op(e->op_mu);
-    {
-        std::lock_guard<std::mutex> lk(e->mu);
-        for (const Segment& s : e->segs)
-            if (s.has_backup && s.backup_tier != FMA_TIER_HOST) return fail(FMA_ESTATE, "parking buffer holds a sleeping image");
-    }
+    if (image_in(e, ImageIn::NotHost)) return fail(FMA_ESTATE, "parking buffer holds a sleeping image");
     DeviceGuard guard(e->device);
     RC(park_release(e));
-    ParkStore p;
-    p.device = kForeignDevice;
-    p.cap = bytes;
-    DRV(g_drv.MemImportFromShareableHandle(&p.handle, reinterpret_cast<void*>(static_cast<uintptr_t>(fd)), CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR));
-    CUresult r = g_drv.MemAddressReserve(&p.va, bytes, FMA_PAGE_BYTES, 0, 0);
-    if (r != CUDA_SUCCESS) {
-        g_drv.MemRelease(p.handle);
-        return fail(FMA_ECUDA, "cuMemAddressReserve(attach) failed: %s", cu_err(r));
-    }
-    r = g_drv.MemMap(p.va, bytes, 0, p.handle, 0);
-    if (r != CUDA_SUCCESS) {
-        g_drv.MemAddressFree(p.va, bytes);
-        g_drv.MemRelease(p.handle);
-        return fail(FMA_ECUDA, "cuMemMap(attach, %zu bytes) failed: %s (is `bytes` the size the owner created?)", bytes, cu_err(r));
-    }
-    CUmemAccessDesc acc;
-    memset(&acc, 0, sizeof(acc));
-    acc.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
-    acc.location.id = e->device;
-    acc.flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;
-    r = g_drv.MemSetAccess(p.va, bytes, &acc, 1);
-    if (r != CUDA_SUCCESS) {
-        g_drv.MemUnmap(p.va, bytes);
-        g_drv.MemAddressFree(p.va, bytes);
-        g_drv.MemRelease(p.handle);
-        return fail(FMA_ECUDA, "cuMemSetAccess(attach) failed: %s (no P2P path from device %d to the buffer's GPU?)", cu_err(r), e->device);
-    }
-    e->park = p;
+    CUmemGenericAllocationHandle h = 0;
+    RC(vmm_import(fd, &h));
+    char what[160];
+    snprintf(what, sizeof(what), "attach, %zu bytes: the size the owner created? a P2P path from device %d to the buffer's GPU?", bytes, e->device);
+    RC(vmm_buffer_map(h, bytes, {e->device}, what, &e->park));
+    e->park.device = kForeignDevice;
     return FMA_OK;
 }
 
@@ -1292,12 +1290,7 @@ int fma_peer_attach(fma_engine_t* e, int fd, size_t bytes) {
 // after it was pinned) is placed again: now, not inside the next sleep.  A store that holds an image, is shared or was adopted
 // stays as it is.
 static int replace_store_for_paths(fma_engine_t* e) {
-    bool image_in_store = false;
-    {
-        std::lock_guard<std::mutex> lk(e->mu);
-        for (const Segment& s : e->segs) image_in_store = image_in_store || (s.has_backup && s.backup_tier == FMA_TIER_HOST);
-    }
-    if (e->host.base && !image_in_store && !e->host.shared && e->host.fd < 0 && e->host.registered && e->host.placed_for != paths_signature(e)) {
+    if (e->host.base && !image_in(e, ImageIn::Host) && !e->host.shared && e->host.fd < 0 && e->host.registered && e->host.placed_for != paths_signature(e)) {
         const size_t cap = e->host.cap;
         if (e->shadow_tier == FMA_TIER_HOST) invalidate_shadows(e);
         host_store_free(e->host);
@@ -1332,48 +1325,24 @@ int fma_paths_set(fma_engine_t* e, const int* helper_devices, int n, size_t slot
     }
     e->path_slot_bytes = slot_bytes;
     e->path_slots = slots;
+    const size_t bytes = slot_bytes * (size_t)slots;
     for (int d : devs) {
-        WakePath p;
+        e->paths.emplace_back();
+        WakePath& p = e->paths.back();
         p.device = d;
         p.numa_node = gpu_numa_node(d);
-        p.bytes = slot_bytes * (size_t)slots;
+        char what[64];
+        snprintf(what, sizeof(what), "path staging on device %d", d);
+        CUmemGenericAllocationHandle h = 0;
         int rc = FMA_OK;
         {
             DeviceGuard g(d);
             if (cudaFree(nullptr) != cudaSuccess) rc = fail(FMA_ECUDA, "cannot initialise helper device %d", d);
-            CUmemAllocationProp prop = device_prop(d);
-            CUmemGenericAllocationHandle h = 0;
-            CUresult r = rc == FMA_OK ? g_drv.MemCreate(&h, p.bytes, &prop, 0) : CUDA_ERROR_UNKNOWN;
-            if (rc == FMA_OK && r != CUDA_SUCCESS) rc = fail(r == CUDA_ERROR_OUT_OF_MEMORY ? FMA_ENOMEM : FMA_ECUDA, "cuMemCreate(path staging on device %d) failed: %s", d, cu_err(r));
-            if (rc == FMA_OK) {
-                r = g_drv.MemAddressReserve(&p.va, p.bytes, FMA_PAGE_BYTES, 0, 0);
-                if (r == CUDA_SUCCESS) r = g_drv.MemMap(p.va, p.bytes, 0, h, 0);
-                CUmemAccessDesc acc[2];
-                memset(acc, 0, sizeof(acc));
-                acc[0].location.type = CU_MEM_LOCATION_TYPE_DEVICE;
-                acc[0].location.id = d;
-                acc[0].flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;
-                acc[1] = acc[0];
-                acc[1].location.id = e->device;
-                if (r == CUDA_SUCCESS) r = g_drv.MemSetAccess(p.va, p.bytes, acc, d != e->device ? 2 : 1);
-                g_drv.MemRelease(h);   // the mapping keeps the memory alive
-                if (r != CUDA_SUCCESS) rc = fail(FMA_ECUDA, "mapping the path staging buffer of device %d failed: %s", d, cu_err(r));
-            }
-            if (rc == FMA_OK && cudaStreamCreateWithFlags(&p.copy, cudaStreamNonBlocking) != cudaSuccess) rc = fail(FMA_ECUDA, "stream on helper %d", d);
-            for (int i = 0; i < slots && rc == FMA_OK; ++i)
-                if (cudaEventCreateWithFlags(&p.ev_full[i], cudaEventDisableTiming) != cudaSuccess) rc = fail(FMA_ECUDA, "event on helper %d", d);
+            if (rc == FMA_OK) rc = vmm_create(d, bytes, false, &h);
+            if (rc == FMA_OK) rc = vmm_buffer_map(h, bytes, {d, e->device}, what, &p.staging);
         }
-        if (rc == FMA_OK && cudaStreamCreateWithFlags(&p.kern, cudaStreamNonBlocking) != cudaSuccess) rc = fail(FMA_ECUDA, "kernel stream for path %d", d);
-        for (int i = 0; i < slots && rc == FMA_OK; ++i)
-            if (cudaEventCreateWithFlags(&p.ev_free[i], cudaEventDisableTiming) != cudaSuccess) rc = fail(FMA_ECUDA, "event for path %d", d);
-        if (rc == FMA_OK && cudaEventCreateWithFlags(&p.ev_done, cudaEventDisableTiming) != cudaSuccess) rc = fail(FMA_ECUDA, "event for path %d", d);
-        e->paths.push_back(p);   // also on failure: paths_release below frees what exists
-        if (rc != FMA_OK) {
-            char keep[512];
-            snprintf(keep, sizeof(keep), "%s", tl_err);
-            paths_release(e);
-            return fail(rc, "%s", keep);
-        }
+        if (rc == FMA_OK) rc = open_path(p, slots);
+        if (rc != FMA_OK) return paths_fail(e, rc);
     }
     return replace_store_for_paths(e);
 }
@@ -1503,10 +1472,7 @@ int fma_op_page_digest(fma_engine_t* e, const uint64_t* pages, uint64_t base, co
 // ---- PACKED image: page layout query + raw K4p / K4 / K5 ----------------------------------------------------
 int fma_image_pages(fma_engine_t* e, uint64_t* out_offsets, uint32_t* out_bytes, uint32_t cap) {
     if (check_engine(e) != FMA_OK) return FMA_EINVAL;
-    bool asleep = false;
-    for (const Segment& s : e->segs)
-        if (s.has_backup && !s.mapped) asleep = true;
-    if (!asleep) return 0;
+    if (!image_in(e, ImageIn::AnyAsleep)) return 0;
     const size_t n = e->image_bytes / FMA_PAGE_BYTES;
     for (size_t p = 0; p < n && p < cap; ++p) {
         if (out_offsets) out_offsets[p] = e->image_packed ? e->img_off[p] : (uint64_t)p * FMA_PAGE_BYTES;
@@ -1674,11 +1640,11 @@ int fma_stats(fma_engine_t* e, fma_stats_t* out) {
     }
     uint64_t own_staging = 0;   // multi-path staging slots that live in THIS GPU's HBM (helpers' slots are their GPUs' business)
     for (const WakePath& wp : e->paths)
-        if (!wp.remote && wp.device == e->device) own_staging += wp.bytes;
+        if (!wp.remote && wp.device == e->device) own_staging += wp.staging.bytes;
     out->hbm_aux_bytes = own_staging + (e->ring_attached ? 0 : (uint64_t)e->n_ring * e->ring_slot_bytes) + 2 * e->d_tab_cap * sizeof(uint64_t) +
                          e->desc_cap * (sizeof(fma_k_page_desc) + sizeof(uint64_t)) +
                          e->pdesc_cap * (sizeof(fma_k_pack_desc) + sizeof(uint32_t));
-    out->parked_bytes = e->park.cap;
+    out->parked_bytes = e->park.bytes;
     out->image_packed = e->image_packed ? 1 : 0;
     out->image_store_bytes = e->image_store_bytes;
     out->resident_bytes = e->res.va ? e->res_store_bytes : 0;

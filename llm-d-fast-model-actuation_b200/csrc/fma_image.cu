@@ -262,7 +262,7 @@ int fma_image_adopt_parked(fma_engine_t* e, const void* desc, size_t desc_bytes,
             if (!s.mapped) return fail(FMA_ESTATE, "adopt needs a fully awake engine");
     }
     ParsedImage pi;
-    RC(image_descriptor_parse(e, static_cast<const char*>(desc), desc_bytes, e->park.cap, tag_mask, &pi));
+    RC(image_descriptor_parse(e, static_cast<const char*>(desc), desc_bytes, e->park.bytes, tag_mask, &pi));
     DeviceGuard guard(e->device);
     cudaDeviceSynchronize();
     if (flags & FMA_FLAG_VERIFY) {  // "sleep by adoption" (see fma_image_adopt): only if this engine's bytes ARE the image's

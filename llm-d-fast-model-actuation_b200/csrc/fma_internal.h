@@ -21,6 +21,7 @@
 #include <cstdlib>
 #include <cerrno>
 #include <cstring>
+#include <initializer_list>
 #include <iterator>
 #include <map>
 #include <mutex>
@@ -178,12 +179,15 @@ struct ImageHeader {
 };
 constexpr uint32_t kFlagAdopt = 1u << 31;  // internal: "sleep" onto an adopted image without copying
 
+struct VmmBuffer {  // one VMM allocation, mapped at a VA of its own; it keeps its handle until vmm_buffer_free
+    CUdeviceptr va = 0;
+    size_t bytes = 0;
+    CUmemGenericAllocationHandle handle = 0;
+};
+
 constexpr int kForeignDevice = -2;  // ParkStore::device of an attached buffer: it lives on a GPU this process may not even see
 
-struct ParkStore {  // peer-HBM or local-HBM parking buffer (VMM, P2P mapped)
-    CUdeviceptr va = 0;
-    size_t cap = 0;
-    CUmemGenericAllocationHandle handle = 0;
+struct ParkStore : VmmBuffer {  // peer-HBM or local-HBM parking buffer (P2P mapped), or the resident share
     int device = -1;            // kForeignDevice: imported from a node-level owner's fd (fma_peer_attach)
 };
 
@@ -198,10 +202,8 @@ constexpr int kMaxPaths = 8;
 struct WakePath {
     int device = -1;                         // -1 for a REMOTE path: a helper GPU this process cannot see (fma_paths_attach)
     bool remote = false;                     // the node-level owner drives the H2D into this path's slots (fma_pull.h)
-    CUmemGenericAllocationHandle handle = 0; // remote: the imported staging allocation
     int numa_node = -1;                      // of `device` (sysfs); -1 unknown
-    CUdeviceptr va = 0;                      // n_slots x slot_bytes in `device`'s HBM; access for `device` and the engine's GPU
-    size_t bytes = 0;
+    VmmBuffer staging;                       // n_slots x slot_bytes in `device`'s HBM (remote: imported); access for `device` and the engine's GPU
     cudaStream_t copy = nullptr;             // on `device`: H2D host store -> slot
     cudaStream_t kern = nullptr;             // on the engine's GPU: K2 slot -> destination pages
     cudaEvent_t ev_full[kMaxRing] = {};      // on `device`
@@ -353,6 +355,14 @@ int check_engine(fma_engine_t* e);
 
 // ---- VMM primitives, arenas (fma_engine.cu) ----
 int vmm_create_and_map(int device, CUdeviceptr va, size_t bytes);
+// A VMM buffer is made in two steps: a handle (created on `device`, exportable as a POSIX fd or not; or imported from an fd),
+// then vmm_buffer_map.  Out of memory in the first step is FMA_ENOMEM; every other failure is FMA_ECUDA.
+int vmm_create(int device, size_t bytes, bool exportable, CUmemGenericAllocationHandle* out);
+int vmm_import(int fd, CUmemGenericAllocationHandle* out);
+// Reserves a VA of its own for `h`, maps it and grants `access_devices` read/write access (a device listed twice once).  Takes `h`:
+// on failure nothing is left, `h` included, and the message names `what`.
+int vmm_buffer_map(CUmemGenericAllocationHandle h, size_t bytes, std::initializer_list<int> access_devices, const char* what, VmmBuffer* out);
+void vmm_buffer_free(VmmBuffer& b);   // unmap, release, free the VA; an empty buffer is left as it is
 int unmap_units(fma_engine_t* e, CUdeviceptr va, size_t span_bytes);
 // drop the (unmapped) units in [va, va + bytes) from the table: zombies' VA back to their arenas, an attached ring detached
 void forget_units(fma_engine_t* e, CUdeviceptr va, size_t bytes);
@@ -374,13 +384,26 @@ int ensure_event_pool(fma_engine_t* e, size_t n);
 void host_store_free(HostStore& h);
 int gpu_numa_node(int device);
 int host_store_reserve(fma_engine_t* e, size_t bytes);
+// A wake path's streams and events for `slots` slots: a local path's copy stream and ev_full on its GPU, then the kernel stream,
+// ev_free and ev_done on the current GPU (the engine's).  On failure the caller closes the path.
+int open_path(WakePath& p, int slots);
+void close_path(fma_engine_t* e, WakePath& p);   // undoes open_path, whatever of it was done, and frees the path's staging
 void paths_release(fma_engine_t* e);
+int paths_fail(fma_engine_t* e, int rc);         // fma_paths_set / fma_paths_attach failed: release every path, keep the message
 int park_release(fma_engine_t* e);
 int park_reserve(fma_engine_t* e, int park_device, size_t bytes);
 int park_store_create(fma_engine_t* e, int device, size_t bytes, ParkStore* out);   // one VMM allocation, mapped for e's GPU (+ device's)
-void park_store_free(ParkStore& p);
 void resident_release(fma_engine_t* e);              // drop the resident buffer (caller: nothing on the device still reads it)
-bool resident_asleep(fma_engine_t* e);               // a sleeping image keeps part of itself in the resident buffer
+// Does a segment's image live in the store `where` names (takes e->mu)?
+enum class ImageIn {
+    Host,           // the host store
+    NotHost,        // the parking buffer: any tier but the host's, so a resident share (FMA_TIER_LOCAL) counts too
+    Local,          // FMA_TIER_LOCAL, with the segment unmapped
+    AnyAsleep,      // any store, with the segment unmapped
+};
+bool image_in(fma_engine_t* e, ImageIn where);
+// a sleeping image keeps part of itself in the resident buffer
+inline bool resident_asleep(fma_engine_t* e) { return e->res.va && image_in(e, ImageIn::Local); }
 CUmemAllocationProp device_prop(int device);
 // ---- image descriptor (fma_image.cu): what a sleeping image is made of, so another engine / process can adopt it ----
 int image_descriptor_build(fma_engine_t* e, int tier, std::vector<char>* out);

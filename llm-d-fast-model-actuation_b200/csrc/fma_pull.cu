@@ -11,9 +11,7 @@ struct HelperStaging {   // owner side: n_slots x slot_bytes in one helper GPU's
     int device = -1;
     size_t slot_bytes = 0;
     int slots = 0;
-    CUmemGenericAllocationHandle handle = 0;
-    CUdeviceptr va = 0;
-    size_t bytes = 0;
+    VmmBuffer buf;
     cudaStream_t copy = nullptr;
     cudaEvent_t ev[kMaxRing] = {};
     std::atomic<int> users{0};          // pulls running on this staging buffer right now
@@ -41,6 +39,17 @@ PullMailbox* map_mailbox(int fd) {
 
 void nap() { std::this_thread::sleep_for(std::chrono::microseconds(20)); }
 
+// what fma_helper_open made, whatever of it exists
+void helper_free(HelperStaging& h) {
+    DeviceGuard guard(h.device);
+    if (h.copy) cudaStreamSynchronize(h.copy);
+    if (h.copy) cudaStreamDestroy(h.copy);
+    for (cudaEvent_t ev : h.ev)
+        if (ev) cudaEventDestroy(ev);
+    vmm_buffer_free(h.buf);
+    cudaGetLastError();
+}
+
 }  // namespace
 
 extern "C" {
@@ -61,28 +70,24 @@ int fma_helper_open(int device, size_t slot_bytes, int slots, uint64_t* out_hand
     h.device = device;
     h.slot_bytes = slot_bytes;
     h.slots = slots;
-    h.bytes = slot_bytes * (size_t)slots;
-    CUmemAllocationProp prop = device_prop(device);
-    prop.requestedHandleTypes = CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR;
-    DRV(g_drv.MemCreate(&h.handle, h.bytes, &prop, 0));
+    const size_t bytes = slot_bytes * (size_t)slots;
+    char what[64];
+    snprintf(what, sizeof(what), "helper staging on device %d", device);
+    CUmemGenericAllocationHandle handle = 0;
+    RC(vmm_create(device, bytes, true, &handle));
+    RC(vmm_buffer_map(handle, bytes, {device}, what, &h.buf));
     int fd = -1;
-    CUresult r = g_drv.MemExportToShareableHandle(&fd, h.handle, CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR, 0);
-    if (r == CUDA_SUCCESS) r = g_drv.MemAddressReserve(&h.va, h.bytes, FMA_PAGE_BYTES, 0, 0);
-    if (r == CUDA_SUCCESS) r = g_drv.MemMap(h.va, h.bytes, 0, h.handle, 0);
-    CUmemAccessDesc acc;
-    memset(&acc, 0, sizeof(acc));
-    acc.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
-    acc.location.id = device;
-    acc.flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;
-    if (r == CUDA_SUCCESS) r = g_drv.MemSetAccess(h.va, h.bytes, &acc, 1);
-    if (r != CUDA_SUCCESS) {
-        if (h.va) { g_drv.MemUnmap(h.va, h.bytes); g_drv.MemAddressFree(h.va, h.bytes); }
-        g_drv.MemRelease(h.handle);
+    int rc = FMA_OK;
+    const CUresult r = g_drv.MemExportToShareableHandle(&fd, h.buf.handle, CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR, 0);
+    if (r != CUDA_SUCCESS) rc = fail(FMA_ECUDA, "cuMemExportToShareableHandle(%s) failed: %s", what, cu_err(r));
+    if (rc == FMA_OK && cudaStreamCreateWithFlags(&h.copy, cudaStreamNonBlocking) != cudaSuccess) rc = fail(FMA_ECUDA, "copy stream on helper device %d", device);
+    for (int i = 0; i < slots && rc == FMA_OK; ++i)
+        if (cudaEventCreateWithFlags(&h.ev[i], cudaEventDisableTiming) != cudaSuccess) rc = fail(FMA_ECUDA, "event on helper device %d", device);
+    if (rc != FMA_OK) {
+        helper_free(h);
         if (fd >= 0) close(fd);
-        return fail(FMA_ECUDA, "helper staging on device %d failed: %s", device, cu_err(r));
+        return rc;
     }
-    RT(cudaStreamCreateWithFlags(&h.copy, cudaStreamNonBlocking));
-    for (int i = 0; i < slots; ++i) RT(cudaEventCreateWithFlags(&h.ev[i], cudaEventDisableTiming));
     std::lock_guard<std::mutex> lk(g_mu);
     *out_handle = g_next++;
     g_helpers[*out_handle] = hp;
@@ -102,14 +107,7 @@ int fma_helper_close(uint64_t handle) {
     HelperStaging& h = *hp;
     h.closing.store(true);
     while (h.users.load() > 0) nap();   // a pull notices `closing` within one poll interval (or one chunk copy)
-    DeviceGuard guard(h.device);
-    cudaStreamSynchronize(h.copy);
-    cudaStreamDestroy(h.copy);
-    for (int i = 0; i < h.slots; ++i) cudaEventDestroy(h.ev[i]);
-    g_drv.MemUnmap(h.va, h.bytes);
-    g_drv.MemAddressFree(h.va, h.bytes);
-    g_drv.MemRelease(h.handle);
-    cudaGetLastError();
+    helper_free(h);
     return FMA_OK;
 }
 
@@ -259,7 +257,7 @@ int fma_helper_pull(uint64_t helper, uint64_t store, int mailbox_fd, int path_in
                 } else {
                     const PullChunk ch = mb->chunks[c];
                     if (ch.store_off + ch.bytes > st.bytes || ch.bytes > h.slot_bytes) { rc = fail(FMA_EINVAL, "chunk %u is outside the store / larger than a slot", c); break; }
-                    cudaError_t ce = cudaMemcpyAsync(reinterpret_cast<void*>(h.va + (size_t)slot * h.slot_bytes), static_cast<char*>(st.base) + ch.store_off, ch.bytes,
+                    cudaError_t ce = cudaMemcpyAsync(reinterpret_cast<void*>(h.buf.va + (size_t)slot * h.slot_bytes), static_cast<char*>(st.base) + ch.store_off, ch.bytes,
                                                      cudaMemcpyDefault, h.copy);
                     if (ce == cudaSuccess) ce = cudaEventRecord(h.ev[slot], h.copy);
                     if (ce != cudaSuccess) { rc = fail(FMA_ECUDA, "H2D on helper device %d failed: %s", h.device, cudaGetErrorString(ce)); break; }
@@ -307,53 +305,27 @@ int fma_paths_attach(fma_engine_t* e, const int* staging_fds, int n, size_t slot
     paths_release(e);
     e->path_slot_bytes = slot_bytes;
     e->path_slots = slots;
-    int rc = FMA_OK;
-    for (int i = -1; i < n && rc == FMA_OK; ++i) {   // i == -1: the engine's own link (a local path, as in fma_paths_set)
-        WakePath p;
-        p.bytes = slot_bytes * (size_t)slots;
-        CUmemAccessDesc acc;
-        memset(&acc, 0, sizeof(acc));
-        acc.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
-        acc.location.id = e->device;
-        acc.flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;
-        CUresult r;
-        if (i < 0) {
+    const size_t bytes = slot_bytes * (size_t)slots;
+    for (int i = -1; i < n; ++i) {   // i == -1: the engine's own link (a local path, as in fma_paths_set)
+        e->paths.emplace_back();
+        WakePath& p = e->paths.back();
+        p.remote = i >= 0;
+        if (!p.remote) {
             p.device = e->device;
             p.numa_node = gpu_numa_node(e->device);
-            CUmemAllocationProp prop = device_prop(e->device);
-            r = g_drv.MemCreate(&p.handle, p.bytes, &prop, 0);
-        } else {
-            p.remote = true;
-            r = g_drv.MemImportFromShareableHandle(&p.handle, reinterpret_cast<void*>(static_cast<uintptr_t>(staging_fds[i])), CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR);
         }
-        if (r == CUDA_SUCCESS) r = g_drv.MemAddressReserve(&p.va, p.bytes, FMA_PAGE_BYTES, 0, 0);
-        if (r == CUDA_SUCCESS) r = g_drv.MemMap(p.va, p.bytes, 0, p.handle, 0);
-        if (r == CUDA_SUCCESS) r = g_drv.MemSetAccess(p.va, p.bytes, &acc, 1);
-        if (r != CUDA_SUCCESS) rc = fail(FMA_ECUDA, "mapping the staging buffer of path %d failed: %s", i + 1, cu_err(r));
-        if (i < 0 && p.handle) {   // a local mapping keeps its memory alive; a remote one keeps the imported handle until release
-            g_drv.MemRelease(p.handle);
-            p.handle = 0;
-        }
-        if (rc == FMA_OK && i < 0 && cudaStreamCreateWithFlags(&p.copy, cudaStreamNonBlocking) != cudaSuccess) rc = fail(FMA_ECUDA, "copy stream");
-        for (int s = 0; s < slots && rc == FMA_OK && i < 0; ++s)
-            if (cudaEventCreateWithFlags(&p.ev_full[s], cudaEventDisableTiming) != cudaSuccess) rc = fail(FMA_ECUDA, "event");
-        if (rc == FMA_OK && cudaStreamCreateWithFlags(&p.kern, cudaStreamNonBlocking) != cudaSuccess) rc = fail(FMA_ECUDA, "kernel stream");
-        for (int s = 0; s < slots && rc == FMA_OK; ++s)
-            if (cudaEventCreateWithFlags(&p.ev_free[s], cudaEventDisableTiming) != cudaSuccess) rc = fail(FMA_ECUDA, "event");
-        if (rc == FMA_OK && cudaEventCreateWithFlags(&p.ev_done, cudaEventDisableTiming) != cudaSuccess) rc = fail(FMA_ECUDA, "event");
-        e->paths.push_back(p);
+        char what[64];
+        snprintf(what, sizeof(what), "staging buffer of path %d", i + 1);
+        CUmemGenericAllocationHandle h = 0;
+        int rc = p.remote ? vmm_import(staging_fds[i], &h) : vmm_create(e->device, bytes, false, &h);
+        if (rc == FMA_OK) rc = vmm_buffer_map(h, bytes, {e->device}, what, &p.staging);
+        if (rc == FMA_OK) rc = open_path(p, slots);
+        if (rc != FMA_OK) return paths_fail(e, rc);
     }
-    if (rc == FMA_OK) {
-        e->mbox_fd = (int)syscall(SYS_memfd_create, "fma-pull-mailbox", 1u);
-        if (e->mbox_fd < 0 || ftruncate(e->mbox_fd, (off_t)sizeof(PullMailbox)) != 0) rc = fail(FMA_ENOMEM, "cannot create the mailbox: %s", strerror(errno));
-        else if (!(e->mbox = map_mailbox(e->mbox_fd))) rc = fail(FMA_ENOMEM, "cannot map the mailbox");
-    }
-    if (rc != FMA_OK) {
-        char keep[512];
-        snprintf(keep, sizeof(keep), "%s", tl_err);
-        paths_release(e);
-        return fail(rc, "%s", keep);
-    }
+    e->mbox_fd = (int)syscall(SYS_memfd_create, "fma-pull-mailbox", 1u);
+    if (e->mbox_fd < 0 || ftruncate(e->mbox_fd, (off_t)sizeof(PullMailbox)) != 0)
+        return paths_fail(e, fail(FMA_ENOMEM, "cannot create the mailbox: %s", strerror(errno)));
+    if (!(e->mbox = map_mailbox(e->mbox_fd))) return paths_fail(e, fail(FMA_ENOMEM, "cannot map the mailbox"));
     PullMailbox* mb = e->mbox;   // a fresh memfd is zero-filled: atomics start at 0
     mb->version = kPullVersion;
     mb->n_slots = (uint32_t)slots;

@@ -470,7 +470,7 @@ int SleepPipe::multipath() {
                 ce = cudaEventSynchronize(path.ev_full[slot]);
                 if (ce != cudaSuccess) return failw(FMA_ECUDA, "cudaEventSynchronize(slot drained)", ce);
             }
-            char* slot_ptr = reinterpret_cast<char*>(path.va) + (size_t)slot * e->path_slot_bytes;
+            char* slot_ptr = reinterpret_cast<char*>(path.staging.va) + (size_t)slot * e->path_slot_bytes;
             {
                 std::lock_guard<std::mutex> lk(kt_mu);
                 const int krc = kt.launch_on(path.kern, e->d_tab + ch.p0, 0, nullptr, (uint64_t)(uintptr_t)slot_ptr, (uint32_t)ch.np);   // K1: gather -> slot
@@ -603,7 +603,7 @@ int split_resident(fma_engine_t* e, SleepPlan& p) {
         cudaGetLastError();
         return FMA_OK;
     }
-    e->tl_add("res_alloc", 0, a, b, buf.cap);
+    e->tl_add("res_alloc", 0, a, b, buf.bytes);
     // the two parts, each laid out back to back in image order: [0] the host store, [1] the resident buffer
     struct Part {
         std::vector<Extent> ex;
@@ -656,7 +656,7 @@ int check_incremental(fma_engine_t* e, SleepPlan& p) {
     p.shadows_match = p.shadows_match && p.res_seqs == e->res_seqs;  // a different split is a full sleep
     e->res_seqs = p.res_seqs;
     const uint64_t W = p.W;
-    if (!p.shadows_match || !W || W != e->shadow_image_bytes || (p.tier == FMA_TIER_HOST ? e->host.cap : e->park.cap) < e->shadow_store_bytes) return FMA_OK;
+    if (!p.shadows_match || !W || W != e->shadow_image_bytes || (p.tier == FMA_TIER_HOST ? e->host.cap : e->park.bytes) < e->shadow_store_bytes) return FMA_OK;
     RT(cudaDeviceSynchronize());  // the caller's streams may still be writing weights
     std::vector<uint64_t> now;
     RC(digest_and_mark(e, p.ex, &now));  // either way these are the digests of what sleeps now
@@ -727,7 +727,7 @@ int size_store(fma_engine_t* e, const SleepPlan& p) {
         RC(host_store_reserve(e, p.Wp));
         if (p.route.mode == FMA_MODE_KERNEL && !e->host.dev_alias) return fail(FMA_ECUDA, "host store has no device alias for zero-copy mode");
     } else if (p.tier == FMA_TIER_PEER) {
-        if (!e->park.va || e->park.cap < p.Wp || e->park.device == e->device)
+        if (!e->park.va || e->park.bytes < p.Wp || e->park.device == e->device)
             return fail(FMA_ESTATE, "peer tier needs fma_peer_reserve(peer_device, >= %llu bytes) first", (unsigned long long)p.Wp);
     } else if (p.tier == FMA_TIER_LOCAL) {
         return park_reserve(e, e->device, p.Wp);

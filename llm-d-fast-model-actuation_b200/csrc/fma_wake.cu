@@ -516,7 +516,7 @@ int WakePipe::multipath() {
                     const Batch& ch = chunks[c];
                     const int mrc = mapper.wait_mapped(ch.need);
                     if (mrc != FMA_OK) return failw(mrc, "mapping", cudaSuccess);
-                    char* slot_ptr = reinterpret_cast<char*>(path.va) + (size_t)slot * e->path_slot_bytes;
+                    char* slot_ptr = reinterpret_cast<char*>(path.staging.va) + (size_t)slot * e->path_slot_bytes;
                     {
                         std::lock_guard<std::mutex> lk(kt_mu);
                         const int krc = kt.launch_on(path.kern, nullptr, (uint64_t)(uintptr_t)slot_ptr, e->d_tab + ch.p0, 0, (uint32_t)ch.np);
@@ -556,7 +556,7 @@ int WakePipe::multipath() {
                 ce = cudaEventSynchronize(path.ev_free[slot]);
                 if (ce != cudaSuccess) return failw(FMA_ECUDA, "cudaEventSynchronize(slot free)", ce);
             }
-            char* slot_ptr = reinterpret_cast<char*>(path.va) + (size_t)slot * e->path_slot_bytes;
+            char* slot_ptr = reinterpret_cast<char*>(path.staging.va) + (size_t)slot * e->path_slot_bytes;
             ce = cudaMemcpyAsync(slot_ptr, store + chunk_off[c], ch.stored, cudaMemcpyDefault, path.copy);
             if (ce != cudaSuccess) return failw(FMA_ECUDA, "cudaMemcpyAsync(H2D)", ce);
             if (!first_copy_seen.exchange(true)) first_copy_delay = now_s() - t_entry;
@@ -795,7 +795,7 @@ int do_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags) {
         if (!still_asleep) {
             if (res.next) RT(cudaEventSynchronize(e->ev_res_done));
             const double a = now_s();
-            const uint64_t cap = e->res.cap;
+            const uint64_t cap = e->res.bytes;
             {
                 GateHold hold(kGateUnmap, 0.1);
                 resident_release(e);

@@ -12,6 +12,8 @@
 //   a range spanning several whole mappings is accepted, a sub-range is CUDA_ERROR_INVALID_VALUE (as the driver does,
 //   scripts/vmm_span_probe.py); memory lives until unmap even if the handle was released right after cuMemMap.
 // Streams execute eagerly (a copy has happened when cudaMemcpyAsync returns); events record wall-clock time.
+// Fault injection: the Nth cuMemCreate (hostsim_fail_create_after), large cudaMemcpyAsync (hostsim_fail_memcpy_after) or call
+// of a named VMM / stream / event function (hostsim_fail_call_after) from now fails as if the device were out of memory.
 #include <cuda.h>
 #include <cuda_runtime.h>
 
@@ -28,6 +30,7 @@
 #include <map>
 #include <mutex>
 #include <set>
+#include <string>
 
 namespace {
 std::mutex g_mu;
@@ -42,6 +45,15 @@ thread_local int tl_device = 0;
 thread_local cudaError_t tl_last = cudaSuccess;
 std::atomic<long> g_fail_create_after{-1};                    // fault injection: fail the Nth cuMemCreate from now
 std::atomic<long> g_fail_memcpy_after{-1};                    // fault injection: fail the Nth large cudaMemcpyAsync from now
+std::map<std::string, long> g_fail_call_after;                // fault injection by call name: fail its Nth call from now (g_mu)
+
+// true when this call of `name` is the one hostsim_fail_call_after picked
+bool injected(const char* name) {
+    std::lock_guard<std::mutex> lk(g_mu);
+    auto it = g_fail_call_after.find(name);
+    if (it == g_fail_call_after.end() || it->second < 0) return false;
+    return it->second-- == 0;
+}
 
 int device_count() {
     const char* v = getenv("HOSTSIM_DEVICES");
@@ -60,6 +72,7 @@ CUresult simMemGetAllocationGranularity(size_t* g, const CUmemAllocationProp*, C
     return CUDA_SUCCESS;
 }
 CUresult simMemAddressReserve(CUdeviceptr* ptr, size_t size, size_t, CUdeviceptr, unsigned long long) {
+    if (injected("cuMemAddressReserve")) return CUDA_ERROR_OUT_OF_MEMORY;
     void* p = mmap(nullptr, size, PROT_NONE, MAP_PRIVATE | MAP_ANONYMOUS | MAP_NORESERVE, -1, 0);
     if (p == MAP_FAILED) return CUDA_ERROR_OUT_OF_MEMORY;
     // 2 MiB alignment like the driver: over-reserve is unnecessary for tests (mmap of GiB-sized ranges is 2 MiB aligned
@@ -101,6 +114,7 @@ CUresult simMemCreate(CUmemGenericAllocationHandle* h, size_t size, const CUmemA
     return CUDA_SUCCESS;
 }
 CUresult simMemExportToShareableHandle(void* out, CUmemGenericAllocationHandle h, CUmemAllocationHandleType t, unsigned long long) {
+    if (injected("cuMemExportToShareableHandle")) return CUDA_ERROR_OUT_OF_MEMORY;
     std::lock_guard<std::mutex> lk(g_mu);
     if (t != CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR || !g_handle_fd.count(h)) return CUDA_ERROR_INVALID_VALUE;
     const int fd = dup(g_handle_fd[h]);
@@ -109,6 +123,7 @@ CUresult simMemExportToShareableHandle(void* out, CUmemGenericAllocationHandle h
     return CUDA_SUCCESS;
 }
 CUresult simMemImportFromShareableHandle(CUmemGenericAllocationHandle* h, void* os_handle, CUmemAllocationHandleType t) {
+    if (injected("cuMemImportFromShareableHandle")) return CUDA_ERROR_OUT_OF_MEMORY;
     if (t != CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR) return CUDA_ERROR_INVALID_VALUE;
     const int fd = dup((int)(uintptr_t)os_handle);
     struct stat sb;
@@ -135,6 +150,7 @@ CUresult simMemRelease(CUmemGenericAllocationHandle h) {
     return CUDA_SUCCESS;
 }
 CUresult simMemMap(CUdeviceptr ptr, size_t size, size_t offset, CUmemGenericAllocationHandle h, unsigned long long) {
+    if (injected("cuMemMap")) return CUDA_ERROR_OUT_OF_MEMORY;
     std::lock_guard<std::mutex> lk(g_mu);
     if (offset != 0 || !g_handles.count(h) || g_handles[h] != size) return CUDA_ERROR_INVALID_VALUE;
     bool inside = false;
@@ -149,6 +165,7 @@ CUresult simMemMap(CUdeviceptr ptr, size_t size, size_t offset, CUmemGenericAllo
     return CUDA_SUCCESS;
 }
 CUresult simMemSetAccess(CUdeviceptr ptr, size_t size, const CUmemAccessDesc* desc, size_t n) {
+    if (injected("cuMemSetAccess")) return CUDA_ERROR_OUT_OF_MEMORY;
     std::lock_guard<std::mutex> lk(g_mu);
     auto it = g_mappings.find(ptr);
     if (it == g_mappings.end() || it->second.bytes != size || !desc || !n) return CUDA_ERROR_INVALID_VALUE;
@@ -188,7 +205,16 @@ extern "C" __attribute__((visibility("default"))) unsigned long long hostsim_liv
     std::lock_guard<std::mutex> lk(g_mu);
     return g_handles.size();
 }
+extern "C" __attribute__((visibility("default"))) unsigned long long hostsim_live_reservations() {
+    std::lock_guard<std::mutex> lk(g_mu);
+    return g_reservations.size();
+}
 extern "C" __attribute__((visibility("default"))) void hostsim_fail_create_after(long n) { g_fail_create_after.store(n); }
+// fail the Nth call of `name` ("cuMemMap", "cudaEventCreateWithFlags", ...) from now; n < 0 disarms it
+extern "C" __attribute__((visibility("default"))) void hostsim_fail_call_after(const char* name, long n) {
+    std::lock_guard<std::mutex> lk(g_mu);
+    g_fail_call_after[name] = n;
+}
 extern "C" __attribute__((visibility("default"))) void hostsim_fail_memcpy_after(long n) { g_fail_memcpy_after.store(n); }
 static std::atomic<long long> g_malloc_limit{0};  // > 0: cudaMalloc of more bytes fails ("HBM full": no staging ring)
 extern "C" __attribute__((visibility("default"))) void hostsim_malloc_limit(long long bytes) { g_malloc_limit.store(bytes); }
@@ -213,12 +239,12 @@ cudaError_t cudaHostRegister(void*, size_t, unsigned) {
 }
 cudaError_t cudaHostUnregister(void*) { return cudaSuccess; }
 cudaError_t cudaHostGetDevicePointer(void** d, void* h, unsigned) { *d = h; return cudaSuccess; }
-cudaError_t cudaStreamCreateWithFlags(cudaStream_t* s, unsigned) { *s = (cudaStream_t) new Stream(); return cudaSuccess; }
+cudaError_t cudaStreamCreateWithFlags(cudaStream_t* s, unsigned) { if (injected("cudaStreamCreateWithFlags")) return tl_last = cudaErrorMemoryAllocation; *s = (cudaStream_t) new Stream(); return cudaSuccess; }
 cudaError_t cudaStreamDestroy(cudaStream_t s) { delete (Stream*)s; return cudaSuccess; }
 cudaError_t cudaStreamSynchronize(cudaStream_t) { return cudaSuccess; }
 cudaError_t cudaStreamWaitEvent(cudaStream_t, cudaEvent_t, unsigned) { return cudaSuccess; }
 cudaError_t cudaEventCreate(cudaEvent_t* e) { *e = (cudaEvent_t) new Event(); return cudaSuccess; }
-cudaError_t cudaEventCreateWithFlags(cudaEvent_t* e, unsigned) { *e = (cudaEvent_t) new Event(); return cudaSuccess; }
+cudaError_t cudaEventCreateWithFlags(cudaEvent_t* e, unsigned) { if (injected("cudaEventCreateWithFlags")) return tl_last = cudaErrorMemoryAllocation; *e = (cudaEvent_t) new Event(); return cudaSuccess; }
 cudaError_t cudaEventDestroy(cudaEvent_t e) { delete (Event*)e; return cudaSuccess; }
 cudaError_t cudaEventRecord(cudaEvent_t e, cudaStream_t) { ((Event*)e)->t_ms = now_ms(); return cudaSuccess; }
 cudaError_t cudaEventSynchronize(cudaEvent_t) { return cudaSuccess; }

@@ -9,7 +9,9 @@ streams) and host stand-ins for the kernel launch wrappers, then
      peer tier, swap, cold load, error handling;
   2. a C++ scenario drives the C-ABI under ThreadSanitizer and under AddressSanitizer+UBSan+LeakSanitizer, including
      a failed wake (injected cuMemCreate failure) followed by the controller's retry, and checks that destroying the
-     engines leaves no mapping and no handle behind.
+     engines leaves no mapping and no handle behind;
+  3. a C++ scenario fails, in turn, each call that sets up one of the engine's own VMM buffers (parking, resident, attached,
+     multi-path and helper staging), under the same two sanitizer builds.
 
 The product library contains none of this: without a GPU it refuses to run (tests/test_abi.py)."""
 import os
@@ -87,6 +89,30 @@ def test_engine_scenario_under_sanitizers(tmp_path):
         results = list(pool.map(lambda a: one(*a), [("tsan", ["-fsanitize=thread"]), ("asan", ["-fsanitize=address,undefined", "-fno-omit-frame-pointer"])]))
     for san, rc, out in results:
         assert rc == 0 and "engine sanitizer scenario ok" in out, (san, out[-3000:])
+        assert "WARNING: ThreadSanitizer" not in out and "ERROR: AddressSanitizer" not in out and "runtime error:" not in out, (san, out[-3000:])
+
+
+def test_vmm_buffer_failures_under_sanitizers(tmp_path):
+    """tests/cpp/hostsim/vmm_failure_test.cpp under ThreadSanitizer and under ASan+UBSan+LeakSan: every call that sets up a parking,
+    resident, attached, multi-path or helper staging buffer fails in turn; the error code follows one rule, nothing is left behind
+    (mapping, handle, VA reservation, fd) and the engine still sleeps and wakes bit-exact."""
+    if not _have_cuda_headers():
+        pytest.skip("CUDA headers not installed")
+    from concurrent.futures import ThreadPoolExecutor
+
+    def one(san, flags):
+        exe = str(tmp_path / f"vmm_{san}")
+        subprocess.check_call(["g++", "-std=c++17", "-O1", "-g", *flags, *INC, *SRCS, os.path.join(SIM, "vmm_failure_test.cpp"), "-o", exe, "-lpthread"])
+        env = dict(os.environ, ASAN_OPTIONS="detect_leaks=1", TSAN_OPTIONS="halt_on_error=1", HOSTSIM_DEVICES="2")
+        for key in ("FMA_RESIDENT_MIB", "FMA_HOST_STORE_SHM", "FMA_NO_RING"):
+            env.pop(key, None)
+        r = subprocess.run([exe], env=env, capture_output=True, text=True, timeout=900)
+        return san, r.returncode, r.stdout + r.stderr
+
+    with ThreadPoolExecutor(2) as pool:
+        results = list(pool.map(lambda a: one(*a), [("tsan", ["-fsanitize=thread"]), ("asan", ["-fsanitize=address,undefined", "-fno-omit-frame-pointer"])]))
+    for san, rc, out in results:
+        assert rc == 0 and "vmm failure scenario ok" in out, (san, out[-3000:])
         assert "WARNING: ThreadSanitizer" not in out and "ERROR: AddressSanitizer" not in out and "runtime error:" not in out, (san, out[-3000:])
 
 
