@@ -515,6 +515,97 @@ inline void set_pack_desc(fma_k_pack_desc& d, uint64_t src, uint64_t dst, uint32
 // Reads the K4 / K5 error counter d_psize[pdesc_cap] (synchronises the kernel stream); a non-zero count fails with
 // FMA_EINTEGRITY and `fmt`, which takes the count as its one %u.
 int check_pack_errors(fma_engine_t* e, const char* fmt);
+
+// "Move these pages with a kernel", the same call for both page forms, so that a copy pipeline is written once: plain 2 MiB
+// pages go through K1 / K2 and page tables, PACKED pages through K4 / K5 and descriptors.  One side of every page is its device
+// address (PagePlan::va).  The other, the store side, is wherever the pipeline says: in the store itself, or in a ring slot.
+struct PageKernels {
+    fma_engine_t* e;
+    KernelTimes& kt;
+    bool to_store;   // a sleep: gather / code into the store side; else a wake: scatter / decode out of it
+    bool packed;
+    size_t at = 0;   // first entry of the engine's table and descriptor buffers to use (a RESIDENT share's sit behind the host part's)
+    // Enqueues, on the kernel stream, the upload of what the launches over `pages` read: descriptors (PACKED), or the two page
+    // tables of a wake.  store_addr(q) is the store side of page q.  clear_errors: zero the K4 / K5 error counter too (an
+    // operation does that once, before its first PACKED launch).  A plain sleep has nothing to add: its table of device addresses
+    // is the image's page table, which SleepPipe::plan uploads for every sleep pipeline, and its store side is always a base.
+    template <class StoreAddr>
+    int prepare(const std::vector<PagePlan>& pages, bool clear_errors, StoreAddr store_addr) {
+        const size_t n = pages.size();
+        if (packed) {
+            RC(ensure_pack_bufs(e, at + n));
+            for (size_t q = 0; q < n; ++q) {
+                const uint64_t st = store_addr(q);
+                set_pack_desc(e->h_pdesc[at + q], to_store ? pages[q].va : st, to_store ? st : pages[q].va, pages[q].bytes);
+            }
+            RT(cudaMemcpyAsync(e->d_pdesc + at, e->h_pdesc + at, n * sizeof(fma_k_pack_desc), cudaMemcpyHostToDevice, e->ks));
+            if (clear_errors) RT(cudaMemsetAsync(e->d_psize + e->pdesc_cap, 0, sizeof(uint32_t), e->ks));
+        } else if (!to_store) {
+            RC(ensure_tables(e, at + n));
+            uint64_t* dev = e->h_tab + at;                  // destination page addresses
+            uint64_t* st = e->h_tab + e->d_tab_cap + at;    // source page addresses (may be sparse in the store)
+            for (size_t q = 0; q < n; ++q) {
+                dev[q] = pages[q].va;
+                st[q] = store_addr(q);
+            }
+            RT(cudaMemcpyAsync(e->d_tab + at, dev, n * sizeof(uint64_t), cudaMemcpyHostToDevice, e->ks));
+            RT(cudaMemcpyAsync(e->d_tab + e->d_tab_cap + at, st, n * sizeof(uint64_t), cudaMemcpyHostToDevice, e->ks));
+        }
+        return FMA_OK;
+    }
+    // One launch over the pages of `b`, timed by `kt`.  Plain pages whose store side is contiguous take its address as
+    // store_base; 0: their store side is the table `prepare` uploaded (a wake in place: a batch may span pages apart in the store).
+    int launch(const Batch& b, uint64_t store_base = 0) {
+        const size_t p = at + b.p0;
+        if (!packed) {
+            const uint64_t* dev = e->d_tab + p;
+            const uint64_t* st = store_base ? nullptr : e->d_tab + e->d_tab_cap + p;
+            return to_store ? kt.launch(dev, 0, st, store_base, (uint32_t)b.np) : kt.launch(st, store_base, dev, 0, (uint32_t)b.np);
+        }
+        uint32_t* d_err = e->d_psize + e->pdesc_cap;
+        RC(kt.begin());
+        if (to_store) RT(fma_k_launch_pack(e->d_pdesc + p, (uint32_t)b.np, d_err, e->ks));
+        else RT(fma_k_launch_unpack(e->d_pdesc + p, (uint32_t)b.np, d_err, e->ks));
+        return kt.end((uint64_t)b.np * FMA_PAGE_BYTES + b.stored);
+    }
+};
+
+// Where each page of `pages` lies in the staging ring when batch c of `slots` goes through slot c % n_ring
+inline std::vector<uint64_t> ring_addresses(const fma_engine_t* e, const std::vector<PagePlan>& pages, const std::vector<Batch>& slots) {
+    std::vector<uint64_t> at(pages.size());
+    for (size_t c = 0; c < slots.size(); ++c)
+        for (size_t q = slots[c].p0; q < slots[c].p0 + slots[c].np; ++q)
+            at[q] = (uint64_t)(uintptr_t)e->ring[c % e->n_ring] + (pages[q].off - pages[slots[c].p0].off);
+    return at;
+}
+
+// What the workers of a MULTI-PATH sleep or wake share: one thread per path, and the first error wins.
+struct PathWorkers {
+    std::atomic<int> error{FMA_OK};
+    char err_msg[512] = "";
+    std::mutex kt_mu;                 // an operation has one KernelTimes: the paths' launches take turns
+    std::vector<uint32_t> per_path;   // chunks each path moved
+    void fail_once(int code, size_t pi, int device, const char* what, const char* why) {
+        int expect = FMA_OK;
+        if (error.compare_exchange_strong(expect, code)) snprintf(err_msg, sizeof(err_msg), "%s failed on path %zu (device %d): %s", what, pi, device, why);
+    }
+    // worker(pi) on a thread per path, on the engine's GPU and with the path's kernel stream behind ev_tab (the page table must be
+    // on the device before any path's kernel reads it); returns when every worker has returned
+    template <class Worker>
+    void run(fma_engine_t* e, cudaEvent_t ev_tab, Worker worker) {
+        per_path.assign(e->paths.size(), 0);
+        std::vector<std::thread> th;
+        for (size_t pi = 0; pi < e->paths.size(); ++pi)
+            th.emplace_back([&, pi] {
+                cudaSetDevice(e->device);
+                const cudaError_t ce = cudaStreamWaitEvent(e->paths[pi].kern, ev_tab, 0);
+                if (ce != cudaSuccess) return fail_once(FMA_ECUDA, pi, e->paths[pi].device, "cudaStreamWaitEvent(table)", cudaGetErrorString(ce));
+                worker(pi);
+            });
+        for (auto& t : th) t.join();
+    }
+};
+
 // No kernel ran in this operation: its kernel statistics read zero.
 inline void zero_kernel_stats(fma_engine_t* e) {
     e->pending_events = 0;

@@ -284,10 +284,8 @@ struct SleepPipe {
         return FMA_OK;
     }
     int direct();
-    int kernel_packed();
-    int kernel();
-    int staged_packed();
-    int staged();
+    int in_place(bool packed);
+    int staged(bool packed);
     int multipath();
 };
 
@@ -319,52 +317,30 @@ int SleepPipe::direct() {
     return FMA_OK;
 }
 
-// KERNEL + PACKED (parking tiers): K4 encodes straight into the peer / local HBM store
-int SleepPipe::kernel_packed() {
+// IN PLACE: K1 / K4 write the store themselves: mapped pinned host memory (PCIe posted writes) or peer / local HBM (a PACKED
+// image: 0.758 of the bytes over NVLink and of the parking GPU's HBM)
+int SleepPipe::in_place(bool packed) {
     std::vector<PagePlan> pages;
-    RC(plan(true, &pages));
-    // PACKED image in a parking tier: K4 encodes straight into the peer / local HBM store (0.758 of the bytes
-    // over NVLink and of the parking GPU's HBM), batches as below
-    RC(ensure_pack_bufs(e, pages.size()));
+    RC(plan(packed, &pages));
     const uint64_t dbase = resident ? (uint64_t)e->res.va : store_dev_base(e, tier);
-    for (size_t p = 0; p < pages.size(); ++p) set_pack_desc(e->h_pdesc[p], pages[p].va, dbase + pages[p].off, pages[p].bytes);
-    uint32_t* d_err = e->d_psize + e->pdesc_cap;
-    RT(cudaMemcpyAsync(e->d_pdesc, e->h_pdesc, pages.size() * sizeof(fma_k_pack_desc), cudaMemcpyHostToDevice, e->ks));
-    RT(cudaMemsetAsync(d_err, 0, sizeof(uint32_t), e->ks));
-    std::vector<Batch> batches;
-    fma_layout::plan_batches(pages, slot_pages(e), UINT64_MAX, false, &batches);
-    for (const Batch& b : batches) {
-        RC(kt.begin());
-        RT(fma_k_launch_pack(e->d_pdesc + b.p0, (uint32_t)b.np, d_err, e->ks));
-        RC(kt.end((uint64_t)b.np * FMA_PAGE_BYTES + b.stored));
-        ++copy_ops;
-        RC(publish_gathered(b.p0 + b.np));
-    }
-    return FMA_OK;
-}
-
-// KERNEL: K1 writes the store itself (mapped pinned host memory, peer or local HBM)
-int SleepPipe::kernel() {
-    std::vector<PagePlan> pages;
-    RC(plan(false, &pages));
-    // K1 writes the store itself: mapped pinned host memory (PCIe posted writes) or peer/local HBM;
+    PageKernels pk{e, kt, true, packed};
+    RC(pk.prepare(pages, true, [&](size_t q) { return dbase + pages[q].off; }));
     // launched in slot-sized batches so finished segments can be released while later ones still move
-    const uint64_t dbase = resident ? (uint64_t)e->res.va : store_dev_base(e, tier);
     std::vector<Batch> batches;
     fma_layout::plan_batches(pages, slot_pages(e), UINT64_MAX, false, &batches);
     for (const Batch& b : batches) {
-        RC(kt.launch(e->d_tab + b.p0, 0, nullptr, dbase + pages[b.p0].off, (uint32_t)b.np));
+        RC(pk.launch(b, dbase + pages[b.p0].off));
         ++copy_ops;
         RC(publish_gathered(b.p0 + b.np));
     }
     return FMA_OK;
 }
 
-// STAGED + PACKED: K4 gather + encode -> ring slot (stored pages back to back) -> one D2H per slot
-int SleepPipe::staged_packed() {
+// STAGED: K1 gather / K4 gather + encode -> HBM ring slot (a PACKED image: stored pages back to back) -> one large D2H per slot
+int SleepPipe::staged(bool packed) {
     std::vector<PagePlan> pages;
-    RC(plan(true, &pages));   // (the route has the ring)
-    // the image pages this sleep codes: all of them, or (incremental) the pages of the changed segments, whose stored size
+    RC(plan(packed, &pages));   // (the route has the ring)
+    // the image pages this sleep moves: all of them, or (incremental) the pages of the changed segments, whose stored size
     // is known not to change, so each goes back to its old place in the kept image
     std::vector<size_t> img_page(pages.size());
     for (size_t p = 0; p < pages.size(); ++p) img_page[p] = p;
@@ -374,50 +350,19 @@ int SleepPipe::staged_packed() {
         for (size_t p : img_page) sel.push_back(pages[p]);
         pages = std::move(sel);
     }
-    std::vector<Batch> slots;  // pages adjacent in the store that together fit a ring slot
-    if (!fma_layout::plan_batches(pages, SIZE_MAX, e->ring_slot_bytes, true, &slots))
+    std::vector<Batch> slots;  // pages adjacent in the store that together fit a ring slot: by their stored bytes, or by their number
+    if (!fma_layout::plan_batches(pages, packed ? SIZE_MAX : e->ring_slot_bytes / FMA_PAGE_BYTES, packed ? e->ring_slot_bytes : UINT64_MAX, true, &slots))
         return fail(FMA_EINVAL, "ring slot of %zu bytes cannot hold one page", e->ring_slot_bytes);
-    for (size_t c = 0; c < slots.size(); ++c)
-        for (size_t k = slots[c].p0; k < slots[c].p0 + slots[c].np; ++k)
-            set_pack_desc(e->h_pdesc[k], pages[k].va, (uint64_t)(uintptr_t)e->ring[c % e->n_ring] + (pages[k].off - pages[slots[c].p0].off), pages[k].bytes);
-    uint32_t* d_err = e->d_psize + e->pdesc_cap;
-    RT(cudaMemcpyAsync(e->d_pdesc, e->h_pdesc, pages.size() * sizeof(fma_k_pack_desc), cudaMemcpyHostToDevice, e->ks));
-    RT(cudaMemsetAsync(d_err, 0, sizeof(uint32_t), e->ks));
+    const std::vector<uint64_t> in_ring = ring_addresses(e, pages, slots);
+    PageKernels pk{e, kt, true, packed};
+    RC(pk.prepare(pages, true, [&](size_t q) { return in_ring[q]; }));
     cudaStream_t last_stream = e->cs[0];
     for (size_t c = 0; c < slots.size(); ++c) {
         const Batch& sl = slots[c];
         const int slot = (int)(c % e->n_ring);
         cudaStream_t cstream = e->cs[c % e->n_cs];
         if (c >= (size_t)e->n_ring) RT(cudaStreamWaitEvent(e->ks, e->ev_ring_free[slot], 0));
-        RC(kt.begin());
-        RT(fma_k_launch_pack(e->d_pdesc + sl.p0, (uint32_t)sl.np, d_err, e->ks));
-        RC(kt.end((uint64_t)sl.np * FMA_PAGE_BYTES + sl.stored));
-        RT(cudaEventRecord(e->ev_ring_full[slot], e->ks));
-        RT(cudaStreamWaitEvent(cstream, e->ev_ring_full[slot], 0));
-        RT(cudaMemcpyAsync(store + pages[sl.p0].off, e->ring[slot], sl.stored, cudaMemcpyDefault, cstream));
-        if (c > 0) RT(cudaStreamWaitEvent(cstream, e->ev_ring_free[(c - 1) % e->n_ring], 0));  // same chaining as below
-        RT(cudaEventRecord(e->ev_ring_free[slot], cstream));
-        ++copy_ops;
-        // every image byte below the last page of this slot is in the store: coded just now, or kept from the last wake
-        RC(publish_consumed((uint64_t)(img_page[sl.p0 + sl.np - 1] + 1) * FMA_PAGE_BYTES, cstream));
-        last_stream = cstream;
-    }
-    return subset ? publish_consumed(W, last_stream) : FMA_OK;  // the clean tail of the image needs no copy
-}
-
-// STAGED: K1 gather -> HBM ring slot -> one large D2H per slot
-int SleepPipe::staged() {
-    std::vector<PagePlan> pages;
-    RC(plan(false, &pages));   // (the route has the ring)
-    std::vector<Batch> slots;
-    if (!fma_layout::plan_batches(pages, e->ring_slot_bytes / FMA_PAGE_BYTES, UINT64_MAX, true, &slots))
-        return fail(FMA_EINVAL, "ring slot of %zu bytes cannot hold one page", e->ring_slot_bytes);
-    for (size_t c = 0; c < slots.size(); ++c) {
-        const Batch& sl = slots[c];
-        const int slot = (int)(c % e->n_ring);
-        cudaStream_t cstream = e->cs[c % e->n_cs];
-        if (c >= (size_t)e->n_ring) RT(cudaStreamWaitEvent(e->ks, e->ev_ring_free[slot], 0));
-        RC(kt.launch(e->d_tab + sl.p0, 0, nullptr, (uint64_t)(uintptr_t)e->ring[slot], (uint32_t)sl.np));
+        RC(pk.launch(sl, (uint64_t)(uintptr_t)e->ring[slot]));
         RT(cudaEventRecord(e->ev_ring_full[slot], e->ks));
         RT(cudaStreamWaitEvent(cstream, e->ev_ring_full[slot], 0));
         RT(cudaMemcpyAsync(store + pages[sl.p0].off, e->ring[slot], sl.stored, cudaMemcpyDefault, cstream));
@@ -426,9 +371,12 @@ int SleepPipe::staged() {
         if (c > 0) RT(cudaStreamWaitEvent(cstream, e->ev_ring_free[(c - 1) % e->n_ring], 0));
         RT(cudaEventRecord(e->ev_ring_free[slot], cstream));
         ++copy_ops;
-        RC(publish_consumed((uint64_t)(sl.p0 + sl.np) * FMA_PAGE_BYTES, cstream));  // units fully in the store are dead
+        // every image byte below the last page of this slot is in the store (moved just now, or kept from the last wake):
+        // units fully in the store are dead
+        RC(publish_consumed((uint64_t)(img_page[sl.p0 + sl.np - 1] + 1) * FMA_PAGE_BYTES, cstream));
+        last_stream = cstream;
     }
-    return FMA_OK;
+    return subset ? publish_consumed(W, last_stream) : FMA_OK;  // the clean tail of the image needs no copy
 }
 
 // MULTI-PATH sleep (fma_paths_set): the mirror image of the multi-path wake.  K1 on the sleeping GPU gathers a chunk of the image
@@ -446,22 +394,14 @@ int SleepPipe::multipath() {
     std::vector<uint64_t> chunk_off;
     for (const Batch& ch : chunks) chunk_off.push_back(pages[ch.p0].off);
     fma_layout::ChunkQueues queues(chunk_off, e->host.ranges);
-    std::atomic<int> error{FMA_OK};
-    std::mutex kt_mu;
-    char err_msg[512] = "";
-    std::vector<uint32_t> per_path(e->paths.size(), 0);
-    auto worker = [&](size_t pi) {
+    PathWorkers pw;
+    pw.run(e, ev_tab, [&](size_t pi) {
         WakePath& path = e->paths[pi];
-        cudaSetDevice(e->device);
-        auto failw = [&](int code, const char* what, cudaError_t ce) {
-            int expect = FMA_OK;
-            if (error.compare_exchange_strong(expect, code)) snprintf(err_msg, sizeof(err_msg), "%s failed on path %zu (device %d): %s", what, pi, path.device, cudaGetErrorString(ce));
-        };
-        cudaError_t ce = cudaStreamWaitEvent(path.kern, ev_tab, 0);
-        if (ce != cudaSuccess) return failw(FMA_ECUDA, "cudaStreamWaitEvent(table)", ce);
+        auto failw = [&](int code, const char* what, cudaError_t ce) { pw.fail_once(code, pi, path.device, what, cudaGetErrorString(ce)); };
+        cudaError_t ce;
         uint32_t mine = 0;
         for (;;) {
-            if (error.load() != FMA_OK) return;
+            if (pw.error.load() != FMA_OK) return;
             size_t c = 0;
             if (!queues.take(path.numa_node, &c)) break;
             const Batch& ch = chunks[c];
@@ -472,7 +412,7 @@ int SleepPipe::multipath() {
             }
             char* slot_ptr = reinterpret_cast<char*>(path.staging.va) + (size_t)slot * e->path_slot_bytes;
             {
-                std::lock_guard<std::mutex> lk(kt_mu);
+                std::lock_guard<std::mutex> lk(pw.kt_mu);
                 const int krc = kt.launch_on(path.kern, e->d_tab + ch.p0, 0, nullptr, (uint64_t)(uintptr_t)slot_ptr, (uint32_t)ch.np);   // K1: gather -> slot
                 if (krc != FMA_OK) return failw(krc, "K1 launch", cudaGetLastError());
             }
@@ -486,22 +426,19 @@ int SleepPipe::multipath() {
             if (ce != cudaSuccess) return failw(FMA_ECUDA, "cudaEventRecord(slot drained)", ce);
             ++mine;
         }
-        per_path[pi] = mine;
-    };
-    std::vector<std::thread> th;
-    for (size_t pi = 0; pi < e->paths.size(); ++pi) th.emplace_back(worker, pi);
-    for (auto& t : th) t.join();
+        pw.per_path[pi] = mine;
+    });
     for (WakePath& path : e->paths) {   // every D2H has landed before anything is released (and before an error is reported)
         cudaError_t ce = cudaStreamSynchronize(path.copy);
-        if (ce != cudaSuccess && error.load() == FMA_OK) {
-            error.store(FMA_ECUDA);
-            snprintf(err_msg, sizeof(err_msg), "D2H on path device %d failed: %s", path.device, cudaGetErrorString(ce));
+        if (ce != cudaSuccess && pw.error.load() == FMA_OK) {
+            pw.error.store(FMA_ECUDA);
+            snprintf(pw.err_msg, sizeof(pw.err_msg), "D2H on path device %d failed: %s", path.device, cudaGetErrorString(ce));
         }
     }
-    if (error.load() != FMA_OK) return fail(error.load(), "%s", err_msg);
+    if (pw.error.load() != FMA_OK) return fail(pw.error.load(), "%s", pw.err_msg);
     for (size_t pi = 0; pi < e->paths.size(); ++pi) {
-        copy_ops += per_path[pi];
-        e->tl_add("path_chunks", e->paths[pi].device, e->tl_entry, now_s(), (uint64_t)per_path[pi] * e->path_slot_bytes);
+        copy_ops += pw.per_path[pi];
+        e->tl_add("path_chunks", e->paths[pi].device, e->tl_entry, now_s(), (uint64_t)pw.per_path[pi] * e->path_slot_bytes);
     }
     return publish_consumed(W, e->ks);   // all bytes are in the store: every offloaded unit may go
 }
@@ -748,7 +685,7 @@ int gather_resident(fma_engine_t* e, SleepPlan& p) {
     SleepPipe rp{e, p.ex_res, p.W_all - p.W, FMA_TIER_LOCAL, nullptr, p.kt, res_launches, nullptr};  // units go with the host part
     rp.resident = true;
     p.kt.kind = "res_gather";
-    const int rc = e->res_packed ? rp.kernel_packed() : rp.kernel();
+    const int rc = rp.in_place(e->res_packed);
     p.kt.kind = "kernel";
     if (rc != FMA_OK) return rc;
     if (e->res_packed) RC(check_pack_errors(e, kPackChanged));
@@ -772,18 +709,18 @@ int run_pipeline(fma_engine_t* e, SleepPlan& p, Unmapper& un) {
         switch (p.route.pipe) {
         case SleepPipeKind::PartialPacked:  // only the changed segments' pages are re-coded, each into its old place
             pipe.subset = &p.dirty_pages;
-            RC(pipe.staged_packed());
+            RC(pipe.staged(true));
             break;
         case SleepPipeKind::PartialDirect:  // only the changed segments move; everything below each of them is in the store already
             RC(pipe.direct());
             RC(un.publish_consumed(p.W, e->cs[0]));  // cs[0] has joined the other streams after the last extent
             break;
         case SleepPipeKind::Direct: RC(pipe.direct()); break;
-        case SleepPipeKind::Kernel: RC(pipe.kernel()); break;
-        case SleepPipeKind::KernelPacked: RC(pipe.kernel_packed()); break;
+        case SleepPipeKind::Kernel: RC(pipe.in_place(false)); break;
+        case SleepPipeKind::KernelPacked: RC(pipe.in_place(true)); break;
         case SleepPipeKind::Multipath: RC(pipe.multipath()); break;
-        case SleepPipeKind::StagedPacked: RC(pipe.staged_packed()); break;
-        case SleepPipeKind::Staged: RC(pipe.staged()); break;
+        case SleepPipeKind::StagedPacked: RC(pipe.staged(true)); break;
+        case SleepPipeKind::Staged: RC(pipe.staged(false)); break;
         case SleepPipeKind::Adopt: return fail(FMA_ESTATE, "an adopted image has no copy pipeline");  // (handled above)
         }
         un.close();

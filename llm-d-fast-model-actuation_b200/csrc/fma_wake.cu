@@ -176,9 +176,10 @@ struct ResidentRestore {
     const std::vector<size_t>& seg_run;
     uint64_t W_res;
     size_t n_host_pages;
-    bool image_packed;             // WakePipe::packed clears the K5 error counter
+    bool image_packed;             // the host part's pipeline clears the K5 error counter
     std::vector<Batch> pieces{};
     size_t next = 0;
+    PageKernels kernels() { return PageKernels{e, kt, false, e->res_packed, n_host_pages}; }
     int setup();
     int launch_next();
     // after (host part's pages launched so far, host part's pages): launch the next piece if due
@@ -197,7 +198,6 @@ struct WakePipe {
     const std::vector<size_t>& seg_run;       // segment -> index of its run in the mapper's work list
     uint64_t W;
     int tier;
-    int mode;
     bool ring_run;                             // the staging ring is work item 0
     const char* store;
     KernelTimes& kt;
@@ -211,9 +211,12 @@ struct WakePipe {
         if (!copy_ops) first_copy_delay = now_s() - t_entry;
         ++copy_ops;
     }
-    int packed();
+    // the pages of the DESTINATIONS in image order (== with_backup order only if every backed-up segment is woken), with the
+    // latest work item each page needs; where they are in the store: in the PACKED layout, or verbatim
+    int plan(bool packed, std::vector<PagePlan>* pages);
     int direct();
-    int paged();
+    int in_place(bool packed);
+    int staged(bool packed);
     int multipath();
 };
 
@@ -224,112 +227,34 @@ std::vector<fma_layout::SegPages> wake_segs(const fma_engine_t* e, const std::ve
     return v;
 }
 
+int WakePipe::plan(bool packed, std::vector<PagePlan>* pages) {
+    uint64_t bad = 0;
+    if (!fma_layout::plan_pages(wake_segs(e, with_backup, seg_run), packed ? &e->img_off : nullptr, &e->img_bytes, pages, &bad))
+        return fail(FMA_ESTATE, "segment at image offset %llu is outside the packed image's page table", (unsigned long long)bad);
+    return FMA_OK;
+}
+
 int ResidentRestore::setup() {
     if (!e->res.va) return fail(FMA_ESTATE, "the resident part of the image is gone");
-    const size_t n_res = W_res / FMA_PAGE_BYTES, n_all = n_host_pages + n_res;
-    RC(ensure_tables(e, n_all));
-    if (e->res_packed) RC(ensure_pack_bufs(e, n_all));
     if (!e->ev_res_done && cudaEventCreateWithFlags(&e->ev_res_done, cudaEventDisableTiming) != cudaSuccess)
         return fail(FMA_ECUDA, "cudaEventCreate(resident) failed");
     std::vector<PagePlan> pages;
     uint64_t bad = 0;
     if (!fma_layout::plan_pages(wake_segs(e, with_res, seg_run), e->res_packed ? &e->res_off : nullptr, &e->res_bytes, &pages, &bad))
         return fail(FMA_ESTATE, "segment outside the resident part's page table");
-    uint64_t* dst_tab = e->h_tab + n_host_pages;
-    uint64_t* src_tab = e->h_tab + e->d_tab_cap + n_host_pages;
-    for (size_t q = 0; q < pages.size(); ++q) {
-        if (e->res_packed) {
-            set_pack_desc(e->h_pdesc[n_host_pages + q], (uint64_t)e->res.va + pages[q].off, pages[q].va, pages[q].bytes);
-        } else {
-            dst_tab[q] = pages[q].va;
-            src_tab[q] = (uint64_t)e->res.va + pages[q].off;
-        }
-    }
+    RC(kernels().prepare(pages, !image_packed, [&](size_t q) { return (uint64_t)e->res.va + pages[q].off; }));   // (else the host part's pipeline clears the counter)
     fma_layout::plan_batches(pages, slot_pages(e), UINT64_MAX, false, &pieces);
-    if (e->res_packed) {
-        RT(cudaMemcpyAsync(e->d_pdesc + n_host_pages, e->h_pdesc + n_host_pages, n_res * sizeof(fma_k_pack_desc), cudaMemcpyHostToDevice, e->ks));
-        if (!image_packed) RT(cudaMemsetAsync(e->d_psize + e->pdesc_cap, 0, sizeof(uint32_t), e->ks));   // (WakePipe::packed clears it otherwise)
-    } else {
-        RT(cudaMemcpyAsync(e->d_tab + n_host_pages, dst_tab, n_res * sizeof(uint64_t), cudaMemcpyHostToDevice, e->ks));
-        RT(cudaMemcpyAsync(e->d_tab + e->d_tab_cap + n_host_pages, src_tab, n_res * sizeof(uint64_t), cudaMemcpyHostToDevice, e->ks));
-    }
     return FMA_OK;
 }
 
 int ResidentRestore::launch_next() {
     const Batch& pc = pieces[next];
     RC(mapper.wait(pc.need));
-    int r;
     kt.kind = "res_restore";
-    if (e->res_packed) {
-        r = kt.begin();
-        if (r == FMA_OK) {
-            cudaError_t ce = fma_k_launch_unpack(e->d_pdesc + n_host_pages + pc.p0, (uint32_t)pc.np, e->d_psize + e->pdesc_cap, e->ks);
-            r = ce == cudaSuccess ? kt.end((uint64_t)pc.np * FMA_PAGE_BYTES + pc.stored) : fail(FMA_ECUDA, "K5 (resident) launch failed: %s", cudaGetErrorString(ce));
-        }
-    } else {
-        r = kt.launch(e->d_tab + e->d_tab_cap + n_host_pages + pc.p0, 0, e->d_tab + n_host_pages + pc.p0, 0, (uint32_t)pc.np);
-    }
+    const int r = kernels().launch(pc);
     kt.kind = "kernel";
     if (r != FMA_OK) return r;
     if (++next == pieces.size()) RT(cudaEventRecord(e->ev_res_done, e->ks));
-    return FMA_OK;
-}
-
-// PACKED image: H2D of the stored pages (0.758 of the bytes) -> ring slot -> K5 decode + scatter; or K5 reads the store itself
-int WakePipe::packed() {
-    // K5 reads the store itself when it is peer / local HBM, or when no ring could be had (then over PCIe)
-    const bool zero_copy = mode != FMA_MODE_STAGED;
-    if (zero_copy && tier == FMA_TIER_HOST && !e->host.dev_alias)
-        return fail(FMA_ENOMEM, "no HBM for a staging ring and the host store has no device alias: a packed image cannot be woken");
-    std::vector<PagePlan> pages;
-    uint64_t bad = 0;
-    if (!fma_layout::plan_pages(wake_segs(e, with_backup, seg_run), &e->img_off, &e->img_bytes, &pages, &bad))
-        return fail(FMA_ESTATE, "segment at image offset %llu is outside the packed image's page table", (unsigned long long)bad);
-    const size_t n_pages = pages.size();
-    RC(ensure_pack_bufs(e, n_pages));
-    uint32_t* d_err = e->d_psize + e->pdesc_cap;
-    RT(cudaMemsetAsync(d_err, 0, sizeof(uint32_t), e->ks));
-    if (!zero_copy) {
-        if (ring_run) RC(mapper.wait(1));   // (else the route has the ring)
-        std::vector<Batch> slots;  // pages that are adjacent in the store and fit one ring slot
-        if (!fma_layout::plan_batches(pages, SIZE_MAX, e->ring_slot_bytes, true, &slots))
-            return fail(FMA_EINVAL, "ring slot of %zu bytes cannot hold one page", e->ring_slot_bytes);
-        for (size_t c = 0; c < slots.size(); ++c)
-            for (size_t q = slots[c].p0; q < slots[c].p0 + slots[c].np; ++q)
-                set_pack_desc(e->h_pdesc[q], (uint64_t)(uintptr_t)e->ring[c % e->n_ring] + (pages[q].off - pages[slots[c].p0].off), pages[q].va, pages[q].bytes);
-        RT(cudaMemcpyAsync(e->d_pdesc, e->h_pdesc, n_pages * sizeof(fma_k_pack_desc), cudaMemcpyHostToDevice, e->ks));
-        for (size_t c = 0; c < slots.size(); ++c) {
-            const Batch& sl = slots[c];
-            const int slot = (int)(c % e->n_ring);
-            cudaStream_t cstream = e->cs[c % e->n_cs];
-            if (c >= (size_t)e->n_ring) RT(cudaStreamWaitEvent(cstream, e->ev_ring_free[slot], 0));
-            RT(cudaMemcpyAsync(e->ring[slot], store + pages[sl.p0].off, sl.stored, cudaMemcpyDefault, cstream));
-            copied();
-            RT(cudaEventRecord(e->ev_ring_full[slot], cstream));
-            RC(mapper.wait(sl.need));
-            RT(cudaStreamWaitEvent(e->ks, e->ev_ring_full[slot], 0));
-            RC(kt.begin());
-            RT(fma_k_launch_unpack(e->d_pdesc + sl.p0, (uint32_t)sl.np, d_err, e->ks));
-            RC(kt.end((uint64_t)sl.np * FMA_PAGE_BYTES + sl.stored));
-            RT(cudaEventRecord(e->ev_ring_free[slot], e->ks));
-            if (between) RC(between->pump(sl.p0 + sl.np, n_pages));
-        }
-    } else {
-        const uint64_t sbase = store_dev_base(e, tier);
-        for (size_t q = 0; q < n_pages; ++q) set_pack_desc(e->h_pdesc[q], sbase + pages[q].off, pages[q].va, pages[q].bytes);
-        RT(cudaMemcpyAsync(e->d_pdesc, e->h_pdesc, n_pages * sizeof(fma_k_pack_desc), cudaMemcpyHostToDevice, e->ks));
-        std::vector<Batch> batches;
-        fma_layout::plan_batches(pages, slot_pages(e), UINT64_MAX, false, &batches);
-        for (const Batch& b : batches) {
-            RC(mapper.wait(b.need));
-            RC(kt.begin());
-            RT(fma_k_launch_unpack(e->d_pdesc + b.p0, (uint32_t)b.np, d_err, e->ks));
-            RC(kt.end((uint64_t)b.np * FMA_PAGE_BYTES + b.stored));
-            copied();
-            if (between) RC(between->pump(b.p0 + b.np, n_pages));
-        }
-    }
     return FMA_OK;
 }
 
@@ -350,60 +275,61 @@ int WakePipe::direct() {
     return FMA_OK;
 }
 
-// KERNEL / STAGED: page-table driven — K2 reads the store itself, or H2D -> ring slot -> K2 scatter
-int WakePipe::paged() {
-    // page table of the DESTINATIONS in image order (== with_backup order only if every backed-up segment is woken), with the
-    // latest work item each page needs
+// IN PLACE: K2 / K5 read the store themselves (zero-copy PCIe reads, or NVLink / HBM loads), in batches as the mapper makes
+// progress, so the scatter overlaps cuMemCreate / Map of later segments
+int WakePipe::in_place(bool packed) {
+    // K5 reads the store itself when it is peer / local HBM, or when no ring could be had (then over PCIe)
+    if (packed && tier == FMA_TIER_HOST && !e->host.dev_alias)
+        return fail(FMA_ENOMEM, "no HBM for a staging ring and the host store has no device alias: a packed image cannot be woken");
     std::vector<PagePlan> pages;
-    uint64_t bad = 0;
-    fma_layout::plan_pages(wake_segs(e, with_backup, seg_run), nullptr, nullptr, &pages, &bad);
+    RC(plan(packed, &pages));
     const size_t n_pages = pages.size();
-    RC(ensure_tables(e, n_pages));
-    uint64_t* dst_tab = e->h_tab;                 // destination page addresses
-    uint64_t* src_tab = e->h_tab + e->d_tab_cap;  // source page addresses inside the store (may be sparse)
     const uint64_t sbase = store_dev_base(e, tier);
-    for (size_t p = 0; p < n_pages; ++p) {
-        dst_tab[p] = pages[p].va;
-        src_tab[p] = sbase + pages[p].off;
-    }
-    RT(cudaMemcpyAsync(e->d_tab, dst_tab, n_pages * sizeof(uint64_t), cudaMemcpyHostToDevice, e->ks));
-    RT(cudaMemcpyAsync(e->d_tab + e->d_tab_cap, src_tab, n_pages * sizeof(uint64_t), cudaMemcpyHostToDevice, e->ks));
-    const uint64_t* d_dst = e->d_tab;
-    const uint64_t* d_src = e->d_tab + e->d_tab_cap;
-    if (mode == FMA_MODE_KERNEL) {
-        // K2 reads the store itself (zero-copy PCIe reads, or NVLink/HBM loads); launch batches as the
-        // mapper makes progress so the scatter overlaps cuMemCreate/Map of later segments
-        for (size_t p0 = 0; p0 < n_pages;) {
-            Batch b = fma_layout::next_batch(pages, p0, slot_pages(e), UINT64_MAX, false);
-            RC(mapper.wait(b.need));
-            // opportunistically extend the batch over everything already mapped
+    PageKernels pk{e, kt, false, packed};
+    RC(pk.prepare(pages, true, [&](size_t q) { return sbase + pages[q].off; }));
+    for (size_t p0 = 0; p0 < n_pages;) {
+        Batch b = fma_layout::next_batch(pages, p0, slot_pages(e), UINT64_MAX, false);
+        RC(mapper.wait(b.need));
+        if (!packed) {  // opportunistically extend the batch over everything already mapped
             const size_t have = mapper.done.load();
             while (p0 + b.np < n_pages && pages[p0 + b.np].need <= have) ++b.np;
-            RC(kt.launch(d_src + p0, 0, d_dst + p0, 0, (uint32_t)b.np));
-            copied();
-            p0 += b.np;
-            if (between) RC(between->pump(p0, n_pages));
         }
-    } else {  // STAGED: copy engine H2D store -> ring slot (starts at t=0), K2 scatter once the targets are mapped
-        if (ring_run) RC(mapper.wait(1));  // the ring is run 0 (1 GiB, ~0.2 ms to map): wait for it before the first H2D
-        // the store image may be only partially woken; H2D works on runs that are contiguous in the store
-        std::vector<Batch> slots;
-        if (!fma_layout::plan_batches(pages, e->ring_slot_bytes / FMA_PAGE_BYTES, UINT64_MAX, true, &slots))
-            return fail(FMA_EINVAL, "ring slot of %zu bytes cannot hold one page", e->ring_slot_bytes);
-        for (size_t c = 0; c < slots.size(); ++c) {
-            const Batch& sl = slots[c];
-            const int slot = (int)(c % e->n_ring);
-            cudaStream_t cstream = e->cs[c % e->n_cs];
-            if (c >= (size_t)e->n_ring) RT(cudaStreamWaitEvent(cstream, e->ev_ring_free[slot], 0));
-            RT(cudaMemcpyAsync(e->ring[slot], store + pages[sl.p0].off, sl.stored, cudaMemcpyDefault, cstream));
-            copied();
-            RT(cudaEventRecord(e->ev_ring_full[slot], cstream));
-            RC(mapper.wait(sl.need));
-            RT(cudaStreamWaitEvent(e->ks, e->ev_ring_full[slot], 0));
-            RC(kt.launch(nullptr, (uint64_t)(uintptr_t)e->ring[slot], d_dst + sl.p0, 0, (uint32_t)sl.np));
-            RT(cudaEventRecord(e->ev_ring_free[slot], e->ks));
-            if (between) RC(between->pump(sl.p0 + sl.np, n_pages));
-        }
+        RC(pk.launch(b));
+        copied();
+        p0 += b.np;
+        if (between) RC(between->pump(p0, n_pages));
+    }
+    return FMA_OK;
+}
+
+// STAGED: copy engine H2D store -> ring slot (starts at t=0; a PACKED image: the stored pages, 0.758 of the bytes), K2 scatter /
+// K5 decode + scatter once the targets are mapped
+int WakePipe::staged(bool packed) {
+    std::vector<PagePlan> pages;
+    RC(plan(packed, &pages));
+    const size_t n_pages = pages.size();
+    // the store image may be only partially woken; H2D works on runs that are contiguous in the store and fit one ring slot: by
+    // their stored bytes, or by their number
+    std::vector<Batch> slots;
+    if (!fma_layout::plan_batches(pages, packed ? SIZE_MAX : e->ring_slot_bytes / FMA_PAGE_BYTES, packed ? e->ring_slot_bytes : UINT64_MAX, true, &slots))
+        return fail(FMA_EINVAL, "ring slot of %zu bytes cannot hold one page", e->ring_slot_bytes);
+    const std::vector<uint64_t> in_ring = ring_addresses(e, pages, slots);
+    PageKernels pk{e, kt, false, packed};
+    RC(pk.prepare(pages, true, [&](size_t q) { return in_ring[q]; }));
+    if (ring_run) RC(mapper.wait(1));  // the ring is run 0 (1 GiB, ~0.2 ms to map): wait for it before the first H2D (else the route has the ring)
+    for (size_t c = 0; c < slots.size(); ++c) {
+        const Batch& sl = slots[c];
+        const int slot = (int)(c % e->n_ring);
+        cudaStream_t cstream = e->cs[c % e->n_cs];
+        if (c >= (size_t)e->n_ring) RT(cudaStreamWaitEvent(cstream, e->ev_ring_free[slot], 0));
+        RT(cudaMemcpyAsync(e->ring[slot], store + pages[sl.p0].off, sl.stored, cudaMemcpyDefault, cstream));
+        copied();
+        RT(cudaEventRecord(e->ev_ring_full[slot], cstream));
+        RC(mapper.wait(sl.need));
+        RT(cudaStreamWaitEvent(e->ks, e->ev_ring_full[slot], 0));
+        RC(pk.launch(sl, (uint64_t)(uintptr_t)e->ring[slot]));
+        RT(cudaEventRecord(e->ev_ring_free[slot], e->ks));
+        if (between) RC(between->pump(sl.p0 + sl.np, n_pages));
     }
     return FMA_OK;
 }
@@ -414,8 +340,7 @@ int WakePipe::paged() {
 // the destination pages.  Self-balancing: a slower path (other NUMA node, busy link) simply takes fewer chunks.
 int WakePipe::multipath() {
     std::vector<PagePlan> pages;
-    uint64_t bad = 0;
-    fma_layout::plan_pages(wake_segs(e, with_backup, seg_run), nullptr, nullptr, &pages, &bad);
+    RC(plan(false, &pages));
     const size_t n_pages = pages.size();
     RC(ensure_tables(e, n_pages));
     for (size_t p = 0; p < n_pages; ++p) e->h_tab[p] = pages[p].va;
@@ -454,20 +379,15 @@ int WakePipe::multipath() {
         }
         return queues.take(my_node, out);
     };
-    std::atomic<int> error{FMA_OK};
+    PathWorkers pw;
     std::atomic<bool> first_copy_seen{false};
-    std::mutex kt_mu;
-    char err_msg[512] = "";
-    std::vector<uint32_t> per_path(e->paths.size(), 0), per_path_local(e->paths.size(), 0);
-    auto worker = [&](size_t pi) {
+    std::vector<uint32_t> per_path_local(e->paths.size(), 0);
+    pw.run(e, ev_tab, [&](size_t pi) {
         WakePath& path = e->paths[pi];
-        cudaSetDevice(e->device);
         auto failw = [&](int code, const char* what, cudaError_t ce) {
-            int expect = FMA_OK;
-            if (error.compare_exchange_strong(expect, code)) snprintf(err_msg, sizeof(err_msg), "%s failed on path %zu (device %d): %s", what, pi, path.device, ce == cudaSuccess ? (code == FMA_ESTATE || code == FMA_EINTEGRITY ? what : mapper.msg) : cudaGetErrorString(ce));
+            pw.fail_once(code, pi, path.device, what, ce == cudaSuccess ? (code == FMA_ESTATE || code == FMA_EINTEGRITY ? what : mapper.msg) : cudaGetErrorString(ce));
         };
-        cudaError_t ce = cudaStreamWaitEvent(path.kern, ev_tab, 0);
-        if (ce != cudaSuccess) return failw(FMA_ECUDA, "cudaStreamWaitEvent(table)", ce);
+        cudaError_t ce;
         uint32_t mine = 0;
         if (path.remote) {
             // The owner's helper fills this path's slots in sequence and publishes "chunk c has landed" per slot; K2 gathers the slot
@@ -477,8 +397,8 @@ int WakePipe::multipath() {
             const double patience = std::max(2.0, (double)env_int("FMA_PULL_TIMEOUT_S", 5));
             double t_last = now_s();
             for (;;) {
-                if (error.load() != FMA_OK || mb->abort.load()) {
-                    if (error.load() == FMA_OK) failw(FMA_ESTATE, "the owner's helper aborted the pull", cudaSuccess);
+                if (pw.error.load() != FMA_OK || mb->abort.load()) {
+                    if (pw.error.load() == FMA_OK) failw(FMA_ESTATE, "the owner's helper aborted the pull", cudaSuccess);
                     return;
                 }
                 bool progressed = false;
@@ -518,7 +438,7 @@ int WakePipe::multipath() {
                     if (mrc != FMA_OK) return failw(mrc, "mapping", cudaSuccess);
                     char* slot_ptr = reinterpret_cast<char*>(path.staging.va) + (size_t)slot * e->path_slot_bytes;
                     {
-                        std::lock_guard<std::mutex> lk(kt_mu);
+                        std::lock_guard<std::mutex> lk(pw.kt_mu);
                         const int krc = kt.launch_on(path.kern, nullptr, (uint64_t)(uintptr_t)slot_ptr, e->d_tab + ch.p0, 0, (uint32_t)ch.np);
                         if (krc != FMA_OK) return failw(krc, "K2 launch", cudaGetLastError());
                     }
@@ -536,13 +456,13 @@ int WakePipe::multipath() {
                     std::this_thread::sleep_for(std::chrono::microseconds(20));
                 }
             }
-            per_path[pi] = mine;
+            pw.per_path[pi] = mine;
             ce = cudaEventRecord(path.ev_done, path.kern);
             if (ce != cudaSuccess) return failw(FMA_ECUDA, "cudaEventRecord(done)", ce);
             return;
         }
         for (;;) {
-            if (error.load() != FMA_OK) return;
+            if (pw.error.load() != FMA_OK) return;
             size_t c = 0;
             if (!take_chunk(path.numa_node, &c)) break;
             const Batch& ch = chunks[c];
@@ -567,7 +487,7 @@ int WakePipe::multipath() {
             ce = cudaStreamWaitEvent(path.kern, path.ev_full[slot], 0);
             if (ce != cudaSuccess) return failw(FMA_ECUDA, "cudaStreamWaitEvent(slot full)", ce);
             {
-                std::lock_guard<std::mutex> lk(kt_mu);
+                std::lock_guard<std::mutex> lk(pw.kt_mu);
                 const int krc = kt.launch_on(path.kern, nullptr, (uint64_t)(uintptr_t)slot_ptr, e->d_tab + ch.p0, 0, (uint32_t)ch.np);
                 if (krc != FMA_OK) return failw(krc, "K2 launch", cudaGetLastError());
             }
@@ -575,24 +495,21 @@ int WakePipe::multipath() {
             if (ce != cudaSuccess) return failw(FMA_ECUDA, "cudaEventRecord(slot free)", ce);
             ++mine;
         }
-        per_path[pi] = mine;
+        pw.per_path[pi] = mine;
         ce = cudaEventRecord(path.ev_done, path.kern);
         if (ce != cudaSuccess) return failw(FMA_ECUDA, "cudaEventRecord(done)", ce);
-    };
-    std::vector<std::thread> th;
-    for (size_t pi = 0; pi < e->paths.size(); ++pi) th.emplace_back(worker, pi);
-    for (auto& t : th) t.join();
-    if (error.load() != FMA_OK) {
+    });
+    if (pw.error.load() != FMA_OK) {
         if (mb) mb->abort.store(1);                                          // the owner's helpers stop pulling
         for (WakePath& path : e->paths)
             if (path.copy) cudaStreamSynchronize(path.copy);                 // nothing may still be writing the staging slots
-        return fail(error.load(), "%s", err_msg);
+        return fail(pw.error.load(), "%s", pw.err_msg);
     }
     for (size_t pi = 0; pi < e->paths.size(); ++pi) {
         RT(cudaStreamWaitEvent(e->ks, e->paths[pi].ev_done, 0));   // the wake's device-time bracket and the final sync cover every path
-        copy_ops += per_path[pi];
+        copy_ops += pw.per_path[pi];
         const int idx = e->paths[pi].remote ? -(int)pi : e->paths[pi].device;   // remote paths: -(path index), their GPU is not visible here
-        e->tl_add("path_chunks", idx, t_entry, now_s(), (uint64_t)per_path[pi] * e->path_slot_bytes);
+        e->tl_add("path_chunks", idx, t_entry, now_s(), (uint64_t)pw.per_path[pi] * e->path_slot_bytes);
         e->tl_add("path_local", idx, t_entry, now_s(), (uint64_t)per_path_local[pi] * e->path_slot_bytes);
     }
     return FMA_OK;
@@ -759,13 +676,15 @@ int do_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags) {
         RC(timer.begin());
         if (W_res) RC(res.setup());
         if (W) {
-            WakePipe pipe{e, with_host, seg_run, W, tier, route.mode, ring_run, store, kt, copy_ops, first_copy_delay, t_entry, mapper, W_res ? &res : nullptr};
+            WakePipe pipe{e, with_host, seg_run, W, tier, ring_run, store, kt, copy_ops, first_copy_delay, t_entry, mapper, W_res ? &res : nullptr};
             const double t_enq0 = now_s();
             switch (route.pipe) {
-            case fma_layout::WakePipeKind::PackedRing: case fma_layout::WakePipeKind::PackedZeroCopy: RC(pipe.packed()); break;
+            case fma_layout::WakePipeKind::PackedRing: RC(pipe.staged(true)); break;
+            case fma_layout::WakePipeKind::PackedZeroCopy: RC(pipe.in_place(true)); break;
             case fma_layout::WakePipeKind::Multipath: RC(pipe.multipath()); break;
             case fma_layout::WakePipeKind::Direct: RC(pipe.direct()); break;
-            case fma_layout::WakePipeKind::Kernel: case fma_layout::WakePipeKind::Staged: RC(pipe.paged()); break;
+            case fma_layout::WakePipeKind::Kernel: RC(pipe.in_place(false)); break;
+            case fma_layout::WakePipeKind::Staged: RC(pipe.staged(false)); break;
             }
             e->tl_add("enqueue", (int)copy_ops, t_enq0, now_s(), W);
         }
