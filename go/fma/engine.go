@@ -220,6 +220,30 @@ func (e *Engine) ImageAdoptParked(desc []byte, tagMask uint64) error {
 	return nil
 }
 
+// FileStore names the file the next file-tier sleep (Sleep(mask, C.FMA_TIER_FILE)) writes; "" forgets it.  The caller owns the file.
+func (e *Engine) FileStore(path string) error {
+	var cs *C.char
+	if path != "" {
+		cs = C.CString(path)
+		defer C.free(unsafe.Pointer(cs))
+	}
+	if rc := C.fma_file_store(e.h, cs); rc != 0 {
+		return lastErr(rc)
+	}
+	return nil
+}
+
+// ImageAdoptFile: a fully awake engine with the same segment sequence becomes "asleep in the file tier" with the image in `path`
+// (written by a file-tier sleep or by image_save); only the descriptor is read, WakeUp streams the data.
+func (e *Engine) ImageAdoptFile(path string, tagMask uint64, flags uint32) error {
+	cs := C.CString(path)
+	defer C.free(unsafe.Pointer(cs))
+	if rc := C.fma_image_adopt_file(e.h, cs, C.uint64_t(tagMask), C.uint32_t(flags)); rc != 0 {
+		return lastErr(rc)
+	}
+	return nil
+}
+
 // PathsSet names idle peer GPUs whose PCIe links a host-tier wake may borrow (MULTI-PATH wake); nil turns it off.
 func (e *Engine) PathsSet(helpers []int, slotBytes uint64, slots int) error {
 	var p *C.int

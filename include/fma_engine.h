@@ -48,6 +48,7 @@ extern "C" {
 #define FMA_ESTATE     -5   /* call not legal in the current sleep state                */
 #define FMA_ENOTFOUND  -6   /* unknown pointer / segment / tag                          */
 #define FMA_EINTEGRITY -7   /* digest mismatch after wake (only with FMA_FLAG_VERIFY)   */
+#define FMA_EIO        -8   /* a read or write of a file failed (a full disk included)  */
 
 /* ---- units ------------------------------------------------------------------------ */
 /* The engine's unit of placement is the 2 MiB VMM page (cuMemGetAllocationGranularity
@@ -61,6 +62,7 @@ extern "C" {
 #define FMA_TIER_HOST   0   /* pinned host-DRAM store over PCIe Gen5 (copy engines)      */
 #define FMA_TIER_PEER   1   /* peer-GPU HBM parking buffer over NVLink / NVSwitch        */
 #define FMA_TIER_LOCAL  2   /* parking buffer in the SAME GPU's HBM (kernel roofline/test)*/
+#define FMA_TIER_FILE   3   /* a file on local disk (fma_file_store): no host store while asleep */
 
 /* ---- data-path modes (how bytes cross the link) ----------------------------------- */
 #define FMA_MODE_AUTO     0
@@ -153,7 +155,9 @@ typedef struct fma_stats {
     uint64_t resident_bytes;        /* HBM the resident part of a sleeping host-tier image holds on this GPU now
                                        (option "resident_bytes"; its stored bytes, in one allocation rounded up to
                                        2 MiB); 0 when there is none                                          */
-    uint64_t reserved[2];
+    uint64_t io_buffer_bytes;       /* pinned host DRAM of the engine's file I/O windows (fma_load_file and the file tier;
+                                       pinned once per engine): all the host DRAM a file-tier sleeper holds        */
+    uint64_t reserved[1];
 } fma_stats_t;
 
 /* ---- library ---------------------------------------------------------------------- */
@@ -245,6 +249,34 @@ FMA_API int  fma_image_export(fma_engine_t* e, int* out_fd);          /* caller 
  * came from) and its device bytes must match the image's digests — then its device side is released and it shares that
  * image (one host copy per node instead of one per replica); on a mismatch nothing is touched and FMA_EINTEGRITY comes back. */
 FMA_API int  fma_image_adopt(fma_engine_t* e, int fd, uint64_t tag_mask, uint32_t flags);  /* fd stays owned by the caller */
+
+/* ---- FILE tier: a sleeping model's image on local disk, no host store while asleep ------------------------------------
+ * A host-tier sleeper holds its whole image in pinned host DRAM, and host DRAM is what limits the sleepers of a node.  In the
+ * reference a model that did not fit is deleted and cold-started (pkg/controller/dual-pods/inference-server.go:416-448).
+ * fma_sleep(..., FMA_TIER_FILE, ...) writes the image to the file named by fma_file_store: the STAGED pipeline (K1 gather, or
+ * K4 gather + encode with config.pack, into the HBM staging ring -> D2H into the engine's pinned I/O windows) with writer threads
+ * that pwrite each window at its place in the file.  fma_wake reads it back: reader threads pread ahead into the windows -> H2D into
+ * the ring -> K2 / K5.  The file has the layout image_save writes: the image bytes (the PACKED form's stored pages back to back),
+ * then the descriptor in the last 2 MiB, written after one fdatasync, so a torn file is never adopted.  I/O goes through O_DIRECT
+ * when the file's filesystem accepts it, else through the page cache with posix_fadvise(DONTNEED) behind it (timeline row
+ * "file_io": idx 1 = O_DIRECT, 0 = buffered; FMA_FILE_BUFFERED=1 forces the buffered path).  What stays in host DRAM is the I/O
+ * windows (fma_stats_t.io_buffer_bytes), pinned once per engine by fma_file_store / fma_image_adopt_file.
+ * Failures: the free space is checked (fstatvfs) before anything is released; if it is short, or the file cannot be opened,
+ * FMA_EIO comes back with the engine fully awake.  A unit is unmapped only after its bytes' pwrite has returned, so a sleep whose
+ * write fails half way (FMA_EIO) leaves every released segment in the file and a wake restores them.  A wake whose read fails
+ * (FMA_EIO, e.g. the file was truncated) is rolled back like any failed wake and can be retried.  The tier needs a staging ring:
+ * without HBM for one a sleep returns FMA_ENOMEM fully awake and a wake FMA_ENOMEM rolled back.  Combinations: PACKED both
+ * ways; INCREMENTAL clean sleeps only (the file outlives the wake: a clean sleep to the same path writes 0 bytes, anything else
+ * is a full sleep); the resident share and multi-path are ignored; fma_image_export, fma_image_describe and
+ * fma_host_store_share return FMA_ESTATE for a file-tier image (the file itself is the hand-over). */
+/* The file the next file-tier sleep writes (created or overwritten; the caller owns the path, the engine never unlinks it);
+ * NULL forgets the path.  Pins the engine's I/O windows if they are not yet pinned. */
+FMA_API int  fma_file_store(fma_engine_t* e, const char* path);
+/* Like fma_image_adopt, from a file written by a file-tier sleep or by image_save: the engine must be fully awake with the same
+ * segment sequence for tag_mask, and FMA_FLAG_VERIFY means sleep by adoption.  Reads only the descriptor tail, pins nothing
+ * else; the engine is then asleep in FMA_TIER_FILE and a wake streams the data from `path`.  A file whose descriptor does not
+ * parse (torn, foreign) is refused with FMA_EINVAL and nothing touched. */
+FMA_API int  fma_image_adopt_file(fma_engine_t* e, const char* path, uint64_t tag_mask, uint32_t flags);
 
 /* ---- MULTI-PATH wake: borrow idle peers' PCIe links ---------------------------------------------------------------------
  * A host-tier wake is bounded by ONE x16 Gen5 link (55.6 GB/s measured of 64): 0.29 s for Llama-3-8B however good the engine
@@ -371,6 +403,7 @@ typedef struct fma_load_stats {
 } fma_load_stats_t;
 
 #define FMA_LOAD_O_DIRECT (1u << 0)  /* bypass the page cache (4 KiB-aligned reads into the bounce ring)  */
+/* The bounce ring is the engine's pinned I/O windows, which the file tier shares; a failed read returns FMA_EINVAL. */
 
 FMA_API int  fma_load_file(fma_engine_t* e, const char* path, const fma_load_span_t* spans, uint32_t n_spans,
                            uint32_t flags, fma_load_stats_t* out_stats);
@@ -398,7 +431,8 @@ FMA_API int  fma_stats(fma_engine_t* e, fma_stats_t* out);
  * enqueue, copies_landed, wait_all_mapped, drain, unmap (sleep), kernel (K1/K2/K4/K5 launches, device-timed), total;
  * multi-path operations add path_chunks / path_local (idx = the path's GPU, bytes = what that path moved / moved NUMA-locally);
  * a resident share adds res_alloc (sleep) / res_free (wake) for the resident buffer's VMM calls, res_fallback (its allocation
- * failed: plain sleep), and res_gather / res_restore rows for its K1 / K4 and K2 / K5 launches (device-timed, like kernel).
+ * failed: plain sleep), and res_gather / res_restore rows for its K1 / K4 and K2 / K5 launches (device-timed, like kernel); the
+ * file tier adds file_io (idx 1 = O_DIRECT, 0 = page cache; from the file's open to its last write / read returned, bytes = file bytes).
  * The reference has no tracing on this path (SURVEY.md section 5); this is what shows WHICH phase bounds a wake.
  * Returns the length of the full text (call with buf=NULL to size it), or a negative error. */
 FMA_API int  fma_timeline(fma_engine_t* e, char* buf, size_t cap);

@@ -9,13 +9,13 @@ FMA_PAGE_BYTES = 2 << 20
 FMA_PACKED_PAGE_BYTES = (3 << 19) + (16 << 10)   # stored size of a page in the "FMP4" code (csrc/fma_codec.h)
 FMA_MAX_TAGS = 64
 
-FMA_OK, FMA_EINVAL, FMA_ENODRIVER, FMA_ECUDA, FMA_ENOMEM, FMA_ESTATE, FMA_ENOTFOUND, FMA_EINTEGRITY = (
-    0, -1, -2, -3, -4, -5, -6, -7)
+FMA_OK, FMA_EINVAL, FMA_ENODRIVER, FMA_ECUDA, FMA_ENOMEM, FMA_ESTATE, FMA_ENOTFOUND, FMA_EINTEGRITY, FMA_EIO = (
+    0, -1, -2, -3, -4, -5, -6, -7, -8)
 ERROR_NAMES = {
     FMA_EINVAL: "FMA_EINVAL", FMA_ENODRIVER: "FMA_ENODRIVER", FMA_ECUDA: "FMA_ECUDA", FMA_ENOMEM: "FMA_ENOMEM",
-    FMA_ESTATE: "FMA_ESTATE", FMA_ENOTFOUND: "FMA_ENOTFOUND", FMA_EINTEGRITY: "FMA_EINTEGRITY",
+    FMA_ESTATE: "FMA_ESTATE", FMA_ENOTFOUND: "FMA_ENOTFOUND", FMA_EINTEGRITY: "FMA_EINTEGRITY", FMA_EIO: "FMA_EIO",
 }
-FMA_TIER_HOST, FMA_TIER_PEER, FMA_TIER_LOCAL = 0, 1, 2
+FMA_TIER_HOST, FMA_TIER_PEER, FMA_TIER_LOCAL, FMA_TIER_FILE = 0, 1, 2, 3
 FMA_MODE_AUTO, FMA_MODE_DIRECT, FMA_MODE_STAGED, FMA_MODE_KERNEL = 0, 1, 2, 3
 FMA_KERNEL_TMA, FMA_KERNEL_LDG = 0, 1
 FMA_FLAG_VERIFY, FMA_FLAG_KEEP_BACKUP = 1, 2
@@ -61,7 +61,7 @@ class fma_stats_t(C.Structure):
         ("total_kernel_launches", C.c_uint64), ("total_copy_ops", C.c_uint64),
         ("hbm_mapped_bytes", C.c_uint64), ("hbm_aux_bytes", C.c_uint64), ("parked_bytes", C.c_uint64),
         ("image_store_bytes", C.c_uint64), ("sleep_bytes_copied", C.c_uint64), ("resident_bytes", C.c_uint64),
-        ("reserved", C.c_uint64 * 2),
+        ("io_buffer_bytes", C.c_uint64), ("reserved", C.c_uint64 * 1),
     ]
 
     def as_dict(self) -> dict:
@@ -136,6 +136,8 @@ _PROTOTYPES = {
                                 C.POINTER(fma_load_stats_t)]),
     "fma_image_export": (C.c_int, [C.c_void_p, C.POINTER(C.c_int)]),
     "fma_image_adopt": (C.c_int, [C.c_void_p, C.c_int, C.c_uint64, C.c_uint32]),
+    "fma_file_store": (C.c_int, [C.c_void_p, C.c_char_p]),
+    "fma_image_adopt_file": (C.c_int, [C.c_void_p, C.c_char_p, C.c_uint64, C.c_uint32]),
     "fma_set_option": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int64]),
     "fma_stats": (C.c_int, [C.c_void_p, C.POINTER(fma_stats_t)]),
     "fma_timeline": (C.c_int, [C.c_void_p, C.c_char_p, C.c_size_t]),

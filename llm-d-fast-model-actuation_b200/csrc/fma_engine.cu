@@ -617,7 +617,7 @@ int paths_fail(fma_engine_t* e, int rc) {
 
 int park_release(fma_engine_t* e) {
     if (!e->park.va) return FMA_OK;
-    if (e->shadow_tier != FMA_TIER_HOST) invalidate_shadows(e);  // the parking buffer held the kept image
+    if (e->shadow_tier == FMA_TIER_PEER || e->shadow_tier == FMA_TIER_LOCAL) invalidate_shadows(e);  // the parking buffer held the kept image
     cudaDeviceSynchronize();
     vmm_buffer_free(e->park);
     return FMA_OK;
@@ -666,7 +666,7 @@ bool image_in(fma_engine_t* e, ImageIn where) {
         if (!s.has_backup) continue;
         switch (where) {
             case ImageIn::Host: if (s.backup_tier == FMA_TIER_HOST) return true; break;
-            case ImageIn::NotHost: if (s.backup_tier != FMA_TIER_HOST) return true; break;
+            case ImageIn::NotHost: if (s.backup_tier != FMA_TIER_HOST && s.backup_tier != FMA_TIER_FILE) return true; break;
             case ImageIn::Local: if (!s.mapped && s.backup_tier == FMA_TIER_LOCAL) return true; break;
             case ImageIn::AnyAsleep: if (!s.mapped) return true; break;
         }
@@ -795,8 +795,8 @@ int check_tma_shape(const fma_engine_t* e, int tier) {
 uint64_t store_dev_base(const fma_engine_t* e, int tier) {
     return tier == FMA_TIER_HOST ? (uint64_t)(uintptr_t)e->host.dev_alias : (uint64_t)e->park.va;
 }
-void* store_copy_base(const fma_engine_t* e, int tier) {
-    return tier == FMA_TIER_HOST ? e->host.base : reinterpret_cast<void*>(e->park.va);
+void* store_copy_base(const fma_engine_t* e, int tier) {   // (the FILE tier has no store in memory)
+    return tier == FMA_TIER_HOST ? e->host.base : tier == FMA_TIER_FILE ? nullptr : reinterpret_cast<void*>(e->park.va);
 }
 
 // ------------------------------------------------------------------------------------
@@ -1648,6 +1648,7 @@ int fma_stats(fma_engine_t* e, fma_stats_t* out) {
     out->image_packed = e->image_packed ? 1 : 0;
     out->image_store_bytes = e->image_store_bytes;
     out->resident_bytes = e->res.va ? e->res_store_bytes : 0;
+    out->io_buffer_bytes = e->load_ring_bytes;
     return FMA_OK;
 }
 

@@ -127,6 +127,7 @@ int fma_image_export(fma_engine_t* e, int* out_fd) {
     std::lock_guard<std::mutex> op(e->op_mu);
     if (!out_fd) return fail(FMA_EINVAL, "out_fd is NULL");
     if (resident_asleep(e)) return fail(FMA_ESTATE, "part of the sleeping image is resident in this process's own HBM (option resident_bytes) and cannot be handed over: set it to 0 and sleep again");
+    if (e->image_tier == FMA_TIER_FILE && image_in(e, ImageIn::AnyAsleep)) return fail(FMA_ESTATE, "the sleeping image is in a file: the file itself is the hand-over");
     if (e->host.fd < 0 || !e->host.base) return fail(FMA_ESTATE, "the host store is not shareable (set FMA_HOST_STORE_SHM=1 before the first sleep)");
     if (e->image_tier != FMA_TIER_HOST) return fail(FMA_ESTATE, "no host-tier image");
     std::vector<char> desc;
@@ -237,6 +238,63 @@ int fma_image_adopt(fma_engine_t* e, int fd, uint64_t tag_mask, uint32_t flags) 
     return FMA_OK;
 }
 
+// ---- FILE tier (see include/fma_engine.h) -----------------------------------------------------------------------------
+
+int fma_file_store(fma_engine_t* e, const char* path) {
+    if (check_engine(e) != FMA_OK) return FMA_EINVAL;
+    std::lock_guard<std::mutex> op(e->op_mu);
+    if (!path) {
+        e->file_path.clear();
+        return FMA_OK;
+    }
+    if (!*path) return fail(FMA_EINVAL, "empty path");
+    DeviceGuard guard(e->device);
+    if (!e->load_ring) RC(ensure_io_windows(e));   // pinned once per engine, never inside a sleep or wake
+    e->file_path = path;
+    return FMA_OK;
+}
+
+int fma_image_adopt_file(fma_engine_t* e, const char* path, uint64_t tag_mask, uint32_t flags) {
+    if (check_engine(e) != FMA_OK) return FMA_EINVAL;
+    std::lock_guard<std::mutex> op(e->op_mu);
+    if (!path || !tag_mask) return fail(FMA_EINVAL, "adopt needs the file and the tag mask the image was slept with");
+    {
+        std::lock_guard<std::mutex> lk(e->mu);
+        for (const Segment& s : e->segs)
+            if (!s.mapped) return fail(FMA_ESTATE, "adopt needs a fully awake engine");
+    }
+    FileFd f;
+    f.fd = open(path, O_RDONLY | O_CLOEXEC);
+    if (f.fd < 0) return fail(FMA_EIO, "cannot open %s: %s", path, strerror(errno));
+    struct stat sb;
+    if (fstat(f.fd, &sb) != 0 || (size_t)sb.st_size <= kImageTail) return fail(FMA_EINVAL, "%s is not an image file", path);
+    const size_t cap = (size_t)sb.st_size - kImageTail;
+    std::vector<char> tail(kImageTail);
+    for (size_t got = 0; got < kImageTail;) {
+        const ssize_t n = pread(f.fd, tail.data() + got, kImageTail - got, (off_t)(cap + got));
+        if (n < 0 && errno == EINTR) continue;
+        if (n <= 0) return fail(FMA_EIO, "cannot read the descriptor of %s: %s", path, n < 0 ? strerror(errno) : "the file ends early");
+        got += (size_t)n;
+    }
+    ParsedImage pi;
+    RC(image_descriptor_parse(e, tail.data(), kImageTail, cap, tag_mask, &pi));
+    DeviceGuard guard(e->device);
+    cudaDeviceSynchronize();
+    if (flags & FMA_FLAG_VERIFY) {  // "sleep by adoption" (see fma_image_adopt): only if this engine's bytes ARE the image's
+        std::vector<uint64_t> now;
+        RC(digest_segments(e, pi.order, &now));
+        for (size_t i = 0; i < pi.ds.size(); ++i)
+            if (!pi.ds[i].digest_valid || pi.ds[i].digest != now[i])
+                return fail(FMA_EINTEGRITY, pi.ds[i].digest_valid ? "the image holds different bytes than this engine's segments" : "the image carries no digests to compare with");
+    }
+    if (!e->load_ring) RC(ensure_io_windows(e));
+    invalidate_shadows(e);
+    RC(do_sleep(e, tag_mask, FMA_TIER_FILE, (flags & ~FMA_FLAG_VERIFY) | kFlagAdopt));
+    image_apply(e, pi);
+    e->image_file = path;
+    return FMA_OK;
+}
+
 // ---- the same hand-over for an image PARKED in peer HBM (fma_peer_attach'ed buffer of a node-level owner) ----------------
 // The buffer itself is the owner's; what has to travel is the descriptor: the owner keeps it next to the fd.
 
@@ -245,6 +303,7 @@ int fma_image_describe(fma_engine_t* e, int tier, void* buf, size_t cap) {
     std::lock_guard<std::mutex> op(e->op_mu);
     if (resident_asleep(e)) return fail(FMA_ESTATE, "part of the sleeping image is resident in this process's own HBM (option resident_bytes) and cannot be handed over: set it to 0 and sleep again");
     if (tier != e->image_tier) return fail(FMA_ESTATE, "no image sleeps in tier %d", tier);
+    if (tier == FMA_TIER_FILE) return fail(FMA_ESTATE, "the sleeping image is in a file: the file itself is the hand-over (its descriptor is its tail)");
     std::vector<char> desc;
     RC(image_descriptor_build(e, tier, &desc));
     if (buf && cap >= desc.size()) memcpy(buf, desc.data(), desc.size());

@@ -3,7 +3,7 @@
 //   fma_engine.cu   errors, driver resolution, VMM primitives, arenas, engine resources, stores, allocator, the C-ABI
 //   fma_sleep.cu    SLEEP pipeline (do_sleep) and the PACKED image plan
 //   fma_wake.cu     WAKE pipeline (do_wake)
-//   fma_load.cu     cold load: file -> HBM (fma_load_file)
+//   fma_load.cu     file I/O: reader / writer threads over the pinned I/O windows (cold load fma_load_file, FILE tier)
 //   fma_image.cu    image hand-over between engines / processes (fma_image_export / fma_image_adopt)
 //
 // Everything below lives in namespace fma_impl; the library is built with -fvisibility=hidden, so none of it is exported.
@@ -298,10 +298,13 @@ struct fma_engine {
     uint64_t* h_dig = nullptr;
     size_t desc_cap = 0;
 
-    // cold-load bounce ring (pinned host), persistent and small
+    // I/O windows (pinned host), persistent and small: the cold load's bounce ring and the FILE tier's disk stage.  Pinned with
+    // the load_* options in force when ensure_io_windows last ran; an operation uses them as they are
     void* load_ring = nullptr;
     size_t load_ring_bytes = 0;
-    std::vector<cudaEvent_t> ev_load;
+    size_t io_window_bytes = 0;          // each window: a load chunk + 8 KiB of O_DIRECT alignment slack
+    int io_windows = 0;
+    std::vector<cudaEvent_t> ev_load;    // per window: the copy into / out of it has finished
     int load_threads = 12;               // pread from the page cache is the limiter: enough readers to keep
     size_t load_chunk = (size_t)16 << 20;  // one PCIe Gen5 link busy (tests/tools/load_bench.py measures it)
     int load_slots = 24;
@@ -313,6 +316,10 @@ struct fma_engine {
     PullMailbox* mbox = nullptr;             // remote paths (fma_paths_attach): shared with the node-level owner
     int mbox_fd = -1;
     uint64_t pull_generation = 0;
+
+    // FILE tier
+    std::string file_path;               // fma_file_store: where the next file-tier sleep writes ("" = nowhere)
+    std::string image_file;              // the file the last file-tier image was written to / adopted from (read by the wake)
 
     fma_k_tma_cfg tma = fma_k_default_tma_cfg();
     fma_stats_t st{};
@@ -397,7 +404,7 @@ void resident_release(fma_engine_t* e);              // drop the resident buffer
 // Does a segment's image live in the store `where` names (takes e->mu)?
 enum class ImageIn {
     Host,           // the host store
-    NotHost,        // the parking buffer: any tier but the host's, so a resident share (FMA_TIER_LOCAL) counts too
+    NotHost,        // the parking buffer: any tier but the host's and the file's, so a resident share (FMA_TIER_LOCAL) counts too
     Local,          // FMA_TIER_LOCAL, with the segment unmapped
     AnyAsleep,      // any store, with the segment unmapped
 };
@@ -408,6 +415,62 @@ CUmemAllocationProp device_prop(int device);
 // ---- image descriptor (fma_image.cu): what a sleeping image is made of, so another engine / process can adopt it ----
 int image_descriptor_build(fma_engine_t* e, int tier, std::vector<char>* out);
 void invalidate_shadows(fma_engine_t* e);   // the host store no longer holds a usable copy of any segment
+// ---- file I/O (fma_load.cu) ----
+int ensure_io_windows(fma_engine_t* e);   // pin the I/O windows for the current load_* options (and their events)
+// Opens `path` for the FILE tier (write: created, not truncated), with O_DIRECT when the filesystem accepts it and
+// FMA_FILE_BUFFERED is not 1; *direct tells which.  Failure: FMA_EIO.
+int open_image_file(const char* path, bool write, int* fd, bool* direct);
+struct FileFd {   // closes on every exit path
+    int fd = -1;
+    ~FileFd() { if (fd >= 0) close(fd); }
+};
+// Reader or writer threads over the engine's pinned I/O windows.  Item k of `items` goes through window k % io_windows, and the
+// caller's thread enqueues the copy of every item, in item order, recording event(k) on the copy's stream right behind it:
+//   read:  readers pread item k into its window -> wait_read(k) returns its bytes -> the caller enqueues the H2D out of them ->
+//          posted(k): the reader of item k + n reuses the window once event(k) has completed
+//   write: wait_free(k) returns item k's window once the pwrite of item k - n has returned -> the caller enqueues the D2H into it ->
+//          posted(k): a writer pwrites item k once event(k) has completed
+// With O_DIRECT a read may start below its item and a write must be 4 KiB aligned (the FILE tier's always are).  In the page
+// cache's mode every range read or written is dropped from it behind the I/O (posix_fadvise DONTNEED).
+class FileIO {
+  public:
+    struct Item {
+        uint64_t file_off, bytes;
+    };
+    FileIO(fma_engine_t* e, int fd, bool write, bool direct, std::vector<Item> items, uint64_t file_bytes, const char* path);
+    ~FileIO();
+    const char* wait_read(size_t k);   // nullptr: the I/O failed (finish() has the error)
+    char* wait_free(size_t k);
+    cudaEvent_t event(size_t k) const { return e_->ev_load[k % n_]; }
+    void posted(size_t k);
+    size_t written();                  // items whose pwrite has returned, as a prefix of `items`
+    int finish();                      // joins the threads and waits for every posted copy; FMA_OK or the first error (FMA_EIO / FMA_ECUDA)
+    double io_seconds() const { return io_ns_.load() * 1e-9; }
+    int threads() const { return (int)th_.size(); }
+
+  private:
+    void worker();
+    void set_error(int code, const char* fmt, ...);
+    int stop();                        // finish() without setting the thread's error message
+    fma_engine_t* e_;
+    int fd_;
+    bool write_, direct_;
+    std::vector<Item> items_;
+    uint64_t file_bytes_;
+    const char* path_;
+    int n_;
+    std::mutex mu_;
+    std::condition_variable cv_;
+    std::vector<char> ready_, posted_, done_;   // read: item read; both: copy enqueued; write: pwrite returned
+    size_t written_ = 0, n_posted_ = 0, n_posted_items_ = 0;   // n_posted_: 1 + the highest item posted
+    std::atomic<size_t> next_{0};
+    std::atomic<uint64_t> io_ns_{0};
+    int error_ = FMA_OK;
+    char msg_[512] = "";
+    std::vector<std::thread> th_;
+    bool stopped_ = false;
+};
+
 // ---- pipelines ----
 int do_sleep(fma_engine_t* e, uint64_t offload_mask, int tier, uint32_t flags);   // fma_sleep.cu
 int do_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags);                  // fma_wake.cu

@@ -249,13 +249,14 @@ inline std::vector<char> resident_split(const std::vector<uint64_t>& stored, uin
 // ---- which pipeline a sleep / wake runs ----
 // The configured mode as a tier runs it: AUTO is STAGED on the host tier, KERNEL on the parking tiers (staging helps over PCIe).
 inline int resolve_mode(int cfg_mode, int tier) {
+    if (tier == FMA_TIER_FILE) return FMA_MODE_STAGED;   // the file tier has one pipeline: the staging ring with a disk stage
     int m = cfg_mode;
     if (m == FMA_MODE_AUTO) m = (tier == FMA_TIER_HOST) ? FMA_MODE_STAGED : FMA_MODE_KERNEL;
     if (tier != FMA_TIER_HOST && m == FMA_MODE_STAGED) m = FMA_MODE_KERNEL;
     return m;
 }
 
-enum class SleepPipeKind { Adopt, PartialDirect, PartialPacked, Direct, Kernel, KernelPacked, Staged, StagedPacked, Multipath };
+enum class SleepPipeKind { Adopt, PartialDirect, PartialPacked, Direct, Kernel, KernelPacked, Staged, StagedPacked, Multipath, File, FilePacked, NoRing };
 
 // What a sleep knows when it picks its pipeline.  `ring` and `worth_packing` are answers of calls with side effects (a ring
 // allocation, the K4p probe): ask with both true, make the calls the route wants, then ask again with the answers.
@@ -278,6 +279,11 @@ inline SleepRoute sleep_route(const SleepFacts& f) {
     if (f.adopt || f.clean) return SleepRoute{SleepPipeKind::Adopt, f.mode, false, false};
     if (f.partial_packed) return SleepRoute{SleepPipeKind::PartialPacked, f.mode, false, false};
     if (f.partial) return SleepRoute{SleepPipeKind::PartialDirect, FMA_MODE_DIRECT, false, false};
+    // FILE: the ring-staged pipeline with a disk stage behind it, PACKED when asked and worth it; without a ring nothing moves
+    if (f.tier == FMA_TIER_FILE) {
+        const SleepPipeKind k = !f.ring ? SleepPipeKind::NoRing : f.pack && f.worth_packing ? SleepPipeKind::FilePacked : SleepPipeKind::File;
+        return SleepRoute{k, FMA_MODE_STAGED, true, f.pack};
+    }
     SleepRoute r{SleepPipeKind::Staged, f.mode, false, false};
     // MULTI-PATH: a full, plain host-tier sleep is striped over the paths' links, each with its own staging slots
     const bool multipath = f.paths && !f.mbox && f.tier == FMA_TIER_HOST && f.mode == FMA_MODE_STAGED && !f.pack && f.multipath_env;
@@ -293,7 +299,7 @@ inline SleepRoute sleep_route(const SleepFacts& f) {
     return r;
 }
 
-enum class WakePipeKind { PackedRing, PackedZeroCopy, Direct, Kernel, Staged, Multipath };
+enum class WakePipeKind { PackedRing, PackedZeroCopy, Direct, Kernel, Staged, Multipath, File, NoRing };
 
 // What a wake knows when it picks its pipeline; `ring` as in SleepFacts (a ring attached to the first run, or allocated).
 struct WakeFacts {
@@ -309,6 +315,8 @@ struct WakeRoute {
 };
 
 inline WakeRoute wake_route(const WakeFacts& f) {
+    // FILE: plain or PACKED pages come through the ring (FMA_NO_RING: as if HBM had no room for one)
+    if (f.tier == FMA_TIER_FILE) return WakeRoute{f.moves && (f.no_ring || !f.ring) ? WakePipeKind::NoRing : WakePipeKind::File, FMA_MODE_STAGED, f.moves && !f.no_ring};
     // a PACKED image can only be read by K5: through the staging ring, or straight from the store
     WakeRoute r{WakePipeKind::Staged, f.image_packed && f.tier == FMA_TIER_HOST ? FMA_MODE_STAGED : f.mode, false};
     const bool multipath = f.paths && f.tier == FMA_TIER_HOST && r.mode == FMA_MODE_STAGED && !f.image_packed;

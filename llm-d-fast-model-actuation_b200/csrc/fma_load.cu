@@ -1,6 +1,194 @@
-// fma_load.cu — cold load: checkpoint file -> HBM through a pinned bounce ring and the copy engines (SURVEY.md §8f-3)
+// fma_load.cu — file I/O: reader / writer threads over a small ring of pinned host windows, for the cold load (checkpoint file ->
+// HBM, SURVEY.md §8f-3) and for the FILE tier's sleep and wake (fma_sleep.cu / fma_wake.cu)
 // Part of the host engine (see fma_internal.h for the map of translation units; C-ABI in include/fma_engine.h).
 #include "fma_internal.h"
+
+namespace fma_impl {
+
+int ensure_io_windows(fma_engine_t* e) {
+    const int n_slots = e->load_slots;
+    const size_t slot_bytes = e->load_chunk + 8192;  // slack for O_DIRECT alignment on both ends
+    if (e->io_windows != n_slots || e->io_window_bytes != slot_bytes) {
+        if (e->load_ring) cudaFreeHost(e->load_ring);
+        e->load_ring = nullptr;
+        e->load_ring_bytes = 0;
+        e->io_windows = 0;
+        e->io_window_bytes = 0;
+        cudaError_t r = cudaHostAlloc(&e->load_ring, slot_bytes * n_slots, cudaHostAllocPortable);
+        if (r != cudaSuccess) {
+            cudaGetLastError();
+            e->load_ring = nullptr;
+            return fail(FMA_ENOMEM, "cannot pin the %zu byte I/O windows: %s", slot_bytes * n_slots, cudaGetErrorString(r));
+        }
+        e->load_ring_bytes = slot_bytes * n_slots;
+        e->io_windows = n_slots;
+        e->io_window_bytes = slot_bytes;
+    }
+    while ((int)e->ev_load.size() < n_slots) {
+        cudaEvent_t ev;
+        RT(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+        e->ev_load.push_back(ev);
+    }
+    return FMA_OK;
+}
+
+int open_image_file(const char* path, bool write, int* fd, bool* direct) {
+    const int flags = (write ? O_WRONLY | O_CREAT : O_RDONLY) | O_CLOEXEC;
+    *direct = env_int("FMA_FILE_BUFFERED", 0) == 0;
+    *fd = *direct ? open(path, flags | O_DIRECT, 0644) : -1;
+    if (*fd < 0 && *direct && errno != EINVAL) return fail(FMA_EIO, "cannot open %s: %s", path, strerror(errno));
+    if (*fd < 0) {   // the filesystem refuses O_DIRECT (EINVAL), or the page cache was asked for
+        *direct = false;
+        *fd = open(path, flags, 0644);
+        if (*fd < 0) return fail(FMA_EIO, "cannot open %s: %s", path, strerror(errno));
+    }
+    return FMA_OK;
+}
+
+FileIO::FileIO(fma_engine_t* e, int fd, bool write, bool direct, std::vector<Item> items, uint64_t file_bytes, const char* path)
+    : e_(e), fd_(fd), write_(write), direct_(direct), items_(std::move(items)), file_bytes_(file_bytes), path_(path), n_(e->io_windows),
+      ready_(items_.size(), 0), posted_(items_.size(), 0), done_(items_.size(), 0) {
+    if (!n_ || !e->load_ring) {
+        set_error(FMA_ESTATE, "the engine's I/O windows are not pinned");
+        return;
+    }
+    for (const Item& it : items_)
+        if (it.bytes > e->io_window_bytes - 8192 || (direct_ && write_ && ((it.file_off | it.bytes) & 4095))) {
+            set_error(FMA_EINVAL, "I/O item of %llu bytes at %llu does not fit a window", (unsigned long long)it.bytes, (unsigned long long)it.file_off);
+            return;
+        }
+    const int n_threads = std::max(1, std::min<int>(e->load_threads, (int)std::max<size_t>(items_.size(), 1)));
+    for (int t = 0; t < n_threads && !items_.empty(); ++t) th_.emplace_back([this] { worker(); });
+}
+
+FileIO::~FileIO() { stop(); }   // (keeps the message of whatever made the caller leave)
+
+void FileIO::set_error(int code, const char* fmt, ...) {
+    std::lock_guard<std::mutex> lk(mu_);
+    if (error_ == FMA_OK) {
+        error_ = code;
+        va_list ap;
+        va_start(ap, fmt);
+        vsnprintf(msg_, sizeof(msg_), fmt, ap);
+        va_end(ap);
+    }
+    cv_.notify_all();
+}
+
+void FileIO::worker() {
+    cudaSetDevice(e_->device);
+    for (;;) {
+        const size_t k = next_.fetch_add(1);
+        if (k >= items_.size()) break;
+        const size_t w = k % n_;
+        {   // read: the window's last copy has been enqueued (k - n posted); write: this item's D2H has been enqueued
+            std::unique_lock<std::mutex> lk(mu_);
+            cv_.wait(lk, [&] { return error_ != FMA_OK || (write_ ? posted_[k] : (k < (size_t)n_ || posted_[k - n_])); });
+            if (error_ != FMA_OK) break;
+        }
+        if (write_ || k >= (size_t)n_) {   // ... and has finished
+            const cudaError_t r = cudaEventSynchronize(e_->ev_load[w]);
+            if (r != cudaSuccess) return set_error(FMA_ECUDA, "cudaEventSynchronize(I/O window) failed: %s", cudaGetErrorString(r));
+        }
+        char* buf = static_cast<char*>(e_->load_ring) + w * e_->io_window_bytes;
+        char* abuf = direct_ ? reinterpret_cast<char*>(round_up(reinterpret_cast<uintptr_t>(buf), 4096)) : buf;
+        const Item& it = items_[k];
+        const double t0 = now_s();
+        uint64_t done = 0;
+        int err = 0;
+        if (write_) {
+            while (done < it.bytes) {
+                const ssize_t n = pwrite(fd_, abuf + done, it.bytes - done, (off_t)(it.file_off + done));
+                if (n < 0 && errno == EINTR) continue;
+                if (n <= 0) { err = n < 0 ? errno : ENOSPC; break; }
+                done += (uint64_t)n;
+            }
+        } else {
+            const uint64_t a_off = direct_ ? (it.file_off & ~4095ull) : it.file_off;
+            const uint64_t delta = it.file_off - a_off, need = delta + it.bytes;
+            uint64_t want = direct_ ? round_up(need, 4096) : it.bytes;   // at most the window (a chunk + 8 KiB of slack)
+            const uint64_t end = round_up(file_bytes_, 4096);              // O_DIRECT reads stop at the file's last block
+            if (direct_) want = a_off >= end ? 0 : std::min(want, end - a_off);
+            while (done < need) {
+                const ssize_t n = pread(fd_, abuf + done, want - done, (off_t)(a_off + done));
+                if (n < 0 && errno == EINTR) continue;
+                if (n <= 0) { err = n < 0 ? errno : 0; break; }
+                done += (uint64_t)n;
+            }
+            if (done < need) done = UINT64_MAX;
+        }
+        io_ns_.fetch_add((uint64_t)((now_s() - t0) * 1e9));
+        if (write_ ? done < it.bytes : done == UINT64_MAX)
+            return set_error(FMA_EIO, "%s of %llu bytes at offset %llu of %s failed: %s", write_ ? "write" : "read", (unsigned long long)it.bytes,
+                             (unsigned long long)it.file_off, path_, err ? strerror(err) : "the file ends early");
+        if (!direct_) posix_fadvise(fd_, (off_t)it.file_off, (off_t)it.bytes, POSIX_FADV_DONTNEED);   // (written pages go after fdatasync)
+        std::lock_guard<std::mutex> lk(mu_);
+        if (write_) {
+            done_[k] = 1;
+            while (written_ < items_.size() && done_[written_]) ++written_;
+        } else {
+            ready_[k] = 1;
+        }
+        cv_.notify_all();
+    }
+}
+
+const char* FileIO::wait_read(size_t k) {
+    std::unique_lock<std::mutex> lk(mu_);
+    cv_.wait(lk, [&] { return error_ != FMA_OK || ready_[k]; });
+    if (error_ != FMA_OK) return nullptr;
+    const char* buf = static_cast<const char*>(e_->load_ring) + (k % n_) * e_->io_window_bytes;
+    if (direct_) buf = reinterpret_cast<const char*>(round_up(reinterpret_cast<uintptr_t>(buf), 4096)) + (items_[k].file_off & 4095);
+    return buf;
+}
+
+char* FileIO::wait_free(size_t k) {
+    std::unique_lock<std::mutex> lk(mu_);
+    cv_.wait(lk, [&] { return error_ != FMA_OK || k < (size_t)n_ || done_[k - n_]; });
+    if (error_ != FMA_OK) return nullptr;
+    char* buf = static_cast<char*>(e_->load_ring) + (k % n_) * e_->io_window_bytes;
+    return direct_ ? reinterpret_cast<char*>(round_up(reinterpret_cast<uintptr_t>(buf), 4096)) : buf;
+}
+
+void FileIO::posted(size_t k) {
+    std::lock_guard<std::mutex> lk(mu_);
+    posted_[k] = 1;
+    n_posted_ = std::max(n_posted_, k + 1);
+    ++n_posted_items_;
+    cv_.notify_all();
+}
+
+size_t FileIO::written() {
+    std::lock_guard<std::mutex> lk(mu_);
+    return written_;
+}
+
+int FileIO::stop() {
+    if (!stopped_) {
+        {   // the caller stopped before its last item (its own error): threads that wait for a copy it will never post leave
+            std::lock_guard<std::mutex> lk(mu_);
+            if (error_ == FMA_OK && n_posted_items_ < items_.size()) {
+                error_ = FMA_ESTATE;
+                snprintf(msg_, sizeof(msg_), "file I/O of %s stopped before its last item", path_);
+            }
+            cv_.notify_all();
+        }
+        for (auto& t : th_) t.join();
+        for (size_t w = 0; w < std::min<size_t>(n_posted_, (size_t)n_); ++w) {   // nothing may still copy into or out of a window
+            const cudaError_t r = cudaEventSynchronize(e_->ev_load[w]);
+            if (r != cudaSuccess && error_ == FMA_OK) {
+                error_ = FMA_ECUDA;
+                snprintf(msg_, sizeof(msg_), "cudaEventSynchronize(I/O window) failed: %s", cudaGetErrorString(r));
+            }
+        }
+        stopped_ = true;
+    }
+    return error_;
+}
+
+int FileIO::finish() { return stop() == FMA_OK ? FMA_OK : fail(error_, "%s", msg_); }
+
+}  // namespace fma_impl
 
 using namespace fma_impl;
 
@@ -14,26 +202,21 @@ int fma_load_file(fma_engine_t* e, const char* path, const fma_load_span_t* span
     DeviceGuard guard(e->device);
     RC(ensure_streams(e));
     const bool direct = (flags & FMA_LOAD_O_DIRECT) != 0;
-    int fd = open(path, O_RDONLY | (direct ? O_DIRECT : 0));
-    if (fd < 0) return fail(FMA_EINVAL, "cannot open %s: %s", path, strerror(errno));
+    FileFd f;
+    f.fd = open(path, O_RDONLY | (direct ? O_DIRECT : 0));
+    if (f.fd < 0) return fail(FMA_EINVAL, "cannot open %s: %s", path, strerror(errno));
     struct stat sb;
-    if (fstat(fd, &sb) != 0) {
-        close(fd);
-        return fail(FMA_EINVAL, "fstat(%s) failed: %s", path, strerror(errno));
-    }
+    if (fstat(f.fd, &sb) != 0) return fail(FMA_EINVAL, "fstat(%s) failed: %s", path, strerror(errno));
     // every destination must be device memory this engine has mapped; every source range must be inside the file
-    struct Item { uint64_t file_off, bytes, dst; };
-    std::vector<Item> items;
+    std::vector<FileIO::Item> items;
+    std::vector<uint64_t> dst;
     uint64_t total = 0;
     {
         std::lock_guard<std::mutex> lk(e->mu);
         for (uint32_t i = 0; i < n_spans; ++i) {
             const fma_load_span_t& sp = spans[i];
             if (!sp.bytes) continue;
-            if (sp.file_offset + sp.bytes > (uint64_t)sb.st_size) {
-                close(fd);
-                return fail(FMA_EINVAL, "span %u reads past the end of %s", i, path);
-            }
+            if (sp.file_offset + sp.bytes > (uint64_t)sb.st_size) return fail(FMA_EINVAL, "span %u reads past the end of %s", i, path);
             // the range may span several VA-adjacent mapping units (segments of one arena sit back to back)
             bool ok = true;
             for (uint64_t pos = sp.dst, end = sp.dst + sp.bytes; pos < end;) {
@@ -44,130 +227,45 @@ int fma_load_file(fma_engine_t* e, const char* path, const fma_load_span_t* span
                 if (pos < it->second.va || pos >= u_end) { ok = false; break; }
                 pos = u_end;
             }
-            if (!ok) {
-                close(fd);
-                return fail(FMA_EINVAL, "span %u: destination 0x%llx+%llu is not inside a mapped segment", i,
-                            (unsigned long long)sp.dst, (unsigned long long)sp.bytes);
+            if (!ok)
+                return fail(FMA_EINVAL, "span %u: destination 0x%llx+%llu is not inside a mapped segment", i, (unsigned long long)sp.dst,
+                            (unsigned long long)sp.bytes);
+            for (uint64_t o = 0; o < sp.bytes; o += e->load_chunk) {
+                items.push_back(FileIO::Item{sp.file_offset + o, std::min<uint64_t>(e->load_chunk, sp.bytes - o)});
+                dst.push_back(sp.dst + o);
             }
-            for (uint64_t o = 0; o < sp.bytes; o += e->load_chunk)
-                items.push_back(Item{sp.file_offset + o, std::min<uint64_t>(e->load_chunk, sp.bytes - o), sp.dst + o});
             total += sp.bytes;
         }
     }
-    const int n_slots = e->load_slots;
-    const size_t slot_bytes = e->load_chunk + 8192;  // slack for O_DIRECT alignment on both ends
-    if (e->load_ring_bytes < slot_bytes * n_slots) {
-        if (e->load_ring) cudaFreeHost(e->load_ring);
-        e->load_ring = nullptr;
-        e->load_ring_bytes = 0;
-        cudaError_t r = cudaHostAlloc(&e->load_ring, slot_bytes * n_slots, cudaHostAllocPortable);
-        if (r != cudaSuccess) {
-            cudaGetLastError();
-            close(fd);
-            return fail(FMA_ENOMEM, "cannot pin the %zu byte load ring: %s", slot_bytes * n_slots, cudaGetErrorString(r));
-        }
-        e->load_ring_bytes = slot_bytes * n_slots;
+    RC(ensure_io_windows(e));
+    // readers pread ahead into the windows; this thread moves each chunk to its destination as soon as it has been read
+    FileIO io(e, f.fd, false, direct, items, (uint64_t)sb.st_size, path);
+    for (size_t k = 0; k < items.size(); ++k) {
+        const char* src = io.wait_read(k);
+        if (!src) break;
+        cudaStream_t st = e->cs[k % e->n_cs];
+        RT(cudaMemcpyAsync(reinterpret_cast<void*>((uintptr_t)dst[k]), src, items[k].bytes, cudaMemcpyHostToDevice, st));
+        RT(cudaEventRecord(io.event(k), st));
+        io.posted(k);
     }
-    while ((int)e->ev_load.size() < n_slots) {
-        cudaEvent_t ev;
-        cudaError_t r = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
-        if (r != cudaSuccess) {
-            close(fd);
-            return fail(FMA_ECUDA, "cudaEventCreate failed: %s", cudaGetErrorString(r));
-        }
-        e->ev_load.push_back(ev);
+    int rc = io.finish();
+    for (int i = 0; i < e->n_cs; ++i) RT(cudaStreamSynchronize(e->cs[i]));
+    if (rc == FMA_EIO) {   // a failed read of a cold load has always been FMA_EINVAL
+        char why[512];
+        snprintf(why, sizeof(why), "%s", tl_err);
+        rc = fail(FMA_EINVAL, "%s", why);
     }
-    // Slot s is used by items s, s+n, s+2n, ... strictly in that order (threads run ahead of each other):
-    // slot_gen[s] counts the uses whose H2D has been ENQUEUED; the event tells when that H2D has finished.
-    std::mutex mu;
-    std::condition_variable cv;
-    std::vector<uint64_t> slot_gen(n_slots, 0);
-    std::atomic<size_t> next{0};
-    std::atomic<uint64_t> read_ns{0};
-    int error = FMA_OK;
-    char msg[512] = "";
-    const int n_threads = std::max(1, std::min<int>(e->load_threads, (int)std::max<size_t>(items.size(), 1)));
-    auto worker = [&]() {
-        cudaSetDevice(e->device);
-        for (;;) {
-            const size_t k = next.fetch_add(1);
-            if (k >= items.size()) break;
-            const int s = (int)(k % n_slots);
-            const uint64_t my_gen = k / n_slots;
-            {
-                std::unique_lock<std::mutex> lk(mu);
-                cv.wait(lk, [&] { return slot_gen[s] == my_gen || error != FMA_OK; });
-                if (error != FMA_OK) break;
-            }
-            char* buf = static_cast<char*>(e->load_ring) + (size_t)s * slot_bytes;
-            if (my_gen > 0) {
-                cudaError_t r = cudaEventSynchronize(e->ev_load[s]);  // the previous chunk in this slot has left
-                if (r != cudaSuccess) {
-                    std::lock_guard<std::mutex> lk(mu);
-                    if (error == FMA_OK) { error = FMA_ECUDA; snprintf(msg, sizeof(msg), "cudaEventSynchronize: %s", cudaGetErrorString(r)); }
-                    cv.notify_all();
-                    break;
-                }
-            }
-            const Item& it = items[k];
-            const uint64_t a_off = direct ? (it.file_off & ~4095ull) : it.file_off;
-            const uint64_t delta = it.file_off - a_off;
-            uint64_t want = direct ? round_up(delta + it.bytes, 4096) : it.bytes;
-            if (direct && a_off + want > (uint64_t)round_up((size_t)sb.st_size, 4096)) want = round_up((size_t)sb.st_size, 4096) - a_off;
-            char* rbuf = direct ? reinterpret_cast<char*>(round_up(reinterpret_cast<uintptr_t>(buf), 4096)) : buf;
-            const double t0 = now_s();
-            uint64_t got = 0;
-            bool io_err = false;
-            while (got < (direct ? delta + it.bytes : it.bytes)) {
-                ssize_t n = pread(fd, rbuf + got, want - got, (off_t)(a_off + got));
-                if (n < 0 && errno == EINTR) continue;
-                if (n <= 0) { io_err = (got < delta + it.bytes); break; }
-                got += (uint64_t)n;
-            }
-            read_ns.fetch_add((uint64_t)((now_s() - t0) * 1e9));
-            cudaError_t r = cudaSuccess;
-            if (!io_err) {
-                cudaStream_t st = e->cs[k % e->n_cs];
-                r = cudaMemcpyAsync(reinterpret_cast<void*>((uintptr_t)it.dst), rbuf + delta, it.bytes, cudaMemcpyHostToDevice, st);
-                if (r == cudaSuccess) r = cudaEventRecord(e->ev_load[s], st);
-            }
-            std::lock_guard<std::mutex> lk(mu);
-            if (io_err || r != cudaSuccess) {
-                if (error == FMA_OK) {
-                    error = io_err ? FMA_EINVAL : FMA_ECUDA;
-                    snprintf(msg, sizeof(msg), io_err ? "short read at offset %llu of %s: %s" : "H2D of chunk at %llu failed (%s): %s",
-                             (unsigned long long)it.file_off, path, io_err ? strerror(errno) : cudaGetErrorString(r));
-                }
-            } else {
-                slot_gen[s] = my_gen + 1;
-            }
-            cv.notify_all();
-            if (error != FMA_OK) break;
-        }
-    };
-    std::vector<std::thread> th;
-    for (int t = 0; t < n_threads; ++t) th.emplace_back(worker);
-    for (auto& t : th) t.join();
-    close(fd);
-    for (int i = 0; i < e->n_cs; ++i) {
-        cudaError_t r = cudaStreamSynchronize(e->cs[i]);
-        if (r != cudaSuccess && error == FMA_OK) {
-            error = FMA_ECUDA;
-            snprintf(msg, sizeof(msg), "cudaStreamSynchronize failed: %s", cudaGetErrorString(r));
-        }
-    }
-    if (error != FMA_OK) return fail(error, "%s", msg);
+    if (rc != FMA_OK) return rc;
     e->st.total_copy_ops += items.size();
     if (out_stats) {
         memset(out_stats, 0, sizeof(*out_stats));
         out_stats->seconds = now_s() - t_entry;
-        out_stats->read_seconds = read_ns.load() * 1e-9;
+        out_stats->read_seconds = io.io_seconds();
         out_stats->bytes = total;
         out_stats->chunks = (uint32_t)items.size();
-        out_stats->threads = (uint32_t)n_threads;
+        out_stats->threads = (uint32_t)io.threads();
     }
     return FMA_OK;
 }
-
 
 }  // extern "C"

@@ -3,6 +3,8 @@
 #include "fma_internal.h"
 #include "fma_gate.h"
 
+#include <sys/statvfs.h>
+
 namespace fma_impl {
 
 namespace {
@@ -146,7 +148,8 @@ struct Unmapper {
         RT(cudaEventRecord(*out, stream));
         return FMA_OK;
     }
-    // everything whose bytes are inside image[0, image_done) and has been read by work enqueued on `stream` so far
+    // everything whose bytes are inside image[0, image_done) and has been read by work enqueued on `stream` so far (no stream:
+    // those bytes are in the store already, the FILE tier's written frontier)
     int publish_consumed(uint64_t image_done, cudaStream_t stream) {
         Stage st;
         while (next_unit < off_units.size() && off_units[next_unit].image_end <= image_done) {
@@ -154,7 +157,8 @@ struct Unmapper {
             ++next_unit;
         }
         if (st.ranges.empty()) return FMA_OK;
-        RC(stage_event(stream, &st.ev));
+        st.ev = nullptr;
+        if (stream) RC(stage_event(stream, &st.ev));
         {
             std::lock_guard<std::mutex> lk(mu);
             stages.push_back(std::move(st));
@@ -198,7 +202,7 @@ struct Unmapper {
                 if (k >= stages.size()) break;
                 st = stages[k];
             }
-            cudaError_t r = cudaEventSynchronize(st.ev);
+            cudaError_t r = st.ev ? cudaEventSynchronize(st.ev) : cudaSuccess;
             if (r != cudaSuccess) {
                 std::lock_guard<std::mutex> lk(mu);
                 if (error == FMA_OK) {
@@ -287,6 +291,7 @@ struct SleepPipe {
     int in_place(bool packed);
     int staged(bool packed);
     int multipath();
+    int file(bool packed, int fd, bool direct, const char* path);
 };
 
 // DIRECT: copy engines move each segment chunk straight into the packed image
@@ -379,6 +384,57 @@ int SleepPipe::staged(bool packed) {
     return subset ? publish_consumed(W, last_stream) : FMA_OK;  // the clean tail of the image needs no copy
 }
 
+// FILE: the STAGED pipeline with a disk stage behind it.  K1 gather / K4 gather + encode -> HBM ring slot -> D2H into the engine's
+// pinned I/O windows -> writer threads pwrite each window at its place in the file.  A unit is released once every byte of it has
+// been WRITTEN (the writes' frontier, not the D2H's), so a sleep whose write fails half way leaves every released segment in the file.
+int SleepPipe::file(bool packed, int fd, bool direct, const char* path) {
+    std::vector<PagePlan> pages;
+    RC(plan(packed, &pages));   // (the route has the ring)
+    std::vector<Batch> slots;
+    if (!fma_layout::plan_batches(pages, packed ? SIZE_MAX : e->ring_slot_bytes / FMA_PAGE_BYTES, packed ? e->ring_slot_bytes : UINT64_MAX, true, &slots))
+        return fail(FMA_EINVAL, "ring slot of %zu bytes cannot hold one page", e->ring_slot_bytes);
+    const std::vector<uint64_t> in_ring = ring_addresses(e, pages, slots);
+    PageKernels pk{e, kt, true, packed};
+    RC(pk.prepare(pages, true, [&](size_t q) { return in_ring[q]; }));
+    // every slot cut into window-sized writes; slot c's are items [slot_end[c - 1], slot_end[c])
+    const uint64_t piece = e->io_window_bytes - 8192;
+    std::vector<FileIO::Item> items;
+    std::vector<size_t> slot_end;
+    for (const Batch& sl : slots) {
+        for (uint64_t o = 0; o < sl.stored; o += piece) items.push_back(FileIO::Item{pages[sl.p0].off + o, std::min(piece, sl.stored - o)});
+        slot_end.push_back(items.size());
+    }
+    FileIO io(e, fd, true, direct, items, 0, path);
+    size_t k = 0, slots_written = 0;
+    auto publish_written = [&]() -> int {   // units whose every page is in a slot that has been written are dead
+        const size_t n = io.written();
+        while (slots_written < slots.size() && slot_end[slots_written] <= n) ++slots_written;
+        return slots_written ? publish_consumed((uint64_t)(slots[slots_written - 1].p0 + slots[slots_written - 1].np) * FMA_PAGE_BYTES, nullptr) : FMA_OK;
+    };
+    for (size_t c = 0; c < slots.size(); ++c) {
+        const Batch& sl = slots[c];
+        const int slot = (int)(c % e->n_ring);
+        cudaStream_t cstream = e->cs[c % e->n_cs];
+        if (c >= (size_t)e->n_ring) RT(cudaStreamWaitEvent(e->ks, e->ev_ring_free[slot], 0));
+        RC(pk.launch(sl, (uint64_t)(uintptr_t)e->ring[slot]));
+        RT(cudaEventRecord(e->ev_ring_full[slot], e->ks));
+        RT(cudaStreamWaitEvent(cstream, e->ev_ring_full[slot], 0));
+        for (; k < slot_end[c]; ++k) {
+            char* window = io.wait_free(k);
+            if (!window) return io.finish();
+            RC(publish_written());
+            RT(cudaMemcpyAsync(window, static_cast<char*>(e->ring[slot]) + (items[k].file_off - pages[sl.p0].off), items[k].bytes,
+                               cudaMemcpyDeviceToHost, cstream));
+            RT(cudaEventRecord(io.event(k), cstream));
+            io.posted(k);
+            ++copy_ops;
+        }
+        RT(cudaEventRecord(e->ev_ring_free[slot], cstream));
+    }
+    RC(io.finish());   // every pwrite has returned
+    return publish_consumed(W, nullptr);
+}
+
 // MULTI-PATH sleep (fma_paths_set): the mirror image of the multi-path wake.  K1 on the sleeping GPU gathers a chunk of the image
 // into a staging slot of a PATH — its own HBM, or a helper GPU's HBM over NVLink — and THAT GPU's copy engine moves the slot into
 // the host store over THAT GPU's x16 link; chunk queues per NUMA node of the (striped) store, self-balancing.  Nothing is unmapped
@@ -468,6 +524,9 @@ struct SleepPlan {
     KernelTimes kt;
     uint32_t copy_ops = 0;
     double copy_s = 0;
+    FileFd file;                      // FILE tier: the file this sleep writes, opened by size_store
+    bool file_direct = false;
+    double file_t0 = 0;
     SleepPlan(fma_engine_t* e, int t, uint32_t f) : tier(t), flags(f), timer{e}, kt{e} {}
     bool adopt() const { return (flags & kFlagAdopt) || clean || !W; }  // not a byte moves (the route is then Adopt)
 };
@@ -475,6 +534,12 @@ struct SleepPlan {
 fma_layout::SleepFacts sleep_facts(const fma_engine_t* e, const SleepPlan& p) {
     return fma_layout::SleepFacts{p.tier, fma_layout::resolve_mode(e->cfg.mode, p.tier), e->cfg.pack != 0, !e->paths.empty(), e->mbox != nullptr,
                                   (p.flags & kFlagAdopt) || !p.W, p.clean, p.partial, p.partial_packed, env_int("FMA_MULTIPATH_SLEEP", 1) != 0};
+}
+
+// `path` is a file of an image of store_bytes (plus the descriptor tail)
+bool file_holds(const std::string& path, uint64_t store_bytes) {
+    struct stat sb;
+    return store_bytes && stat(path.c_str(), &sb) == 0 && (uint64_t)sb.st_size == store_bytes + kImageTail;
 }
 
 // 1. offloaded segments -> packed image, in (arena, VA) order.  Arenas are bump-allocated per tag, so this is allocation order
@@ -487,7 +552,9 @@ void plan_image(fma_engine_t* e, uint64_t offload_mask, SleepPlan& p) {
         return x.arena != y.arena ? x.arena < y.arena : x.va < y.va;
     });
     // the store that would hold the kept image: the host store, or the parking buffer of the same (peer / local) tier
+    // or (FILE) the file the last file-tier image went to, when this sleep writes the same path and the file has that image's size
     p.kept_store = p.tier == FMA_TIER_HOST ? e->host.base != nullptr
+                 : p.tier == FMA_TIER_FILE ? !e->file_path.empty() && e->file_path == e->image_file && file_holds(e->image_file, e->shadow_store_bytes)
                                            : (e->park.va != 0 && (p.tier == FMA_TIER_LOCAL ? e->park.device == e->device : e->park.device != e->device));
     p.shadows_match = e->incremental && p.tier == e->shadow_tier && !(p.flags & kFlagAdopt) && p.kept_store;
     for (size_t i : by_addr) {
@@ -593,7 +660,7 @@ int check_incremental(fma_engine_t* e, SleepPlan& p) {
     p.shadows_match = p.shadows_match && p.res_seqs == e->res_seqs;  // a different split is a full sleep
     e->res_seqs = p.res_seqs;
     const uint64_t W = p.W;
-    if (!p.shadows_match || !W || W != e->shadow_image_bytes || (p.tier == FMA_TIER_HOST ? e->host.cap : e->park.bytes) < e->shadow_store_bytes) return FMA_OK;
+    if (!p.shadows_match || !W || W != e->shadow_image_bytes || (p.tier == FMA_TIER_HOST ? e->host.cap : p.tier == FMA_TIER_FILE ? e->shadow_store_bytes : e->park.bytes) < e->shadow_store_bytes) return FMA_OK;
     RT(cudaDeviceSynchronize());  // the caller's streams may still be writing weights
     std::vector<uint64_t> now;
     RC(digest_and_mark(e, p.ex, &now));  // either way these are the digests of what sleeps now
@@ -629,6 +696,7 @@ int route_sleep(fma_engine_t* e, SleepPlan& p) {
     fma_layout::SleepFacts f = sleep_facts(e, p);
     if (fma_layout::sleep_route(f).wants_ring) f.ring = !no_ring() && ensure_ring(e, p.W) == FMA_OK;
     p.route = fma_layout::sleep_route(f);
+    if (p.route.pipe == fma_layout::SleepPipeKind::NoRing) return fail(FMA_ENOMEM, "the file tier needs an HBM staging ring and there is no room for one");
     const bool kept = p.clean || p.partial_packed;  // the image in the store, its form and its page table stay as they are
     if (kept) {
         p.packed = e->shadow_packed;
@@ -651,8 +719,51 @@ int route_sleep(fma_engine_t* e, SleepPlan& p) {
     return FMA_OK;
 }
 
+// FILE: open the file, check that the filesystem has room for the image and its descriptor, and only then empty the file
+int open_file_store(fma_engine_t* e, SleepPlan& p) {
+    if (e->file_path.empty()) return fail(FMA_ESTATE, "the file tier needs fma_file_store(path) first");
+    if (!e->load_ring) return fail(FMA_ESTATE, "the engine's I/O windows are not pinned");
+    p.file_t0 = now_s();
+    RC(open_image_file(e->file_path.c_str(), true, &p.file.fd, &p.file_direct));
+    struct statvfs vs;
+    struct stat sb;
+    if (fstatvfs(p.file.fd, &vs) != 0 || fstat(p.file.fd, &sb) != 0) return fail(FMA_EIO, "fstatvfs(%s) failed: %s", e->file_path.c_str(), strerror(errno));
+    const uint64_t need = p.Wp + kImageTail, room = (uint64_t)vs.f_bavail * vs.f_frsize + (uint64_t)sb.st_blocks * 512;  // (its own blocks come back)
+    if (room < need)
+        return fail(FMA_EIO, "%s: %llu bytes free, the image needs %llu", e->file_path.c_str(), (unsigned long long)room, (unsigned long long)need);
+    if (ftruncate(p.file.fd, 0) != 0) return fail(FMA_EIO, "ftruncate(%s) failed: %s", e->file_path.c_str(), strerror(errno));
+    e->image_file = e->file_path;
+    return FMA_OK;
+}
+
+// After the last write: fdatasync, then the descriptor in the last kImageTail bytes (a torn file fails descriptor parsing).
+int close_file_store(fma_engine_t* e, SleepPlan& p) {
+    const char* path = e->image_file.c_str();
+    if (fdatasync(p.file.fd) != 0) return fail(FMA_EIO, "fdatasync(%s) failed: %s", path, strerror(errno));
+    std::vector<char> desc;
+    RC(image_descriptor_build(e, FMA_TIER_FILE, &desc));
+    desc.resize(kImageTail, 0);
+    void* buf = nullptr;
+    if (posix_memalign(&buf, 4096, kImageTail) != 0) return fail(FMA_ENOMEM, "no memory for the descriptor");
+    memcpy(buf, desc.data(), kImageTail);
+    uint64_t done = 0;
+    while (done < kImageTail) {
+        const ssize_t n = pwrite(p.file.fd, static_cast<char*>(buf) + done, kImageTail - done, (off_t)(p.Wp + done));
+        if (n < 0 && errno == EINTR) continue;
+        if (n <= 0) break;
+        done += (uint64_t)n;
+    }
+    const int err = errno;
+    free(buf);
+    if (done < kImageTail) return fail(FMA_EIO, "writing the descriptor of %s failed: %s", path, strerror(err));
+    if (fdatasync(p.file.fd) != 0) return fail(FMA_EIO, "fdatasync(%s) failed: %s", path, strerror(errno));
+    if (!p.file_direct) posix_fadvise(p.file.fd, 0, 0, POSIX_FADV_DONTNEED);   // clean now: the page cache lets go of the image
+    e->tl_add("file_io", p.file_direct ? 1 : 0, p.file_t0, now_s(), p.Wp + kImageTail);
+    return FMA_OK;
+}
+
 // 5. a store of the tier that holds Wp bytes
-int size_store(fma_engine_t* e, const SleepPlan& p) {
+int size_store(fma_engine_t* e, SleepPlan& p) {
     if (!p.W) return FMA_OK;
     if (p.tier == FMA_TIER_HOST && p.adopt()) {
         if (!e->host.base) return fail(FMA_ESTATE, "adopt without a store");  // the adopted store IS the image: never re-sized
@@ -668,6 +779,8 @@ int size_store(fma_engine_t* e, const SleepPlan& p) {
             return fail(FMA_ESTATE, "peer tier needs fma_peer_reserve(peer_device, >= %llu bytes) first", (unsigned long long)p.Wp);
     } else if (p.tier == FMA_TIER_LOCAL) {
         return park_reserve(e, e->device, p.Wp);
+    } else if (p.tier == FMA_TIER_FILE) {
+        if (!p.adopt()) return open_file_store(e, p);   // (an adopted or clean image is in its file already)
     } else {
         return fail(FMA_EINVAL, "unknown tier %d", p.tier);
     }
@@ -721,6 +834,9 @@ int run_pipeline(fma_engine_t* e, SleepPlan& p, Unmapper& un) {
         case SleepPipeKind::Multipath: RC(pipe.multipath()); break;
         case SleepPipeKind::StagedPacked: RC(pipe.staged(true)); break;
         case SleepPipeKind::Staged: RC(pipe.staged(false)); break;
+        case SleepPipeKind::File: RC(pipe.file(false, p.file.fd, p.file_direct, e->image_file.c_str())); break;
+        case SleepPipeKind::FilePacked: RC(pipe.file(true, p.file.fd, p.file_direct, e->image_file.c_str())); break;
+        case SleepPipeKind::NoRing:   // (refused by route_sleep)
         case SleepPipeKind::Adopt: return fail(FMA_ESTATE, "an adopted image has no copy pipeline");  // (handled above)
         }
         un.close();
@@ -738,7 +854,7 @@ int run_pipeline(fma_engine_t* e, SleepPlan& p, Unmapper& un) {
 
 // 8. apply what the unmapper did to the table, then unmap whatever is left (FMA_OVERLAP_UNMAP=0, nothing offloaded, ...) —
 // every unit goes (cumem.py:213), VAs stay reserved; then the stats
-int finish_sleep(fma_engine_t* e, const SleepPlan& p, Unmapper& un, ApplyUnmapped& apply_unmapped, double t_entry) {
+int finish_sleep(fma_engine_t* e, SleepPlan& p, Unmapper& un, ApplyUnmapped& apply_unmapped, double t_entry) {
     un.finish();
     if (un.error != FMA_OK) return fail(un.error, "%s", un.msg);
     for (const Extent& x : p.ex) mark_backed_up(e, x, p.tier);
@@ -757,6 +873,7 @@ int finish_sleep(fma_engine_t* e, const SleepPlan& p, Unmapper& un, ApplyUnmappe
     }
     e->image_bytes = p.W;
     e->image_tier = p.tier;
+    if (p.file.fd >= 0) RC(close_file_store(e, p));   // (the image is asleep in the file either way: a wake reads what was written)
 
     e->tl_add("total", 0, t_entry, now_s(), p.W_all);
     e->st.sleep_seconds = now_s() - t_entry;

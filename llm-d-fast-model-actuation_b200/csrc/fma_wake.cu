@@ -152,6 +152,12 @@ struct Mapper {
         retract_gate();
         cudaDeviceSynchronize();
         cudaGetLastError();
+        // a wake that failed before the mapper reached the ring run: that ring never came to exist (as when its mapping fails),
+        // so its VA goes back to the arena and the engine forgets it; else a retry would take the unmapped range for its ring
+        if (ring_run && !item_done[0] && e->ring_attached && e->ring_unit_va == runs[0].va) {
+            arena_give_back(e->arenas[runs[0].arena], runs[0].va - e->arenas[runs[0].arena].base, runs[0].bytes);
+            release_ring(e);
+        }
         for (size_t k = 0; k < runs.size(); ++k) {
             if (!item_done[k]) continue;
             for (size_t i : runs[k].segs) {
@@ -218,6 +224,7 @@ struct WakePipe {
     int in_place(bool packed);
     int staged(bool packed);
     int multipath();
+    int file(bool packed);
 };
 
 // The segments `idx` as the page planner sees them: each waits for the mapper work item of its run.
@@ -331,6 +338,66 @@ int WakePipe::staged(bool packed) {
         RT(cudaEventRecord(e->ev_ring_free[slot], e->ks));
         if (between) RC(between->pump(sl.p0 + sl.np, n_pages));
     }
+    return FMA_OK;
+}
+
+// FILE: the STAGED pipeline with a disk stage in front of it.  Reader threads pread ahead into the engine's pinned I/O windows ->
+// H2D window -> ring slot -> K2 scatter / K5 decode + scatter once the targets are mapped (the same mapper.wait / ev_ring_* protocol).
+int WakePipe::file(bool packed) {
+    std::vector<PagePlan> pages;
+    RC(plan(packed, &pages));
+    std::vector<Batch> slots;
+    if (!fma_layout::plan_batches(pages, packed ? SIZE_MAX : e->ring_slot_bytes / FMA_PAGE_BYTES, packed ? e->ring_slot_bytes : UINT64_MAX, true, &slots))
+        return fail(FMA_EINVAL, "ring slot of %zu bytes cannot hold one page", e->ring_slot_bytes);
+    const std::vector<uint64_t> in_ring = ring_addresses(e, pages, slots);
+    PageKernels pk{e, kt, false, packed};
+    RC(pk.prepare(pages, true, [&](size_t q) { return in_ring[q]; }));
+    const double t_io = now_s();
+    const char* path = e->image_file.c_str();
+    FileFd f;
+    bool direct = false;
+    RC(open_image_file(path, false, &f.fd, &direct));
+    struct stat sb;
+    if (fstat(f.fd, &sb) != 0) return fail(FMA_EIO, "fstat(%s) failed: %s", path, strerror(errno));
+    const uint64_t piece = e->io_window_bytes - 8192;
+    std::vector<FileIO::Item> items;
+    std::vector<size_t> slot_end;
+    uint64_t file_bytes = 0;
+    for (const Batch& sl : slots) {
+        for (uint64_t o = 0; o < sl.stored; o += piece) items.push_back(FileIO::Item{pages[sl.p0].off + o, std::min(piece, sl.stored - o)});
+        slot_end.push_back(items.size());
+        file_bytes += sl.stored;
+    }
+    // the file must hold every byte this wake reads (else it was truncated or replaced): refused before a read is issued
+    const uint64_t file_end = items.empty() ? 0 : items.back().file_off + items.back().bytes;
+    for (const FileIO::Item& it : items)
+        if (it.file_off + it.bytes > (uint64_t)sb.st_size)
+            return fail(FMA_EIO, "%s holds %llu bytes, the image needs %llu", path, (unsigned long long)sb.st_size, (unsigned long long)file_end);
+    FileIO io(e, f.fd, false, direct, items, (uint64_t)sb.st_size, path);
+    if (ring_run) RC(mapper.wait(1));  // (as in staged)
+    size_t k = 0;
+    for (size_t c = 0; c < slots.size(); ++c) {
+        const Batch& sl = slots[c];
+        const int slot = (int)(c % e->n_ring);
+        cudaStream_t cstream = e->cs[c % e->n_cs];
+        if (c >= (size_t)e->n_ring) RT(cudaStreamWaitEvent(cstream, e->ev_ring_free[slot], 0));
+        for (; k < slot_end[c]; ++k) {
+            const char* src = io.wait_read(k);
+            if (!src) return io.finish();
+            RT(cudaMemcpyAsync(static_cast<char*>(e->ring[slot]) + (items[k].file_off - pages[sl.p0].off), src, items[k].bytes,
+                               cudaMemcpyHostToDevice, cstream));
+            RT(cudaEventRecord(io.event(k), cstream));
+            io.posted(k);
+            copied();
+        }
+        RT(cudaEventRecord(e->ev_ring_full[slot], cstream));
+        RC(mapper.wait(sl.need));
+        RT(cudaStreamWaitEvent(e->ks, e->ev_ring_full[slot], 0));
+        RC(pk.launch(sl, (uint64_t)(uintptr_t)e->ring[slot]));
+        RT(cudaEventRecord(e->ev_ring_free[slot], e->ks));
+    }
+    RC(io.finish());   // every read has returned and every H2D out of a window has finished
+    e->tl_add("file_io", direct ? 1 : 0, t_io, now_s(), file_bytes);
     return FMA_OK;
 }
 
@@ -670,7 +737,7 @@ int do_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags) {
     const bool res_packed = W_res && e->res_packed;   // (the buffer may be released before the K5 error count is read)
     if (W || W_res) {
         const char* store = static_cast<const char*>(store_copy_base(e, tier));
-        if (W && !store) return fail(FMA_ESTATE, "backup store of tier %d is gone", tier);
+        if (W && !store && tier != FMA_TIER_FILE) return fail(FMA_ESTATE, "backup store of tier %d is gone", tier);
         if (W && tier == FMA_TIER_HOST && route.mode == FMA_MODE_KERNEL && !e->host.dev_alias)
             return fail(FMA_ECUDA, "host store has no device alias for zero-copy mode");
         RC(timer.begin());
@@ -685,6 +752,8 @@ int do_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags) {
             case fma_layout::WakePipeKind::Direct: RC(pipe.direct()); break;
             case fma_layout::WakePipeKind::Kernel: RC(pipe.in_place(false)); break;
             case fma_layout::WakePipeKind::Staged: RC(pipe.staged(false)); break;
+            case fma_layout::WakePipeKind::File: RC(pipe.file(facts.image_packed)); break;
+            case fma_layout::WakePipeKind::NoRing: return fail(FMA_ENOMEM, "the file tier needs an HBM staging ring and there is no room for one");
             }
             e->tl_add("enqueue", (int)copy_ops, t_enq0, now_s(), W);
         }

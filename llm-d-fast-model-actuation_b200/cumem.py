@@ -24,6 +24,7 @@ over several copy-engine streams overlapped with cuMemCreate/cuMemMap.
 """
 from __future__ import annotations
 
+import atexit
 import dataclasses
 import gc
 import json
@@ -53,8 +54,23 @@ class AllocationData:
 
 
 def _tier_from_env() -> int:
-    return {"host": L.FMA_TIER_HOST, "peer": L.FMA_TIER_PEER, "local": L.FMA_TIER_LOCAL}[
+    return {"host": L.FMA_TIER_HOST, "peer": L.FMA_TIER_PEER, "local": L.FMA_TIER_LOCAL, "file": L.FMA_TIER_FILE}[
         os.environ.get("FMA_TIER", "host").lower()]
+
+
+def _file_tier_path() -> str:
+    """FMA_TIER=file: this rank's image file, ``<FMA_FILE_DIR>/<instance id>-r<rank>.fmaimg`` (removed when the process exits)."""
+    d = os.environ.get("FMA_FILE_DIR")
+    if not d:
+        raise L.FmaError(L.FMA_EINVAL, "FMA_TIER=file needs FMA_FILE_DIR=<directory on a local disk>")
+    return os.path.join(d, f"{_instance_id()}-r{_rank()}.fmaimg")
+
+
+def _remove_file(path: str) -> None:
+    try:
+        os.unlink(path)
+    except OSError:
+        pass
 
 
 class CuMemAllocator:
@@ -86,6 +102,7 @@ class CuMemAllocator:
         self.current_tag: str = CuMemAllocator.default_tag
         self.allocator_and_pools: dict[str, Any] = {}
         self._reserve_thread: threading.Thread | None = None
+        self._file_path: str | None = None     # FMA_TIER=file: this rank's image file, once named
         # MULTI-PATH wake across processes (FMA_REMOTE_PATHS=k): the node agent's helper GPUs pull for this instance; that needs the
         # host store as a memfd the agent can map, so the switch is thrown before the store is first reserved
         self._remote = None
@@ -142,6 +159,10 @@ class CuMemAllocator:
                         raise
                     logger.warning("fma_b200: GPU %d cannot take %.2f GiB right now (%s): sleeping to the host tier instead", peer, nbytes / 1024**3, e.message)
                     tier = L.FMA_TIER_HOST
+        elif tier == L.FMA_TIER_FILE and self._file_path is None:
+            self._file_path = _file_tier_path()
+            self.engine.file_store(self._file_path)
+            atexit.register(_remove_file, self._file_path)
         deposit_host = (tier == L.FMA_TIER_HOST and os.environ.get("FMA_DEPOSIT_HOST_IMAGE") == "1" and os.environ.get("FMA_NODE_AGENT_SOCK")
                         and os.environ.get("FMA_HOST_STORE_SHM") == "1")
         if deposit_host:
@@ -149,7 +170,14 @@ class CuMemAllocator:
             if int(os.environ.get("FMA_RESIDENT_MIB", "0") or 0) > 0:
                 logger.warning("fma_b200: FMA_DEPOSIT_HOST_IMAGE=1 takes precedence over FMA_RESIDENT_MIB: the whole image goes to the host store")
             self.engine.set_option("resident_bytes", 0)
-        self.engine.sleep(offload_tags, tier=tier)
+        try:
+            self.engine.sleep(offload_tags, tier=tier)
+        except L.FmaError as e:
+            # the file tier refused before releasing anything (no room on the disk, no HBM for its staging ring): the host tier works
+            if tier != L.FMA_TIER_FILE or e.code not in (L.FMA_EIO, L.FMA_ENOMEM) or self.engine.is_sleeping():
+                raise
+            logger.warning("fma_b200: cannot sleep to %s (%s): sleeping to the host tier instead", self._file_path, e.message)
+            self.engine.sleep(offload_tags, tier=L.FMA_TIER_HOST)
         if owner is not None and self.engine.stats()["sleep_bytes_offloaded"]:
             owner.deposit(self.engine, _instance_id(), _rank(), tier)
         elif deposit_host and self.engine.stats()["sleep_bytes_offloaded"]:
@@ -268,7 +296,7 @@ class CuMemAllocator:
             self.engine.wake(["weights"], flags=L.FMA_FLAG_VERIFY)
             st = self.engine.stats()
             logger.info("fma_b200: adopted the parked image of instance %s rank %d: %.2f GiB restored from %s in %.3f s (digests verified)",
-                        _instance_id(), _rank(), st["wake_bytes_restored"] / 1024**3, "the host store" if st["tier"] == L.FMA_TIER_HOST else "peer HBM",
+                        _instance_id(), _rank(), st["wake_bytes_restored"] / 1024**3, {L.FMA_TIER_HOST: "the host store", L.FMA_TIER_PEER: "peer HBM"}.get(st["tier"], f"tier {st['tier']}"),
                         time.perf_counter() - t0)
         except L.FmaError as e:
             if self.engine.is_sleeping():

@@ -331,6 +331,17 @@ class Engine:
         finally:
             os.close(fd)
 
+    # -- FILE tier ------------------------------------------------------------------------
+    def file_store(self, path: str | None) -> None:
+        """The file the next ``sleep(tier=FMA_TIER_FILE)`` writes (None forgets it).  The caller owns the file; the engine never
+        removes it.  Pins the engine's I/O windows (``stats()["io_buffer_bytes"]``) the first time."""
+        check(self._lib.fma_file_store(self._h, None if path is None else path.encode()))
+
+    def image_adopt_file(self, path: str, tags: Sequence[str], flags: int = 0) -> None:
+        """Become 'asleep in the file tier' with the image in ``path`` (written by a file-tier sleep or by ``image_save``): this
+        engine must hold the same segment sequence for ``tags``.  Reads only the descriptor; ``wake`` streams the data."""
+        check(self._lib.fma_image_adopt_file(self._h, path.encode(), self.tag_mask(tags), flags))
+
     # -- cold load -------------------------------------------------------------------------
     def load_file(self, path: str, spans: Sequence[tuple[int, int, int]], o_direct: bool = False) -> dict:
         """Stream (file_offset, nbytes, device_address) spans of one file into mapped segments."""
