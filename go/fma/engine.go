@@ -244,6 +244,15 @@ func (e *Engine) ImageAdoptFile(path string, tagMask uint64, flags uint32) error
 	return nil
 }
 
+// MoveImage moves the sleeping image to `tier` without waking it (host DRAM, a file named by FileStore, a peer's or this GPU's
+// parking buffer).  The source store stays allocated until HostRelease / PeerRelease; a source file is never touched.
+func (e *Engine) MoveImage(tier int) error {
+	if rc := C.fma_image_move(e.h, C.int(tier)); rc != 0 {
+		return lastErr(rc)
+	}
+	return nil
+}
+
 // PathsSet names idle peer GPUs whose PCIe links a host-tier wake may borrow (MULTI-PATH wake); nil turns it off.
 func (e *Engine) PathsSet(helpers []int, slotBytes uint64, slots int) error {
 	var p *C.int

@@ -278,6 +278,31 @@ FMA_API int  fma_file_store(fma_engine_t* e, const char* path);
  * parse (torn, foreign) is refused with FMA_EINVAL and nothing touched. */
 FMA_API int  fma_image_adopt_file(fma_engine_t* e, const char* path, uint64_t tag_mask, uint32_t flags);
 
+/* ---- moving a sleeping image between tiers, without waking it ----------------------------------------------------------
+ * A sleeper's tier is otherwise fixed at sleep time, and waking it to sleep again takes HBM that belongs to whoever serves on the
+ * GPU.  fma_image_move copies the image of a sleeping engine to `tier` and makes it sleep there: a host-tier sleeper is demoted to
+ * disk when host DRAM runs short, a parked image leaves the parking GPU's HBM, a file-tier image is promoted to host DRAM ahead of
+ * an expected wake.  Every tier stores the image in one layout, so a move is a byte copy (nothing is decoded or re-encoded, no
+ * weight memory is mapped): host <-> parking buffer by the copy engines (direct_chunk pieces over the engine's copy streams);
+ * host <-> file by the file tier's reader / writer threads, pread / pwrite straight into / out of the pinned store (O_DIRECT under
+ * the file tier's rule); parking buffer <-> file through the pinned I/O windows.
+ * The destination is prepared as a sleep to its tier prepares it: FMA_TIER_HOST reserves the host store (a shared one is first
+ * swapped for a private one), FMA_TIER_LOCAL reserves the parking buffer on the engine's own GPU (the only move that allocates HBM),
+ * FMA_TIER_PEER needs a parking buffer (fma_peer_reserve / fma_peer_attach) of at least image_store_bytes, FMA_TIER_FILE needs
+ * fma_file_store(path): free space is checked (fstatvfs) before a byte is written, and the file is completed like a file-tier
+ * sleep's (fdatasync, descriptor, fdatasync), so fma_image_adopt_file and image_load open it.
+ * After success every backed-up segment and fma_stats_t.tier report `tier`, K3 digests still hold (FMA_FLAG_VERIFY on the next wake
+ * checks them), and the next fma_wake takes that tier's route.  The source is left as it was: the host store and the parking buffer
+ * stay allocated (fma_host_release / fma_peer_release now succeed) and a source file is never touched.
+ * Refusals leave the engine unchanged: FMA_ESTATE when nothing sleeps, a backed-up segment is mapped (a KEEP_BACKUP or partial
+ * wake), part of the image is in a resident share, or the destination is not prepared; FMA_EINVAL for an unknown tier, the tier
+ * the image is in (FILE -> FILE included) and PEER <-> LOCAL (there is one parking buffer).  A move that fails (FMA_EIO, FMA_ENOMEM,
+ * FMA_ECUDA) leaves the image where it was: records and statistics unchanged, a host store or local buffer it created released, a
+ * destination file emptied (never with a descriptor).  Only the engine's own streams and events are synchronised, so another
+ * engine of the process may serve meanwhile; host <-> file moves make no CUDA call beyond pinning a host store they create.  fma_timeline: op "move", rows file_io,
+ * copies_landed (the copy engines ran) and total (bytes = image_store_bytes). */
+FMA_API int  fma_image_move(fma_engine_t* e, int tier);
+
 /* ---- MULTI-PATH wake: borrow idle peers' PCIe links ---------------------------------------------------------------------
  * A host-tier wake is bounded by ONE x16 Gen5 link (55.6 GB/s measured of 64): 0.29 s for Llama-3-8B however good the engine
  * is.  When other GPUs of the box are idle (BASELINE config 5: the GPUs that only park sleepers; any N=1 deployment on an
@@ -425,7 +450,7 @@ FMA_API int  fma_set_option(fma_engine_t* e, const char* key, int64_t value);
 /* ---- stats ------------------------------------------------------------------------ */
 FMA_API int  fma_stats(fma_engine_t* e, fma_stats_t* out);
 
-/* Per-phase timeline of the last fma_sleep / fma_wake as text, one event per line:
+/* Per-phase timeline of the last fma_sleep / fma_wake / fma_image_move as text, one event per line:
  *   "<op>,<kind>,<idx>,<t0_ms>,<t1_ms>,<bytes>\n"   (times since the call's entry)
  * kinds: plan, map_ring / map_backed / map_remap (one cuMemCreate+Map+SetAccess each, mapper thread), gate_wait,
  * enqueue, copies_landed, wait_all_mapped, drain, unmap (sleep), kernel (K1/K2/K4/K5 launches, device-timed), total;

@@ -117,6 +117,156 @@ void image_apply(fma_engine_t* e, ParsedImage& pi) {
     }
 }
 
+// ---- moves of a sleeping image between tiers (fma_image_move) ----
+// Every tier holds the image in one layout (plain pages back to back, or the PACKED form's stored pages at img_off[p]), so a move
+// copies image_store_bytes bytes from offset 0 of one store to offset 0 of the other and changes nothing but the engine's records.
+
+// Copy engines between the pinned host store and the parking buffer: direct_chunk pieces round-robin over the copy streams.
+int move_host_park(fma_engine_t* e, bool to_park, uint64_t bytes, uint32_t* ops) {
+    char* host = static_cast<char*>(e->host.base);
+    char* park = reinterpret_cast<char*>(e->park.va);
+    const size_t chunk = direct_chunk(e);
+    size_t k = 0;
+    for (uint64_t o = 0; o < bytes; o += chunk, ++k) {
+        const size_t n = (size_t)std::min<uint64_t>(chunk, bytes - o);
+        RT(cudaMemcpyAsync(to_park ? park + o : host + o, to_park ? host + o : park + o, n, cudaMemcpyDefault, e->cs[k % e->n_cs]));
+        ++*ops;
+    }
+    return FMA_OK;
+}
+
+// The pinned host store <-> a file: FileIO's threads pread / pwrite straight into / out of the store, no copy engine involved.
+int move_host_file(fma_engine_t* e, bool to_file, int fd, bool direct, uint64_t bytes, uint64_t file_bytes, const char* path) {
+    const uint64_t piece = round_up(std::max<size_t>(e->load_chunk, 4096), 4096);
+    std::vector<FileIO::Item> items;
+    for (uint64_t o = 0; o < bytes; o += piece) items.push_back(FileIO::Item{o, std::min(piece, bytes - o)});
+    FileIO io(e, fd, to_file, direct, std::move(items), file_bytes, path, static_cast<char*>(e->host.base));
+    return io.finish();
+}
+
+// The parking buffer <-> a file through the engine's pinned I/O windows: the file tier's disk stage without the HBM ring.
+int move_park_file(fma_engine_t* e, bool to_file, int fd, bool direct, uint64_t bytes, uint64_t file_bytes, const char* path, uint32_t* ops) {
+    char* park = reinterpret_cast<char*>(e->park.va);
+    const uint64_t piece = e->io_window_bytes - 8192;
+    std::vector<FileIO::Item> items;
+    for (uint64_t o = 0; o < bytes && piece; o += piece) items.push_back(FileIO::Item{o, std::min(piece, bytes - o)});
+    FileIO io(e, fd, to_file, direct, items, file_bytes, path);
+    for (size_t k = 0; k < items.size(); ++k) {
+        cudaStream_t st = e->cs[k % e->n_cs];
+        char* dev = park + items[k].file_off;
+        if (to_file) {
+            char* window = io.wait_free(k);
+            if (!window) return io.finish();
+            RT(cudaMemcpyAsync(window, dev, items[k].bytes, cudaMemcpyDefault, st));
+        } else {
+            const char* window = io.wait_read(k);
+            if (!window) return io.finish();
+            RT(cudaMemcpyAsync(dev, window, items[k].bytes, cudaMemcpyDefault, st));
+        }
+        RT(cudaEventRecord(io.event(k), st));
+        io.posted(k);
+        ++*ops;
+    }
+    return io.finish();   // every pread / pwrite has returned and every copy into or out of a window has finished
+}
+
+// What a move has set up so far, so that a failure can undo it
+struct MoveState {
+    FileFd file;
+    bool direct = false;
+    bool file_emptied = false;   // the destination file has been emptied: a failure leaves no descriptor in it
+    bool made_host = false;      // the host store, or the local parking buffer, was created by this move
+    bool made_park = false;
+    bool copies = false;         // the copy streams ran
+};
+
+int run_move(fma_engine_t* e, fma_layout::MovePipeKind pipe, int from, int to, MoveState& ms) {
+    using fma_layout::MovePipeKind;
+    const uint64_t bytes = e->image_store_bytes;
+    const bool park_side = pipe != MovePipeKind::HostFile && pipe != MovePipeKind::FileHost;
+    ms.copies = park_side;
+    if (park_side) RC(ensure_streams(e));
+    // the destination, prepared as a sleep to its tier prepares it
+    if (to == FMA_TIER_HOST) {
+        if (e->host.shared) {   // the shared image is read-only: leave it to its other holders and take a private store
+            invalidate_shadows(e);
+            host_store_free(e->host);
+            e->st.host_store_bytes = 0;
+        }
+        ms.made_host = !e->host.base || e->host.cap < round_up(std::max<size_t>(bytes, FMA_PAGE_BYTES), FMA_PAGE_BYTES);
+        RC(host_store_reserve(e, bytes));
+    } else if (to == FMA_TIER_LOCAL) {
+        const size_t need = round_up(std::max<size_t>(bytes, FMA_PAGE_BYTES), e->gran);
+        ms.made_park = !(e->park.va && e->park.device == e->device && e->park.bytes >= need);
+        if (ms.made_park && e->park.va) {   // a buffer that does not fit, or a peer's (it holds nothing of this image), goes
+            if (e->shadow_tier == FMA_TIER_PEER || e->shadow_tier == FMA_TIER_LOCAL) invalidate_shadows(e);
+            vmm_buffer_free(e->park);
+        }
+        if (ms.made_park) RC(park_store_create(e, e->device, need, &e->park));
+    }
+    // the file side: the destination emptied once the filesystem has room; the source checked to hold the whole image
+    const double t_io = now_s();
+    const std::string path = to == FMA_TIER_FILE ? e->file_path : e->image_file;
+    uint64_t file_bytes = 0;
+    if (to == FMA_TIER_FILE) {
+        RC(open_image_file(path.c_str(), true, &ms.file.fd, &ms.direct));
+        RC(open_file_store(ms.file.fd, bytes, path.c_str()));
+        ms.file_emptied = true;
+    } else if (from == FMA_TIER_FILE) {
+        RC(open_image_file(path.c_str(), false, &ms.file.fd, &ms.direct));
+        struct stat sb;
+        if (fstat(ms.file.fd, &sb) != 0) return fail(FMA_EIO, "fstat(%s) failed: %s", path.c_str(), strerror(errno));
+        if ((uint64_t)sb.st_size < bytes)
+            return fail(FMA_EIO, "%s holds %llu bytes, the image needs %llu", path.c_str(), (unsigned long long)sb.st_size, (unsigned long long)bytes);
+        file_bytes = (uint64_t)sb.st_size;
+    }
+    // the bytes
+    uint32_t ops = 0;
+    CopyTimer timer{e};
+    const double t_copy = now_s();
+    if (park_side) RC(timer.begin());
+    switch (pipe) {
+    case MovePipeKind::HostPark: RC(move_host_park(e, true, bytes, &ops)); break;
+    case MovePipeKind::ParkHost: RC(move_host_park(e, false, bytes, &ops)); break;
+    case MovePipeKind::HostFile: RC(move_host_file(e, true, ms.file.fd, ms.direct, bytes, 0, path.c_str())); break;
+    case MovePipeKind::FileHost: RC(move_host_file(e, false, ms.file.fd, ms.direct, bytes, file_bytes, path.c_str())); break;
+    case MovePipeKind::ParkFile: RC(move_park_file(e, true, ms.file.fd, ms.direct, bytes, 0, path.c_str(), &ops)); break;
+    case MovePipeKind::FilePark: RC(move_park_file(e, false, ms.file.fd, ms.direct, bytes, file_bytes, path.c_str(), &ops)); break;
+    case MovePipeKind::Refused: return fail(FMA_EINVAL, "a refused move has no copy");   // (refused before)
+    }
+    if (park_side) {
+        double copy_s = 0;
+        RC(timer.end(&copy_s));   // joins the copy streams only
+        e->tl_add("copies_landed", (int)ops, t_copy, now_s(), bytes);
+    }
+    // a file written by a move is completed as a file-tier sleep completes it: it opens with fma_image_adopt_file and image_load
+    if (to == FMA_TIER_FILE) {
+        std::vector<char> desc;
+        RC(image_descriptor_build(e, from, &desc));
+        RC(close_file_store(ms.file.fd, bytes, path.c_str(), ms.direct, desc));
+    }
+    if (ms.file.fd >= 0) e->tl_add("file_io", ms.direct ? 1 : 0, t_io, now_s(), to == FMA_TIER_FILE ? bytes + kImageTail : bytes);
+    e->st.copy_ops = ops;
+    e->st.total_copy_ops += ops;
+    return FMA_OK;
+}
+
+// A failed move: nothing may still copy into what goes, what the move created goes, and a destination file keeps no descriptor
+void undo_move(fma_engine_t* e, MoveState& ms) {
+    if (ms.copies)
+        for (int i = 0; i < e->n_cs; ++i) cudaStreamSynchronize(e->cs[i]);
+    if (ms.made_host) {
+        host_store_free(e->host);
+        e->st.host_store_bytes = 0;
+    }
+    if (ms.made_park) vmm_buffer_free(e->park);
+    if (ms.file_emptied) {   // what was written goes too (best effort: without its descriptor the file is refused anyway)
+        const int r = ftruncate(ms.file.fd, 0);
+        (void)r;
+    }
+    cudaGetLastError();
+}
+
 }  // namespace
 }  // namespace fma_impl
 
@@ -334,6 +484,48 @@ int fma_image_adopt_parked(fma_engine_t* e, const void* desc, size_t desc_bytes,
     if (e->shadow_tier != FMA_TIER_HOST) invalidate_shadows(e);
     RC(do_sleep(e, tag_mask, FMA_TIER_PEER, (flags & ~FMA_FLAG_VERIFY) | kFlagAdopt));
     image_apply(e, pi);
+    return FMA_OK;
+}
+
+// ---- moving a sleeping image to another tier (see include/fma_engine.h) -------------------------------------------------
+int fma_image_move(fma_engine_t* e, int tier) {
+    if (check_engine(e) != FMA_OK) return FMA_EINVAL;
+    std::lock_guard<std::mutex> op(e->op_mu);
+    const int from = e->image_tier;
+    fma_layout::MoveFacts facts{};
+    {
+        std::lock_guard<std::mutex> lk(e->mu);
+        for (const Segment& s : e->segs)
+            if (s.has_backup) (s.mapped ? facts.backup_mapped : facts.asleep) = true;
+    }
+    facts.resident = resident_asleep(e);
+    facts.prepared = tier == FMA_TIER_PEER ? e->park.va && e->park.device != e->device && e->park.bytes >= e->image_store_bytes
+                   : tier == FMA_TIER_FILE ? !e->file_path.empty()
+                                           : true;
+    const fma_layout::MoveRoute route = fma_layout::move_route(from, tier, facts);
+    if (route.error != FMA_OK) return fail(route.error, "image move from tier %d to tier %d: %s", from, tier, route.why);
+
+    DeviceGuard guard(e->device);
+    RC(flush_kernel_times(e));
+    const double t_entry = now_s();
+    e->tl_begin("move", t_entry);
+    MoveState ms;
+    const int rc = run_move(e, route.pipe, from, tier, ms);
+    if (rc != FMA_OK) {
+        undo_move(e, ms);   // the image stays where it was, its records untouched
+        return rc;
+    }
+    {
+        std::lock_guard<std::mutex> lk(e->mu);
+        for (Segment& s : e->segs)
+            if (s.has_backup && !s.mapped) s.backup_tier = tier;
+    }
+    e->image_tier = tier;
+    if (tier == FMA_TIER_FILE) e->image_file = e->file_path;
+    // INCREMENTAL: the copy a clean sleep may keep lay in the store the image left; the next wake records the new one
+    invalidate_shadows(e);
+    e->st.tier = tier;
+    e->tl_add("total", 0, t_entry, now_s(), e->image_store_bytes);
     return FMA_OK;
 }
 

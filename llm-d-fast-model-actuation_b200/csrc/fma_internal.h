@@ -4,7 +4,7 @@
 //   fma_sleep.cu    SLEEP pipeline (do_sleep) and the PACKED image plan
 //   fma_wake.cu     WAKE pipeline (do_wake)
 //   fma_load.cu     file I/O: reader / writer threads over the pinned I/O windows (cold load fma_load_file, FILE tier)
-//   fma_image.cu    image hand-over between engines / processes (fma_image_export / fma_image_adopt)
+//   fma_image.cu    image hand-over between engines / processes (fma_image_export / fma_image_adopt), moves between tiers (fma_image_move)
 //
 // Everything below lives in namespace fma_impl; the library is built with -fvisibility=hidden, so none of it is exported.
 #pragma once
@@ -432,12 +432,15 @@ struct FileFd {   // closes on every exit path
 //          posted(k): a writer pwrites item k once event(k) has completed
 // With O_DIRECT a read may start below its item and a write must be 4 KiB aligned (the FILE tier's always are).  In the page
 // cache's mode every range read or written is dropped from it behind the I/O (posix_fadvise DONTNEED).
+// With `mem` (a pinned host store: fma_image_move between the host and file tiers) there are no windows and no copies: item k is
+// read into / written from mem + its file offset, and the threads run on their own until finish().  With O_DIRECT, `mem` and every
+// item must then be 4 KiB aligned.
 class FileIO {
   public:
     struct Item {
         uint64_t file_off, bytes;
     };
-    FileIO(fma_engine_t* e, int fd, bool write, bool direct, std::vector<Item> items, uint64_t file_bytes, const char* path);
+    FileIO(fma_engine_t* e, int fd, bool write, bool direct, std::vector<Item> items, uint64_t file_bytes, const char* path, char* mem = nullptr);
     ~FileIO();
     const char* wait_read(size_t k);   // nullptr: the I/O failed (finish() has the error)
     char* wait_free(size_t k);
@@ -458,6 +461,7 @@ class FileIO {
     std::vector<Item> items_;
     uint64_t file_bytes_;
     const char* path_;
+    char* mem_;
     int n_;
     std::mutex mu_;
     std::condition_variable cv_;
@@ -470,6 +474,14 @@ class FileIO {
     std::vector<std::thread> th_;
     bool stopped_ = false;
 };
+
+// ---- the FILE tier's store (fma_sleep.cu), for a file-tier sleep and a move to the file tier (fma_image_move) ----
+// The filesystem of the open file `fd` has room for an image of `bytes` and its descriptor (fstatvfs), and only then the file is
+// emptied.  Short of room: FMA_EIO with the file untouched.
+int open_file_store(int fd, uint64_t bytes, const char* path);
+// After the image's last write: fdatasync, then `desc` (image_descriptor_build) in the kImageTail bytes behind the image, then
+// fdatasync again, so a torn file fails descriptor parsing.
+int close_file_store(int fd, uint64_t bytes, const char* path, bool direct, const std::vector<char>& desc);
 
 // ---- pipelines ----
 int do_sleep(fma_engine_t* e, uint64_t offload_mask, int tier, uint32_t flags);   // fma_sleep.cu

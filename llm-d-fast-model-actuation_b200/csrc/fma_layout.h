@@ -329,4 +329,39 @@ inline WakeRoute wake_route(const WakeFacts& f) {
     return r;
 }
 
+// ---- which copy a move of a sleeping image between tiers runs (fma_image_move) ----
+// Park: the parking buffer, of the peer tier or the local one.  Every tier stores the image in one layout, so a move is a byte copy.
+enum class MovePipeKind { HostPark, ParkHost, HostFile, FileHost, ParkFile, FilePark, Refused };
+
+struct MoveFacts {
+    bool asleep;          // a segment with a backup is unmapped
+    bool backup_mapped;   // a segment with a backup is mapped (a KEEP_BACKUP wake, a partly woken image)
+    bool resident;        // part of the image sleeps in a resident share
+    bool prepared;        // the destination is ready: PEER, a peer parking buffer that holds the image; FILE, a path (HOST and LOCAL: always)
+};
+struct MoveRoute {
+    MovePipeKind pipe;
+    int error;            // FMA_OK, or the code of the refusal
+    const char* why;      // the refusal's reason
+};
+
+inline bool is_park_tier(int tier) { return tier == FMA_TIER_PEER || tier == FMA_TIER_LOCAL; }
+
+inline MoveRoute move_route(int from, int to, const MoveFacts& f) {
+    auto refuse = [](int code, const char* why) { return MoveRoute{MovePipeKind::Refused, code, why}; };
+    if (to < FMA_TIER_HOST || to > FMA_TIER_FILE) return refuse(FMA_EINVAL, "unknown tier");
+    if (!f.asleep) return refuse(FMA_ESTATE, "no image is asleep");
+    if (f.backup_mapped) return refuse(FMA_ESTATE, "a segment with a backup is mapped (a KEEP_BACKUP or partial wake): wake or sleep it fully first");
+    if (f.resident) return refuse(FMA_ESTATE, "part of the image sleeps in the resident share, which does not move");
+    if (from < FMA_TIER_HOST || from > FMA_TIER_FILE) return refuse(FMA_EINVAL, "the image's tier is unknown");
+    if (to == from) return refuse(FMA_EINVAL, "the image already sleeps in that tier");
+    if (is_park_tier(from) && is_park_tier(to)) return refuse(FMA_EINVAL, "there is one parking buffer: no move between the peer and local tiers");
+    if (!f.prepared)
+        return refuse(FMA_ESTATE, to == FMA_TIER_FILE ? "a move to the file tier needs fma_file_store(path) first"
+                                                      : "a move to the peer tier needs a peer parking buffer that holds the image (fma_peer_reserve / fma_peer_attach)");
+    if (from == FMA_TIER_HOST) return MoveRoute{to == FMA_TIER_FILE ? MovePipeKind::HostFile : MovePipeKind::HostPark, FMA_OK, ""};
+    if (from == FMA_TIER_FILE) return MoveRoute{to == FMA_TIER_HOST ? MovePipeKind::FileHost : MovePipeKind::FilePark, FMA_OK, ""};
+    return MoveRoute{to == FMA_TIER_HOST ? MovePipeKind::ParkHost : MovePipeKind::ParkFile, FMA_OK, ""};
+}
+
 }  // namespace fma_layout

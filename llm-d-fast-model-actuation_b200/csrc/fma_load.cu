@@ -45,18 +45,27 @@ int open_image_file(const char* path, bool write, int* fd, bool* direct) {
     return FMA_OK;
 }
 
-FileIO::FileIO(fma_engine_t* e, int fd, bool write, bool direct, std::vector<Item> items, uint64_t file_bytes, const char* path)
-    : e_(e), fd_(fd), write_(write), direct_(direct), items_(std::move(items)), file_bytes_(file_bytes), path_(path), n_(e->io_windows),
-      ready_(items_.size(), 0), posted_(items_.size(), 0), done_(items_.size(), 0) {
-    if (!n_ || !e->load_ring) {
-        set_error(FMA_ESTATE, "the engine's I/O windows are not pinned");
-        return;
-    }
-    for (const Item& it : items_)
-        if (it.bytes > e->io_window_bytes - 8192 || (direct_ && write_ && ((it.file_off | it.bytes) & 4095))) {
-            set_error(FMA_EINVAL, "I/O item of %llu bytes at %llu does not fit a window", (unsigned long long)it.bytes, (unsigned long long)it.file_off);
+FileIO::FileIO(fma_engine_t* e, int fd, bool write, bool direct, std::vector<Item> items, uint64_t file_bytes, const char* path, char* mem)
+    : e_(e), fd_(fd), write_(write), direct_(direct), items_(std::move(items)), file_bytes_(file_bytes), path_(path), mem_(mem), n_(e->io_windows),
+      ready_(items_.size(), 0), posted_(items_.size(), mem ? 1 : 0), done_(items_.size(), 0) {
+    if (mem_) {   // nothing is copied into or out of a window: every item is "posted" from the start
+        n_posted_items_ = items_.size();
+        for (const Item& it : items_)
+            if (direct_ && ((it.file_off | it.bytes | (uint64_t)(uintptr_t)mem_) & 4095)) {
+                set_error(FMA_EINVAL, "I/O item of %llu bytes at %llu is not aligned for O_DIRECT", (unsigned long long)it.bytes, (unsigned long long)it.file_off);
+                return;
+            }
+    } else {
+        if (!n_ || !e->load_ring) {
+            set_error(FMA_ESTATE, "the engine's I/O windows are not pinned");
             return;
         }
+        for (const Item& it : items_)
+            if (it.bytes > e->io_window_bytes - 8192 || (direct_ && write_ && ((it.file_off | it.bytes) & 4095))) {
+                set_error(FMA_EINVAL, "I/O item of %llu bytes at %llu does not fit a window", (unsigned long long)it.bytes, (unsigned long long)it.file_off);
+                return;
+            }
+    }
     const int n_threads = std::max(1, std::min<int>(e->load_threads, (int)std::max<size_t>(items_.size(), 1)));
     for (int t = 0; t < n_threads && !items_.empty(); ++t) th_.emplace_back([this] { worker(); });
 }
@@ -76,23 +85,29 @@ void FileIO::set_error(int code, const char* fmt, ...) {
 }
 
 void FileIO::worker() {
-    cudaSetDevice(e_->device);
+    if (!mem_) cudaSetDevice(e_->device);
     for (;;) {
         const size_t k = next_.fetch_add(1);
         if (k >= items_.size()) break;
-        const size_t w = k % n_;
-        {   // read: the window's last copy has been enqueued (k - n posted); write: this item's D2H has been enqueued
-            std::unique_lock<std::mutex> lk(mu_);
-            cv_.wait(lk, [&] { return error_ != FMA_OK || (write_ ? posted_[k] : (k < (size_t)n_ || posted_[k - n_])); });
-            if (error_ != FMA_OK) break;
-        }
-        if (write_ || k >= (size_t)n_) {   // ... and has finished
-            const cudaError_t r = cudaEventSynchronize(e_->ev_load[w]);
-            if (r != cudaSuccess) return set_error(FMA_ECUDA, "cudaEventSynchronize(I/O window) failed: %s", cudaGetErrorString(r));
-        }
-        char* buf = static_cast<char*>(e_->load_ring) + w * e_->io_window_bytes;
-        char* abuf = direct_ ? reinterpret_cast<char*>(round_up(reinterpret_cast<uintptr_t>(buf), 4096)) : buf;
         const Item& it = items_[k];
+        char* abuf = mem_ ? mem_ + it.file_off : nullptr;
+        if (!mem_) {
+            const size_t w = k % n_;
+            {   // read: the window's last copy has been enqueued (k - n posted); write: this item's D2H has been enqueued
+                std::unique_lock<std::mutex> lk(mu_);
+                cv_.wait(lk, [&] { return error_ != FMA_OK || (write_ ? posted_[k] : (k < (size_t)n_ || posted_[k - n_])); });
+                if (error_ != FMA_OK) break;
+            }
+            if (write_ || k >= (size_t)n_) {   // ... and has finished
+                const cudaError_t r = cudaEventSynchronize(e_->ev_load[w]);
+                if (r != cudaSuccess) return set_error(FMA_ECUDA, "cudaEventSynchronize(I/O window) failed: %s", cudaGetErrorString(r));
+            }
+            char* buf = static_cast<char*>(e_->load_ring) + w * e_->io_window_bytes;
+            abuf = direct_ ? reinterpret_cast<char*>(round_up(reinterpret_cast<uintptr_t>(buf), 4096)) : buf;
+        } else {
+            std::lock_guard<std::mutex> lk(mu_);
+            if (error_ != FMA_OK) break;   // another item failed: the I/O stops
+        }
         const double t0 = now_s();
         uint64_t done = 0;
         int err = 0;

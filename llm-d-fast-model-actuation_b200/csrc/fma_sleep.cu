@@ -719,36 +719,27 @@ int route_sleep(fma_engine_t* e, SleepPlan& p) {
     return FMA_OK;
 }
 
-// FILE: open the file, check that the filesystem has room for the image and its descriptor, and only then empty the file
-int open_file_store(fma_engine_t* e, SleepPlan& p) {
-    if (e->file_path.empty()) return fail(FMA_ESTATE, "the file tier needs fma_file_store(path) first");
-    if (!e->load_ring) return fail(FMA_ESTATE, "the engine's I/O windows are not pinned");
-    p.file_t0 = now_s();
-    RC(open_image_file(e->file_path.c_str(), true, &p.file.fd, &p.file_direct));
+}  // namespace
+
+int open_file_store(int fd, uint64_t bytes, const char* path) {
     struct statvfs vs;
     struct stat sb;
-    if (fstatvfs(p.file.fd, &vs) != 0 || fstat(p.file.fd, &sb) != 0) return fail(FMA_EIO, "fstatvfs(%s) failed: %s", e->file_path.c_str(), strerror(errno));
-    const uint64_t need = p.Wp + kImageTail, room = (uint64_t)vs.f_bavail * vs.f_frsize + (uint64_t)sb.st_blocks * 512;  // (its own blocks come back)
-    if (room < need)
-        return fail(FMA_EIO, "%s: %llu bytes free, the image needs %llu", e->file_path.c_str(), (unsigned long long)room, (unsigned long long)need);
-    if (ftruncate(p.file.fd, 0) != 0) return fail(FMA_EIO, "ftruncate(%s) failed: %s", e->file_path.c_str(), strerror(errno));
-    e->image_file = e->file_path;
+    if (fstatvfs(fd, &vs) != 0 || fstat(fd, &sb) != 0) return fail(FMA_EIO, "fstatvfs(%s) failed: %s", path, strerror(errno));
+    const uint64_t need = bytes + kImageTail, room = (uint64_t)vs.f_bavail * vs.f_frsize + (uint64_t)sb.st_blocks * 512;  // (its own blocks come back)
+    if (room < need) return fail(FMA_EIO, "%s: %llu bytes free, the image needs %llu", path, (unsigned long long)room, (unsigned long long)need);
+    if (ftruncate(fd, 0) != 0) return fail(FMA_EIO, "ftruncate(%s) failed: %s", path, strerror(errno));
     return FMA_OK;
 }
 
-// After the last write: fdatasync, then the descriptor in the last kImageTail bytes (a torn file fails descriptor parsing).
-int close_file_store(fma_engine_t* e, SleepPlan& p) {
-    const char* path = e->image_file.c_str();
-    if (fdatasync(p.file.fd) != 0) return fail(FMA_EIO, "fdatasync(%s) failed: %s", path, strerror(errno));
-    std::vector<char> desc;
-    RC(image_descriptor_build(e, FMA_TIER_FILE, &desc));
-    desc.resize(kImageTail, 0);
+int close_file_store(int fd, uint64_t bytes, const char* path, bool direct, const std::vector<char>& desc) {
+    if (fdatasync(fd) != 0) return fail(FMA_EIO, "fdatasync(%s) failed: %s", path, strerror(errno));
     void* buf = nullptr;
-    if (posix_memalign(&buf, 4096, kImageTail) != 0) return fail(FMA_ENOMEM, "no memory for the descriptor");
-    memcpy(buf, desc.data(), kImageTail);
+    if (desc.size() > kImageTail || posix_memalign(&buf, 4096, kImageTail) != 0) return fail(FMA_ENOMEM, "no memory for the descriptor");
+    memset(buf, 0, kImageTail);
+    memcpy(buf, desc.data(), desc.size());
     uint64_t done = 0;
     while (done < kImageTail) {
-        const ssize_t n = pwrite(p.file.fd, static_cast<char*>(buf) + done, kImageTail - done, (off_t)(p.Wp + done));
+        const ssize_t n = pwrite(fd, static_cast<char*>(buf) + done, kImageTail - done, (off_t)(bytes + done));
         if (n < 0 && errno == EINTR) continue;
         if (n <= 0) break;
         done += (uint64_t)n;
@@ -756,8 +747,29 @@ int close_file_store(fma_engine_t* e, SleepPlan& p) {
     const int err = errno;
     free(buf);
     if (done < kImageTail) return fail(FMA_EIO, "writing the descriptor of %s failed: %s", path, strerror(err));
-    if (fdatasync(p.file.fd) != 0) return fail(FMA_EIO, "fdatasync(%s) failed: %s", path, strerror(errno));
-    if (!p.file_direct) posix_fadvise(p.file.fd, 0, 0, POSIX_FADV_DONTNEED);   // clean now: the page cache lets go of the image
+    if (fdatasync(fd) != 0) return fail(FMA_EIO, "fdatasync(%s) failed: %s", path, strerror(errno));
+    if (!direct) posix_fadvise(fd, 0, 0, POSIX_FADV_DONTNEED);   // clean now: the page cache lets go of the image
+    return FMA_OK;
+}
+
+namespace {
+
+// FILE: open the file, check that the filesystem has room for the image and its descriptor, and only then empty the file
+int open_sleep_file(fma_engine_t* e, SleepPlan& p) {
+    if (e->file_path.empty()) return fail(FMA_ESTATE, "the file tier needs fma_file_store(path) first");
+    if (!e->load_ring) return fail(FMA_ESTATE, "the engine's I/O windows are not pinned");
+    p.file_t0 = now_s();
+    RC(open_image_file(e->file_path.c_str(), true, &p.file.fd, &p.file_direct));
+    RC(open_file_store(p.file.fd, p.Wp, e->file_path.c_str()));
+    e->image_file = e->file_path;
+    return FMA_OK;
+}
+
+// After the last write: the descriptor of the image the file now holds
+int close_sleep_file(fma_engine_t* e, SleepPlan& p) {
+    std::vector<char> desc;
+    RC(image_descriptor_build(e, FMA_TIER_FILE, &desc));
+    RC(close_file_store(p.file.fd, p.Wp, e->image_file.c_str(), p.file_direct, desc));
     e->tl_add("file_io", p.file_direct ? 1 : 0, p.file_t0, now_s(), p.Wp + kImageTail);
     return FMA_OK;
 }
@@ -780,7 +792,7 @@ int size_store(fma_engine_t* e, SleepPlan& p) {
     } else if (p.tier == FMA_TIER_LOCAL) {
         return park_reserve(e, e->device, p.Wp);
     } else if (p.tier == FMA_TIER_FILE) {
-        if (!p.adopt()) return open_file_store(e, p);   // (an adopted or clean image is in its file already)
+        if (!p.adopt()) return open_sleep_file(e, p);   // (an adopted or clean image is in its file already)
     } else {
         return fail(FMA_EINVAL, "unknown tier %d", p.tier);
     }
@@ -873,7 +885,7 @@ int finish_sleep(fma_engine_t* e, SleepPlan& p, Unmapper& un, ApplyUnmapped& app
     }
     e->image_bytes = p.W;
     e->image_tier = p.tier;
-    if (p.file.fd >= 0) RC(close_file_store(e, p));   // (the image is asleep in the file either way: a wake reads what was written)
+    if (p.file.fd >= 0) RC(close_sleep_file(e, p));   // (the image is asleep in the file either way: a wake reads what was written)
 
     e->tl_add("total", 0, t_entry, now_s(), p.W_all);
     e->st.sleep_seconds = now_s() - t_entry;

@@ -216,6 +216,24 @@ class CuMemAllocator:
             logger.info("fma_b200: wake %.3f s, H2D %.1f GB/s", st["wake_seconds"],
                         st["wake_bytes_restored"] / st["wake_copy_seconds"] / 1e9)
 
+    def move_image(self, tier: str) -> None:
+        """Move this rank's sleeping image without waking it.  ``"file"`` demotes it to ``<FMA_FILE_DIR>/<instance id>-r<rank>.fmaimg``
+        (the file tier's name, removed when the process exits) and then releases the host store; ``"host"`` promotes it back to
+        host DRAM ahead of a wake and leaves the file to the exit hook."""
+        self._join_reserve()
+        if tier == "file":
+            if self._file_path is None:
+                self._file_path = _file_tier_path()
+                self.engine.file_store(self._file_path)
+                atexit.register(_remove_file, self._file_path)
+            self.engine.move_image(L.FMA_TIER_FILE)
+            self.engine.host_release()
+        elif tier == "host":
+            self.engine.move_image(L.FMA_TIER_HOST)
+        else:
+            raise L.FmaError(L.FMA_EINVAL, f"move_image: tier {tier!r} is not 'host' or 'file'")
+        logger.info("fma_b200: sleeping image moved to the %s tier (%.2f GiB)", tier, self.engine.stats()["image_store_bytes"] / 1024**3)
+
     # ---- pool --------------------------------------------------------------------------
     @contextmanager
     def use_memory_pool(self, tag: str | None = None):

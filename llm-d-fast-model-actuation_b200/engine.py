@@ -342,6 +342,12 @@ class Engine:
         engine must hold the same segment sequence for ``tags``.  Reads only the descriptor; ``wake`` streams the data."""
         check(self._lib.fma_image_adopt_file(self._h, path.encode(), self.tag_mask(tags), flags))
 
+    def move_image(self, tier: int) -> None:
+        """Move the sleeping image to ``tier`` without waking it (fma_image_move): host DRAM, a file (``file_store`` first), a peer's
+        parking buffer (``peer_reserve`` first) or this GPU's.  The source store stays allocated until ``host_release`` /
+        ``peer_release``; a source file is never touched."""
+        check(self._lib.fma_image_move(self._h, tier))
+
     # -- cold load -------------------------------------------------------------------------
     def load_file(self, path: str, spans: Sequence[tuple[int, int, int]], o_direct: bool = False) -> dict:
         """Stream (file_offset, nbytes, device_address) spans of one file into mapped segments."""
