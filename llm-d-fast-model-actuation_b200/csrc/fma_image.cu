@@ -146,27 +146,10 @@ int move_host_file(fma_engine_t* e, bool to_file, int fd, bool direct, uint64_t 
 
 // The parking buffer <-> a file through the engine's pinned I/O windows: the file tier's disk stage without the HBM ring.
 int move_park_file(fma_engine_t* e, bool to_file, int fd, bool direct, uint64_t bytes, uint64_t file_bytes, const char* path, uint32_t* ops) {
-    char* park = reinterpret_cast<char*>(e->park.va);
-    const uint64_t piece = e->io_window_bytes - 8192;
-    std::vector<FileIO::Item> items;
-    for (uint64_t o = 0; o < bytes && piece; o += piece) items.push_back(FileIO::Item{o, std::min(piece, bytes - o)});
+    const std::vector<FileIO::Item> items = FileIO::cut(e, {FileIO::Item{0, bytes}});
     FileIO io(e, fd, to_file, direct, items, file_bytes, path);
-    for (size_t k = 0; k < items.size(); ++k) {
-        cudaStream_t st = e->cs[k % e->n_cs];
-        char* dev = park + items[k].file_off;
-        if (to_file) {
-            char* window = io.wait_free(k);
-            if (!window) return io.finish();
-            RT(cudaMemcpyAsync(window, dev, items[k].bytes, cudaMemcpyDefault, st));
-        } else {
-            const char* window = io.wait_read(k);
-            if (!window) return io.finish();
-            RT(cudaMemcpyAsync(dev, window, items[k].bytes, cudaMemcpyDefault, st));
-        }
-        RT(cudaEventRecord(io.event(k), st));
-        io.posted(k);
-        ++*ops;
-    }
+    for (size_t k = 0; k < items.size(); ++k, ++*ops)
+        RC(io.copy(k, reinterpret_cast<char*>(e->park.va) + items[k].file_off, e->cs[k % e->n_cs]));
     return io.finish();   // every pread / pwrite has returned and every copy into or out of a window has finished
 }
 
@@ -213,12 +196,7 @@ int run_move(fma_engine_t* e, fma_layout::MovePipeKind pipe, int from, int to, M
         RC(open_file_store(ms.file.fd, bytes, path.c_str()));
         ms.file_emptied = true;
     } else if (from == FMA_TIER_FILE) {
-        RC(open_image_file(path.c_str(), false, &ms.file.fd, &ms.direct));
-        struct stat sb;
-        if (fstat(ms.file.fd, &sb) != 0) return fail(FMA_EIO, "fstat(%s) failed: %s", path.c_str(), strerror(errno));
-        if ((uint64_t)sb.st_size < bytes)
-            return fail(FMA_EIO, "%s holds %llu bytes, the image needs %llu", path.c_str(), (unsigned long long)sb.st_size, (unsigned long long)bytes);
-        file_bytes = (uint64_t)sb.st_size;
+        RC(open_image_source(path.c_str(), bytes, &ms.file.fd, &ms.direct, &file_bytes));
     }
     // the bytes
     uint32_t ops = 0;

@@ -25,6 +25,7 @@
 #include <iterator>
 #include <map>
 #include <mutex>
+#include <optional>
 #include <string>
 #include <thread>
 #include <vector>
@@ -420,16 +421,19 @@ int ensure_io_windows(fma_engine_t* e);   // pin the I/O windows for the current
 // Opens `path` for the FILE tier (write: created, not truncated), with O_DIRECT when the filesystem accepts it and
 // FMA_FILE_BUFFERED is not 1; *direct tells which.  Failure: FMA_EIO.
 int open_image_file(const char* path, bool write, int* fd, bool* direct);
+// open_image_file for reading an image of `need` bytes: a file that holds fewer is refused with FMA_EIO; *file_bytes: its size
+int open_image_source(const char* path, uint64_t need, int* fd, bool* direct, uint64_t* file_bytes);
 struct FileFd {   // closes on every exit path
     int fd = -1;
     ~FileFd() { if (fd >= 0) close(fd); }
 };
 // Reader or writer threads over the engine's pinned I/O windows.  Item k of `items` goes through window k % io_windows, and the
-// caller's thread enqueues the copy of every item, in item order, recording event(k) on the copy's stream right behind it:
-//   read:  readers pread item k into its window -> wait_read(k) returns its bytes -> the caller enqueues the H2D out of them ->
-//          posted(k): the reader of item k + n reuses the window once event(k) has completed
-//   write: wait_free(k) returns item k's window once the pwrite of item k - n has returned -> the caller enqueues the D2H into it ->
-//          posted(k): a writer pwrites item k once event(k) has completed
+// caller's thread calls copy(k, dev, stream) for every item, in item order.  copy enqueues the item's copy between its window and
+// the device memory `dev` on `stream`, and records the window's event behind it:
+//   read:  readers pread item k into its window -> copy(k) waits for that, enqueues the H2D out of the window -> the reader of
+//          item k + n reuses the window once that H2D has finished
+//   write: copy(k) waits until the pwrite of item k - n has returned, enqueues the D2H into the window -> a writer pwrites item k
+//          once that D2H has finished
 // With O_DIRECT a read may start below its item and a write must be 4 KiB aligned (the FILE tier's always are).  In the page
 // cache's mode every range read or written is dropped from it behind the I/O (posix_fadvise DONTNEED).
 // With `mem` (a pinned host store: fma_image_move between the host and file tiers) there are no windows and no copies: item k is
@@ -440,12 +444,11 @@ class FileIO {
     struct Item {
         uint64_t file_off, bytes;
     };
+    // `ranges` cut into items of at most one window each, in order; (*ends)[r]: one past the last item of range r
+    static std::vector<Item> cut(const fma_engine_t* e, const std::vector<Item>& ranges, std::vector<size_t>* ends = nullptr);
     FileIO(fma_engine_t* e, int fd, bool write, bool direct, std::vector<Item> items, uint64_t file_bytes, const char* path, char* mem = nullptr);
     ~FileIO();
-    const char* wait_read(size_t k);   // nullptr: the I/O failed (finish() has the error)
-    char* wait_free(size_t k);
-    cudaEvent_t event(size_t k) const { return e_->ev_load[k % n_]; }
-    void posted(size_t k);
+    int copy(size_t k, void* dev, cudaStream_t stream);   // FMA_OK, a CUDA error, or (the I/O failed) finish()'s error
     size_t written();                  // items whose pwrite has returned, as a prefix of `items`
     int finish();                      // joins the threads and waits for every posted copy; FMA_OK or the first error (FMA_EIO / FMA_ECUDA)
     double io_seconds() const { return io_ns_.load() * 1e-9; }
@@ -453,6 +456,7 @@ class FileIO {
 
   private:
     void worker();
+    char* window(size_t k) const;      // where item k's I/O starts in its window (4 KiB aligned for O_DIRECT)
     void set_error(int code, const char* fmt, ...);
     int stop();                        // finish() without setting the thread's error message
     fma_engine_t* e_;
@@ -645,13 +649,19 @@ struct PageKernels {
     }
 };
 
-// Where each page of `pages` lies in the staging ring when batch c of `slots` goes through slot c % n_ring
-inline std::vector<uint64_t> ring_addresses(const fma_engine_t* e, const std::vector<PagePlan>& pages, const std::vector<Batch>& slots) {
-    std::vector<uint64_t> at(pages.size());
-    for (size_t c = 0; c < slots.size(); ++c)
-        for (size_t q = slots[c].p0; q < slots[c].p0 + slots[c].np; ++q)
-            at[q] = (uint64_t)(uintptr_t)e->ring[c % e->n_ring] + (pages[q].off - pages[slots[c].p0].off);
-    return at;
+// The ring slots of a staged sleep or wake: runs of `pages` adjacent in the store that fit one slot, by their stored bytes (PACKED)
+// or by their number.  Batch c of *slots goes through slot c % n_ring, and (*in_ring)[q] is where page q lies in it.
+inline int plan_ring_slots(const fma_engine_t* e, bool packed, const std::vector<PagePlan>& pages, std::vector<Batch>* slots,
+                           std::vector<uint64_t>* in_ring) {
+    if (!fma_layout::plan_batches(pages, packed ? SIZE_MAX : e->ring_slot_bytes / FMA_PAGE_BYTES, packed ? e->ring_slot_bytes : UINT64_MAX, true, slots))
+        return fail(FMA_EINVAL, "ring slot of %zu bytes cannot hold one page", e->ring_slot_bytes);
+    in_ring->assign(pages.size(), 0);
+    for (size_t c = 0; c < slots->size(); ++c) {
+        const Batch& sl = (*slots)[c];
+        for (size_t q = sl.p0; q < sl.p0 + sl.np; ++q)
+            (*in_ring)[q] = (uint64_t)(uintptr_t)e->ring[c % e->n_ring] + (pages[q].off - pages[sl.p0].off);
+    }
+    return FMA_OK;
 }
 
 // What the workers of a MULTI-PATH sleep or wake share: one thread per path, and the first error wins.

@@ -45,6 +45,26 @@ int open_image_file(const char* path, bool write, int* fd, bool* direct) {
     return FMA_OK;
 }
 
+int open_image_source(const char* path, uint64_t need, int* fd, bool* direct, uint64_t* file_bytes) {
+    RC(open_image_file(path, false, fd, direct));
+    struct stat sb;
+    if (fstat(*fd, &sb) != 0) return fail(FMA_EIO, "fstat(%s) failed: %s", path, strerror(errno));
+    if ((uint64_t)sb.st_size < need)
+        return fail(FMA_EIO, "%s holds %llu bytes, the image needs %llu", path, (unsigned long long)sb.st_size, (unsigned long long)need);
+    *file_bytes = (uint64_t)sb.st_size;
+    return FMA_OK;
+}
+
+std::vector<FileIO::Item> FileIO::cut(const fma_engine_t* e, const std::vector<Item>& ranges, std::vector<size_t>* ends) {
+    const uint64_t piece = e->io_window_bytes - 8192;   // (the windows' O_DIRECT slack, ensure_io_windows)
+    std::vector<Item> items;
+    for (const Item& r : ranges) {
+        for (uint64_t o = 0; o < r.bytes; o += piece) items.push_back(Item{r.file_off + o, std::min(piece, r.bytes - o)});
+        if (ends) ends->push_back(items.size());
+    }
+    return items;
+}
+
 FileIO::FileIO(fma_engine_t* e, int fd, bool write, bool direct, std::vector<Item> items, uint64_t file_bytes, const char* path, char* mem)
     : e_(e), fd_(fd), write_(write), direct_(direct), items_(std::move(items)), file_bytes_(file_bytes), path_(path), mem_(mem), n_(e->io_windows),
       ready_(items_.size(), 0), posted_(items_.size(), mem ? 1 : 0), done_(items_.size(), 0) {
@@ -102,8 +122,7 @@ void FileIO::worker() {
                 const cudaError_t r = cudaEventSynchronize(e_->ev_load[w]);
                 if (r != cudaSuccess) return set_error(FMA_ECUDA, "cudaEventSynchronize(I/O window) failed: %s", cudaGetErrorString(r));
             }
-            char* buf = static_cast<char*>(e_->load_ring) + w * e_->io_window_bytes;
-            abuf = direct_ ? reinterpret_cast<char*>(round_up(reinterpret_cast<uintptr_t>(buf), 4096)) : buf;
+            abuf = window(k);
         } else {
             std::lock_guard<std::mutex> lk(mu_);
             if (error_ != FMA_OK) break;   // another item failed: the I/O stops
@@ -148,29 +167,29 @@ void FileIO::worker() {
     }
 }
 
-const char* FileIO::wait_read(size_t k) {
-    std::unique_lock<std::mutex> lk(mu_);
-    cv_.wait(lk, [&] { return error_ != FMA_OK || ready_[k]; });
-    if (error_ != FMA_OK) return nullptr;
-    const char* buf = static_cast<const char*>(e_->load_ring) + (k % n_) * e_->io_window_bytes;
-    if (direct_) buf = reinterpret_cast<const char*>(round_up(reinterpret_cast<uintptr_t>(buf), 4096)) + (items_[k].file_off & 4095);
-    return buf;
-}
-
-char* FileIO::wait_free(size_t k) {
-    std::unique_lock<std::mutex> lk(mu_);
-    cv_.wait(lk, [&] { return error_ != FMA_OK || k < (size_t)n_ || done_[k - n_]; });
-    if (error_ != FMA_OK) return nullptr;
+char* FileIO::window(size_t k) const {
     char* buf = static_cast<char*>(e_->load_ring) + (k % n_) * e_->io_window_bytes;
     return direct_ ? reinterpret_cast<char*>(round_up(reinterpret_cast<uintptr_t>(buf), 4096)) : buf;
 }
 
-void FileIO::posted(size_t k) {
+int FileIO::copy(size_t k, void* dev, cudaStream_t stream) {
+    bool failed;
+    {   // read: item k is in its window; write: the window's last pwrite (item k - n) has returned
+        std::unique_lock<std::mutex> lk(mu_);
+        cv_.wait(lk, [&] { return error_ != FMA_OK || (write_ ? k < (size_t)n_ || done_[k - n_] : ready_[k]); });
+        failed = error_ != FMA_OK;
+    }
+    if (failed) return finish();
+    char* win = window(k);
+    if (direct_ && !write_) win += items_[k].file_off & 4095;   // the O_DIRECT read started at the block below the item
+    RT(cudaMemcpyAsync(write_ ? win : dev, write_ ? dev : win, items_[k].bytes, cudaMemcpyDefault, stream));
+    RT(cudaEventRecord(e_->ev_load[k % n_], stream));
     std::lock_guard<std::mutex> lk(mu_);
     posted_[k] = 1;
     n_posted_ = std::max(n_posted_, k + 1);
     ++n_posted_items_;
     cv_.notify_all();
+    return FMA_OK;
 }
 
 size_t FileIO::written() {
@@ -255,15 +274,10 @@ int fma_load_file(fma_engine_t* e, const char* path, const fma_load_span_t* span
     RC(ensure_io_windows(e));
     // readers pread ahead into the windows; this thread moves each chunk to its destination as soon as it has been read
     FileIO io(e, f.fd, false, direct, items, (uint64_t)sb.st_size, path);
-    for (size_t k = 0; k < items.size(); ++k) {
-        const char* src = io.wait_read(k);
-        if (!src) break;
-        cudaStream_t st = e->cs[k % e->n_cs];
-        RT(cudaMemcpyAsync(reinterpret_cast<void*>((uintptr_t)dst[k]), src, items[k].bytes, cudaMemcpyHostToDevice, st));
-        RT(cudaEventRecord(io.event(k), st));
-        io.posted(k);
-    }
-    int rc = io.finish();
+    int rc = FMA_OK;
+    for (size_t k = 0; k < items.size(); ++k)
+        if ((rc = io.copy(k, reinterpret_cast<void*>((uintptr_t)dst[k]), e->cs[k % e->n_cs])) != FMA_OK) break;
+    if (rc == FMA_OK) rc = io.finish();
     for (int i = 0; i < e->n_cs; ++i) RT(cudaStreamSynchronize(e->cs[i]));
     if (rc == FMA_EIO) {   // a failed read of a cold load has always been FMA_EINVAL
         char why[512];

@@ -271,6 +271,9 @@ struct SleepPipe {
     Unmapper* un;          // releases units behind the pipeline; null: nothing is released (the resident gather)
     const std::vector<size_t>* subset = nullptr;  // INCREMENTAL + PACKED: only these image pages (ascending) are re-coded, in place
     bool resident = false;  // the extents go to the resident buffer (e->res, its own page layout res_off / res_bytes), not the tier's store
+    int file_fd = -1;       // FILE tier: the staged pipeline writes the image to this file, not to `store`
+    bool file_direct = false;
+    const char* file_path = nullptr;
     int publish_consumed(uint64_t image_done, cudaStream_t stream) { return un ? un->publish_consumed(image_done, stream) : FMA_OK; }
     int publish_gathered(size_t pages_done) { return publish_consumed((uint64_t)pages_done * FMA_PAGE_BYTES, e->ks); }
     // the image's pages, stored in the PACKED layout or verbatim; their device addresses in order -> e->h_tab / e->d_tab
@@ -291,7 +294,6 @@ struct SleepPipe {
     int in_place(bool packed);
     int staged(bool packed);
     int multipath();
-    int file(bool packed, int fd, bool direct, const char* path);
 };
 
 // DIRECT: copy engines move each segment chunk straight into the packed image
@@ -341,7 +343,10 @@ int SleepPipe::in_place(bool packed) {
     return FMA_OK;
 }
 
-// STAGED: K1 gather / K4 gather + encode -> HBM ring slot (a PACKED image: stored pages back to back) -> one large D2H per slot
+// STAGED: K1 gather / K4 gather + encode -> HBM ring slot (a PACKED image: stored pages back to back) -> one large D2H per slot.
+// The FILE tier (file_fd) puts a disk stage behind the ring: each slot drains into the engine's pinned I/O windows, one D2H per
+// window, and writer threads pwrite each window at its place in the file.  A unit is then released once every byte of it has been
+// WRITTEN (the writes' frontier, not the D2H's), so a sleep whose write fails half way leaves every released segment in the file.
 int SleepPipe::staged(bool packed) {
     std::vector<PagePlan> pages;
     RC(plan(packed, &pages));   // (the route has the ring)
@@ -355,84 +360,59 @@ int SleepPipe::staged(bool packed) {
         for (size_t p : img_page) sel.push_back(pages[p]);
         pages = std::move(sel);
     }
-    std::vector<Batch> slots;  // pages adjacent in the store that together fit a ring slot: by their stored bytes, or by their number
-    if (!fma_layout::plan_batches(pages, packed ? SIZE_MAX : e->ring_slot_bytes / FMA_PAGE_BYTES, packed ? e->ring_slot_bytes : UINT64_MAX, true, &slots))
-        return fail(FMA_EINVAL, "ring slot of %zu bytes cannot hold one page", e->ring_slot_bytes);
-    const std::vector<uint64_t> in_ring = ring_addresses(e, pages, slots);
+    std::vector<Batch> slots;
+    std::vector<uint64_t> in_ring;
+    RC(plan_ring_slots(e, packed, pages, &slots, &in_ring));
     PageKernels pk{e, kt, true, packed};
     RC(pk.prepare(pages, true, [&](size_t q) { return in_ring[q]; }));
+    // every image byte below the last page of slot c is in the store once slot c is (moved, or kept from the last wake)
+    auto image_end = [&](size_t c) { return (uint64_t)(img_page[slots[c].p0 + slots[c].np - 1] + 1) * FMA_PAGE_BYTES; };
+    // FILE: every slot cut into window-sized writes; slot c's are items [slot_end[c - 1], slot_end[c])
+    std::vector<FileIO::Item> items;
+    std::vector<size_t> slot_end;
+    std::optional<FileIO> io;
+    if (file_fd >= 0) {
+        for (const Batch& sl : slots) items.push_back(FileIO::Item{pages[sl.p0].off, sl.stored});
+        items = FileIO::cut(e, items, &slot_end);
+        io.emplace(e, file_fd, true, file_direct, items, 0, file_path);
+    }
+    size_t k = 0, slots_written = 0;
+    auto publish_written = [&]() -> int {   // units whose every page is in a slot that has been written are dead
+        const size_t n = io->written();
+        while (slots_written < slots.size() && slot_end[slots_written] <= n) ++slots_written;
+        return slots_written ? publish_consumed(image_end(slots_written - 1), nullptr) : FMA_OK;
+    };
     cudaStream_t last_stream = e->cs[0];
     for (size_t c = 0; c < slots.size(); ++c) {
         const Batch& sl = slots[c];
         const int slot = (int)(c % e->n_ring);
+        char* ring = static_cast<char*>(e->ring[slot]);
         cudaStream_t cstream = e->cs[c % e->n_cs];
         if (c >= (size_t)e->n_ring) RT(cudaStreamWaitEvent(e->ks, e->ev_ring_free[slot], 0));
-        RC(pk.launch(sl, (uint64_t)(uintptr_t)e->ring[slot]));
+        RC(pk.launch(sl, (uint64_t)(uintptr_t)ring));
         RT(cudaEventRecord(e->ev_ring_full[slot], e->ks));
         RT(cudaStreamWaitEvent(cstream, e->ev_ring_full[slot], 0));
-        RT(cudaMemcpyAsync(store + pages[sl.p0].off, e->ring[slot], sl.stored, cudaMemcpyDefault, cstream));
-        // "slot free" also means "every earlier slot has reached the store" (chained through the previous
-        // slot's event), so the unmapper below never releases device memory whose bytes are not yet on the host
-        if (c > 0) RT(cudaStreamWaitEvent(cstream, e->ev_ring_free[(c - 1) % e->n_ring], 0));
-        RT(cudaEventRecord(e->ev_ring_free[slot], cstream));
-        ++copy_ops;
-        // every image byte below the last page of this slot is in the store (moved just now, or kept from the last wake):
-        // units fully in the store are dead
-        RC(publish_consumed((uint64_t)(img_page[sl.p0 + sl.np - 1] + 1) * FMA_PAGE_BYTES, cstream));
-        last_stream = cstream;
-    }
-    return subset ? publish_consumed(W, last_stream) : FMA_OK;  // the clean tail of the image needs no copy
-}
-
-// FILE: the STAGED pipeline with a disk stage behind it.  K1 gather / K4 gather + encode -> HBM ring slot -> D2H into the engine's
-// pinned I/O windows -> writer threads pwrite each window at its place in the file.  A unit is released once every byte of it has
-// been WRITTEN (the writes' frontier, not the D2H's), so a sleep whose write fails half way leaves every released segment in the file.
-int SleepPipe::file(bool packed, int fd, bool direct, const char* path) {
-    std::vector<PagePlan> pages;
-    RC(plan(packed, &pages));   // (the route has the ring)
-    std::vector<Batch> slots;
-    if (!fma_layout::plan_batches(pages, packed ? SIZE_MAX : e->ring_slot_bytes / FMA_PAGE_BYTES, packed ? e->ring_slot_bytes : UINT64_MAX, true, &slots))
-        return fail(FMA_EINVAL, "ring slot of %zu bytes cannot hold one page", e->ring_slot_bytes);
-    const std::vector<uint64_t> in_ring = ring_addresses(e, pages, slots);
-    PageKernels pk{e, kt, true, packed};
-    RC(pk.prepare(pages, true, [&](size_t q) { return in_ring[q]; }));
-    // every slot cut into window-sized writes; slot c's are items [slot_end[c - 1], slot_end[c])
-    const uint64_t piece = e->io_window_bytes - 8192;
-    std::vector<FileIO::Item> items;
-    std::vector<size_t> slot_end;
-    for (const Batch& sl : slots) {
-        for (uint64_t o = 0; o < sl.stored; o += piece) items.push_back(FileIO::Item{pages[sl.p0].off + o, std::min(piece, sl.stored - o)});
-        slot_end.push_back(items.size());
-    }
-    FileIO io(e, fd, true, direct, items, 0, path);
-    size_t k = 0, slots_written = 0;
-    auto publish_written = [&]() -> int {   // units whose every page is in a slot that has been written are dead
-        const size_t n = io.written();
-        while (slots_written < slots.size() && slot_end[slots_written] <= n) ++slots_written;
-        return slots_written ? publish_consumed((uint64_t)(slots[slots_written - 1].p0 + slots[slots_written - 1].np) * FMA_PAGE_BYTES, nullptr) : FMA_OK;
-    };
-    for (size_t c = 0; c < slots.size(); ++c) {
-        const Batch& sl = slots[c];
-        const int slot = (int)(c % e->n_ring);
-        cudaStream_t cstream = e->cs[c % e->n_cs];
-        if (c >= (size_t)e->n_ring) RT(cudaStreamWaitEvent(e->ks, e->ev_ring_free[slot], 0));
-        RC(pk.launch(sl, (uint64_t)(uintptr_t)e->ring[slot]));
-        RT(cudaEventRecord(e->ev_ring_full[slot], e->ks));
-        RT(cudaStreamWaitEvent(cstream, e->ev_ring_full[slot], 0));
-        for (; k < slot_end[c]; ++k) {
-            char* window = io.wait_free(k);
-            if (!window) return io.finish();
-            RC(publish_written());
-            RT(cudaMemcpyAsync(window, static_cast<char*>(e->ring[slot]) + (items[k].file_off - pages[sl.p0].off), items[k].bytes,
-                               cudaMemcpyDeviceToHost, cstream));
-            RT(cudaEventRecord(io.event(k), cstream));
-            io.posted(k);
+        if (io) {
+            for (; k < slot_end[c]; ++k, ++copy_ops) {
+                RC(io->copy(k, ring + (items[k].file_off - pages[sl.p0].off), cstream));
+                RC(publish_written());
+            }
+        } else {
+            RT(cudaMemcpyAsync(store + pages[sl.p0].off, ring, sl.stored, cudaMemcpyDefault, cstream));
             ++copy_ops;
+            // "slot free" also means "every earlier slot has reached the store" (chained through the previous
+            // slot's event), so the unmapper below never releases device memory whose bytes are not yet on the host
+            if (c > 0) RT(cudaStreamWaitEvent(cstream, e->ev_ring_free[(c - 1) % e->n_ring], 0));
         }
         RT(cudaEventRecord(e->ev_ring_free[slot], cstream));
+        if (!io) RC(publish_consumed(image_end(c), cstream));   // units fully in the store are dead
+        last_stream = cstream;
     }
-    RC(io.finish());   // every pwrite has returned
-    return publish_consumed(W, nullptr);
+    if (io) {
+        RC(io->finish());   // every pwrite has returned
+        return publish_consumed(W, nullptr);
+    }
+    return subset ? publish_consumed(W, last_stream) : FMA_OK;  // the clean tail of the image needs no copy
 }
 
 // MULTI-PATH sleep (fma_paths_set): the mirror image of the multi-path wake.  K1 on the sleeping GPU gathers a chunk of the image
@@ -846,8 +826,13 @@ int run_pipeline(fma_engine_t* e, SleepPlan& p, Unmapper& un) {
         case SleepPipeKind::Multipath: RC(pipe.multipath()); break;
         case SleepPipeKind::StagedPacked: RC(pipe.staged(true)); break;
         case SleepPipeKind::Staged: RC(pipe.staged(false)); break;
-        case SleepPipeKind::File: RC(pipe.file(false, p.file.fd, p.file_direct, e->image_file.c_str())); break;
-        case SleepPipeKind::FilePacked: RC(pipe.file(true, p.file.fd, p.file_direct, e->image_file.c_str())); break;
+        case SleepPipeKind::File:
+        case SleepPipeKind::FilePacked:
+            pipe.file_fd = p.file.fd;
+            pipe.file_direct = p.file_direct;
+            pipe.file_path = e->image_file.c_str();
+            RC(pipe.staged(p.route.pipe == SleepPipeKind::FilePacked));
+            break;
         case SleepPipeKind::NoRing:   // (refused by route_sleep)
         case SleepPipeKind::Adopt: return fail(FMA_ESTATE, "an adopted image has no copy pipeline");  // (handled above)
         }

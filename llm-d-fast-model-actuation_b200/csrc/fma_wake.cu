@@ -224,7 +224,6 @@ struct WakePipe {
     int in_place(bool packed);
     int staged(bool packed);
     int multipath();
-    int file(bool packed);
 };
 
 // The segments `idx` as the page planner sees them: each waits for the mapper work item of its run.
@@ -310,94 +309,67 @@ int WakePipe::in_place(bool packed) {
 }
 
 // STAGED: copy engine H2D store -> ring slot (starts at t=0; a PACKED image: the stored pages, 0.758 of the bytes), K2 scatter /
-// K5 decode + scatter once the targets are mapped
+// K5 decode + scatter once the targets are mapped.  The FILE tier puts a disk stage in front of the ring: reader threads pread
+// ahead into the engine's pinned I/O windows, and each slot fills from them, one H2D per window.
 int WakePipe::staged(bool packed) {
     std::vector<PagePlan> pages;
     RC(plan(packed, &pages));
     const size_t n_pages = pages.size();
-    // the store image may be only partially woken; H2D works on runs that are contiguous in the store and fit one ring slot: by
-    // their stored bytes, or by their number
+    // the store image may be only partially woken; H2D works on runs that are contiguous in the store and fit one ring slot
     std::vector<Batch> slots;
-    if (!fma_layout::plan_batches(pages, packed ? SIZE_MAX : e->ring_slot_bytes / FMA_PAGE_BYTES, packed ? e->ring_slot_bytes : UINT64_MAX, true, &slots))
-        return fail(FMA_EINVAL, "ring slot of %zu bytes cannot hold one page", e->ring_slot_bytes);
-    const std::vector<uint64_t> in_ring = ring_addresses(e, pages, slots);
+    std::vector<uint64_t> in_ring;
+    RC(plan_ring_slots(e, packed, pages, &slots, &in_ring));
     PageKernels pk{e, kt, false, packed};
     RC(pk.prepare(pages, true, [&](size_t q) { return in_ring[q]; }));
-    if (ring_run) RC(mapper.wait(1));  // the ring is run 0 (1 GiB, ~0.2 ms to map): wait for it before the first H2D (else the route has the ring)
-    for (size_t c = 0; c < slots.size(); ++c) {
-        const Batch& sl = slots[c];
-        const int slot = (int)(c % e->n_ring);
-        cudaStream_t cstream = e->cs[c % e->n_cs];
-        if (c >= (size_t)e->n_ring) RT(cudaStreamWaitEvent(cstream, e->ev_ring_free[slot], 0));
-        RT(cudaMemcpyAsync(e->ring[slot], store + pages[sl.p0].off, sl.stored, cudaMemcpyDefault, cstream));
-        copied();
-        RT(cudaEventRecord(e->ev_ring_full[slot], cstream));
-        RC(mapper.wait(sl.need));
-        RT(cudaStreamWaitEvent(e->ks, e->ev_ring_full[slot], 0));
-        RC(pk.launch(sl, (uint64_t)(uintptr_t)e->ring[slot]));
-        RT(cudaEventRecord(e->ev_ring_free[slot], e->ks));
-        if (between) RC(between->pump(sl.p0 + sl.np, n_pages));
-    }
-    return FMA_OK;
-}
-
-// FILE: the STAGED pipeline with a disk stage in front of it.  Reader threads pread ahead into the engine's pinned I/O windows ->
-// H2D window -> ring slot -> K2 scatter / K5 decode + scatter once the targets are mapped (the same mapper.wait / ev_ring_* protocol).
-int WakePipe::file(bool packed) {
-    std::vector<PagePlan> pages;
-    RC(plan(packed, &pages));
-    std::vector<Batch> slots;
-    if (!fma_layout::plan_batches(pages, packed ? SIZE_MAX : e->ring_slot_bytes / FMA_PAGE_BYTES, packed ? e->ring_slot_bytes : UINT64_MAX, true, &slots))
-        return fail(FMA_EINVAL, "ring slot of %zu bytes cannot hold one page", e->ring_slot_bytes);
-    const std::vector<uint64_t> in_ring = ring_addresses(e, pages, slots);
-    PageKernels pk{e, kt, false, packed};
-    RC(pk.prepare(pages, true, [&](size_t q) { return in_ring[q]; }));
+    // FILE: every slot cut into window-sized reads; slot c's are items [slot_end[c - 1], slot_end[c])
     const double t_io = now_s();
-    const char* path = e->image_file.c_str();
-    FileFd f;
-    bool direct = false;
-    RC(open_image_file(path, false, &f.fd, &direct));
-    struct stat sb;
-    if (fstat(f.fd, &sb) != 0) return fail(FMA_EIO, "fstat(%s) failed: %s", path, strerror(errno));
-    const uint64_t piece = e->io_window_bytes - 8192;
     std::vector<FileIO::Item> items;
     std::vector<size_t> slot_end;
-    uint64_t file_bytes = 0;
-    for (const Batch& sl : slots) {
-        for (uint64_t o = 0; o < sl.stored; o += piece) items.push_back(FileIO::Item{pages[sl.p0].off + o, std::min(piece, sl.stored - o)});
-        slot_end.push_back(items.size());
-        file_bytes += sl.stored;
+    uint64_t read_bytes = 0;
+    FileFd f;
+    bool direct = false;
+    std::optional<FileIO> io;
+    if (tier == FMA_TIER_FILE) {
+        for (const Batch& sl : slots) {
+            items.push_back(FileIO::Item{pages[sl.p0].off, sl.stored});
+            read_bytes += sl.stored;
+        }
+        items = FileIO::cut(e, items, &slot_end);
+        // the file must hold every byte this wake reads (else it was truncated or replaced): refused before a read is issued.
+        // The items ascend in image order, so the last one ends furthest into the file.
+        const uint64_t need = items.empty() ? 0 : items.back().file_off + items.back().bytes;
+        uint64_t file_bytes = 0;
+        RC(open_image_source(e->image_file.c_str(), need, &f.fd, &direct, &file_bytes));
+        io.emplace(e, f.fd, false, direct, items, file_bytes, e->image_file.c_str());   // the readers start now, ahead of the ring's mapping
     }
-    // the file must hold every byte this wake reads (else it was truncated or replaced): refused before a read is issued
-    const uint64_t file_end = items.empty() ? 0 : items.back().file_off + items.back().bytes;
-    for (const FileIO::Item& it : items)
-        if (it.file_off + it.bytes > (uint64_t)sb.st_size)
-            return fail(FMA_EIO, "%s holds %llu bytes, the image needs %llu", path, (unsigned long long)sb.st_size, (unsigned long long)file_end);
-    FileIO io(e, f.fd, false, direct, items, (uint64_t)sb.st_size, path);
-    if (ring_run) RC(mapper.wait(1));  // (as in staged)
+    if (ring_run) RC(mapper.wait(1));  // the ring is run 0 (1 GiB, ~0.2 ms to map): wait for it before the first H2D (else the route has the ring)
     size_t k = 0;
     for (size_t c = 0; c < slots.size(); ++c) {
         const Batch& sl = slots[c];
         const int slot = (int)(c % e->n_ring);
+        char* ring = static_cast<char*>(e->ring[slot]);
         cudaStream_t cstream = e->cs[c % e->n_cs];
         if (c >= (size_t)e->n_ring) RT(cudaStreamWaitEvent(cstream, e->ev_ring_free[slot], 0));
-        for (; k < slot_end[c]; ++k) {
-            const char* src = io.wait_read(k);
-            if (!src) return io.finish();
-            RT(cudaMemcpyAsync(static_cast<char*>(e->ring[slot]) + (items[k].file_off - pages[sl.p0].off), src, items[k].bytes,
-                               cudaMemcpyHostToDevice, cstream));
-            RT(cudaEventRecord(io.event(k), cstream));
-            io.posted(k);
+        if (io) {
+            for (; k < slot_end[c]; ++k) {
+                RC(io->copy(k, ring + (items[k].file_off - pages[sl.p0].off), cstream));
+                copied();
+            }
+        } else {
+            RT(cudaMemcpyAsync(ring, store + pages[sl.p0].off, sl.stored, cudaMemcpyDefault, cstream));
             copied();
         }
         RT(cudaEventRecord(e->ev_ring_full[slot], cstream));
         RC(mapper.wait(sl.need));
         RT(cudaStreamWaitEvent(e->ks, e->ev_ring_full[slot], 0));
-        RC(pk.launch(sl, (uint64_t)(uintptr_t)e->ring[slot]));
+        RC(pk.launch(sl, (uint64_t)(uintptr_t)ring));
         RT(cudaEventRecord(e->ev_ring_free[slot], e->ks));
+        if (between) RC(between->pump(sl.p0 + sl.np, n_pages));
     }
-    RC(io.finish());   // every read has returned and every H2D out of a window has finished
-    e->tl_add("file_io", direct ? 1 : 0, t_io, now_s(), file_bytes);
+    if (io) {
+        RC(io->finish());   // every read has returned and every H2D out of a window has finished
+        e->tl_add("file_io", direct ? 1 : 0, t_io, now_s(), read_bytes);
+    }
     return FMA_OK;
 }
 
@@ -752,7 +724,7 @@ int do_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags) {
             case fma_layout::WakePipeKind::Direct: RC(pipe.direct()); break;
             case fma_layout::WakePipeKind::Kernel: RC(pipe.in_place(false)); break;
             case fma_layout::WakePipeKind::Staged: RC(pipe.staged(false)); break;
-            case fma_layout::WakePipeKind::File: RC(pipe.file(facts.image_packed)); break;
+            case fma_layout::WakePipeKind::File: RC(pipe.staged(facts.image_packed)); break;   // (a file as its store)
             case fma_layout::WakePipeKind::NoRing: return fail(FMA_ENOMEM, "the file tier needs an HBM staging ring and there is no room for one");
             }
             e->tl_add("enqueue", (int)copy_ops, t_enq0, now_s(), W);
