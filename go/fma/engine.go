@@ -253,6 +253,25 @@ func (e *Engine) MoveImage(tier int) error {
 	return nil
 }
 
+// VerifyImage checks the sleeping image against the digests it carries, where it lies, without waking it.  It returns the indices
+// of the segments whose stored bytes do not match (empty: intact).
+func (e *Engine) VerifyImage() ([]int, error) {
+	n := int(C.fma_segment_count(e.h))
+	if n < 0 {
+		return nil, lastErr(C.int(n))
+	}
+	buf := make([]C.int, n+1)
+	rc := C.fma_image_verify(e.h, &buf[0], C.int(n))
+	if rc < 0 {
+		return nil, lastErr(rc)
+	}
+	bad := make([]int, 0, int(rc))
+	for i := 0; i < int(rc) && i < n; i++ {
+		bad = append(bad, int(buf[i]))
+	}
+	return bad, nil
+}
+
 // PathsSet names idle peer GPUs whose PCIe links a host-tier wake may borrow (MULTI-PATH wake); nil turns it off.
 func (e *Engine) PathsSet(helpers []int, slotBytes uint64, slots int) error {
 	var p *C.int

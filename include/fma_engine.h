@@ -303,6 +303,22 @@ FMA_API int  fma_image_adopt_file(fma_engine_t* e, const char* path, uint64_t ta
  * copies_landed (the copy engines ran) and total (bytes = image_store_bytes). */
 FMA_API int  fma_image_move(fma_engine_t* e, int tier);
 
+/* Check the sleeping image against the K3 digests it carries, where it lies (host store, parking buffer, resident share, file),
+ * without mapping a segment.  Returns the number of segments whose stored bytes do not match (0 = intact) and writes up to `cap`
+ * of their indices (fma_segment_info order) to `out_bad`; or a negative error.
+ * Every segment that has a backup and is unmapped is checked: plain pages by K3 and PACKED pages by K6, which decodes a stored page
+ * as K5 would and digests it without writing it.  A stored PACKED page that cannot be decoded (bad magic, too many exceptions, a
+ * size that disagrees with the page table) counts its segment as bad.  The kernels read the parking buffer and the resident share
+ * in HBM, the host store through its device alias and a file through the engine's pinned I/O windows (reader threads pread whole
+ * stored pages into them, O_DIRECT when the filesystem accepts it), so no HBM is taken; a host store without a device alias is
+ * copied through 2 x 64 MiB of HBM scratch, freed before the call returns.  An adopted image (fma_image_adopt, _adopt_file,
+ * _adopt_parked) is checked against the digests that came with it: fma_image_adopt_file reads only the descriptor, and this call
+ * reads the rest.  FMA_ESTATE, with the engine unchanged: nothing is asleep, a segment to check carries no digest (sleep with
+ * FMA_FLAG_VERIFY or the "incremental" option), or a mapped segment keeps a backup (a KEEP_BACKUP or partial wake).  FMA_EIO: the
+ * image file cannot be opened or is shorter than the image.  No segment, tier, store, statistic or INCREMENTAL shadow changes;
+ * the timeline records op "verify" with file_io, kernel and total rows (total's idx = the number of bad segments). */
+FMA_API int  fma_image_verify(fma_engine_t* e, int* out_bad, int cap);
+
 /* ---- MULTI-PATH wake: borrow idle peers' PCIe links ---------------------------------------------------------------------
  * A host-tier wake is bounded by ONE x16 Gen5 link (55.6 GB/s measured of 64): 0.29 s for Llama-3-8B however good the engine
  * is.  When other GPUs of the box are idle (BASELINE config 5: the GPUs that only park sleepers; any N=1 deployment on an
@@ -450,10 +466,10 @@ FMA_API int  fma_set_option(fma_engine_t* e, const char* key, int64_t value);
 /* ---- stats ------------------------------------------------------------------------ */
 FMA_API int  fma_stats(fma_engine_t* e, fma_stats_t* out);
 
-/* Per-phase timeline of the last fma_sleep / fma_wake / fma_image_move as text, one event per line:
+/* Per-phase timeline of the last fma_sleep / fma_wake / fma_image_move / fma_image_verify as text, one event per line:
  *   "<op>,<kind>,<idx>,<t0_ms>,<t1_ms>,<bytes>\n"   (times since the call's entry)
  * kinds: plan, map_ring / map_backed / map_remap (one cuMemCreate+Map+SetAccess each, mapper thread), gate_wait,
- * enqueue, copies_landed, wait_all_mapped, drain, unmap (sleep), kernel (K1/K2/K4/K5 launches, device-timed), total;
+ * enqueue, copies_landed, wait_all_mapped, drain, unmap (sleep), kernel (K1/K2/K4/K5 launches, K3/K6 pairs of a verify, device-timed), total;
  * multi-path operations add path_chunks / path_local (idx = the path's GPU, bytes = what that path moved / moved NUMA-locally);
  * a resident share adds res_alloc (sleep) / res_free (wake) for the resident buffer's VMM calls, res_fallback (its allocation
  * failed: plain sleep), and res_gather / res_restore rows for its K1 / K4 and K2 / K5 launches (device-timed, like kernel); the

@@ -139,6 +139,7 @@ _PROTOTYPES = {
     "fma_file_store": (C.c_int, [C.c_void_p, C.c_char_p]),
     "fma_image_adopt_file": (C.c_int, [C.c_void_p, C.c_char_p, C.c_uint64, C.c_uint32]),
     "fma_image_move": (C.c_int, [C.c_void_p, C.c_int]),
+    "fma_image_verify": (C.c_int, [C.c_void_p, C.POINTER(C.c_int), C.c_int]),
     "fma_set_option": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int64]),
     "fma_stats": (C.c_int, [C.c_void_p, C.POINTER(fma_stats_t)]),
     "fma_timeline": (C.c_int, [C.c_void_p, C.c_char_p, C.c_size_t]),

@@ -245,6 +245,182 @@ void undo_move(fma_engine_t* e, MoveState& ms) {
     cudaGetLastError();
 }
 
+// ---- checking a sleeping image where it lies (fma_image_verify) ----
+// K3 digests plain pages and K6 decodes and digests PACKED ones, both straight out of the store: the parking buffer or the
+// resident share in HBM, the pinned host store through its device alias, a file through the pinned I/O windows.  Each kernel adds
+// a page's digest into that page's accumulator (d_dig, one per page of the check), and the host sums a segment's pages.
+struct Verifier {
+    explicit Verifier(fma_engine_t* engine) : e(engine) {}
+    fma_engine_t* e;
+    struct Seg { size_t index; uint64_t va, digest; };
+    std::vector<Seg> segs;            // the segments checked, by engine index
+    std::vector<uint64_t> sum;        // their digests as computed
+    std::vector<size_t> seg_of;       // accumulator i -> position in `segs`
+    std::vector<uint64_t> kbytes;     // stored bytes read by each timed launch pair
+    size_t n_ev = 0;
+    static constexpr size_t kScratch = (size_t)64 << 20;   // host store without a device alias: two HBM buffers of this size
+    void* scratch[2] = {};
+
+    // The pages of the segments `pos` (positions in `segs`) in a store with the page table (off, bytes), off == nullptr: pages stored
+    // verbatim at their image offsets.  PagePlan::need carries the page's segment position (nothing waits for a mapper here).
+    int plan(const std::vector<size_t>& pos, const std::vector<uint64_t>* off, const std::vector<uint32_t>* bytes, std::vector<PagePlan>* pages) {
+        std::vector<fma_layout::SegPages> v;
+        for (size_t k : pos) {
+            const Segment& s = e->segs[segs[k].index];
+            v.push_back(fma_layout::SegPages{s.va, s.bytes, s.packed_off, k});
+        }
+        uint64_t bad = 0;
+        if (!fma_layout::plan_pages(v, off, bytes, pages, &bad))
+            return fail(FMA_ESTATE, "segment at image offset %llu is outside the packed image's page table", (unsigned long long)bad);
+        return FMA_OK;
+    }
+
+    // One launch pair over pages [b.p0, b.p0 + b.np) of `pages`, whose accumulators start at `at`: K6 over the coded pages, K3 over
+    // the raw ones.  src(q) is where page q can be read on the device now.
+    template <class Src>
+    int launch(const std::vector<PagePlan>& pages, size_t at, const Batch& b, Src src) {
+        size_t lo = at + b.p0, hi = at + b.p0 + b.np;   // coded pages fill the accumulators from the front, raw ones from the back
+        for (size_t q = b.p0; q < b.p0 + b.np; ++q) {
+            const size_t i = pages[q].bytes == FMA_PAGE_BYTES ? --hi : lo++;
+            e->h_desc[i].addr = src(q);
+            e->h_desc[i].first_word = (pages[q].va - segs[pages[q].need].va) / 8;
+            seg_of[i] = pages[q].need;
+        }
+        const size_t p0 = at + b.p0, n_coded = lo - p0, n_raw = b.np - n_coded;
+        RT(cudaMemcpyAsync(e->d_desc + p0, e->h_desc + p0, b.np * sizeof(fma_k_page_desc), cudaMemcpyHostToDevice, e->ks));
+        RC(ensure_event_pool(e, n_ev + 2));
+        RT(cudaEventRecord(e->ev_pool[n_ev], e->ks));
+        if (n_coded) {
+            if (!fma_k_launch_unpack_digest) return fail(FMA_ECUDA, "this library was built without K6: a PACKED image cannot be checked");
+            RT(fma_k_launch_unpack_digest(e->d_desc + p0, (uint32_t)n_coded, e->d_dig + p0, e->d_psize + e->pdesc_cap, e->ks));
+        }
+        RT(fma_k_launch_page_digest(e->d_desc + lo, (uint32_t)n_raw, e->d_dig + lo, e->ks));
+        RT(cudaEventRecord(e->ev_pool[n_ev + 1], e->ks));
+        n_ev += 2;
+        kbytes.push_back(b.stored);
+        return FMA_OK;
+    }
+
+    // a store the device reads in place (HBM, or pinned host memory through its alias) at `base`
+    int in_place(const std::vector<PagePlan>& pages, size_t at, uint64_t base) {
+        std::vector<Batch> batches;
+        fma_layout::plan_batches(pages, slot_pages(e), UINT64_MAX, false, &batches);
+        for (const Batch& b : batches) RC(launch(pages, at, b, [&](size_t q) { return base + pages[q].off; }));
+        return FMA_OK;
+    }
+
+    // a host store without a device alias: runs of pages copied into two HBM scratch buffers in turn, checked there
+    int staged_host(const std::vector<PagePlan>& pages, size_t at) {
+        std::vector<Batch> batches;
+        if (!fma_layout::plan_batches(pages, SIZE_MAX, kScratch, true, &batches)) return fail(FMA_EINVAL, "a stored page does not fit %zu bytes of scratch", kScratch);
+        RC(ensure_ring_events(e, 2));
+        for (int i = 0; i < 2 && i < (int)batches.size(); ++i)
+            if (cudaMalloc(&scratch[i], kScratch) != cudaSuccess) {
+                cudaGetLastError();
+                return fail(FMA_ENOMEM, "cannot allocate 2 x %zu bytes of HBM scratch to check a host store without a device alias", kScratch);
+            }
+        for (size_t c = 0; c < batches.size(); ++c) {
+            const Batch& b = batches[c];
+            const int s = (int)(c % 2);
+            char* buf = static_cast<char*>(scratch[s]);
+            if (c >= 2) RT(cudaStreamWaitEvent(e->cs[0], e->ev_ring_free[s], 0));
+            RT(cudaMemcpyAsync(buf, static_cast<const char*>(e->host.base) + pages[b.p0].off, b.stored, cudaMemcpyHostToDevice, e->cs[0]));
+            RT(cudaEventRecord(e->ev_ring_full[s], e->cs[0]));
+            RT(cudaStreamWaitEvent(e->ks, e->ev_ring_full[s], 0));
+            RC(launch(pages, at, b, [&](size_t q) { return (uint64_t)(uintptr_t)buf + (pages[q].off - pages[b.p0].off); }));
+            RT(cudaEventRecord(e->ev_ring_free[s], e->ks));
+        }
+        return FMA_OK;
+    }
+
+    // the image file: reader threads pread runs of whole stored pages into the pinned I/O windows, the kernels read each window
+    // over the link, and the window goes back to its reader behind them
+    int file(const std::vector<PagePlan>& pages, size_t at) {
+        if (!e->load_ring) RC(ensure_io_windows(e));
+        const uint64_t window = e->io_window_bytes - 8192;   // (the windows' O_DIRECT slack, ensure_io_windows)
+        std::vector<Batch> batches;
+        if (!fma_layout::plan_batches(pages, SIZE_MAX, window, true, &batches))
+            return fail(FMA_EINVAL, "a stored page does not fit an I/O window of %llu bytes", (unsigned long long)window);
+        std::vector<FileIO::Item> items;
+        uint64_t need = 0, read_bytes = 0;
+        for (const Batch& b : batches) {
+            items.push_back(FileIO::Item{pages[b.p0].off, b.stored});
+            need = std::max(need, pages[b.p0].off + b.stored);
+            read_bytes += b.stored;
+        }
+        const double t_io = now_s();
+        FileFd f;
+        bool direct = false;
+        uint64_t file_bytes = 0;
+        RC(open_image_source(e->image_file.c_str(), need, &f.fd, &direct, &file_bytes));
+        FileIO io(e, f.fd, false, direct, items, file_bytes, e->image_file.c_str());
+        for (size_t c = 0; c < batches.size(); ++c) {
+            const Batch& b = batches[c];
+            RC(io.read_in_place(c, e->ks, [&](const char* win) {
+                return launch(pages, at, b, [&](size_t q) { return (uint64_t)(uintptr_t)win + (pages[q].off - pages[b.p0].off); });
+            }));
+        }
+        RC(io.finish());   // every read has returned and every kernel over a window has finished
+        e->tl_add("file_io", direct ? 1 : 0, t_io, now_s(), read_bytes);
+        return FMA_OK;
+    }
+
+    int run(const std::vector<size_t>& main, const std::vector<size_t>& res) {
+        std::vector<PagePlan> mp, rp;
+        RC(plan(main, e->image_packed ? &e->img_off : nullptr, &e->img_bytes, &mp));
+        RC(plan(res, e->res_packed ? &e->res_off : nullptr, &e->res_bytes, &rp));
+        const size_t n = mp.size() + rp.size();
+        RC(ensure_streams(e));
+        RC(ensure_desc(e, n));
+        seg_of.assign(n, 0);
+        RT(cudaEventRecord(e->ev_start, e->ks));
+        e->tl_dev_base = now_s() - e->tl_entry;
+        RT(cudaMemsetAsync(e->d_dig, 0, n * sizeof(uint64_t), e->ks));
+        const auto coded = [](const PagePlan& q) { return q.bytes != FMA_PAGE_BYTES; };
+        if (std::any_of(mp.begin(), mp.end(), coded) || std::any_of(rp.begin(), rp.end(), coded)) {
+            RC(ensure_pack_bufs(e, 1));   // (K6 counts malformed pages in K5's error counter)
+            RT(cudaMemsetAsync(e->d_psize + e->pdesc_cap, 0, sizeof(uint32_t), e->ks));
+        }
+        if (!mp.empty()) {
+            switch (e->image_tier) {
+            case FMA_TIER_HOST:
+                RC(e->host.dev_alias ? in_place(mp, 0, (uint64_t)(uintptr_t)e->host.dev_alias) : staged_host(mp, 0));
+                break;
+            case FMA_TIER_FILE: RC(file(mp, 0)); break;
+            default:
+                if (!e->park.va) return fail(FMA_ESTATE, "the parking buffer that holds the image is gone");
+                RC(in_place(mp, 0, (uint64_t)e->park.va));
+            }
+        }
+        if (!rp.empty()) {
+            if (!e->res.va) return fail(FMA_ESTATE, "the resident part of the image is gone");
+            RC(in_place(rp, mp.size(), (uint64_t)e->res.va));
+        }
+        RT(cudaMemcpyAsync(e->h_dig, e->d_dig, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, e->ks));
+        RT(cudaStreamSynchronize(e->ks));
+        sum.assign(segs.size(), 0);
+        for (size_t i = 0; i < n; ++i) sum[seg_of[i]] += e->h_dig[i];
+        for (size_t i = 0; i + 1 < n_ev; i += 2) {   // device-timed launch rows
+            float ms0 = 0, ms = 0;
+            RT(cudaEventElapsedTime(&ms0, e->ev_start, e->ev_pool[i]));
+            RT(cudaEventElapsedTime(&ms, e->ev_pool[i], e->ev_pool[i + 1]));
+            const double t0 = e->tl_entry + e->tl_dev_base + ms0 * 1e-3;
+            e->tl_add("kernel", (int)(i / 2), t0, t0 + ms * 1e-3, kbytes[i / 2]);
+        }
+        return FMA_OK;
+    }
+
+    ~Verifier() {   // nothing may still read the scratch when it goes
+        if (scratch[0] || scratch[1]) {
+            cudaStreamSynchronize(e->cs[0]);
+            cudaStreamSynchronize(e->ks);
+        }
+        for (void* p : scratch)
+            if (p) cudaFree(p);
+        cudaGetLastError();
+    }
+};
+
 }  // namespace
 }  // namespace fma_impl
 
@@ -505,6 +681,44 @@ int fma_image_move(fma_engine_t* e, int tier) {
     e->st.tier = tier;
     e->tl_add("total", 0, t_entry, now_s(), e->image_store_bytes);
     return FMA_OK;
+}
+
+// ---- checking a sleeping image against its digests where it lies (see include/fma_engine.h) ------------------------------
+int fma_image_verify(fma_engine_t* e, int* out_bad, int cap) {
+    if (check_engine(e) != FMA_OK) return FMA_EINVAL;
+    std::lock_guard<std::mutex> op(e->op_mu);
+    if (cap < 0 || (cap > 0 && !out_bad)) return fail(FMA_EINVAL, "out_bad is NULL or cap is negative");
+    Verifier v(e);
+    std::vector<size_t> main, res;   // positions in v.segs: the image's own store, the resident share
+    {
+        std::lock_guard<std::mutex> lk(e->mu);
+        for (size_t i = 0; i < e->segs.size(); ++i) {
+            const Segment& s = e->segs[i];
+            if (!s.has_backup) continue;
+            if (s.mapped) return fail(FMA_ESTATE, "segment %zu is mapped and keeps a backup (a KEEP_BACKUP or partial wake): wake the rest or sleep again first", i);
+            if (!s.digest_valid)
+                return fail(FMA_ESTATE, "segment %zu of the sleeping image carries no digest: sleep with FMA_FLAG_VERIFY or the incremental option to record them", i);
+            const bool resident = s.backup_tier == FMA_TIER_LOCAL && e->image_tier == FMA_TIER_HOST;
+            (resident ? res : main).push_back(v.segs.size());
+            v.segs.push_back(Verifier::Seg{i, (uint64_t)s.va, s.digest});
+        }
+    }
+    if (v.segs.empty()) return fail(FMA_ESTATE, "nothing is asleep");
+    DeviceGuard guard(e->device);
+    RC(flush_kernel_times(e));   // (the last operation's kernel rows and times, before the timeline turns to this call)
+    const double t_entry = now_s();
+    e->tl_begin("verify", t_entry);
+    const int rc = v.run(main, res);
+    if (e->ks) cudaStreamSynchronize(e->ks);   // nothing still reads a store or the descriptors, also after a failure
+    if (rc != FMA_OK) return rc;
+    int n_bad = 0;
+    for (size_t k = 0; k < v.segs.size(); ++k)
+        if (v.sum[k] != v.segs[k].digest) {
+            if (n_bad < cap) out_bad[n_bad] = (int)v.segs[k].index;
+            ++n_bad;
+        }
+    e->tl_add("total", n_bad, t_entry, now_s(), e->image_store_bytes + e->res_store_bytes);
+    return n_bad;
 }
 
 

@@ -449,12 +449,39 @@ class FileIO {
     FileIO(fma_engine_t* e, int fd, bool write, bool direct, std::vector<Item> items, uint64_t file_bytes, const char* path, char* mem = nullptr);
     ~FileIO();
     int copy(size_t k, void* dev, cudaStream_t stream);   // FMA_OK, a CUDA error, or (the I/O failed) finish()'s error
+    // read: copy() without the copy.  enqueue(window) puts work on `stream` that reads item k in place in its pinned window (a
+    // kernel reading it over the link, fma_image_verify), and the window is handed back behind that work.
+    template <class Enqueue>
+    int read_in_place(size_t k, cudaStream_t stream, Enqueue enqueue) {
+        return post(k, stream, [&](char* win) { return enqueue(static_cast<const char*>(win)); });
+    }
     size_t written();                  // items whose pwrite has returned, as a prefix of `items`
     int finish();                      // joins the threads and waits for every posted copy; FMA_OK or the first error (FMA_EIO / FMA_ECUDA)
     double io_seconds() const { return io_ns_.load() * 1e-9; }
     int threads() const { return (int)th_.size(); }
 
   private:
+    // waits for item k's window, enqueue(window) on `stream`, records the window's event behind it and marks the item posted
+    template <class Enqueue>
+    int post(size_t k, cudaStream_t stream, Enqueue enqueue) {
+        bool failed;
+        {   // read: item k is in its window; write: the window's last pwrite (item k - n) has returned
+            std::unique_lock<std::mutex> lk(mu_);
+            cv_.wait(lk, [&] { return error_ != FMA_OK || (write_ ? k < (size_t)n_ || done_[k - n_] : ready_[k]); });
+            failed = error_ != FMA_OK;
+        }
+        if (failed) return finish();
+        char* win = window(k);
+        if (direct_ && !write_) win += items_[k].file_off & 4095;   // the O_DIRECT read started at the block below the item
+        RC(enqueue(win));
+        RT(cudaEventRecord(e_->ev_load[k % n_], stream));
+        std::lock_guard<std::mutex> lk(mu_);
+        posted_[k] = 1;
+        n_posted_ = std::max(n_posted_, k + 1);
+        ++n_posted_items_;
+        cv_.notify_all();
+        return FMA_OK;
+    }
     void worker();
     char* window(size_t k) const;      // where item k's I/O starts in its window (4 KiB aligned for O_DIRECT)
     void set_error(int code, const char* fmt, ...);

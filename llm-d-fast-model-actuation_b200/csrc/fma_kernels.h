@@ -62,3 +62,9 @@ cudaError_t fma_k_launch_pack_probe(const uint64_t* src_tab, uint32_t n_pages, u
 // K4 / K5: *err_count (device, zeroed by the caller) counts pages that could not be coded / decoded
 cudaError_t fma_k_launch_pack(fma_k_pack_desc* descs, uint32_t n_pages, uint32_t* err_count, cudaStream_t stream);   // writes descs[].state
 cudaError_t fma_k_launch_unpack(const fma_k_pack_desc* descs, uint32_t n_pages, uint32_t* err_count, cudaStream_t stream);
+// K6: out_zeroed[p] += the K3 digest of the page K5 would decode from the coded page pages[p].addr (first_word as for K3); nothing
+// else is written.  *err_count counts malformed pages as K5 does, and such a page adds nothing to its accumulator.
+// Declared weak: the engine's host translation units are also built without the kernels, against stand-ins for the launch
+// wrappers (a host simulation), and fma_image_verify refuses a PACKED image when this wrapper is absent.
+__attribute__((weak)) cudaError_t fma_k_launch_unpack_digest(const fma_k_page_desc* pages, uint32_t n_pages, uint64_t* out_zeroed,
+                                                             uint32_t* err_count, cudaStream_t stream);

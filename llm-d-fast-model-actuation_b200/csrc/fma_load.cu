@@ -173,23 +173,10 @@ char* FileIO::window(size_t k) const {
 }
 
 int FileIO::copy(size_t k, void* dev, cudaStream_t stream) {
-    bool failed;
-    {   // read: item k is in its window; write: the window's last pwrite (item k - n) has returned
-        std::unique_lock<std::mutex> lk(mu_);
-        cv_.wait(lk, [&] { return error_ != FMA_OK || (write_ ? k < (size_t)n_ || done_[k - n_] : ready_[k]); });
-        failed = error_ != FMA_OK;
-    }
-    if (failed) return finish();
-    char* win = window(k);
-    if (direct_ && !write_) win += items_[k].file_off & 4095;   // the O_DIRECT read started at the block below the item
-    RT(cudaMemcpyAsync(write_ ? win : dev, write_ ? dev : win, items_[k].bytes, cudaMemcpyDefault, stream));
-    RT(cudaEventRecord(e_->ev_load[k % n_], stream));
-    std::lock_guard<std::mutex> lk(mu_);
-    posted_[k] = 1;
-    n_posted_ = std::max(n_posted_, k + 1);
-    ++n_posted_items_;
-    cv_.notify_all();
-    return FMA_OK;
+    return post(k, stream, [&](char* win) -> int {
+        RT(cudaMemcpyAsync(write_ ? win : dev, write_ ? dev : win, items_[k].bytes, cudaMemcpyDefault, stream));
+        return FMA_OK;
+    });
 }
 
 size_t FileIO::written() {

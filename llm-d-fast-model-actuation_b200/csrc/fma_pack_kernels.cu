@@ -3,6 +3,7 @@
 //   K4p fma_k_pack_probe   per page: would it pack?  -> stored size (kPackedBytes or 2 MiB raw)
 //   K4  fma_k_pack         gather + encode: scattered 2 MiB device pages -> packed pages in a contiguous ring slot
 //   K5  fma_k_unpack       decode + scatter: packed pages in a ring slot -> the segments' device pages
+//   K6  fma_k_unpack_digest decode + K3 digest of stored pages where they lie, writing no page (fma_image_verify)
 //
 // They take the place of K1/K2 (fma_kernels.cu) when the engine's `pack` option is on and the tier is host DRAM: the
 // copy engines then move 0.758 x the bytes over PCIe Gen5, which is what bounds a wake (DESIGN.md §4).  The reference
@@ -233,6 +234,104 @@ fma_k_unpack(const fma_k_pack_desc* __restrict__ descs, uint32_t n_pages, uint32
     }
 }
 
+// ------------------------------------------------------------------------------------
+// K6: decode + digest.  The K3 digest (fma_kernels.cu) of the page K5 would write, without writing it: a sleeping image is
+// checked where it lies, with nothing mapped.  K5's work items; each decoded 64-bit word goes straight into
+// sum_j fmix64(w_j + (first_word + j + 1) * GOLDEN).  The exceptions of a part then correct the words they patch: a word's
+// term as decoded (exponent 0) is replaced by its term with every patch of that word applied, as K5's patch loop leaves it.
+// ------------------------------------------------------------------------------------
+#define FMA_DIGEST_GOLDEN 0x9E3779B97F4A7C15ull
+__device__ __forceinline__ uint64_t digest_mix(uint64_t z) {   // fmix64, as K3 and oracle/fma_oracle.c define it
+    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+    return z ^ (z >> 31);
+}
+__device__ __forceinline__ uint64_t digest_term(uint64_t w, uint64_t pos) { return digest_mix(w + (pos + 1) * FMA_DIGEST_GOLDEN); }
+
+// word `wd` (4 values) of a coded page as lane_decode leaves it, before any exception patch
+__device__ __forceinline__ uint64_t decoded_word(const unsigned char* src, uint32_t wd) {
+    const uint32_t v0 = (wd * 4u) & ~7u;   // the lane's first value
+    const uint2 sm = ld_stream8(src + kSmOff + v0);
+    uint32_t w[4];
+    lane_decode(sm.x, sm.y, ld_stream4(src + kNibOff + v0 / 2), __ldg(src + kEmaxOff + v0 / kTileValues), w);
+    return (wd & 1) ? ((uint64_t)w[3] << 32 | w[2]) : ((uint64_t)w[1] << 32 | w[0]);
+}
+
+__global__ void __launch_bounds__(kThreads, 8)   // K5's shape: 32 registers, 8 CTAs per SM
+fma_k_unpack_digest(const fma_k_page_desc* __restrict__ pages, uint32_t n_pages, unsigned long long* __restrict__ out,
+                    uint32_t* __restrict__ err) {
+    __shared__ uint32_t s_exc[kExcCap];          // the part's exception entries
+    __shared__ uint32_t s_n;
+    __shared__ unsigned long long s_sum[kWarps];
+    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint32_t n_items = n_pages * kParts;
+    for (uint32_t item = blockIdx.x; item < n_items; item += gridDim.x) {
+        const uint32_t p = item / kParts, part = item % kParts;
+        const unsigned char* src = reinterpret_cast<const unsigned char*>(pages[p].addr);
+        const uint64_t first_word = pages[p].first_word;
+        const uint32_t magic = ld_stream4(src + kHdrOff), n_exc = ld_stream4(src + kHdrOff + 4);
+        if (magic != kMagic || n_exc > kExcCap) {  // uniform per CTA; counted once per page, and the page adds nothing
+            if (threadIdx.x == 0 && part == 0) atomicAdd(err, 1u);
+            continue;
+        }
+        if (threadIdx.x == 0) s_n = 0;
+        uint64_t acc = 0;
+        for (uint32_t it = part * kItersPart; it < (part + 1) * kItersPart; ++it) {
+            uint2 sm[kU];
+            uint32_t nib[kU], emax[kU];
+#pragma unroll
+            for (int u = 0; u < kU; ++u) {
+                const uint32_t tile = tile_of(it, warp, u);
+                sm[u] = ld_stream8(src + kSmOff + tile * kTileValues + lane * 8u);
+                nib[u] = ld_stream4(src + kNibOff + tile * (kTileValues / 2) + lane * 4u);
+                emax[u] = __ldg(src + kEmaxOff + tile);
+            }
+#pragma unroll
+            for (int u = 0; u < kU; ++u) {
+                uint32_t w[4];
+                lane_decode(sm[u].x, sm[u].y, nib[u], emax[u], w);
+                const uint64_t j = first_word + tile_of(it, warp, u) * (kTileValues / 4) + lane * 2u;   // the lane's first word
+                acc += digest_term((uint64_t)w[1] << 32 | w[0], j);
+                acc += digest_term((uint64_t)w[3] << 32 | w[2], j + 1);
+            }
+        }
+        __syncthreads();   // s_n is zero
+        const uint32_t* exc = reinterpret_cast<const uint32_t*>(src + kExcOff);
+        for (uint32_t i = threadIdx.x; i < n_exc; i += kThreads) {   // every part scans the page's list for its own range, as K5
+            const uint32_t entry = ld_stream4(exc + i);
+            if (exc_index(entry) / kValuesPart == part) s_exc[atomicAdd(&s_n, 1u)] = entry;
+        }
+        __syncthreads();
+        const uint32_t m = s_n;
+        for (uint32_t i = threadIdx.x; i < m; i += kThreads) {   // rare: one thread per patched word, the word's first entry here
+            const uint32_t wd = exc_index(s_exc[i]) / 4u;
+            bool first = true;
+            for (uint32_t k = 0; k < i && first; ++k) first = exc_index(s_exc[k]) / 4u != wd;
+            if (!first) continue;
+            const uint64_t before = decoded_word(src, wd);
+            uint64_t after = before;
+            for (uint32_t k = i; k < m; ++k) {
+                const uint32_t entry = s_exc[k], v = exc_index(entry);
+                if (v / 4u != wd) continue;
+                const uint32_t sh = 16u * (v & 3u);
+                after = (after & ~(0xFFFFull << sh)) | (uint64_t)apply_exception((uint32_t)(after >> sh) & 0xFFFFu, entry) << sh;
+            }
+            acc += digest_term(after, first_word + wd) - digest_term(before, first_word + wd);
+        }
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) acc += __shfl_down_sync(0xffffffffu, acc, off);
+        if (lane == 0) s_sum[warp] = acc;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            unsigned long long tot = 0;
+#pragma unroll
+            for (int w = 0; w < kWarps; ++w) tot += s_sum[w];
+            atomicAdd(out + p, tot);
+        }
+        __syncthreads();   // s_exc, s_n and s_sum are free for the next item
+    }
+}
+
 int g_pack_sm_count = 0;
 int pack_sm_count() {
     if (!g_pack_sm_count) {
@@ -272,5 +371,13 @@ cudaError_t fma_k_launch_pack(fma_k_pack_desc* descs, uint32_t n_pages, uint32_t
 cudaError_t fma_k_launch_unpack(const fma_k_pack_desc* descs, uint32_t n_pages, uint32_t* err_count, cudaStream_t stream) {
     if (n_pages == 0) return cudaSuccess;
     FMA_LAUNCH(fma_k_unpack, pack_grid(n_pages * kParts), kThreads, 0, stream, descs, n_pages, err_count);
+    return cudaGetLastError();
+}
+
+cudaError_t fma_k_launch_unpack_digest(const fma_k_page_desc* pages, uint32_t n_pages, uint64_t* out_zeroed, uint32_t* err_count,
+                                       cudaStream_t stream) {
+    if (n_pages == 0) return cudaSuccess;
+    FMA_LAUNCH(fma_k_unpack_digest, pack_grid(n_pages * kParts), kThreads, 0, stream, pages, n_pages,
+               reinterpret_cast<unsigned long long*>(out_zeroed), err_count);
     return cudaGetLastError();
 }

@@ -234,6 +234,15 @@ class CuMemAllocator:
             raise L.FmaError(L.FMA_EINVAL, f"move_image: tier {tier!r} is not 'host' or 'file'")
         logger.info("fma_b200: sleeping image moved to the %s tier (%.2f GiB)", tier, self.engine.stats()["image_store_bytes"] / 1024**3)
 
+    def verify_image(self) -> bool:
+        """Check this rank's sleeping image where it lies (host DRAM, disk or parking HBM) against the digests recorded when it
+        slept with FMA_FLAG_VERIFY, without waking it: False when a segment's stored bytes do not match, so the caller can cold-start
+        instead of waking wrong weights.  Raises FmaError if the image carries no digests or nothing is asleep."""
+        bad = self.engine.verify_image()
+        if bad:
+            logger.warning("fma_b200: sleeping image fails verification in %d segment(s): %s", len(bad), bad[:8])
+        return not bad
+
     # ---- pool --------------------------------------------------------------------------
     @contextmanager
     def use_memory_pool(self, tag: str | None = None):

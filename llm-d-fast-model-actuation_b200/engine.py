@@ -348,6 +348,16 @@ class Engine:
         ``peer_release``; a source file is never touched."""
         check(self._lib.fma_image_move(self._h, tier))
 
+    def verify_image(self) -> list[int]:
+        """Check the sleeping image against the digests it carries, where it lies, without waking it (fma_image_verify): the
+        indices of the segments whose stored bytes do not match, [] when it is intact.  Raises FmaError when nothing is asleep, a
+        segment carries no digest (sleep with FMA_FLAG_VERIFY or ``incremental``), a mapped segment keeps a backup, or the image
+        file cannot be read whole (FMA_EIO)."""
+        n = self.segment_count()
+        bad = (C.c_int * max(n, 1))()
+        k = check(self._lib.fma_image_verify(self._h, bad, n))
+        return sorted(bad[i] for i in range(min(k, n)))
+
     # -- cold load -------------------------------------------------------------------------
     def load_file(self, path: str, spans: Sequence[tuple[int, int, int]], o_direct: bool = False) -> dict:
         """Stream (file_offset, nbytes, device_address) spans of one file into mapped segments."""
