@@ -146,7 +146,7 @@ func (e *Engine) LoadFile(path string, spans []LoadSpan) (seconds float64, err e
 }
 
 // Stats returns the engine's fma_stats_t as cgo sees it, so every field of include/fma_engine.h is there without a Go copy of
-// the struct, resident_bytes (the HBM a sleeping image's resident share holds on this GPU) included.
+// the struct, resident_bytes (the HBM a sleeping image's resident share holds on this GPU) and prefetched_bytes included.
 func (e *Engine) Stats() (C.fma_stats_t, error) {
 	var st C.fma_stats_t
 	if rc := C.fma_stats(e.h, &st); rc != 0 {
@@ -248,6 +248,16 @@ func (e *Engine) ImageAdoptFile(path string, tagMask uint64, flags uint32) error
 // parking buffer).  The source store stays allocated until HostRelease / PeerRelease; a source file is never touched.
 func (e *Engine) MoveImage(tier int) error {
 	if rc := C.fma_image_move(e.h, C.int(tier)); rc != 0 {
+		return lastErr(rc)
+	}
+	return nil
+}
+
+// PrefetchImage copies the tail of the sleeping image, up to `bytes` of stored bytes (rounded down to 2 MiB), from host DRAM or
+// its file into this GPU's HBM ahead of a wake, without waking it; the next Wake moves only the rest over the link.  0 frees that
+// HBM again.  Stats().prefetched_bytes reports what the copy holds.
+func (e *Engine) PrefetchImage(bytes uint64) error {
+	if rc := C.fma_image_prefetch(e.h, C.uint64_t(bytes)); rc != 0 {
 		return lastErr(rc)
 	}
 	return nil

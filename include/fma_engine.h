@@ -157,7 +157,8 @@ typedef struct fma_stats {
                                        2 MiB); 0 when there is none                                          */
     uint64_t io_buffer_bytes;       /* pinned host DRAM of the engine's file I/O windows (fma_load_file and the file tier;
                                        pinned once per engine): all the host DRAM a file-tier sleeper holds        */
-    uint64_t reserved[1];
+    uint64_t prefetched_bytes;      /* HBM the prefetched copy of a sleeping image holds on this GPU now (fma_image_prefetch;
+                                       its stored bytes, in one allocation rounded up to 2 MiB); not in resident_bytes */
 } fma_stats_t;
 
 /* ---- library ---------------------------------------------------------------------- */
@@ -319,6 +320,36 @@ FMA_API int  fma_image_move(fma_engine_t* e, int tier);
  * the timeline records op "verify" with file_io, kernel and total rows (total's idx = the number of bad segments). */
 FMA_API int  fma_image_verify(fma_engine_t* e, int* out_bad, int cap);
 
+/* Prefetch part or all of the sleeping image into this engine's own GPU ahead of a wake, or drop that copy, without waking it.
+ * A wake is bounded by the link its image crosses (PCIe for the host tier, the disk for the file tier); the resident share keeps
+ * bytes off it too, but is fixed at sleep time and only given back by a wake.  Once a caller knows which sleeper wakes next, and
+ * how much HBM the GPU can spare, it copies that much of the image into HBM here, and gives it back with bytes = 0.
+ * `bytes` is rounded down to 2 MiB.  The segments copied follow the resident share's rule over stored sizes: from the last segment
+ * in image order to the first, a segment is taken if its stored size still fits what is left (a budget of image_store_bytes or
+ * more takes all of it).  They go, back to back, into ONE VMM allocation on the engine's GPU; a PACKED image's stored pages stay
+ * coded (0.758 of the bf16 weights).  From the host store the copy engines move them (direct_chunk pieces over the engine's copy
+ * streams); from a file, the file tier's reader threads pread them into the pinned I/O windows and the copy engines take them from
+ * there (O_DIRECT under the file tier's rule).  The tier's store keeps every byte: the prefetch is a copy, so dropping it copies
+ * nothing, and hand-overs (fma_image_export, _describe, fma_host_store_share, a file adopted elsewhere), the K3 digests and the
+ * INCREMENTAL shadows are unaffected.  Nothing is mapped and no segment record but the prefetch's own table changes.
+ * The next fma_wake restores the prefetched segments from HBM through the resident share's restore (K2 / K5 pieces between the link
+ * part's launches, as soon as their runs are mapped) and moves only the others over the link (a file-tier wake reads only their
+ * pages); the buffer is freed once that restore has completed and every run is mapped, while a prefetched segment still sleeps
+ * after a tag-selective wake it stays, after an FMA_FLAG_KEEP_BACKUP wake it goes (the store is the backup), and a wake that fails
+ * is rolled back with the buffer kept for the retry.  fma_image_move between the host and file tiers keeps it; a move to the peer
+ * or local tier frees it after success.  fma_image_verify checks the prefetched copy as well as the store (K3 plain, K6 PACKED).
+ * A segment freed while asleep leaves the table; fma_engine_destroy frees the buffer.
+ * A call while a prefetch exists replaces it: the old buffer is freed first, so only the new part's HBM is needed.  bytes = 0
+ * frees it and succeeds when there is none, whatever the engine's state.  Refusals leave the engine unchanged: FMA_ESTATE when
+ * nothing is asleep, a backed-up segment is mapped (a KEEP_BACKUP or partial wake), or the image keeps a resident share from its
+ * sleep (set resident_bytes to 0 and sleep again); FMA_EINVAL when the image sleeps in the peer or local tier (it is in HBM already).
+ * Failures leave no buffer and the image, its tier and every statistic as they were: FMA_ENOMEM (no HBM for the buffer), FMA_EIO
+ * (the image file cannot be opened, is shorter than the image or a read fails), FMA_ECUDA.  Like every image call it runs alone on
+ * the engine (it waits for a sleep, wake, move or verify in flight), synchronises only the engine's own streams and events, and
+ * records timeline op "prefetch" with rows file_io, copies_landed and total (idx = segments, bytes = stored bytes prefetched).
+ * fma_stats_t.prefetched_bytes reports the buffer's stored bytes. */
+FMA_API int  fma_image_prefetch(fma_engine_t* e, uint64_t bytes);
+
 /* ---- MULTI-PATH wake: borrow idle peers' PCIe links ---------------------------------------------------------------------
  * A host-tier wake is bounded by ONE x16 Gen5 link (55.6 GB/s measured of 64): 0.29 s for Llama-3-8B however good the engine
  * is.  When other GPUs of the box are idle (BASELINE config 5: the GPUs that only park sleepers; any N=1 deployment on an
@@ -466,7 +497,7 @@ FMA_API int  fma_set_option(fma_engine_t* e, const char* key, int64_t value);
 /* ---- stats ------------------------------------------------------------------------ */
 FMA_API int  fma_stats(fma_engine_t* e, fma_stats_t* out);
 
-/* Per-phase timeline of the last fma_sleep / fma_wake / fma_image_move / fma_image_verify as text, one event per line:
+/* Per-phase timeline of the last fma_sleep / fma_wake / fma_image_move / fma_image_verify / fma_image_prefetch as text, one event per line:
  *   "<op>,<kind>,<idx>,<t0_ms>,<t1_ms>,<bytes>\n"   (times since the call's entry)
  * kinds: plan, map_ring / map_backed / map_remap (one cuMemCreate+Map+SetAccess each, mapper thread), gate_wait,
  * enqueue, copies_landed, wait_all_mapped, drain, unmap (sleep), kernel (K1/K2/K4/K5 launches, K3/K6 pairs of a verify, device-timed), total;

@@ -61,7 +61,7 @@ class fma_stats_t(C.Structure):
         ("total_kernel_launches", C.c_uint64), ("total_copy_ops", C.c_uint64),
         ("hbm_mapped_bytes", C.c_uint64), ("hbm_aux_bytes", C.c_uint64), ("parked_bytes", C.c_uint64),
         ("image_store_bytes", C.c_uint64), ("sleep_bytes_copied", C.c_uint64), ("resident_bytes", C.c_uint64),
-        ("io_buffer_bytes", C.c_uint64), ("reserved", C.c_uint64 * 1),
+        ("io_buffer_bytes", C.c_uint64), ("prefetched_bytes", C.c_uint64),
     ]
 
     def as_dict(self) -> dict:
@@ -140,6 +140,7 @@ _PROTOTYPES = {
     "fma_image_adopt_file": (C.c_int, [C.c_void_p, C.c_char_p, C.c_uint64, C.c_uint32]),
     "fma_image_move": (C.c_int, [C.c_void_p, C.c_int]),
     "fma_image_verify": (C.c_int, [C.c_void_p, C.POINTER(C.c_int), C.c_int]),
+    "fma_image_prefetch": (C.c_int, [C.c_void_p, C.c_uint64]),
     "fma_set_option": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int64]),
     "fma_stats": (C.c_int, [C.c_void_p, C.POINTER(fma_stats_t)]),
     "fma_timeline": (C.c_int, [C.c_void_p, C.c_char_p, C.c_size_t]),

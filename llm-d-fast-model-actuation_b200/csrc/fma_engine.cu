@@ -660,6 +660,15 @@ void resident_release(fma_engine_t* e) {
     e->res_store_bytes = 0;
 }
 
+void prefetch_release(fma_engine_t* e) {
+    vmm_buffer_free(e->pf);
+    e->pf_off.clear();
+    e->pf_bytes.clear();
+    e->pf_store_bytes = 0;
+    std::lock_guard<std::mutex> lk(e->mu);
+    for (Segment& s : e->segs) s.prefetch_off = kNoOffset;
+}
+
 bool image_in(fma_engine_t* e, ImageIn where) {
     std::lock_guard<std::mutex> lk(e->mu);
     for (const Segment& s : e->segs) {
@@ -923,6 +932,7 @@ int fma_engine_destroy(fma_engine_t* e) {
     host_store_free(e->host);
     park_release(e);
     resident_release(e);
+    prefetch_release(e);
     paths_release(e);
     release_ring(e);
     for (int i = 0; i < kMaxRing; ++i) {
@@ -1649,6 +1659,7 @@ int fma_stats(fma_engine_t* e, fma_stats_t* out) {
     out->image_store_bytes = e->image_store_bytes;
     out->resident_bytes = e->res.va ? e->res_store_bytes : 0;
     out->io_buffer_bytes = e->load_ring_bytes;
+    out->prefetched_bytes = e->pf_store_bytes.load();
     return FMA_OK;
 }
 

@@ -263,11 +263,13 @@ struct Verifier {
 
     // The pages of the segments `pos` (positions in `segs`) in a store with the page table (off, bytes), off == nullptr: pages stored
     // verbatim at their image offsets.  PagePlan::need carries the page's segment position (nothing waits for a mapper here).
-    int plan(const std::vector<size_t>& pos, const std::vector<uint64_t>* off, const std::vector<uint32_t>* bytes, std::vector<PagePlan>* pages) {
+    // prefetched: the segments' copies in the prefetch buffer (offsets prefetch_off), not the store's.
+    int plan(const std::vector<size_t>& pos, const std::vector<uint64_t>* off, const std::vector<uint32_t>* bytes, std::vector<PagePlan>* pages,
+             bool prefetched = false) {
         std::vector<fma_layout::SegPages> v;
         for (size_t k : pos) {
             const Segment& s = e->segs[segs[k].index];
-            v.push_back(fma_layout::SegPages{s.va, s.bytes, s.packed_off, k});
+            v.push_back(fma_layout::SegPages{s.va, s.bytes, prefetched ? s.prefetch_off : s.packed_off, k});
         }
         uint64_t bad = 0;
         if (!fma_layout::plan_pages(v, off, bytes, pages, &bad))
@@ -365,11 +367,12 @@ struct Verifier {
         return FMA_OK;
     }
 
-    int run(const std::vector<size_t>& main, const std::vector<size_t>& res) {
-        std::vector<PagePlan> mp, rp;
+    int run(const std::vector<size_t>& main, const std::vector<size_t>& res, const std::vector<size_t>& pf) {
+        std::vector<PagePlan> mp, rp, fp;
         RC(plan(main, e->image_packed ? &e->img_off : nullptr, &e->img_bytes, &mp));
         RC(plan(res, e->res_packed ? &e->res_off : nullptr, &e->res_bytes, &rp));
-        const size_t n = mp.size() + rp.size();
+        RC(plan(pf, e->image_packed ? &e->pf_off : nullptr, &e->pf_bytes, &fp, true));
+        const size_t n = mp.size() + rp.size() + fp.size();
         RC(ensure_streams(e));
         RC(ensure_desc(e, n));
         seg_of.assign(n, 0);
@@ -377,7 +380,7 @@ struct Verifier {
         e->tl_dev_base = now_s() - e->tl_entry;
         RT(cudaMemsetAsync(e->d_dig, 0, n * sizeof(uint64_t), e->ks));
         const auto coded = [](const PagePlan& q) { return q.bytes != FMA_PAGE_BYTES; };
-        if (std::any_of(mp.begin(), mp.end(), coded) || std::any_of(rp.begin(), rp.end(), coded)) {
+        if (std::any_of(mp.begin(), mp.end(), coded) || std::any_of(rp.begin(), rp.end(), coded) || std::any_of(fp.begin(), fp.end(), coded)) {
             RC(ensure_pack_bufs(e, 1));   // (K6 counts malformed pages in K5's error counter)
             RT(cudaMemsetAsync(e->d_psize + e->pdesc_cap, 0, sizeof(uint32_t), e->ks));
         }
@@ -395,6 +398,10 @@ struct Verifier {
         if (!rp.empty()) {
             if (!e->res.va) return fail(FMA_ESTATE, "the resident part of the image is gone");
             RC(in_place(rp, mp.size(), (uint64_t)e->res.va));
+        }
+        if (!fp.empty()) {   // the prefetched copy, checked in HBM beside the store it came from
+            if (!e->pf.va) return fail(FMA_ESTATE, "the prefetched part of the image is gone");
+            RC(in_place(fp, mp.size() + rp.size(), (uint64_t)e->pf.va));
         }
         RT(cudaMemcpyAsync(e->h_dig, e->d_dig, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, e->ks));
         RT(cudaStreamSynchronize(e->ks));
@@ -420,6 +427,106 @@ struct Verifier {
         cudaGetLastError();
     }
 };
+
+// ---- prefetching part of a sleeping image into its GPU's HBM (fma_image_prefetch) ----
+// The segments a budget takes, in image order, and the copies that bring them: store range r (file_off = its offset in the store)
+// lands at at[r] in the buffer.  The buffer holds the segments back to back, so store-adjacent segments make one range.
+struct PrefetchPlan {
+    std::vector<size_t> segs;           // engine indices
+    std::vector<uint64_t> seg_off;      // their prefetch_off
+    std::vector<uint64_t> off;          // PACKED: stored offset and size of each page of the prefetched part
+    std::vector<uint32_t> bytes;
+    std::vector<FileIO::Item> ranges;
+    std::vector<uint64_t> at;
+    uint64_t stored = 0;
+};
+
+int plan_prefetch(fma_engine_t* e, uint64_t budget, PrefetchPlan* p) {
+    std::vector<size_t> order;   // the sleeping segments, image order
+    {
+        std::lock_guard<std::mutex> lk(e->mu);
+        for (size_t i = 0; i < e->segs.size(); ++i)
+            if (e->segs[i].has_backup && !e->segs[i].mapped) order.push_back(i);
+    }
+    std::sort(order.begin(), order.end(), [&](size_t a, size_t b) { return e->segs[a].packed_off < e->segs[b].packed_off; });
+    std::vector<uint64_t> stored(order.size(), 0);
+    for (size_t k = 0; k < order.size(); ++k) {
+        const Segment& s = e->segs[order[k]];
+        if (!e->image_packed) {
+            stored[k] = s.bytes;
+            continue;
+        }
+        const uint64_t p0 = s.packed_off / FMA_PAGE_BYTES, np = s.bytes / FMA_PAGE_BYTES;
+        if (p0 + np > e->img_bytes.size()) return fail(FMA_ESTATE, "segment %zu lies outside the packed image's page table", order[k]);
+        for (uint64_t q = p0; q < p0 + np; ++q) stored[k] += e->img_bytes[q];
+    }
+    const std::vector<char> keep = fma_layout::resident_split(stored, budget);
+    uint64_t image_off = 0;
+    for (size_t k = 0; k < order.size(); ++k) {
+        if (!keep[k]) continue;
+        const Segment& s = e->segs[order[k]];
+        const uint64_t p0 = s.packed_off / FMA_PAGE_BYTES;
+        const uint64_t from = e->image_packed ? e->img_off[p0] : s.packed_off;
+        p->segs.push_back(order[k]);
+        p->seg_off.push_back(image_off);
+        image_off += s.bytes;
+        if (e->image_packed)
+            for (uint64_t q = p0; q < p0 + s.bytes / FMA_PAGE_BYTES; ++q) {
+                p->off.push_back(p->stored + (e->img_off[q] - from));
+                p->bytes.push_back(e->img_bytes[q]);
+            }
+        if (!p->ranges.empty() && p->ranges.back().file_off + p->ranges.back().bytes == from) {
+            p->ranges.back().bytes += stored[k];
+        } else {
+            p->ranges.push_back(FileIO::Item{from, stored[k]});
+            p->at.push_back(p->stored);
+        }
+        p->stored += stored[k];
+    }
+    return FMA_OK;
+}
+
+// The copies into `dst` (the new buffer), timed on the engine's streams only.  Host store: direct_chunk pieces round-robin over the
+// copy streams.  File: reader threads pread the ranges into the pinned I/O windows, one H2D per window.
+int prefetch_copy(fma_engine_t* e, const PrefetchPlan& p, char* dst) {
+    RC(ensure_streams(e));
+    CopyTimer timer{e};
+    uint32_t ops = 0;
+    const double t_copy = now_s();
+    RC(timer.begin());
+    if (e->image_tier == FMA_TIER_FILE) {
+        if (!e->load_ring) RC(ensure_io_windows(e));
+        std::vector<size_t> ends;
+        const std::vector<FileIO::Item> items = FileIO::cut(e, p.ranges, &ends);
+        // the ranges ascend in the file: the last one ends furthest into it
+        const uint64_t need = p.ranges.back().file_off + p.ranges.back().bytes;
+        const double t_io = now_s();
+        FileFd f;
+        bool direct = false;
+        uint64_t file_bytes = 0;
+        RC(open_image_source(e->image_file.c_str(), need, &f.fd, &direct, &file_bytes));
+        FileIO io(e, f.fd, false, direct, items, file_bytes, e->image_file.c_str());
+        for (size_t k = 0, r = 0; k < items.size(); ++k, ++ops) {
+            while (k >= ends[r]) ++r;
+            RC(io.copy(k, dst + p.at[r] + (items[k].file_off - p.ranges[r].file_off), e->cs[k % e->n_cs]));
+        }
+        RC(io.finish());   // every read has returned and every H2D out of a window has finished
+        e->tl_add("file_io", direct ? 1 : 0, t_io, now_s(), p.stored);
+    } else {
+        const char* host = static_cast<const char*>(e->host.base);
+        if (!host) return fail(FMA_ESTATE, "the host store that holds the image is gone");
+        const size_t chunk = direct_chunk(e);
+        for (size_t r = 0; r < p.ranges.size(); ++r)
+            for (uint64_t o = 0; o < p.ranges[r].bytes; o += chunk, ++ops) {
+                const size_t n = (size_t)std::min<uint64_t>(chunk, p.ranges[r].bytes - o);
+                RT(cudaMemcpyAsync(dst + p.at[r] + o, host + p.ranges[r].file_off + o, n, cudaMemcpyDefault, e->cs[ops % e->n_cs]));
+            }
+    }
+    double copy_s = 0;
+    RC(timer.end(&copy_s));   // joins the copy streams only
+    e->tl_add("copies_landed", (int)ops, t_copy, now_s(), p.stored);
+    return FMA_OK;
+}
 
 }  // namespace
 }  // namespace fma_impl
@@ -676,6 +783,7 @@ int fma_image_move(fma_engine_t* e, int tier) {
     }
     e->image_tier = tier;
     if (tier == FMA_TIER_FILE) e->image_file = e->file_path;
+    if (fma_layout::is_park_tier(tier)) prefetch_release(e);   // the whole image is in HBM now; host <-> file keeps the copy
     // INCREMENTAL: the copy a clean sleep may keep lay in the store the image left; the next wake records the new one
     invalidate_shadows(e);
     e->st.tier = tier;
@@ -689,7 +797,7 @@ int fma_image_verify(fma_engine_t* e, int* out_bad, int cap) {
     std::lock_guard<std::mutex> op(e->op_mu);
     if (cap < 0 || (cap > 0 && !out_bad)) return fail(FMA_EINVAL, "out_bad is NULL or cap is negative");
     Verifier v(e);
-    std::vector<size_t> main, res;   // positions in v.segs: the image's own store, the resident share
+    std::vector<size_t> main, res, pf;   // positions in v.segs: the image's own store, the resident share, the prefetched copy
     {
         std::lock_guard<std::mutex> lk(e->mu);
         for (size_t i = 0; i < e->segs.size(); ++i) {
@@ -701,6 +809,10 @@ int fma_image_verify(fma_engine_t* e, int* out_bad, int cap) {
             const bool resident = s.backup_tier == FMA_TIER_LOCAL && e->image_tier == FMA_TIER_HOST;
             (resident ? res : main).push_back(v.segs.size());
             v.segs.push_back(Verifier::Seg{i, (uint64_t)s.va, s.digest});
+            if (s.prefetch_off != kNoOffset) {   // checked a second time, where the wake will read it
+                pf.push_back(v.segs.size());
+                v.segs.push_back(Verifier::Seg{i, (uint64_t)s.va, s.digest});
+            }
         }
     }
     if (v.segs.empty()) return fail(FMA_ESTATE, "nothing is asleep");
@@ -708,18 +820,64 @@ int fma_image_verify(fma_engine_t* e, int* out_bad, int cap) {
     RC(flush_kernel_times(e));   // (the last operation's kernel rows and times, before the timeline turns to this call)
     const double t_entry = now_s();
     e->tl_begin("verify", t_entry);
-    const int rc = v.run(main, res);
+    const int rc = v.run(main, res, pf);
     if (e->ks) cudaStreamSynchronize(e->ks);   // nothing still reads a store or the descriptors, also after a failure
     if (rc != FMA_OK) return rc;
     int n_bad = 0;
-    for (size_t k = 0; k < v.segs.size(); ++k)
-        if (v.sum[k] != v.segs[k].digest) {
+    for (size_t k = 0; k < v.segs.size(); ++k)   // a segment checked in two places and bad in both counts once
+        if (v.sum[k] != v.segs[k].digest && (k == 0 || v.segs[k - 1].index != v.segs[k].index || v.sum[k - 1] == v.segs[k - 1].digest)) {
             if (n_bad < cap) out_bad[n_bad] = (int)v.segs[k].index;
             ++n_bad;
         }
-    e->tl_add("total", n_bad, t_entry, now_s(), e->image_store_bytes + e->res_store_bytes);
+    e->tl_add("total", n_bad, t_entry, now_s(), e->image_store_bytes + e->res_store_bytes + e->pf_store_bytes.load());
     return n_bad;
 }
 
+// ---- prefetching part of a sleeping image into HBM ahead of a wake (see include/fma_engine.h) ------------------------------
+int fma_image_prefetch(fma_engine_t* e, uint64_t bytes) {
+    if (check_engine(e) != FMA_OK) return FMA_EINVAL;
+    std::lock_guard<std::mutex> op(e->op_mu);
+    DeviceGuard guard(e->device);
+    if (!bytes) {   // the hand-back: nothing on the device reads the buffer between operations
+        prefetch_release(e);
+        return FMA_OK;
+    }
+    fma_layout::PrefetchFacts facts{e->image_tier, false, false, e->res.va != 0};
+    {
+        std::lock_guard<std::mutex> lk(e->mu);
+        for (const Segment& s : e->segs)
+            if (s.has_backup) (s.mapped ? facts.backup_mapped : facts.asleep) = true;
+    }
+    const fma_layout::PrefetchRoute route = fma_layout::prefetch_route(facts);
+    if (route.error != FMA_OK) return fail(route.error, "image prefetch: %s", route.why);
+    RC(flush_kernel_times(e));   // (the last operation's kernel rows and times, before the timeline turns to this call)
+    const double t_entry = now_s();
+    e->tl_begin("prefetch", t_entry);
+    prefetch_release(e);   // a new prefetch replaces the old one, whose HBM goes first
+    PrefetchPlan p;
+    RC(plan_prefetch(e, bytes & ~(uint64_t)(FMA_PAGE_BYTES - 1), &p));
+    if (p.stored) {
+        ParkStore buf;
+        RC(park_store_create(e, e->device, p.stored, &buf));
+        const int rc = prefetch_copy(e, p, reinterpret_cast<char*>(buf.va));
+        if (rc != FMA_OK) {   // nothing may still copy into the buffer when it goes
+            for (int i = 0; i < e->n_cs; ++i) cudaStreamSynchronize(e->cs[i]);
+            if (e->ks) cudaStreamSynchronize(e->ks);
+            cudaGetLastError();
+            vmm_buffer_free(buf);
+            return rc;
+        }
+        {
+            std::lock_guard<std::mutex> lk(e->mu);
+            for (size_t k = 0; k < p.segs.size(); ++k) e->segs[p.segs[k]].prefetch_off = p.seg_off[k];
+        }
+        e->pf = buf;
+        e->pf_off = std::move(p.off);
+        e->pf_bytes = std::move(p.bytes);
+        e->pf_store_bytes = p.stored;
+    }
+    e->tl_add("total", (int)p.segs.size(), t_entry, now_s(), p.stored);
+    return FMA_OK;
+}
 
 }  // extern "C"

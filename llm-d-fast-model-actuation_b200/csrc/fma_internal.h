@@ -4,7 +4,8 @@
 //   fma_sleep.cu    SLEEP pipeline (do_sleep) and the PACKED image plan
 //   fma_wake.cu     WAKE pipeline (do_wake)
 //   fma_load.cu     file I/O: reader / writer threads over the pinned I/O windows (cold load fma_load_file, FILE tier)
-//   fma_image.cu    image hand-over between engines / processes (fma_image_export / fma_image_adopt), moves between tiers (fma_image_move)
+//   fma_image.cu    image hand-over between engines / processes (fma_image_export / fma_image_adopt), moves between tiers (fma_image_move),
+//                  checks in place (fma_image_verify), prefetch into HBM (fma_image_prefetch)
 //
 // Everything below lives in namespace fma_impl; the library is built with -fvisibility=hidden, so none of it is exported.
 #pragma once
@@ -128,6 +129,9 @@ struct Segment {
     // INCREMENTAL sleep: after a host-tier wake the store still holds this segment's bytes at shadow_off, and `digest` is
     // their K3 digest; kNoOffset = no such copy (never slept, image overwritten or released, layout changed)
     uint64_t shadow_off = kNoOffset;
+    // PREFETCH (fma_image_prefetch): a copy of its stored bytes is in the prefetch buffer, at this offset of the prefetch part's
+    // image space; backup_tier and packed_off still name the tier's store, which keeps every byte
+    uint64_t prefetch_off = kNoOffset;
 };
 
 using fma_layout::Arena;
@@ -252,6 +256,13 @@ struct fma_engine {
     uint64_t res_store_bytes = 0;     // bytes the resident part occupies in `res`
     cudaEvent_t ev_res_done = nullptr;  // wake: the resident part's last restore launch has completed
     std::vector<uint64_t> res_seqs;   // Segment::seq of the segments the last sleep kept resident (INCREMENTAL: same split or full sleep)
+    // PREFETCH (fma_image_prefetch): a copy of part of a sleeping host- or file-tier image in ONE VMM allocation on this GPU (`pf`),
+    // the prefetched segments back to back in image order and laid out like the resident part (pf_off / pf_bytes: each page's
+    // stored offset and size when the image is PACKED).  The tier's store stays complete, so dropping it copies nothing.
+    ParkStore pf;
+    std::vector<uint64_t> pf_off;
+    std::vector<uint32_t> pf_bytes;
+    std::atomic<uint64_t> pf_store_bytes{0};   // bytes the prefetched part occupies in `pf` (fma_stats reads it without op_mu)
     uint64_t image_bytes = 0;  // W of the current packed image
     int image_tier = FMA_TIER_HOST;
     // PACKED host image (option "pack", fma_codec.h): image page p (= packed_off / 2 MiB) is stored at
@@ -332,7 +343,7 @@ struct fma_engine {
     std::vector<TimelineEv> tl;
     std::vector<uint64_t> tl_kbytes;   // algorithmic bytes of each pending kernel launch (pairs in ev_pool)
     std::vector<const char*> tl_kkind; // timeline kind of each pending kernel launch ("kernel", "res_gather", "res_restore")
-    char tl_op[8] = "";
+    char tl_op[16] = "";
     double tl_entry = 0;               // now_s() at the operation's entry
     double tl_dev_base = 0;            // host time (since entry) at which ev_start was recorded: origin of the device-side events
     void tl_begin(const char* op, double t_entry) {
@@ -402,6 +413,7 @@ int park_release(fma_engine_t* e);
 int park_reserve(fma_engine_t* e, int park_device, size_t bytes);
 int park_store_create(fma_engine_t* e, int device, size_t bytes, ParkStore* out);   // one VMM allocation, mapped for e's GPU (+ device's)
 void resident_release(fma_engine_t* e);              // drop the resident buffer (caller: nothing on the device still reads it)
+void prefetch_release(fma_engine_t* e);              // drop the prefetch buffer and its table (same condition; takes e->mu)
 // Does a segment's image live in the store `where` names (takes e->mu)?
 enum class ImageIn {
     Host,           // the host store
@@ -412,6 +424,23 @@ enum class ImageIn {
 bool image_in(fma_engine_t* e, ImageIn where);
 // a sleeping image keeps part of itself in the resident buffer
 inline bool resident_asleep(fma_engine_t* e) { return e->res.va && image_in(e, ImageIn::Local); }
+// A wake restores a segment from HBM instead of its tier's store when its bytes are in the resident share or in the prefetch
+// buffer (an image has one or the other, never both).  Its offset in that part's image space, or kNoOffset.
+inline uint64_t hbm_offset(const fma_engine_t* e, const Segment& s) {
+    if (!s.has_backup) return kNoOffset;
+    if (s.backup_tier == FMA_TIER_LOCAL && e->image_tier == FMA_TIER_HOST) return s.packed_off;   // the resident share
+    return s.prefetch_off;
+}
+struct HbmPart {   // that part: its buffer, its form and (PACKED) its page table
+    uint64_t base;
+    bool packed;
+    const std::vector<uint64_t>* off;
+    const std::vector<uint32_t>* bytes;
+};
+inline HbmPart hbm_part(const fma_engine_t* e) {
+    if (e->pf.va) return HbmPart{(uint64_t)e->pf.va, e->image_packed, &e->pf_off, &e->pf_bytes};
+    return HbmPart{(uint64_t)e->res.va, e->res_packed, &e->res_off, &e->res_bytes};
+}
 CUmemAllocationProp device_prop(int device);
 // ---- image descriptor (fma_image.cu): what a sleeping image is made of, so another engine / process can adopt it ----
 int image_descriptor_build(fma_engine_t* e, int tier, std::vector<char>* out);

@@ -364,4 +364,26 @@ inline MoveRoute move_route(int from, int to, const MoveFacts& f) {
     return MoveRoute{to == FMA_TIER_HOST ? MovePipeKind::ParkHost : MovePipeKind::ParkFile, FMA_OK, ""};
 }
 
+// ---- whether part of a sleeping image may be prefetched into its GPU's HBM (fma_image_prefetch with a budget) ----
+// The segments it copies are the resident share's choice over stored sizes (resident_split); what is decided here is the refusal.
+struct PrefetchFacts {
+    int tier;             // the image's tier
+    bool asleep;          // a segment with a backup is unmapped
+    bool backup_mapped;   // a segment with a backup is mapped (a KEEP_BACKUP wake, a partly woken image)
+    bool resident;        // the image keeps a resident share from its sleep
+};
+struct PrefetchRoute {
+    int error;            // FMA_OK, or the code of the refusal
+    const char* why;
+};
+
+inline PrefetchRoute prefetch_route(const PrefetchFacts& f) {
+    if (f.backup_mapped) return PrefetchRoute{FMA_ESTATE, "a segment with a backup is mapped (a KEEP_BACKUP or partial wake): wake or sleep it fully first"};
+    if (!f.asleep) return PrefetchRoute{FMA_ESTATE, "no image is asleep"};
+    if (f.resident)
+        return PrefetchRoute{FMA_ESTATE, "part of the image sleeps in a resident share (option resident_bytes): set it to 0 and sleep again to prefetch instead"};
+    if (f.tier != FMA_TIER_HOST && f.tier != FMA_TIER_FILE) return PrefetchRoute{FMA_EINVAL, "the image sleeps in a parking buffer: it is in HBM already"};
+    return PrefetchRoute{FMA_OK, ""};
+}
+
 }  // namespace fma_layout

@@ -913,6 +913,10 @@ int do_sleep(fma_engine_t* e, uint64_t offload_mask, int tier, uint32_t flags) {
         GateHold hold(kGateUnmap, 0.1);
         resident_release(e);
     }
+    if (e->pf.va) {  // a prefetch left behind by segments freed while asleep: this sleep writes a new image
+        RT(cudaDeviceSynchronize());
+        prefetch_release(e);
+    }
 
     SleepPlan p(e, tier, flags);
     plan_image(e, offload_mask, p);

@@ -171,9 +171,10 @@ struct Mapper {
     }
 };
 
-// RESIDENT share: K2 / K5 copy the resident segments from e->res into their pages, on the kernel stream in pieces of at most one
-// ring slot, each launched between two of the host part's launches once its destination is mapped (in the second half of the
-// host part's launches the pipeline waits for that mapping); the tables sit behind the host part's in the same buffers.
+// RESIDENT share or PREFETCH (hbm_part): K2 / K5 copy the segments whose bytes are in HBM into their pages, on the kernel stream in
+// pieces of at most one ring slot, each launched between two of the host part's launches once its destination is mapped (in the
+// second half of the host part's launches the pipeline waits for that mapping); the tables sit behind the host part's in the same
+// buffers.  With no host part the pieces go one after the other as their runs are mapped.
 struct ResidentRestore {
     fma_engine_t* e;
     Mapper& mapper;
@@ -183,9 +184,10 @@ struct ResidentRestore {
     uint64_t W_res;
     size_t n_host_pages;
     bool image_packed;             // the host part's pipeline clears the K5 error counter
+    HbmPart part = hbm_part(e);
     std::vector<Batch> pieces{};
     size_t next = 0;
-    PageKernels kernels() { return PageKernels{e, kt, false, e->res_packed, n_host_pages}; }
+    PageKernels kernels() { return PageKernels{e, kt, false, part.packed, n_host_pages}; }
     int setup();
     int launch_next();
     // after (host part's pages launched so far, host part's pages): launch the next piece if due
@@ -226,10 +228,12 @@ struct WakePipe {
     int multipath();
 };
 
-// The segments `idx` as the page planner sees them: each waits for the mapper work item of its run.
-std::vector<fma_layout::SegPages> wake_segs(const fma_engine_t* e, const std::vector<size_t>& idx, const std::vector<size_t>& seg_run) {
+// The segments `idx` as the page planner sees them: each waits for the mapper work item of its run.  hbm: placed by their offsets
+// in the HBM part (hbm_offset) rather than in the tier's store.
+std::vector<fma_layout::SegPages> wake_segs(const fma_engine_t* e, const std::vector<size_t>& idx, const std::vector<size_t>& seg_run, bool hbm = false) {
     std::vector<fma_layout::SegPages> v;
-    for (size_t i : idx) v.push_back(fma_layout::SegPages{(uint64_t)e->segs[i].va, e->segs[i].bytes, e->segs[i].packed_off, seg_run[i] + 1});
+    for (size_t i : idx)
+        v.push_back(fma_layout::SegPages{(uint64_t)e->segs[i].va, e->segs[i].bytes, hbm ? hbm_offset(e, e->segs[i]) : e->segs[i].packed_off, seg_run[i] + 1});
     return v;
 }
 
@@ -241,14 +245,14 @@ int WakePipe::plan(bool packed, std::vector<PagePlan>* pages) {
 }
 
 int ResidentRestore::setup() {
-    if (!e->res.va) return fail(FMA_ESTATE, "the resident part of the image is gone");
+    if (!part.base) return fail(FMA_ESTATE, "the part of the image kept in HBM is gone");
     if (!e->ev_res_done && cudaEventCreateWithFlags(&e->ev_res_done, cudaEventDisableTiming) != cudaSuccess)
         return fail(FMA_ECUDA, "cudaEventCreate(resident) failed");
     std::vector<PagePlan> pages;
     uint64_t bad = 0;
-    if (!fma_layout::plan_pages(wake_segs(e, with_res, seg_run), e->res_packed ? &e->res_off : nullptr, &e->res_bytes, &pages, &bad))
-        return fail(FMA_ESTATE, "segment outside the resident part's page table");
-    RC(kernels().prepare(pages, !image_packed, [&](size_t q) { return (uint64_t)e->res.va + pages[q].off; }));   // (else the host part's pipeline clears the counter)
+    if (!fma_layout::plan_pages(wake_segs(e, with_res, seg_run, true), part.packed ? part.off : nullptr, part.bytes, &pages, &bad))
+        return fail(FMA_ESTATE, "segment outside the page table of the part kept in HBM");
+    RC(kernels().prepare(pages, !image_packed, [&](size_t q) { return part.base + pages[q].off; }));   // (else the host part's pipeline clears the counter)
     fma_layout::plan_batches(pages, slot_pages(e), UINT64_MAX, false, &pieces);
     return FMA_OK;
 }
@@ -256,7 +260,7 @@ int ResidentRestore::setup() {
 int ResidentRestore::launch_next() {
     const Batch& pc = pieces[next];
     RC(mapper.wait(pc.need));
-    kt.kind = "res_restore";
+    kt.kind = e->pf.va ? "pf_restore" : "res_restore";
     const int r = kernels().launch(pc);
     kt.kind = "kernel";
     if (r != FMA_OK) return r;
@@ -578,8 +582,9 @@ int plan_wake_runs(fma_engine_t* e, uint64_t tag_mask, double t_entry, std::vect
     std::vector<fma_layout::SegView> view;
     for (size_t i : cand) {
         const Segment& s = e->segs[i];
-        // a RESIDENT share's segments (their offsets are in the resident part) are mapped after the host part's
-        const uint64_t key = is_resident(e, s) ? (1ull << 62) + s.packed_off : s.packed_off;
+        // the segments restored from HBM (their offsets are in the resident or prefetched part) are mapped after the host part's
+        const uint64_t h = hbm_offset(e, s);
+        const uint64_t key = h != kNoOffset ? (1ull << 62) + h : s.packed_off;
         view.push_back(fma_layout::SegView{i, s.arena, (uint64_t)s.va, s.bytes, s.has_backup, key});
     }
     // FMA_MAP_PIECE_MIB (default 2048; 0 = whole runs): backed-up runs are mapped in pieces of about that size, cut at segment
@@ -647,6 +652,7 @@ void drop_backups(fma_engine_t* e, const std::vector<size_t>& with_backup, uint6
         s.shadow_off = kept ? s.packed_off : kNoOffset;   // host store or parking buffer: both outlive the wake
         s.has_backup = false;
         s.packed_off = kNoOffset;
+        s.prefetch_off = kNoOffset;
     }
     if (W) {
         e->shadow_tier = tier;
@@ -671,9 +677,9 @@ int do_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags) {
     if (runs.empty()) return FMA_OK;
     const int tier = e->image_tier;
 
-    std::vector<size_t> with_backup, with_host, with_res;  // segment indices, image order; with_backup by store: host part, RESIDENT share
+    std::vector<size_t> with_backup, with_host, with_res;  // segment indices, image order; with_backup by store: host part, HBM part
     std::vector<size_t> seg_run(e->segs.size(), 0);       // segment -> index of its run in `runs`
-    uint64_t W = 0, W_res = 0, remapped_only = 0;         // W: what crosses the link (a resident share's segments do not)
+    uint64_t W = 0, W_res = 0, remapped_only = 0;         // W: what crosses the link (the resident or prefetched segments do not)
     for (size_t r = 0; r < runs.size(); ++r) {
         for (size_t i : runs[r].segs) {
             seg_run[i] = r;
@@ -682,7 +688,7 @@ int do_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags) {
                 continue;
             }
             with_backup.push_back(i);
-            const bool res = is_resident(e, e->segs[i]);
+            const bool res = hbm_offset(e, e->segs[i]) != kNoOffset;
             (res ? with_res : with_host).push_back(i);
             (res ? W_res : W) += e->segs[i].bytes;
         }
@@ -705,8 +711,10 @@ int do_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags) {
     KernelTimes kt{e};
     uint32_t copy_ops = 0;
     double copy_s = 0, first_copy_delay = 0;
-    ResidentRestore res{e, mapper, kt, with_res, seg_run, W_res, W / FMA_PAGE_BYTES, facts.image_packed};
-    const bool res_packed = W_res && e->res_packed;   // (the buffer may be released before the K5 error count is read)
+    // (a prefetched part with no host part beside it clears the K5 error counter itself)
+    ResidentRestore res{e, mapper, kt, with_res, seg_run, W_res, W / FMA_PAGE_BYTES, facts.image_packed && (W || !e->pf.va)};
+    const bool res_packed = W_res && res.part.packed;   // (the buffer may be released before the K5 error count is read)
+    const uint64_t W_store = W + (e->pf.va ? W_res : 0);  // of these bytes the tier's store holds a copy (a prefetch is one of it)
     if (W || W_res) {
         const char* store = static_cast<const char*>(store_copy_base(e, tier));
         if (W && !store && tier != FMA_TIER_FILE) return fail(FMA_ESTATE, "backup store of tier %d is gone", tier);
@@ -746,21 +754,25 @@ int do_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags) {
     }
     mapper.join();
     mapper.retract_gate();
-    // RESIDENT share: the buffer goes once its restore has completed and every run is mapped (a wake that fails before that is
-    // rolled back and its retry needs the buffer), under the host part's copy; it stays while a resident segment still sleeps
-    // (tag-selective wake) and with FMA_FLAG_KEEP_BACKUP.
-    if (e->res.va && !(flags & FMA_FLAG_KEEP_BACKUP)) {
+    // RESIDENT share / PREFETCH: the buffer goes once its restore has completed and every run is mapped (a wake that fails before
+    // that is rolled back and its retry needs the buffer), under the host part's copy; it stays while a segment it holds still
+    // sleeps (tag-selective wake).  With FMA_FLAG_KEEP_BACKUP a resident share stays (it is the backup), a prefetch goes (the
+    // store is).
+    const bool from_pf = e->pf.va != 0;
+    const ParkStore& hbm = from_pf ? e->pf : e->res;
+    if (hbm.va && (from_pf || !(flags & FMA_FLAG_KEEP_BACKUP))) {
         bool still_asleep = false;
-        for (const Segment& s : e->segs) still_asleep = still_asleep || (is_resident(e, s) && !s.mapped);
+        if (!(flags & FMA_FLAG_KEEP_BACKUP))
+            for (const Segment& s : e->segs) still_asleep = still_asleep || (hbm_offset(e, s) != kNoOffset && !s.mapped);
         if (!still_asleep) {
             if (res.next) RT(cudaEventSynchronize(e->ev_res_done));
             const double a = now_s();
-            const uint64_t cap = e->res.bytes;
+            const uint64_t cap = hbm.bytes;
             {
                 GateHold hold(kGateUnmap, 0.1);
-                resident_release(e);
+                from_pf ? prefetch_release(e) : resident_release(e);
             }
-            e->tl_add("res_free", 0, a, now_s(), cap);
+            e->tl_add(from_pf ? "pf_free" : "res_free", 0, a, now_s(), cap);
         }
     }
     const double t_joined = now_s();
@@ -780,7 +792,7 @@ int do_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags) {
 
     int verify_rc = FMA_OK;
     if ((flags & FMA_FLAG_VERIFY) && (W || W_res)) RC(verify_wake(e, with_backup, &verify_rc));
-    if (!(flags & FMA_FLAG_KEEP_BACKUP)) drop_backups(e, with_backup, W, tier, verify_rc == FMA_OK);
+    if (!(flags & FMA_FLAG_KEEP_BACKUP)) drop_backups(e, with_backup, W_store, tier, verify_rc == FMA_OK);
 
     e->tl_add("total", 0, t_entry, now_s(), W + W_res);
     e->st.wake_seconds = now_s() - t_entry;

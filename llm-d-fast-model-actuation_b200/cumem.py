@@ -243,6 +243,18 @@ class CuMemAllocator:
             logger.warning("fma_b200: sleeping image fails verification in %d segment(s): %s", len(bad), bad[:8])
         return not bad
 
+    def prefetch_image(self, mib: int) -> int:
+        """Copy up to ``mib`` MiB of this rank's sleeping image (its tail, in stored bytes) from host DRAM or disk into its own GPU's
+        HBM ahead of a wake, so that the wake moves that much less over the link; 0 gives the HBM back.  A no-op while awake.
+        Returns the bytes prefetched."""
+        if not self.engine.is_sleeping():
+            return 0
+        self._join_reserve()
+        self.engine.prefetch_image(int(mib) << 20)
+        n = self.engine.stats()["prefetched_bytes"]
+        logger.info("fma_b200: %.2f GiB of the sleeping image prefetched into HBM", n / 1024**3)
+        return n
+
     # ---- pool --------------------------------------------------------------------------
     @contextmanager
     def use_memory_pool(self, tag: str | None = None):

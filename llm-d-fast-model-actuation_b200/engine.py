@@ -358,6 +358,14 @@ class Engine:
         k = check(self._lib.fma_image_verify(self._h, bad, n))
         return sorted(bad[i] for i in range(min(k, n)))
 
+    def prefetch_image(self, nbytes: int) -> None:
+        """Copy the tail of the sleeping image, up to ``nbytes`` of stored bytes (rounded down to 2 MiB), into this GPU's HBM ahead
+        of a wake, without waking it (fma_image_prefetch); 0 gives that HBM back.  The next ``wake`` restores those segments from
+        HBM and moves only the others over PCIe or from disk.  ``stats()["prefetched_bytes"]`` is what the copy holds.  Raises
+        FmaError when nothing is asleep, a mapped segment keeps a backup, the image has a resident share (FMA_ESTATE) or sleeps in
+        a parking buffer (FMA_EINVAL), or when HBM (FMA_ENOMEM) or the image file (FMA_EIO) fails it."""
+        check(self._lib.fma_image_prefetch(self._h, nbytes))
+
     # -- cold load -------------------------------------------------------------------------
     def load_file(self, path: str, spans: Sequence[tuple[int, int, int]], o_direct: bool = False) -> dict:
         """Stream (file_offset, nbytes, device_address) spans of one file into mapped segments."""
