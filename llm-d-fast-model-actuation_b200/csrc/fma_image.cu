@@ -6,17 +6,35 @@ using namespace fma_impl;
 
 namespace fma_impl {
 
+namespace {
+
+// The sleeping segments (they keep a backup and are unmapped) that `pick` takes, by engine index in image order (takes e->mu)
+template <class Pick>
+std::vector<size_t> sleeping_segments(fma_engine_t* e, Pick pick) {
+    std::vector<size_t> v;
+    std::lock_guard<std::mutex> lk(e->mu);
+    for (size_t i = 0; i < e->segs.size(); ++i)
+        if (e->segs[i].has_backup && !e->segs[i].mapped && pick(e->segs[i])) v.push_back(i);
+    std::sort(v.begin(), v.end(), [&](size_t a, size_t b) { return e->segs[a].packed_off < e->segs[b].packed_off; });
+    return v;
+}
+
+// Is a segment's image asleep (kept and unmapped), and is one mapped again while it keeps its backup (takes e->mu)?
+void sleep_state(fma_engine_t* e, bool* asleep, bool* backup_mapped) {
+    std::lock_guard<std::mutex> lk(e->mu);
+    for (const Segment& s : e->segs)
+        if (s.has_backup) *(s.mapped ? backup_mapped : asleep) = true;
+}
+
+}  // namespace
+
 // Descriptor of the image sleeping in `tier`'s store: header, one ImageSegDesc per offloaded segment in image order and, for a
 // PACKED image (version 2), the per-page stored sizes (offsets are their prefix sums).  At most kImageTail bytes.
 int image_descriptor_build(fma_engine_t* e, int tier, std::vector<char>* out) {
-    std::vector<const Segment*> segs;
-    {
-        std::lock_guard<std::mutex> lk(e->mu);
-        for (const Segment& s : e->segs)
-            if (s.has_backup && (tier == FMA_TIER_HOST ? s.backup_tier == FMA_TIER_HOST : s.backup_tier != FMA_TIER_HOST) && !s.mapped) segs.push_back(&s);
-    }
+    const std::vector<size_t> segs = sleeping_segments(e, [&](const Segment& s) {
+        return tier == FMA_TIER_HOST ? s.backup_tier == FMA_TIER_HOST : s.backup_tier != FMA_TIER_HOST;
+    });
     if (segs.empty()) return fail(FMA_ESTATE, "nothing is asleep in that store");
-    std::sort(segs.begin(), segs.end(), [](const Segment* a, const Segment* b) { return a->packed_off < b->packed_off; });
     const size_t n_img_pages = e->image_packed ? e->img_bytes.size() : 0;
     const size_t total = sizeof(ImageHeader) + segs.size() * sizeof(ImageSegDesc) + sizeof(uint32_t) * (1 + n_img_pages);
     if (total > kImageTail) return fail(FMA_ENOMEM, "too many segments / pages for the descriptor");
@@ -25,13 +43,14 @@ int image_descriptor_build(fma_engine_t* e, int tier, std::vector<char>* out) {
     ImageHeader hd{kImageMagic, e->image_packed ? 2u : 1u, (uint32_t)segs.size(), e->image_bytes};
     memcpy(tail, &hd, sizeof(hd));
     for (size_t i = 0; i < segs.size(); ++i) {
+        const Segment& s = e->segs[segs[i]];
         ImageSegDesc d;
         memset(&d, 0, sizeof(d));
-        d.bytes = segs[i]->bytes;
-        d.packed_off = segs[i]->packed_off;
-        d.digest = segs[i]->digest;
-        d.digest_valid = segs[i]->digest_valid ? 1 : 0;
-        const std::string& t = e->tags[segs[i]->tag];
+        d.bytes = s.bytes;
+        d.packed_off = s.packed_off;
+        d.digest = s.digest;
+        d.digest_valid = s.digest_valid ? 1 : 0;
+        const std::string& t = e->tags[s.tag];
         d.tag_len = (uint32_t)std::min<size_t>(t.size(), sizeof(d.tag) - 1);
         memcpy(d.tag, t.data(), d.tag_len);
         memcpy(tail + sizeof(hd) + i * sizeof(d), &d, sizeof(d));
@@ -102,7 +121,7 @@ int image_descriptor_parse(fma_engine_t* e, const char* tail, size_t tail_bytes,
     return FMA_OK;
 }
 
-// after do_sleep(kFlagAdopt): take over the exporter's page table and integrity data
+// after do_sleep(kFlagAdopt): take over the exporter's page table and integrity data (caller holds e->mu)
 void image_apply(fma_engine_t* e, ParsedImage& pi) {
     if (pi.hd.version == 2) {  // wake through K5 with the exporter's page table
         e->image_packed = true;
@@ -117,46 +136,167 @@ void image_apply(fma_engine_t* e, ParsedImage& pi) {
     }
 }
 
+// An adoption releases the device side as a sleep would: every segment must be mapped (takes e->mu)
+int adopt_needs_awake(fma_engine_t* e) {
+    std::lock_guard<std::mutex> lk(e->mu);
+    for (const Segment& s : e->segs)
+        if (!s.mapped) return fail(FMA_ESTATE, "adopt needs a fully awake engine");
+    return FMA_OK;
+}
+
+// What every adoption does once its entry point holds the descriptor (`desc`, the image's store: store_cap bytes): parse it against
+// the segments of `tag_mask`; with FMA_FLAG_VERIFY, check that the device holds what the image holds; take_store() sets the store
+// up; then the device side goes exactly as a sleep to `tier` would release it, without copying anything out, and the engine takes
+// over the exporter's page table and digests.
+template <class TakeStore>
+int adopt(fma_engine_t* e, const char* desc, size_t desc_bytes, size_t store_cap, uint64_t tag_mask, uint32_t flags, int tier, TakeStore take_store) {
+    ParsedImage pi;
+    RC(image_descriptor_parse(e, desc, desc_bytes, store_cap, tag_mask, &pi));
+    DeviceGuard guard(e->device);
+    cudaDeviceSynchronize();
+    if (flags & FMA_FLAG_VERIFY) {
+        // "Sleep by adoption": this engine HAS the weights and wants to share somebody else's image of the same model (a second
+        // replica on the node: one host copy for all).  Only legal if its device bytes are what the image holds — K3 digests
+        // against the descriptor's; a mismatch leaves the engine awake and untouched.
+        std::vector<uint64_t> now;
+        RC(digest_segments(e, pi.order, &now));
+        for (size_t i = 0; i < pi.ds.size(); ++i)
+            if (!pi.ds[i].digest_valid || pi.ds[i].digest != now[i])
+                return fail(FMA_EINTEGRITY, pi.ds[i].digest_valid ? "the image holds different bytes than this engine's segments" : "the image carries no digests to compare with");
+    }
+    RC(take_store());
+    RC(do_sleep(e, tag_mask, tier, (flags & ~FMA_FLAG_VERIFY) | kFlagAdopt));
+    std::lock_guard<std::mutex> lk(e->mu);
+    image_apply(e, pi);
+    return FMA_OK;
+}
+
+// An exported image's memfd (a dup of it) and its shared mapping: unmapped and closed on every exit path, unless the host store
+// takes them over
+struct ImageMapping {
+    int fd = -1;
+    void* base = nullptr;
+    size_t bytes = 0;
+    ~ImageMapping() {
+        if (base) munmap(base, bytes);
+        if (fd >= 0) close(fd);
+    }
+};
+
+// The adopted memfd image becomes the host store: pinned in place, or copied once into anonymous pinned memory
+int adopt_host_store(fma_engine_t* e, ImageMapping& m) {
+    const size_t cap = m.bytes - kImageTail;
+    invalidate_shadows(e);
+    host_store_free(e->host);
+    const double t0 = now_s();
+    void* p = m.base;
+    cudaError_t r = cudaHostRegister(p, m.bytes, cudaHostRegisterPortable | cudaHostRegisterMapped);
+    HostStore h;
+    if (r != cudaSuccess) {
+        // The mapping cannot be pinned in place (e.g. an image FILE on a filesystem whose pages the driver will not lock):
+        // copy it once into an anonymous pinned store — a load from the page cache, several threads — and let go of the fd.
+        cudaGetLastError();
+        void* q = nullptr;
+        r = cudaHostAlloc(&q, m.bytes, cudaHostAllocPortable | cudaHostAllocMapped);
+        if (r != cudaSuccess) {
+            cudaGetLastError();
+            return fail(FMA_ENOMEM, "cannot pin the adopted image, in place or as a copy");
+        }
+        const int nt = std::max(1, std::min(env_int("FMA_TOUCH_THREADS", 8), 32));
+        const size_t per = round_up((m.bytes + nt - 1) / nt, FMA_PAGE_BYTES);
+        std::vector<std::thread> th;
+        for (int t = 0; t < nt; ++t) {
+            const size_t lo = (size_t)t * per, hi = std::min(m.bytes, lo + per);
+            if (lo >= hi) break;
+            th.emplace_back([p, q, lo, hi] { memcpy(static_cast<char*>(q) + lo, static_cast<const char*>(p) + lo, hi - lo); });
+        }
+        for (auto& t : th) t.join();
+        h.base = q; h.cap = cap; h.map_bytes = 0; h.fd = -1; h.registered = false;
+        p = q;
+    } else {
+        h.base = p; h.cap = cap; h.map_bytes = m.bytes; h.fd = m.fd; h.registered = true;
+        h.shared = true;  // the exporter (and other adopters) map the same pages
+        m.base = nullptr;   // the store's now
+        m.fd = -1;
+    }
+    void* alias = nullptr;
+    if (cudaHostGetDevicePointer(&alias, p, 0) == cudaSuccess) h.dev_alias = alias;
+    else cudaGetLastError();
+    h.pin_seconds = now_s() - t0;
+    e->host = h;
+    e->st.host_store_bytes = cap;
+    e->st.host_store_pin_seconds = h.pin_seconds;
+    return FMA_OK;
+}
+
+// ---- copies between a store and an HBM buffer, for moves and prefetches ----
+
+// Nothing the engine's streams were given still runs (a failure's clean-up, before what they copy into or out of goes)
+inline void drain(fma_engine_t* e) {
+    for (int i = 0; i < e->n_cs; ++i) cudaStreamSynchronize(e->cs[i]);
+    if (e->ks) cudaStreamSynchronize(e->ks);
+    cudaGetLastError();
+}
+
+// Copies store ranges into (to_hbm) or out of the HBM buffer `hbm`: range r (its offset in the store, its bytes) is at hbm + at[r].
+// The host store: direct_chunk pieces round-robin over the copy streams.  A file (io: the readers or writers of
+// FileIO::cut(ranges)): one copy per window item, item k on copy stream k % n_cs.  *ops counts the copies.
+int copy_ranges(fma_engine_t* e, const std::vector<FileIO::Item>& ranges, const std::vector<uint64_t>& at, char* hbm, bool to_hbm, FileIO* io,
+                uint32_t* ops) {
+    if (io) {
+        std::vector<size_t> ends;
+        const std::vector<FileIO::Item> items = FileIO::cut(e, ranges, &ends);
+        for (size_t k = 0, r = 0; k < items.size(); ++k, ++*ops) {
+            while (k >= ends[r]) ++r;
+            RC(io->copy(k, hbm + at[r] + (items[k].file_off - ranges[r].file_off), e->cs[k % e->n_cs]));
+        }
+        return io->finish();   // every pread / pwrite has returned and every copy into or out of a window has finished
+    }
+    char* host = static_cast<char*>(e->host.base);
+    if (!host) return fail(FMA_ESTATE, "the host store that holds the image is gone");
+    const size_t chunk = direct_chunk(e);
+    for (size_t r = 0; r < ranges.size(); ++r)
+        for (uint64_t o = 0; o < ranges[r].bytes; o += chunk, ++*ops) {
+            const size_t n = (size_t)std::min<uint64_t>(chunk, ranges[r].bytes - o);
+            char* h = host + ranges[r].file_off + o;
+            char* d = hbm + at[r] + o;
+            RT(cudaMemcpyAsync(to_hbm ? d : h, to_hbm ? h : d, n, cudaMemcpyDefault, e->cs[*ops % e->n_cs]));
+        }
+    return FMA_OK;
+}
+
+// The copy engines' part of an operation, timed on the engine's streams only: the CopyTimer bracket around copy(), which counts
+// the copies it enqueues in *ops, and the "copies_landed" row over `bytes`
+template <class Copy>
+int timed_copies(fma_engine_t* e, uint64_t bytes, uint32_t* ops, Copy copy) {
+    RC(ensure_streams(e));
+    CopyTimer timer{e};
+    const double t0 = now_s();
+    RC(timer.begin());
+    RC(copy());
+    double copy_s = 0;
+    RC(timer.end(&copy_s));   // joins the copy streams only
+    e->tl_add("copies_landed", (int)*ops, t0, now_s(), bytes);
+    return FMA_OK;
+}
+
 // ---- moves of a sleeping image between tiers (fma_image_move) ----
 // Every tier holds the image in one layout (plain pages back to back, or the PACKED form's stored pages at img_off[p]), so a move
 // copies image_store_bytes bytes from offset 0 of one store to offset 0 of the other and changes nothing but the engine's records.
 
-// Copy engines between the pinned host store and the parking buffer: direct_chunk pieces round-robin over the copy streams.
-int move_host_park(fma_engine_t* e, bool to_park, uint64_t bytes, uint32_t* ops) {
-    char* host = static_cast<char*>(e->host.base);
-    char* park = reinterpret_cast<char*>(e->park.va);
-    const size_t chunk = direct_chunk(e);
-    size_t k = 0;
-    for (uint64_t o = 0; o < bytes; o += chunk, ++k) {
-        const size_t n = (size_t)std::min<uint64_t>(chunk, bytes - o);
-        RT(cudaMemcpyAsync(to_park ? park + o : host + o, to_park ? host + o : park + o, n, cudaMemcpyDefault, e->cs[k % e->n_cs]));
-        ++*ops;
-    }
-    return FMA_OK;
-}
-
-// The pinned host store <-> a file: FileIO's threads pread / pwrite straight into / out of the store, no copy engine involved.
-int move_host_file(fma_engine_t* e, bool to_file, int fd, bool direct, uint64_t bytes, uint64_t file_bytes, const char* path) {
+// The items of a move between the pinned host store and a file: FileIO's threads pread / pwrite them straight into / out of the
+// store, no copy engine involved.
+std::vector<FileIO::Item> move_host_file(const fma_engine_t* e, uint64_t bytes) {
     const uint64_t piece = round_up(std::max<size_t>(e->load_chunk, 4096), 4096);
     std::vector<FileIO::Item> items;
     for (uint64_t o = 0; o < bytes; o += piece) items.push_back(FileIO::Item{o, std::min(piece, bytes - o)});
-    FileIO io(e, fd, to_file, direct, std::move(items), file_bytes, path, static_cast<char*>(e->host.base));
-    return io.finish();
-}
-
-// The parking buffer <-> a file through the engine's pinned I/O windows: the file tier's disk stage without the HBM ring.
-int move_park_file(fma_engine_t* e, bool to_file, int fd, bool direct, uint64_t bytes, uint64_t file_bytes, const char* path, uint32_t* ops) {
-    const std::vector<FileIO::Item> items = FileIO::cut(e, {FileIO::Item{0, bytes}});
-    FileIO io(e, fd, to_file, direct, items, file_bytes, path);
-    for (size_t k = 0; k < items.size(); ++k, ++*ops)
-        RC(io.copy(k, reinterpret_cast<char*>(e->park.va) + items[k].file_off, e->cs[k % e->n_cs]));
-    return io.finish();   // every pread / pwrite has returned and every copy into or out of a window has finished
+    return items;
 }
 
 // What a move has set up so far, so that a failure can undo it
 struct MoveState {
-    FileFd file;
-    bool direct = false;
+    explicit MoveState(fma_engine_t* e) : file(e) {}
+    ImageFile file;
     bool file_emptied = false;   // the destination file has been emptied: a failure leaves no descriptor in it
     bool made_host = false;      // the host store, or the local parking buffer, was created by this move
     bool made_park = false;
@@ -168,7 +308,6 @@ int run_move(fma_engine_t* e, fma_layout::MovePipeKind pipe, int from, int to, M
     const uint64_t bytes = e->image_store_bytes;
     const bool park_side = pipe != MovePipeKind::HostFile && pipe != MovePipeKind::FileHost;
     ms.copies = park_side;
-    if (park_side) RC(ensure_streams(e));
     // the destination, prepared as a sleep to its tier prepares it
     if (to == FMA_TIER_HOST) {
         if (e->host.shared) {   // the shared image is read-only: leave it to its other holders and take a private store
@@ -187,43 +326,36 @@ int run_move(fma_engine_t* e, fma_layout::MovePipeKind pipe, int from, int to, M
         }
         if (ms.made_park) RC(park_store_create(e, e->device, need, &e->park));
     }
-    // the file side: the destination emptied once the filesystem has room; the source checked to hold the whole image
-    const double t_io = now_s();
-    const std::string path = to == FMA_TIER_FILE ? e->file_path : e->image_file;
-    uint64_t file_bytes = 0;
-    if (to == FMA_TIER_FILE) {
-        RC(open_image_file(path.c_str(), true, &ms.file.fd, &ms.direct));
-        RC(open_file_store(ms.file.fd, bytes, path.c_str()));
-        ms.file_emptied = true;
-    } else if (from == FMA_TIER_FILE) {
-        RC(open_image_source(path.c_str(), bytes, &ms.file.fd, &ms.direct, &file_bytes));
+    // the file side: the destination emptied once the filesystem has room; the source checked to hold the whole image.  A
+    // parking buffer's bytes go through the engine's pinned I/O windows (the file tier's disk stage without the HBM ring).
+    std::optional<FileIO> io;
+    if (to == FMA_TIER_FILE || from == FMA_TIER_FILE) {
+        std::vector<FileIO::Item> items = park_side ? FileIO::cut(e, {FileIO::Item{0, bytes}}) : move_host_file(e, bytes);
+        char* mem = park_side ? nullptr : static_cast<char*>(e->host.base);
+        if (to == FMA_TIER_FILE) {
+            RC(ms.file.create(e->file_path, bytes));
+            ms.file_emptied = true;
+            ms.file.write(std::move(items), &io, mem);
+        } else {
+            RC(ms.file.read(e->image_file, std::move(items), &io, mem));
+        }
     }
     // the bytes
     uint32_t ops = 0;
-    CopyTimer timer{e};
-    const double t_copy = now_s();
-    if (park_side) RC(timer.begin());
-    switch (pipe) {
-    case MovePipeKind::HostPark: RC(move_host_park(e, true, bytes, &ops)); break;
-    case MovePipeKind::ParkHost: RC(move_host_park(e, false, bytes, &ops)); break;
-    case MovePipeKind::HostFile: RC(move_host_file(e, true, ms.file.fd, ms.direct, bytes, 0, path.c_str())); break;
-    case MovePipeKind::FileHost: RC(move_host_file(e, false, ms.file.fd, ms.direct, bytes, file_bytes, path.c_str())); break;
-    case MovePipeKind::ParkFile: RC(move_park_file(e, true, ms.file.fd, ms.direct, bytes, 0, path.c_str(), &ops)); break;
-    case MovePipeKind::FilePark: RC(move_park_file(e, false, ms.file.fd, ms.direct, bytes, file_bytes, path.c_str(), &ops)); break;
-    case MovePipeKind::Refused: return fail(FMA_EINVAL, "a refused move has no copy");   // (refused before)
-    }
     if (park_side) {
-        double copy_s = 0;
-        RC(timer.end(&copy_s));   // joins the copy streams only
-        e->tl_add("copies_landed", (int)ops, t_copy, now_s(), bytes);
+        const bool to_park = fma_layout::is_park_tier(to);
+        RC(timed_copies(e, bytes, &ops, [&] {
+            return copy_ranges(e, {FileIO::Item{0, bytes}}, {0}, reinterpret_cast<char*>(e->park.va), to_park, io ? &*io : nullptr, &ops);
+        }));
+    } else {
+        RC(io->finish());
     }
     // a file written by a move is completed as a file-tier sleep completes it: it opens with fma_image_adopt_file and image_load
     if (to == FMA_TIER_FILE) {
-        std::vector<char> desc;
-        RC(image_descriptor_build(e, from, &desc));
-        RC(close_file_store(ms.file.fd, bytes, path.c_str(), ms.direct, desc));
+        RC(ms.file.seal(from));
+    } else if (from == FMA_TIER_FILE) {
+        RC(ms.file.finish(*io));
     }
-    if (ms.file.fd >= 0) e->tl_add("file_io", ms.direct ? 1 : 0, t_io, now_s(), to == FMA_TIER_FILE ? bytes + kImageTail : bytes);
     e->st.copy_ops = ops;
     e->st.total_copy_ops += ops;
     return FMA_OK;
@@ -231,15 +363,14 @@ int run_move(fma_engine_t* e, fma_layout::MovePipeKind pipe, int from, int to, M
 
 // A failed move: nothing may still copy into what goes, what the move created goes, and a destination file keeps no descriptor
 void undo_move(fma_engine_t* e, MoveState& ms) {
-    if (ms.copies)
-        for (int i = 0; i < e->n_cs; ++i) cudaStreamSynchronize(e->cs[i]);
+    if (ms.copies) drain(e);
     if (ms.made_host) {
         host_store_free(e->host);
         e->st.host_store_bytes = 0;
     }
     if (ms.made_park) vmm_buffer_free(e->park);
     if (ms.file_emptied) {   // what was written goes too (best effort: without its descriptor the file is refused anyway)
-        const int r = ftruncate(ms.file.fd, 0);
+        const int r = ftruncate(ms.file.fd(), 0);
         (void)r;
     }
     cudaGetLastError();
@@ -339,32 +470,22 @@ struct Verifier {
     // over the link, and the window goes back to its reader behind them
     int file(const std::vector<PagePlan>& pages, size_t at) {
         if (!e->load_ring) RC(ensure_io_windows(e));
-        const uint64_t window = e->io_window_bytes - 8192;   // (the windows' O_DIRECT slack, ensure_io_windows)
+        const uint64_t window = FileIO::max_item(e);
         std::vector<Batch> batches;
         if (!fma_layout::plan_batches(pages, SIZE_MAX, window, true, &batches))
             return fail(FMA_EINVAL, "a stored page does not fit an I/O window of %llu bytes", (unsigned long long)window);
         std::vector<FileIO::Item> items;
-        uint64_t need = 0, read_bytes = 0;
-        for (const Batch& b : batches) {
-            items.push_back(FileIO::Item{pages[b.p0].off, b.stored});
-            need = std::max(need, pages[b.p0].off + b.stored);
-            read_bytes += b.stored;
-        }
-        const double t_io = now_s();
-        FileFd f;
-        bool direct = false;
-        uint64_t file_bytes = 0;
-        RC(open_image_source(e->image_file.c_str(), need, &f.fd, &direct, &file_bytes));
-        FileIO io(e, f.fd, false, direct, items, file_bytes, e->image_file.c_str());
+        for (const Batch& b : batches) items.push_back(FileIO::Item{pages[b.p0].off, b.stored});
+        ImageFile file(e);
+        std::optional<FileIO> io;
+        RC(file.read(e->image_file, std::move(items), &io));
         for (size_t c = 0; c < batches.size(); ++c) {
             const Batch& b = batches[c];
-            RC(io.read_in_place(c, e->ks, [&](const char* win) {
+            RC(io->read_in_place(c, e->ks, [&](const char* win) {
                 return launch(pages, at, b, [&](size_t q) { return (uint64_t)(uintptr_t)win + (pages[q].off - pages[b.p0].off); });
             }));
         }
-        RC(io.finish());   // every read has returned and every kernel over a window has finished
-        e->tl_add("file_io", direct ? 1 : 0, t_io, now_s(), read_bytes);
-        return FMA_OK;
+        return file.finish(*io);   // every read has returned and every kernel over a window has finished
     }
 
     int run(const std::vector<size_t>& main, const std::vector<size_t>& res, const std::vector<size_t>& pf) {
@@ -442,13 +563,7 @@ struct PrefetchPlan {
 };
 
 int plan_prefetch(fma_engine_t* e, uint64_t budget, PrefetchPlan* p) {
-    std::vector<size_t> order;   // the sleeping segments, image order
-    {
-        std::lock_guard<std::mutex> lk(e->mu);
-        for (size_t i = 0; i < e->segs.size(); ++i)
-            if (e->segs[i].has_backup && !e->segs[i].mapped) order.push_back(i);
-    }
-    std::sort(order.begin(), order.end(), [&](size_t a, size_t b) { return e->segs[a].packed_off < e->segs[b].packed_off; });
+    const std::vector<size_t> order = sleeping_segments(e, [](const Segment&) { return true; });
     std::vector<uint64_t> stored(order.size(), 0);
     for (size_t k = 0; k < order.size(); ++k) {
         const Segment& s = e->segs[order[k]];
@@ -486,46 +601,19 @@ int plan_prefetch(fma_engine_t* e, uint64_t budget, PrefetchPlan* p) {
     return FMA_OK;
 }
 
-// The copies into `dst` (the new buffer), timed on the engine's streams only.  Host store: direct_chunk pieces round-robin over the
-// copy streams.  File: reader threads pread the ranges into the pinned I/O windows, one H2D per window.
+// The copies into `dst` (the new buffer), timed on the engine's streams only.  From a file, reader threads pread the ranges into
+// the pinned I/O windows, one H2D per window.
 int prefetch_copy(fma_engine_t* e, const PrefetchPlan& p, char* dst) {
-    RC(ensure_streams(e));
-    CopyTimer timer{e};
+    ImageFile file(e);
+    std::optional<FileIO> io;
     uint32_t ops = 0;
-    const double t_copy = now_s();
-    RC(timer.begin());
-    if (e->image_tier == FMA_TIER_FILE) {
+    return timed_copies(e, p.stored, &ops, [&] {
+        if (e->image_tier != FMA_TIER_FILE) return copy_ranges(e, p.ranges, p.at, dst, true, nullptr, &ops);
         if (!e->load_ring) RC(ensure_io_windows(e));
-        std::vector<size_t> ends;
-        const std::vector<FileIO::Item> items = FileIO::cut(e, p.ranges, &ends);
-        // the ranges ascend in the file: the last one ends furthest into it
-        const uint64_t need = p.ranges.back().file_off + p.ranges.back().bytes;
-        const double t_io = now_s();
-        FileFd f;
-        bool direct = false;
-        uint64_t file_bytes = 0;
-        RC(open_image_source(e->image_file.c_str(), need, &f.fd, &direct, &file_bytes));
-        FileIO io(e, f.fd, false, direct, items, file_bytes, e->image_file.c_str());
-        for (size_t k = 0, r = 0; k < items.size(); ++k, ++ops) {
-            while (k >= ends[r]) ++r;
-            RC(io.copy(k, dst + p.at[r] + (items[k].file_off - p.ranges[r].file_off), e->cs[k % e->n_cs]));
-        }
-        RC(io.finish());   // every read has returned and every H2D out of a window has finished
-        e->tl_add("file_io", direct ? 1 : 0, t_io, now_s(), p.stored);
-    } else {
-        const char* host = static_cast<const char*>(e->host.base);
-        if (!host) return fail(FMA_ESTATE, "the host store that holds the image is gone");
-        const size_t chunk = direct_chunk(e);
-        for (size_t r = 0; r < p.ranges.size(); ++r)
-            for (uint64_t o = 0; o < p.ranges[r].bytes; o += chunk, ++ops) {
-                const size_t n = (size_t)std::min<uint64_t>(chunk, p.ranges[r].bytes - o);
-                RT(cudaMemcpyAsync(dst + p.at[r] + o, host + p.ranges[r].file_off + o, n, cudaMemcpyDefault, e->cs[ops % e->n_cs]));
-            }
-    }
-    double copy_s = 0;
-    RC(timer.end(&copy_s));   // joins the copy streams only
-    e->tl_add("copies_landed", (int)ops, t_copy, now_s(), p.stored);
-    return FMA_OK;
+        RC(file.read(e->image_file, FileIO::cut(e, p.ranges), &io));
+        RC(copy_ranges(e, p.ranges, p.at, dst, true, &*io, &ops));
+        return file.finish(*io);
+    });
 }
 
 }  // namespace
@@ -537,7 +625,7 @@ int fma_image_export(fma_engine_t* e, int* out_fd) {
     if (check_engine(e) != FMA_OK) return FMA_EINVAL;
     std::lock_guard<std::mutex> op(e->op_mu);
     if (!out_fd) return fail(FMA_EINVAL, "out_fd is NULL");
-    if (resident_asleep(e)) return fail(FMA_ESTATE, "part of the sleeping image is resident in this process's own HBM (option resident_bytes) and cannot be handed over: set it to 0 and sleep again");
+    RC(refuse_resident_handover(e));
     if (e->image_tier == FMA_TIER_FILE && image_in(e, ImageIn::AnyAsleep)) return fail(FMA_ESTATE, "the sleeping image is in a file: the file itself is the hand-over");
     if (e->host.fd < 0 || !e->host.base) return fail(FMA_ESTATE, "the host store is not shareable (set FMA_HOST_STORE_SHM=1 before the first sleep)");
     if (e->image_tier != FMA_TIER_HOST) return fail(FMA_ESTATE, "no host-tier image");
@@ -556,97 +644,18 @@ int fma_image_adopt(fma_engine_t* e, int fd, uint64_t tag_mask, uint32_t flags) 
     if (check_engine(e) != FMA_OK) return FMA_EINVAL;
     std::lock_guard<std::mutex> op(e->op_mu);
     if (!tag_mask) return fail(FMA_EINVAL, "adopt needs the tag mask the image was slept with");
-    for (const Segment& s : e->segs)
-        if (!s.mapped) return fail(FMA_ESTATE, "adopt needs a fully awake engine");
+    RC(adopt_needs_awake(e));
     struct stat sb;
     if (fstat(fd, &sb) != 0 || (size_t)sb.st_size <= kImageTail) return fail(FMA_EINVAL, "not an image fd");
-    const size_t map_bytes = (size_t)sb.st_size, cap = map_bytes - kImageTail;
-    int myfd = dup(fd);
-    if (myfd < 0) return fail(FMA_ENOMEM, "dup failed: %s", strerror(errno));
-    void* p = mmap(nullptr, map_bytes, PROT_READ | PROT_WRITE, MAP_SHARED, myfd, 0);
-    if (p == MAP_FAILED) {
-        close(myfd);
-        return fail(FMA_ENOMEM, "cannot map the image: %s", strerror(errno));
-    }
-    auto bail = [&](int code, const char* why) {
-        munmap(p, map_bytes);
-        close(myfd);
-        return fail(code, "%s", why);
-    };
-    const char* tail = static_cast<const char*>(p) + cap;
-    ParsedImage pi;
-    {
-        int prc = image_descriptor_parse(e, tail, kImageTail, cap, tag_mask, &pi);
-        if (prc != FMA_OK) {
-            char why[512];
-            snprintf(why, sizeof(why), "%s", tl_err);
-            return bail(prc, why);
-        }
-    }
-    const ImageHeader& hd = pi.hd;
-    std::vector<ImageSegDesc>& ds = pi.ds;
-    const std::vector<size_t>& order = pi.order;
-    DeviceGuard guard(e->device);
-    cudaDeviceSynchronize();
-    if (flags & FMA_FLAG_VERIFY) {
-        // "Sleep by adoption": this engine HAS the weights and wants to share somebody else's image of the same model (a second
-        // replica on the node: one host copy for all).  Only legal if its device bytes are what the image holds — K3 digests
-        // against the descriptor's; a mismatch leaves the engine awake and untouched.
-        std::vector<uint64_t> now;
-        int vrc = digest_segments(e, order, &now);
-        if (vrc != FMA_OK) {
-            munmap(p, map_bytes);
-            close(myfd);
-            return vrc;
-        }
-        for (size_t i = 0; i < ds.size(); ++i)
-            if (!ds[i].digest_valid || ds[i].digest != now[i])
-                return bail(FMA_EINTEGRITY, ds[i].digest_valid ? "the image holds different bytes than this engine's segments" : "the image carries no digests to compare with");
-    }
-    invalidate_shadows(e);
-    host_store_free(e->host);
-    const double t0 = now_s();
-    cudaError_t r = cudaHostRegister(p, map_bytes, cudaHostRegisterPortable | cudaHostRegisterMapped);
-    HostStore h;
-    if (r != cudaSuccess) {
-        // The mapping cannot be pinned in place (e.g. an image FILE on a filesystem whose pages the driver will not lock):
-        // copy it once into an anonymous pinned store — a load from the page cache, several threads — and let go of the fd.
-        cudaGetLastError();
-        void* q = nullptr;
-        r = cudaHostAlloc(&q, map_bytes, cudaHostAllocPortable | cudaHostAllocMapped);
-        if (r != cudaSuccess) {
-            cudaGetLastError();
-            return bail(FMA_ENOMEM, "cannot pin the adopted image, in place or as a copy");
-        }
-        const int nt = std::max(1, std::min(env_int("FMA_TOUCH_THREADS", 8), 32));
-        const size_t per = round_up((map_bytes + nt - 1) / nt, FMA_PAGE_BYTES);
-        std::vector<std::thread> th;
-        for (int t = 0; t < nt; ++t) {
-            const size_t lo = (size_t)t * per, hi = std::min(map_bytes, lo + per);
-            if (lo >= hi) break;
-            th.emplace_back([p, q, lo, hi] { memcpy(static_cast<char*>(q) + lo, static_cast<const char*>(p) + lo, hi - lo); });
-        }
-        for (auto& t : th) t.join();
-        munmap(p, map_bytes);
-        close(myfd);
-        h.base = q; h.cap = cap; h.map_bytes = 0; h.fd = -1; h.registered = false;
-        p = q;
-    } else {
-        h.base = p; h.cap = cap; h.map_bytes = map_bytes; h.fd = myfd; h.registered = true;
-        h.shared = true;  // the exporter (and other adopters) map the same pages
-    }
-    void* alias = nullptr;
-    if (cudaHostGetDevicePointer(&alias, p, 0) == cudaSuccess) h.dev_alias = alias;
-    else cudaGetLastError();
-    h.pin_seconds = now_s() - t0;
-    e->host = h;
-    e->st.host_store_bytes = cap;
-    e->st.host_store_pin_seconds = h.pin_seconds;
-    // release the device side exactly as a sleep would, without copying anything out
-    RC(do_sleep(e, tag_mask, FMA_TIER_HOST, (flags & ~FMA_FLAG_VERIFY) | kFlagAdopt));
-    (void)hd;
-    image_apply(e, pi);
-    return FMA_OK;
+    ImageMapping m;
+    m.bytes = (size_t)sb.st_size;
+    const size_t cap = m.bytes - kImageTail;
+    m.fd = dup(fd);
+    if (m.fd < 0) return fail(FMA_ENOMEM, "dup failed: %s", strerror(errno));
+    void* p = mmap(nullptr, m.bytes, PROT_READ | PROT_WRITE, MAP_SHARED, m.fd, 0);
+    if (p == MAP_FAILED) return fail(FMA_ENOMEM, "cannot map the image: %s", strerror(errno));
+    m.base = p;
+    return adopt(e, static_cast<const char*>(p) + cap, kImageTail, cap, tag_mask, flags, FMA_TIER_HOST, [&] { return adopt_host_store(e, m); });
 }
 
 // ---- FILE tier (see include/fma_engine.h) -----------------------------------------------------------------------------
@@ -669,11 +678,7 @@ int fma_image_adopt_file(fma_engine_t* e, const char* path, uint64_t tag_mask, u
     if (check_engine(e) != FMA_OK) return FMA_EINVAL;
     std::lock_guard<std::mutex> op(e->op_mu);
     if (!path || !tag_mask) return fail(FMA_EINVAL, "adopt needs the file and the tag mask the image was slept with");
-    {
-        std::lock_guard<std::mutex> lk(e->mu);
-        for (const Segment& s : e->segs)
-            if (!s.mapped) return fail(FMA_ESTATE, "adopt needs a fully awake engine");
-    }
+    RC(adopt_needs_awake(e));
     FileFd f;
     f.fd = open(path, O_RDONLY | O_CLOEXEC);
     if (f.fd < 0) return fail(FMA_EIO, "cannot open %s: %s", path, strerror(errno));
@@ -687,21 +692,11 @@ int fma_image_adopt_file(fma_engine_t* e, const char* path, uint64_t tag_mask, u
         if (n <= 0) return fail(FMA_EIO, "cannot read the descriptor of %s: %s", path, n < 0 ? strerror(errno) : "the file ends early");
         got += (size_t)n;
     }
-    ParsedImage pi;
-    RC(image_descriptor_parse(e, tail.data(), kImageTail, cap, tag_mask, &pi));
-    DeviceGuard guard(e->device);
-    cudaDeviceSynchronize();
-    if (flags & FMA_FLAG_VERIFY) {  // "sleep by adoption" (see fma_image_adopt): only if this engine's bytes ARE the image's
-        std::vector<uint64_t> now;
-        RC(digest_segments(e, pi.order, &now));
-        for (size_t i = 0; i < pi.ds.size(); ++i)
-            if (!pi.ds[i].digest_valid || pi.ds[i].digest != now[i])
-                return fail(FMA_EINTEGRITY, pi.ds[i].digest_valid ? "the image holds different bytes than this engine's segments" : "the image carries no digests to compare with");
-    }
-    if (!e->load_ring) RC(ensure_io_windows(e));
-    invalidate_shadows(e);
-    RC(do_sleep(e, tag_mask, FMA_TIER_FILE, (flags & ~FMA_FLAG_VERIFY) | kFlagAdopt));
-    image_apply(e, pi);
+    RC(adopt(e, tail.data(), kImageTail, cap, tag_mask, flags, FMA_TIER_FILE, [&] {
+        if (!e->load_ring) RC(ensure_io_windows(e));
+        invalidate_shadows(e);
+        return FMA_OK;
+    }));
     e->image_file = path;
     return FMA_OK;
 }
@@ -712,7 +707,7 @@ int fma_image_adopt_file(fma_engine_t* e, const char* path, uint64_t tag_mask, u
 int fma_image_describe(fma_engine_t* e, int tier, void* buf, size_t cap) {
     if (check_engine(e) != FMA_OK) return FMA_EINVAL;
     std::lock_guard<std::mutex> op(e->op_mu);
-    if (resident_asleep(e)) return fail(FMA_ESTATE, "part of the sleeping image is resident in this process's own HBM (option resident_bytes) and cannot be handed over: set it to 0 and sleep again");
+    RC(refuse_resident_handover(e));
     if (tier != e->image_tier) return fail(FMA_ESTATE, "no image sleeps in tier %d", tier);
     if (tier == FMA_TIER_FILE) return fail(FMA_ESTATE, "the sleeping image is in a file: the file itself is the hand-over (its descriptor is its tail)");
     std::vector<char> desc;
@@ -726,26 +721,11 @@ int fma_image_adopt_parked(fma_engine_t* e, const void* desc, size_t desc_bytes,
     std::lock_guard<std::mutex> op(e->op_mu);
     if (!desc || !tag_mask) return fail(FMA_EINVAL, "adopt needs the descriptor and the tag mask the image was slept with");
     if (!e->park.va || e->park.device == e->device) return fail(FMA_ESTATE, "adopt_parked needs an attached / reserved peer parking buffer first");
-    {
-        std::lock_guard<std::mutex> lk(e->mu);
-        for (const Segment& s : e->segs)
-            if (!s.mapped) return fail(FMA_ESTATE, "adopt needs a fully awake engine");
-    }
-    ParsedImage pi;
-    RC(image_descriptor_parse(e, static_cast<const char*>(desc), desc_bytes, e->park.bytes, tag_mask, &pi));
-    DeviceGuard guard(e->device);
-    cudaDeviceSynchronize();
-    if (flags & FMA_FLAG_VERIFY) {  // "sleep by adoption" (see fma_image_adopt): only if this engine's bytes ARE the image's
-        std::vector<uint64_t> now;
-        RC(digest_segments(e, pi.order, &now));
-        for (size_t i = 0; i < pi.ds.size(); ++i)
-            if (!pi.ds[i].digest_valid || pi.ds[i].digest != now[i])
-                return fail(FMA_EINTEGRITY, pi.ds[i].digest_valid ? "the image holds different bytes than this engine's segments" : "the image carries no digests to compare with");
-    }
-    if (e->shadow_tier != FMA_TIER_HOST) invalidate_shadows(e);
-    RC(do_sleep(e, tag_mask, FMA_TIER_PEER, (flags & ~FMA_FLAG_VERIFY) | kFlagAdopt));
-    image_apply(e, pi);
-    return FMA_OK;
+    RC(adopt_needs_awake(e));
+    return adopt(e, static_cast<const char*>(desc), desc_bytes, e->park.bytes, tag_mask, flags, FMA_TIER_PEER, [&] {
+        if (e->shadow_tier != FMA_TIER_HOST) invalidate_shadows(e);
+        return FMA_OK;
+    });
 }
 
 // ---- moving a sleeping image to another tier (see include/fma_engine.h) -------------------------------------------------
@@ -754,11 +734,7 @@ int fma_image_move(fma_engine_t* e, int tier) {
     std::lock_guard<std::mutex> op(e->op_mu);
     const int from = e->image_tier;
     fma_layout::MoveFacts facts{};
-    {
-        std::lock_guard<std::mutex> lk(e->mu);
-        for (const Segment& s : e->segs)
-            if (s.has_backup) (s.mapped ? facts.backup_mapped : facts.asleep) = true;
-    }
+    sleep_state(e, &facts.asleep, &facts.backup_mapped);
     facts.resident = resident_asleep(e);
     facts.prepared = tier == FMA_TIER_PEER ? e->park.va && e->park.device != e->device && e->park.bytes >= e->image_store_bytes
                    : tier == FMA_TIER_FILE ? !e->file_path.empty()
@@ -770,7 +746,7 @@ int fma_image_move(fma_engine_t* e, int tier) {
     RC(flush_kernel_times(e));
     const double t_entry = now_s();
     e->tl_begin("move", t_entry);
-    MoveState ms;
+    MoveState ms(e);
     const int rc = run_move(e, route.pipe, from, tier, ms);
     if (rc != FMA_OK) {
         undo_move(e, ms);   // the image stays where it was, its records untouched
@@ -843,11 +819,7 @@ int fma_image_prefetch(fma_engine_t* e, uint64_t bytes) {
         return FMA_OK;
     }
     fma_layout::PrefetchFacts facts{e->image_tier, false, false, e->res.va != 0};
-    {
-        std::lock_guard<std::mutex> lk(e->mu);
-        for (const Segment& s : e->segs)
-            if (s.has_backup) (s.mapped ? facts.backup_mapped : facts.asleep) = true;
-    }
+    sleep_state(e, &facts.asleep, &facts.backup_mapped);
     const fma_layout::PrefetchRoute route = fma_layout::prefetch_route(facts);
     if (route.error != FMA_OK) return fail(route.error, "image prefetch: %s", route.why);
     RC(flush_kernel_times(e));   // (the last operation's kernel rows and times, before the timeline turns to this call)
@@ -861,9 +833,7 @@ int fma_image_prefetch(fma_engine_t* e, uint64_t bytes) {
         RC(park_store_create(e, e->device, p.stored, &buf));
         const int rc = prefetch_copy(e, p, reinterpret_cast<char*>(buf.va));
         if (rc != FMA_OK) {   // nothing may still copy into the buffer when it goes
-            for (int i = 0; i < e->n_cs; ++i) cudaStreamSynchronize(e->cs[i]);
-            if (e->ks) cudaStreamSynchronize(e->ks);
-            cudaGetLastError();
+            drain(e);
             vmm_buffer_free(buf);
             return rc;
         }

@@ -424,6 +424,11 @@ enum class ImageIn {
 bool image_in(fma_engine_t* e, ImageIn where);
 // a sleeping image keeps part of itself in the resident buffer
 inline bool resident_asleep(fma_engine_t* e) { return e->res.va && image_in(e, ImageIn::Local); }
+// A hand-over of the sleeping image (fma_image_export / _describe, fma_host_store_share) cannot take that part along
+inline int refuse_resident_handover(fma_engine_t* e) {
+    if (!resident_asleep(e)) return FMA_OK;
+    return fail(FMA_ESTATE, "part of the sleeping image is resident in this process's own HBM (option resident_bytes) and cannot be handed over: set it to 0 and sleep again");
+}
 // A wake restores a segment from HBM instead of its tier's store when its bytes are in the resident share or in the prefetch
 // buffer (an image has one or the other, never both).  Its offset in that part's image space, or kNoOffset.
 inline uint64_t hbm_offset(const fma_engine_t* e, const Segment& s) {
@@ -447,11 +452,6 @@ int image_descriptor_build(fma_engine_t* e, int tier, std::vector<char>* out);
 void invalidate_shadows(fma_engine_t* e);   // the host store no longer holds a usable copy of any segment
 // ---- file I/O (fma_load.cu) ----
 int ensure_io_windows(fma_engine_t* e);   // pin the I/O windows for the current load_* options (and their events)
-// Opens `path` for the FILE tier (write: created, not truncated), with O_DIRECT when the filesystem accepts it and
-// FMA_FILE_BUFFERED is not 1; *direct tells which.  Failure: FMA_EIO.
-int open_image_file(const char* path, bool write, int* fd, bool* direct);
-// open_image_file for reading an image of `need` bytes: a file that holds fewer is refused with FMA_EIO; *file_bytes: its size
-int open_image_source(const char* path, uint64_t need, int* fd, bool* direct, uint64_t* file_bytes);
 struct FileFd {   // closes on every exit path
     int fd = -1;
     ~FileFd() { if (fd >= 0) close(fd); }
@@ -473,6 +473,8 @@ class FileIO {
     struct Item {
         uint64_t file_off, bytes;
     };
+    // the most one item through a window moves: the window less its O_DIRECT slack (ensure_io_windows)
+    static uint64_t max_item(const fma_engine_t* e) { return e->io_window_bytes - 8192; }
     // `ranges` cut into items of at most one window each, in order; (*ends)[r]: one past the last item of range r
     static std::vector<Item> cut(const fma_engine_t* e, const std::vector<Item>& ranges, std::vector<size_t>* ends = nullptr);
     FileIO(fma_engine_t* e, int fd, bool write, bool direct, std::vector<Item> items, uint64_t file_bytes, const char* path, char* mem = nullptr);
@@ -535,13 +537,36 @@ class FileIO {
     bool stopped_ = false;
 };
 
-// ---- the FILE tier's store (fma_sleep.cu), for a file-tier sleep and a move to the file tier (fma_image_move) ----
-// The filesystem of the open file `fd` has room for an image of `bytes` and its descriptor (fstatvfs), and only then the file is
-// emptied.  Short of room: FMA_EIO with the file untouched.
-int open_file_store(int fd, uint64_t bytes, const char* path);
-// After the image's last write: fdatasync, then `desc` (image_descriptor_build) in the kImageTail bytes behind the image, then
-// fdatasync again, so a torn file fails descriptor parsing.
-int close_file_store(int fd, uint64_t bytes, const char* path, bool direct, const std::vector<char>& desc);
+// The FILE tier's image file as one operation reads or writes it: a wake, a verify, a prefetch or a move out of the tier reads it;
+// a file-tier sleep or a move into the tier writes it.  It owns the fd, whether that is O_DIRECT (when the filesystem accepts it
+// and FMA_FILE_BUFFERED is not 1), the time it was opened and the operation's "file_io" timeline row: from the open to the end,
+// idx 1 with O_DIRECT, over every byte read, or over the image and its descriptor written.  Failures to open: FMA_EIO.
+class ImageFile {
+  public:
+    explicit ImageFile(fma_engine_t* e) : e_(e) {}
+    // Reads `items` of `path`.  A file that ends before the furthest item does (truncated or replaced) is refused before a read
+    // is issued; then *io's readers start (`mem`: see FileIO).
+    int read(const std::string& path, std::vector<FileIO::Item> items, std::optional<FileIO>* io, char* mem = nullptr);
+    // Opens `path` (created if need be) to write an image of `bytes`, and empties it only once its filesystem has room for the
+    // image and its descriptor (fstatvfs).  Short of room, the file is left untouched.
+    int create(const std::string& path, uint64_t bytes);
+    void write(std::vector<FileIO::Item> items, std::optional<FileIO>* io, char* mem = nullptr);   // *io's writers of `items`
+    // Read: every read has returned and every copy out of a window has finished (io.finish()), then the row.
+    int finish(FileIO& io);
+    // Write, after the last item: fdatasync, then the descriptor of the image sleeping in `tier`'s store (image_descriptor_build)
+    // in the kImageTail bytes behind the image, then fdatasync again, so a torn file fails descriptor parsing; then the row.
+    int seal(int tier);
+    int fd() const { return file_.fd; }
+
+  private:
+    int row(uint64_t bytes);
+    fma_engine_t* e_;
+    std::string path_;
+    FileFd file_;
+    bool direct_ = false;
+    double t0_ = 0;
+    uint64_t bytes_ = 0;   // read: every item's; write: the image's
+};
 
 // ---- pipelines ----
 int do_sleep(fma_engine_t* e, uint64_t offload_mask, int tier, uint32_t flags);   // fma_sleep.cu

@@ -3,6 +3,8 @@
 // Part of the host engine (see fma_internal.h for the map of translation units; C-ABI in include/fma_engine.h).
 #include "fma_internal.h"
 
+#include <sys/statvfs.h>
+
 namespace fma_impl {
 
 int ensure_io_windows(fma_engine_t* e) {
@@ -32,6 +34,10 @@ int ensure_io_windows(fma_engine_t* e) {
     return FMA_OK;
 }
 
+namespace {
+
+// Opens `path` for the FILE tier (write: created, not truncated), with O_DIRECT when the filesystem accepts it and
+// FMA_FILE_BUFFERED is not 1; *direct tells which.  Failure: FMA_EIO.
 int open_image_file(const char* path, bool write, int* fd, bool* direct) {
     const int flags = (write ? O_WRONLY | O_CREAT : O_RDONLY) | O_CLOEXEC;
     *direct = env_int("FMA_FILE_BUFFERED", 0) == 0;
@@ -45,6 +51,7 @@ int open_image_file(const char* path, bool write, int* fd, bool* direct) {
     return FMA_OK;
 }
 
+// open_image_file for reading an image of `need` bytes: a file that holds fewer is refused with FMA_EIO; *file_bytes: its size
 int open_image_source(const char* path, uint64_t need, int* fd, bool* direct, uint64_t* file_bytes) {
     RC(open_image_file(path, false, fd, direct));
     struct stat sb;
@@ -55,8 +62,86 @@ int open_image_source(const char* path, uint64_t need, int* fd, bool* direct, ui
     return FMA_OK;
 }
 
+// The filesystem of the open file `fd` has room for an image of `bytes` and its descriptor (fstatvfs), and only then the file is
+// emptied.  Short of room: FMA_EIO with the file untouched.
+int open_file_store(int fd, uint64_t bytes, const char* path) {
+    struct statvfs vs;
+    struct stat sb;
+    if (fstatvfs(fd, &vs) != 0 || fstat(fd, &sb) != 0) return fail(FMA_EIO, "fstatvfs(%s) failed: %s", path, strerror(errno));
+    const uint64_t need = bytes + kImageTail, room = (uint64_t)vs.f_bavail * vs.f_frsize + (uint64_t)sb.st_blocks * 512;  // (its own blocks come back)
+    if (room < need) return fail(FMA_EIO, "%s: %llu bytes free, the image needs %llu", path, (unsigned long long)room, (unsigned long long)need);
+    if (ftruncate(fd, 0) != 0) return fail(FMA_EIO, "ftruncate(%s) failed: %s", path, strerror(errno));
+    return FMA_OK;
+}
+
+// After the image's last write: fdatasync, then `desc` in the kImageTail bytes behind the image, then fdatasync again
+int close_file_store(int fd, uint64_t bytes, const char* path, bool direct, const std::vector<char>& desc) {
+    if (fdatasync(fd) != 0) return fail(FMA_EIO, "fdatasync(%s) failed: %s", path, strerror(errno));
+    void* buf = nullptr;
+    if (desc.size() > kImageTail || posix_memalign(&buf, 4096, kImageTail) != 0) return fail(FMA_ENOMEM, "no memory for the descriptor");
+    memset(buf, 0, kImageTail);
+    memcpy(buf, desc.data(), desc.size());
+    uint64_t done = 0;
+    while (done < kImageTail) {
+        const ssize_t n = pwrite(fd, static_cast<char*>(buf) + done, kImageTail - done, (off_t)(bytes + done));
+        if (n < 0 && errno == EINTR) continue;
+        if (n <= 0) break;
+        done += (uint64_t)n;
+    }
+    const int err = errno;
+    free(buf);
+    if (done < kImageTail) return fail(FMA_EIO, "writing the descriptor of %s failed: %s", path, strerror(err));
+    if (fdatasync(fd) != 0) return fail(FMA_EIO, "fdatasync(%s) failed: %s", path, strerror(errno));
+    if (!direct) posix_fadvise(fd, 0, 0, POSIX_FADV_DONTNEED);   // clean now: the page cache lets go of the image
+    return FMA_OK;
+}
+
+}  // namespace
+
+int ImageFile::read(const std::string& path, std::vector<FileIO::Item> items, std::optional<FileIO>* io, char* mem) {
+    path_ = path;
+    t0_ = now_s();
+    uint64_t need = 0, file_bytes = 0;
+    for (const FileIO::Item& it : items) {
+        need = std::max(need, it.file_off + it.bytes);
+        bytes_ += it.bytes;
+    }
+    RC(open_image_source(path_.c_str(), need, &file_.fd, &direct_, &file_bytes));
+    io->emplace(e_, file_.fd, false, direct_, std::move(items), file_bytes, path_.c_str(), mem);
+    return FMA_OK;
+}
+
+int ImageFile::create(const std::string& path, uint64_t bytes) {
+    path_ = path;
+    t0_ = now_s();
+    bytes_ = bytes;
+    RC(open_image_file(path_.c_str(), true, &file_.fd, &direct_));
+    return open_file_store(file_.fd, bytes, path_.c_str());
+}
+
+void ImageFile::write(std::vector<FileIO::Item> items, std::optional<FileIO>* io, char* mem) {
+    io->emplace(e_, file_.fd, true, direct_, std::move(items), 0, path_.c_str(), mem);
+}
+
+int ImageFile::finish(FileIO& io) {
+    RC(io.finish());
+    return row(bytes_);
+}
+
+int ImageFile::seal(int tier) {
+    std::vector<char> desc;
+    RC(image_descriptor_build(e_, tier, &desc));
+    RC(close_file_store(file_.fd, bytes_, path_.c_str(), direct_, desc));
+    return row(bytes_ + kImageTail);
+}
+
+int ImageFile::row(uint64_t bytes) {
+    e_->tl_add("file_io", direct_ ? 1 : 0, t0_, now_s(), bytes);
+    return FMA_OK;
+}
+
 std::vector<FileIO::Item> FileIO::cut(const fma_engine_t* e, const std::vector<Item>& ranges, std::vector<size_t>* ends) {
-    const uint64_t piece = e->io_window_bytes - 8192;   // (the windows' O_DIRECT slack, ensure_io_windows)
+    const uint64_t piece = max_item(e);
     std::vector<Item> items;
     for (const Item& r : ranges) {
         for (uint64_t o = 0; o < r.bytes; o += piece) items.push_back(Item{r.file_off + o, std::min(piece, r.bytes - o)});
@@ -81,7 +166,7 @@ FileIO::FileIO(fma_engine_t* e, int fd, bool write, bool direct, std::vector<Ite
             return;
         }
         for (const Item& it : items_)
-            if (it.bytes > e->io_window_bytes - 8192 || (direct_ && write_ && ((it.file_off | it.bytes) & 4095))) {
+            if (it.bytes > max_item(e) || (direct_ && write_ && ((it.file_off | it.bytes) & 4095))) {
                 set_error(FMA_EINVAL, "I/O item of %llu bytes at %llu does not fit a window", (unsigned long long)it.bytes, (unsigned long long)it.file_off);
                 return;
             }

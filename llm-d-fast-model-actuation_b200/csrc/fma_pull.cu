@@ -345,7 +345,7 @@ int fma_host_store_share(fma_engine_t* e, int* out_fd) {
     if (check_engine(e) != FMA_OK) return FMA_EINVAL;
     if (!out_fd) return fail(FMA_EINVAL, "out_fd is NULL");
     std::lock_guard<std::mutex> op(e->op_mu);
-    if (resident_asleep(e)) return fail(FMA_ESTATE, "part of the sleeping image is resident in this process's own HBM (option resident_bytes) and cannot be handed over: set it to 0 and sleep again");
+    RC(refuse_resident_handover(e));
     if (e->image_tier == FMA_TIER_FILE && image_in(e, ImageIn::AnyAsleep)) return fail(FMA_ESTATE, "the sleeping image is in a file: the file itself is the hand-over");
     if (e->host.fd < 0 || !e->host.base) return fail(FMA_ESTATE, "the host store is not shareable (set FMA_HOST_STORE_SHM=1 before the first sleep / host_reserve)");
     const int fd = dup(e->host.fd);

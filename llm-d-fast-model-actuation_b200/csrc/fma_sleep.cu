@@ -3,8 +3,6 @@
 #include "fma_internal.h"
 #include "fma_gate.h"
 
-#include <sys/statvfs.h>
-
 namespace fma_impl {
 
 namespace {
@@ -271,9 +269,7 @@ struct SleepPipe {
     Unmapper* un;          // releases units behind the pipeline; null: nothing is released (the resident gather)
     const std::vector<size_t>* subset = nullptr;  // INCREMENTAL + PACKED: only these image pages (ascending) are re-coded, in place
     bool resident = false;  // the extents go to the resident buffer (e->res, its own page layout res_off / res_bytes), not the tier's store
-    int file_fd = -1;       // FILE tier: the staged pipeline writes the image to this file, not to `store`
-    bool file_direct = false;
-    const char* file_path = nullptr;
+    ImageFile* file = nullptr;   // FILE tier: the staged pipeline writes the image to this file, not to `store`
     int publish_consumed(uint64_t image_done, cudaStream_t stream) { return un ? un->publish_consumed(image_done, stream) : FMA_OK; }
     int publish_gathered(size_t pages_done) { return publish_consumed((uint64_t)pages_done * FMA_PAGE_BYTES, e->ks); }
     // the image's pages, stored in the PACKED layout or verbatim; their device addresses in order -> e->h_tab / e->d_tab
@@ -371,10 +367,10 @@ int SleepPipe::staged(bool packed) {
     std::vector<FileIO::Item> items;
     std::vector<size_t> slot_end;
     std::optional<FileIO> io;
-    if (file_fd >= 0) {
+    if (file) {
         for (const Batch& sl : slots) items.push_back(FileIO::Item{pages[sl.p0].off, sl.stored});
         items = FileIO::cut(e, items, &slot_end);
-        io.emplace(e, file_fd, true, file_direct, items, 0, file_path);
+        file->write(items, &io);
     }
     size_t k = 0, slots_written = 0;
     auto publish_written = [&]() -> int {   // units whose every page is in a slot that has been written are dead
@@ -504,10 +500,8 @@ struct SleepPlan {
     KernelTimes kt;
     uint32_t copy_ops = 0;
     double copy_s = 0;
-    FileFd file;                      // FILE tier: the file this sleep writes, opened by size_store
-    bool file_direct = false;
-    double file_t0 = 0;
-    SleepPlan(fma_engine_t* e, int t, uint32_t f) : tier(t), flags(f), timer{e}, kt{e} {}
+    ImageFile file;                   // FILE tier: the file this sleep writes, opened by size_store
+    SleepPlan(fma_engine_t* e, int t, uint32_t f) : tier(t), flags(f), timer{e}, kt{e}, file(e) {}
     bool adopt() const { return (flags & kFlagAdopt) || clean || !W; }  // not a byte moves (the route is then Adopt)
 };
 
@@ -699,58 +693,12 @@ int route_sleep(fma_engine_t* e, SleepPlan& p) {
     return FMA_OK;
 }
 
-}  // namespace
-
-int open_file_store(int fd, uint64_t bytes, const char* path) {
-    struct statvfs vs;
-    struct stat sb;
-    if (fstatvfs(fd, &vs) != 0 || fstat(fd, &sb) != 0) return fail(FMA_EIO, "fstatvfs(%s) failed: %s", path, strerror(errno));
-    const uint64_t need = bytes + kImageTail, room = (uint64_t)vs.f_bavail * vs.f_frsize + (uint64_t)sb.st_blocks * 512;  // (its own blocks come back)
-    if (room < need) return fail(FMA_EIO, "%s: %llu bytes free, the image needs %llu", path, (unsigned long long)room, (unsigned long long)need);
-    if (ftruncate(fd, 0) != 0) return fail(FMA_EIO, "ftruncate(%s) failed: %s", path, strerror(errno));
-    return FMA_OK;
-}
-
-int close_file_store(int fd, uint64_t bytes, const char* path, bool direct, const std::vector<char>& desc) {
-    if (fdatasync(fd) != 0) return fail(FMA_EIO, "fdatasync(%s) failed: %s", path, strerror(errno));
-    void* buf = nullptr;
-    if (desc.size() > kImageTail || posix_memalign(&buf, 4096, kImageTail) != 0) return fail(FMA_ENOMEM, "no memory for the descriptor");
-    memset(buf, 0, kImageTail);
-    memcpy(buf, desc.data(), desc.size());
-    uint64_t done = 0;
-    while (done < kImageTail) {
-        const ssize_t n = pwrite(fd, static_cast<char*>(buf) + done, kImageTail - done, (off_t)(bytes + done));
-        if (n < 0 && errno == EINTR) continue;
-        if (n <= 0) break;
-        done += (uint64_t)n;
-    }
-    const int err = errno;
-    free(buf);
-    if (done < kImageTail) return fail(FMA_EIO, "writing the descriptor of %s failed: %s", path, strerror(err));
-    if (fdatasync(fd) != 0) return fail(FMA_EIO, "fdatasync(%s) failed: %s", path, strerror(errno));
-    if (!direct) posix_fadvise(fd, 0, 0, POSIX_FADV_DONTNEED);   // clean now: the page cache lets go of the image
-    return FMA_OK;
-}
-
-namespace {
-
 // FILE: open the file, check that the filesystem has room for the image and its descriptor, and only then empty the file
 int open_sleep_file(fma_engine_t* e, SleepPlan& p) {
     if (e->file_path.empty()) return fail(FMA_ESTATE, "the file tier needs fma_file_store(path) first");
     if (!e->load_ring) return fail(FMA_ESTATE, "the engine's I/O windows are not pinned");
-    p.file_t0 = now_s();
-    RC(open_image_file(e->file_path.c_str(), true, &p.file.fd, &p.file_direct));
-    RC(open_file_store(p.file.fd, p.Wp, e->file_path.c_str()));
+    RC(p.file.create(e->file_path, p.Wp));
     e->image_file = e->file_path;
-    return FMA_OK;
-}
-
-// After the last write: the descriptor of the image the file now holds
-int close_sleep_file(fma_engine_t* e, SleepPlan& p) {
-    std::vector<char> desc;
-    RC(image_descriptor_build(e, FMA_TIER_FILE, &desc));
-    RC(close_file_store(p.file.fd, p.Wp, e->image_file.c_str(), p.file_direct, desc));
-    e->tl_add("file_io", p.file_direct ? 1 : 0, p.file_t0, now_s(), p.Wp + kImageTail);
     return FMA_OK;
 }
 
@@ -828,9 +776,7 @@ int run_pipeline(fma_engine_t* e, SleepPlan& p, Unmapper& un) {
         case SleepPipeKind::Staged: RC(pipe.staged(false)); break;
         case SleepPipeKind::File:
         case SleepPipeKind::FilePacked:
-            pipe.file_fd = p.file.fd;
-            pipe.file_direct = p.file_direct;
-            pipe.file_path = e->image_file.c_str();
+            pipe.file = &p.file;
             RC(pipe.staged(p.route.pipe == SleepPipeKind::FilePacked));
             break;
         case SleepPipeKind::NoRing:   // (refused by route_sleep)
@@ -870,7 +816,7 @@ int finish_sleep(fma_engine_t* e, SleepPlan& p, Unmapper& un, ApplyUnmapped& app
     }
     e->image_bytes = p.W;
     e->image_tier = p.tier;
-    if (p.file.fd >= 0) RC(close_sleep_file(e, p));   // (the image is asleep in the file either way: a wake reads what was written)
+    if (p.file.fd() >= 0) RC(p.file.seal(FMA_TIER_FILE));   // (the image is asleep in the file either way: a wake reads what was written)
 
     e->tl_add("total", 0, t_entry, now_s(), p.W_all);
     e->st.sleep_seconds = now_s() - t_entry;

@@ -326,25 +326,14 @@ int WakePipe::staged(bool packed) {
     PageKernels pk{e, kt, false, packed};
     RC(pk.prepare(pages, true, [&](size_t q) { return in_ring[q]; }));
     // FILE: every slot cut into window-sized reads; slot c's are items [slot_end[c - 1], slot_end[c])
-    const double t_io = now_s();
     std::vector<FileIO::Item> items;
     std::vector<size_t> slot_end;
-    uint64_t read_bytes = 0;
-    FileFd f;
-    bool direct = false;
+    ImageFile file(e);
     std::optional<FileIO> io;
     if (tier == FMA_TIER_FILE) {
-        for (const Batch& sl : slots) {
-            items.push_back(FileIO::Item{pages[sl.p0].off, sl.stored});
-            read_bytes += sl.stored;
-        }
+        for (const Batch& sl : slots) items.push_back(FileIO::Item{pages[sl.p0].off, sl.stored});
         items = FileIO::cut(e, items, &slot_end);
-        // the file must hold every byte this wake reads (else it was truncated or replaced): refused before a read is issued.
-        // The items ascend in image order, so the last one ends furthest into the file.
-        const uint64_t need = items.empty() ? 0 : items.back().file_off + items.back().bytes;
-        uint64_t file_bytes = 0;
-        RC(open_image_source(e->image_file.c_str(), need, &f.fd, &direct, &file_bytes));
-        io.emplace(e, f.fd, false, direct, items, file_bytes, e->image_file.c_str());   // the readers start now, ahead of the ring's mapping
+        RC(file.read(e->image_file, items, &io));   // the readers start now, ahead of the ring's mapping
     }
     if (ring_run) RC(mapper.wait(1));  // the ring is run 0 (1 GiB, ~0.2 ms to map): wait for it before the first H2D (else the route has the ring)
     size_t k = 0;
@@ -370,10 +359,7 @@ int WakePipe::staged(bool packed) {
         RT(cudaEventRecord(e->ev_ring_free[slot], e->ks));
         if (between) RC(between->pump(sl.p0 + sl.np, n_pages));
     }
-    if (io) {
-        RC(io->finish());   // every read has returned and every H2D out of a window has finished
-        e->tl_add("file_io", direct ? 1 : 0, t_io, now_s(), read_bytes);
-    }
+    if (io) RC(file.finish(*io));   // every read has returned and every H2D out of a window has finished
     return FMA_OK;
 }
 

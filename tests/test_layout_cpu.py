@@ -2,6 +2,7 @@
 split of the sleep / wake copy pipelines) is plain C++ in csrc/fma_layout.h and is what the engine (csrc/fma_engine.cu,
 fma_sleep.cu, fma_wake.cu) compiles in; exercised here on CPU with g++ (incl. a 20k-step randomised alloc/free invariant check)."""
 import os
+import re
 import subprocess
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -14,6 +15,22 @@ def test_layout_logic(tmp_path):
                            os.path.join(ROOT, "tests", "cpp", "layout_test.cpp"), "-o", exe])
     out = subprocess.check_output([exe], text=True)
     assert "layout ok" in out
+
+
+def test_image_operations_write_each_shared_step_once():
+    """The operations on a sleeping image (adoption from a memfd, a file or a parking buffer; move, verify, prefetch) and the
+    file tier's sleep and wake share one adoption path, one reader and writer of the image file and one store <-> HBM copy."""
+    csrc = os.path.join(ROOT, "llm-d-fast-model-actuation_b200", "csrc")
+    read = {f: open(os.path.join(csrc, f)).read() for f in sorted(os.listdir(csrc)) if f.endswith((".cu", ".h", ".cpp"))}
+    src, image = "".join(read.values()), read["fma_image.cu"]
+    for msg in ("the image holds different bytes than this engine's segments", "the image carries no digests to compare with",
+                "adopt needs a fully awake engine"):
+        assert image.count(msg) == 1, msg
+    assert src.count("cannot be handed over") == 1   # the resident share's hand-over refusal
+    for fn in ("open_image_source", "open_file_store", "close_file_store"):   # call sites, not the definition
+        assert len(re.findall(r"(?<!int )\b%s\(" % fn, src)) == 1, fn
+    assert src.count('tl_add("file_io"') == 1
+    assert image.count("direct_chunk(e)") == 1
 
 
 def test_engine_uses_the_tested_header():
