@@ -298,8 +298,9 @@ FMA_API int  fma_image_adopt_file(fma_engine_t* e, const char* path, uint64_t ta
  * Refusals leave the engine unchanged: FMA_ESTATE when nothing sleeps, a backed-up segment is mapped (a KEEP_BACKUP or partial
  * wake), part of the image is in a resident share, or the destination is not prepared; FMA_EINVAL for an unknown tier, the tier
  * the image is in (FILE -> FILE included) and PEER <-> LOCAL (there is one parking buffer).  A move that fails (FMA_EIO, FMA_ENOMEM,
- * FMA_ECUDA) leaves the image where it was: records and statistics unchanged, a host store or local buffer it created released, a
- * destination file emptied (never with a descriptor).  Only the engine's own streams and events are synchronised, so another
+ * FMA_ECUDA) leaves the image where it was: records and statistics unchanged, a host store or local buffer it created released, and
+ * the host store or parking buffer (a peer's or an attached one included) that it would have replaced kept, a destination file
+ * emptied (never with a descriptor).  A replaced store or buffer is released only once the move has succeeded.  Only the engine's own streams and events are synchronised, so another
  * engine of the process may serve meanwhile; host <-> file moves make no CUDA call beyond pinning a host store they create.  fma_timeline: op "move", rows file_io,
  * copies_landed (the copy engines ran) and total (bytes = image_store_bytes). */
 FMA_API int  fma_image_move(fma_engine_t* e, int tier);

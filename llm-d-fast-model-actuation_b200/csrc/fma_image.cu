@@ -301,6 +301,9 @@ struct MoveState {
     bool made_host = false;      // the host store, or the local parking buffer, was created by this move
     bool made_park = false;
     bool copies = false;         // the copy streams ran
+    HostStore old_host;          // what the created store or buffer replaces: released once the move has succeeded, kept if it fails
+    uint64_t old_host_bytes = 0;
+    ParkStore old_park;
 };
 
 int run_move(fma_engine_t* e, fma_layout::MovePipeKind pipe, int from, int to, MoveState& ms) {
@@ -309,22 +312,25 @@ int run_move(fma_engine_t* e, fma_layout::MovePipeKind pipe, int from, int to, M
     const bool park_side = pipe != MovePipeKind::HostFile && pipe != MovePipeKind::FileHost;
     ms.copies = park_side;
     // the destination, prepared as a sleep to its tier prepares it
+    // (a shared host store is read-only: its other holders keep it, and this engine takes a private one)
     if (to == FMA_TIER_HOST) {
-        if (e->host.shared) {   // the shared image is read-only: leave it to its other holders and take a private store
+        ms.made_host = e->host.shared || !e->host.base || e->host.cap < round_up(std::max<size_t>(bytes, FMA_PAGE_BYTES), FMA_PAGE_BYTES);
+        if (ms.made_host) {   // a store that does not fit holds nothing of this image, but it goes only once the move has succeeded
             invalidate_shadows(e);
-            host_store_free(e->host);
+            ms.old_host = e->host;
+            ms.old_host_bytes = e->st.host_store_bytes;
+            e->host = HostStore{};
             e->st.host_store_bytes = 0;
         }
-        ms.made_host = !e->host.base || e->host.cap < round_up(std::max<size_t>(bytes, FMA_PAGE_BYTES), FMA_PAGE_BYTES);
         RC(host_store_reserve(e, bytes));
     } else if (to == FMA_TIER_LOCAL) {
         const size_t need = round_up(std::max<size_t>(bytes, FMA_PAGE_BYTES), e->gran);
         ms.made_park = !(e->park.va && e->park.device == e->device && e->park.bytes >= need);
-        if (ms.made_park && e->park.va) {   // a buffer that does not fit, or a peer's (it holds nothing of this image), goes
-            if (e->shadow_tier == FMA_TIER_PEER || e->shadow_tier == FMA_TIER_LOCAL) invalidate_shadows(e);
-            vmm_buffer_free(e->park);
+        if (ms.made_park) {   // likewise a buffer that does not fit, or a peer's (an attached one included)
+            ms.old_park = e->park;
+            e->park = ParkStore{};
+            RC(park_store_create(e, e->device, need, &e->park));
         }
-        if (ms.made_park) RC(park_store_create(e, e->device, need, &e->park));
     }
     // the file side: the destination emptied once the filesystem has room; the source checked to hold the whole image.  A
     // parking buffer's bytes go through the engine's pinned I/O windows (the file tier's disk stage without the HBM ring).
@@ -361,14 +367,19 @@ int run_move(fma_engine_t* e, fma_layout::MovePipeKind pipe, int from, int to, M
     return FMA_OK;
 }
 
-// A failed move: nothing may still copy into what goes, what the move created goes, and a destination file keeps no descriptor
+// A failed move: nothing may still copy into what goes, what the move created goes (the store or buffer it replaced comes back),
+// and a destination file keeps no descriptor
 void undo_move(fma_engine_t* e, MoveState& ms) {
     if (ms.copies) drain(e);
-    if (ms.made_host) {
+    if (ms.made_host) {   // the store the engine had before, as it was
         host_store_free(e->host);
-        e->st.host_store_bytes = 0;
+        e->host = ms.old_host;
+        e->st.host_store_bytes = ms.old_host_bytes;
     }
-    if (ms.made_park) vmm_buffer_free(e->park);
+    if (ms.made_park) {
+        vmm_buffer_free(e->park);
+        e->park = ms.old_park;
+    }
     if (ms.file_emptied) {   // what was written goes too (best effort: without its descriptor the file is refused anyway)
         const int r = ftruncate(ms.file.fd(), 0);
         (void)r;
@@ -757,6 +768,8 @@ int fma_image_move(fma_engine_t* e, int tier) {
         for (Segment& s : e->segs)
             if (s.has_backup && !s.mapped) s.backup_tier = tier;
     }
+    host_store_free(ms.old_host);   // (what the new store or buffer replaced: nothing of the image was in it)
+    vmm_buffer_free(ms.old_park);
     e->image_tier = tier;
     if (tier == FMA_TIER_FILE) e->image_file = e->file_path;
     if (fma_layout::is_park_tier(tier)) prefetch_release(e);   // the whole image is in HBM now; host <-> file keeps the copy

@@ -13,7 +13,7 @@
 //   scripts/vmm_span_probe.py); memory lives until unmap even if the handle was released right after cuMemMap.
 // Streams execute eagerly (a copy has happened when cudaMemcpyAsync returns); events record wall-clock time.
 // Fault injection: the Nth cuMemCreate (hostsim_fail_create_after), large cudaMemcpyAsync (hostsim_fail_memcpy_after) or call
-// of a named VMM / stream / event function (hostsim_fail_call_after) from now fails as if the device were out of memory.
+// of a named VMM / stream / event / memset function (hostsim_fail_call_after) from now fails as if the device were out of memory.
 #include <cuda.h>
 #include <cuda_runtime.h>
 
@@ -259,7 +259,11 @@ cudaError_t cudaMemcpyAsync(void* d, const void* s, size_t n, cudaMemcpyKind, cu
     return cudaSuccess;
 }
 cudaError_t cudaMemcpy(void* d, const void* s, size_t n, cudaMemcpyKind) { memcpy(d, s, n); return cudaSuccess; }
-cudaError_t cudaMemsetAsync(void* d, int v, size_t n, cudaStream_t) { memset(d, v, n); return cudaSuccess; }
+cudaError_t cudaMemsetAsync(void* d, int v, size_t n, cudaStream_t) {
+    if (injected("cudaMemsetAsync")) return tl_last = cudaErrorLaunchFailure;   // (fma_image_verify clears its digest accumulators first)
+    memset(d, v, n);
+    return cudaSuccess;
+}
 cudaError_t cudaGetDriverEntryPoint(const char* name, void** fn, unsigned long long, cudaDriverEntryPointQueryResult* st) {
     struct { const char* n; void* f; } tab[] = {
         {"cuGetErrorString", (void*)simGetErrorString}, {"cuMemAddressReserve", (void*)simMemAddressReserve},

@@ -268,11 +268,21 @@ def test_move_to_a_file_that_cannot_be_written_leaves_the_image_in_place(built, 
 
 
 @gpu
-@pytest.mark.parametrize("dst", ["host", "local"])
+@pytest.mark.parametrize("dst", ["host", "local", "host_replacing", "local_replacing"])
 def test_move_from_a_truncated_file_fails_and_retries(engine, oracle, tmp_path, dst):
+    """*_replacing: the engine already has a host store or a local parking buffer too small for the image, from an earlier sleep
+    of one segment.  The failed move keeps it (found by a seeded history of tests/test_image_histories.py, seed 9 of its first
+    version: a failed move to the local tier released the parking buffer it would have replaced)."""
     L = _L()
     table, ptrs, ref = _load(engine, oracle, bf16=False)
     engine.set_option("load_chunk_bytes", 1 << 20)
+    name = dst.split("_")[0]
+    if dst.endswith("replacing"):
+        engine.sleep(["kv_cache"], tier=_tier(name))          # a store that fits 32 MiB of kv_cache, not the weights
+        engine.wake(None)
+        for i in ref:
+            engine.write(i, ref[i].tobytes())
+    before = engine.stats()
     path = str(tmp_path / "m.fmaimg")
     engine.file_store(path)
     engine.sleep(["weights"], tier=L.FMA_TIER_FILE, flags=L.FMA_FLAG_VERIFY)
@@ -280,14 +290,17 @@ def test_move_from_a_truncated_file_fails_and_retries(engine, oracle, tmp_path, 
     shutil.copyfile(path, keep)
     os.truncate(path, engine.stats()["image_store_bytes"] // 2 + 1000)
     with pytest.raises(L.FmaError) as ei:
-        engine.move_image(_tier(dst))
+        engine.move_image(_tier(name))
     assert ei.value.code == L.FMA_EIO
     _reports(engine, L.FMA_TIER_FILE)
     st = engine.stats()
-    assert st["host_store_bytes"] == 0 and st["parked_bytes"] == 0   # what the move created went with it
+    # what the move created went with it, and what it would have replaced is still there
+    assert (st["host_store_bytes"], st["parked_bytes"]) == (before["host_store_bytes"], before["parked_bytes"])
+    if dst.endswith("replacing"):
+        assert (st["host_store_bytes"] if name == "host" else st["parked_bytes"]) > 0
     shutil.copyfile(keep, path)
-    engine.move_image(_tier(dst))
-    _reports(engine, _tier(dst))
+    engine.move_image(_tier(name))
+    _reports(engine, _tier(name))
     engine.wake(None, flags=L.FMA_FLAG_VERIFY)
     _check_restored(engine, oracle, ptrs, ref)
 
