@@ -244,6 +244,33 @@ func (e *Engine) ImageAdoptFile(path string, tagMask uint64, flags uint32) error
 	return nil
 }
 
+// ImageFileInfo describes an image file from its descriptor tail alone (fma_image_file_info): no engine and no GPU are needed.
+type ImageFileInfo struct {
+	ImageBytes  uint64 // stored bytes in front of the descriptor
+	WeightBytes uint64 // bytes of the segments the image restores
+	Segments    int
+	Version     int
+	Packed      bool
+	Digests     bool // every segment carries a K3 digest
+	Tags        []string
+}
+
+// ReadImageFileInfo reads what the image file at `path` holds, without an engine.
+func ReadImageFileInfo(path string) (ImageFileInfo, error) {
+	cs := C.CString(path)
+	defer C.free(unsafe.Pointer(cs))
+	var out C.fma_image_file_info_t
+	if rc := C.fma_image_file_info(cs, &out); rc != 0 {
+		return ImageFileInfo{}, lastErr(rc)
+	}
+	info := ImageFileInfo{ImageBytes: uint64(out.image_bytes), WeightBytes: uint64(out.weight_bytes), Segments: int(out.n_segments),
+		Version: int(out.version), Packed: out.packed != 0, Digests: out.digests != 0}
+	for i := 0; i < int(out.n_tags); i++ {
+		info.Tags = append(info.Tags, C.GoString(&out.tags[i][0]))
+	}
+	return info, nil
+}
+
 // MoveImage moves the sleeping image to `tier` without waking it (host DRAM, a file named by FileStore, a peer's or this GPU's
 // parking buffer).  The source store stays allocated until HostRelease / PeerRelease; a source file is never touched.
 func (e *Engine) MoveImage(tier int) error {

@@ -57,6 +57,9 @@ extern "C" {
  * gather / scatter are page-table driven (K1/K2, csrc/fma_kernels.cu).                  */
 #define FMA_PAGE_BYTES  ((size_t)2u << 20)
 #define FMA_MAX_TAGS    64
+/* An image file or exported host store ends in its descriptor: the last FMA_IMAGE_TAIL_BYTES bytes (fma_image_export,
+ * fma_image_adopt_file, fma_image_file_info). */
+#define FMA_IMAGE_TAIL_BYTES ((size_t)2u << 20)
 
 /* ---- tiers ------------------------------------------------------------------------ */
 #define FMA_TIER_HOST   0   /* pinned host-DRAM store over PCIe Gen5 (copy engines)      */
@@ -278,6 +281,26 @@ FMA_API int  fma_file_store(fma_engine_t* e, const char* path);
  * else; the engine is then asleep in FMA_TIER_FILE and a wake streams the data from `path`.  A file whose descriptor does not
  * parse (torn, foreign) is refused with FMA_EINVAL and nothing touched. */
 FMA_API int  fma_image_adopt_file(fma_engine_t* e, const char* path, uint64_t tag_mask, uint32_t flags);
+/* What an image file holds, read from its descriptor tail alone: no engine, no driver and no CUDA call, so a node-level owner can
+ * judge a dead instance's image file (keep it for a warm start, or delete it) on any host.  The tail is read by the same parser
+ * every adoption uses.  Tags are reported by name, in image order of first appearance: tag ids belong to one engine
+ * (fma_tag_intern), so a caller that adopts the file interns these names in its own engine.
+ * Errors: FMA_EIO when the file cannot be opened or read, or is shorter than an image and its descriptor (including a file of at
+ * most FMA_IMAGE_TAIL_BYTES); FMA_EINVAL for a torn, foreign or malformed tail (what fma_image_adopt_file refuses before it looks
+ * at an engine). */
+typedef struct {
+    uint64_t image_bytes;         /* stored bytes in front of the descriptor (the PACKED form's pages back to back)       */
+    uint64_t weight_bytes;        /* bytes of the segments the image restores                                             */
+    uint32_t n_segments;
+    uint32_t version;             /* descriptor version: 1 plain, 2 PACKED                                                */
+    int32_t  packed;
+    int32_t  digests;             /* 1: every segment carries a K3 digest (a wake with FMA_FLAG_VERIFY checks them all)    */
+    uint32_t n_tags;
+    uint32_t reserved0;
+    char     tags[FMA_MAX_TAGS][32];   /* NUL-terminated names, n_tags of them                                            */
+    uint64_t reserved[4];
+} fma_image_file_info_t;
+FMA_API int  fma_image_file_info(const char* path, fma_image_file_info_t* out);
 
 /* ---- moving a sleeping image between tiers, without waking it ----------------------------------------------------------
  * A sleeper's tier is otherwise fixed at sleep time, and waking it to sleep again takes HBM that belongs to whoever serves on the

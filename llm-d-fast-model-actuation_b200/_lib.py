@@ -8,6 +8,7 @@ FMA_ABI_VERSION = 2
 FMA_PAGE_BYTES = 2 << 20
 FMA_PACKED_PAGE_BYTES = (3 << 19) + (16 << 10)   # stored size of a page in the "FMP4" code (csrc/fma_codec.h)
 FMA_MAX_TAGS = 64
+FMA_IMAGE_TAIL_BYTES = 2 << 20   # the descriptor at the end of an image file or exported host store
 
 FMA_OK, FMA_EINVAL, FMA_ENODRIVER, FMA_ECUDA, FMA_ENOMEM, FMA_ESTATE, FMA_ENOTFOUND, FMA_EINTEGRITY, FMA_EIO = (
     0, -1, -2, -3, -4, -5, -6, -7, -8)
@@ -80,6 +81,12 @@ class fma_load_stats_t(C.Structure):
 FMA_LOAD_O_DIRECT = 1
 
 
+class fma_image_file_info_t(C.Structure):
+    _fields_ = [("image_bytes", C.c_uint64), ("weight_bytes", C.c_uint64), ("n_segments", C.c_uint32), ("version", C.c_uint32),
+                ("packed", C.c_int32), ("digests", C.c_int32), ("n_tags", C.c_uint32), ("reserved0", C.c_uint32),
+                ("tags", (C.c_char * 32) * FMA_MAX_TAGS), ("reserved", C.c_uint64 * 4)]
+
+
 def lib_path() -> str:
     """Path of the in-tree shared library (built by ``__graft_entry__.build()`` / csrc/Makefile)."""
     return os.environ.get("FMA_B200_LIB") or os.path.join(os.path.dirname(os.path.abspath(__file__)), "libfma_b200.so")
@@ -138,6 +145,7 @@ _PROTOTYPES = {
     "fma_image_adopt": (C.c_int, [C.c_void_p, C.c_int, C.c_uint64, C.c_uint32]),
     "fma_file_store": (C.c_int, [C.c_void_p, C.c_char_p]),
     "fma_image_adopt_file": (C.c_int, [C.c_void_p, C.c_char_p, C.c_uint64, C.c_uint32]),
+    "fma_image_file_info": (C.c_int, [C.c_char_p, C.POINTER(fma_image_file_info_t)]),
     "fma_image_move": (C.c_int, [C.c_void_p, C.c_int]),
     "fma_image_verify": (C.c_int, [C.c_void_p, C.POINTER(C.c_int), C.c_int]),
     "fma_image_prefetch": (C.c_int, [C.c_void_p, C.c_uint64]),

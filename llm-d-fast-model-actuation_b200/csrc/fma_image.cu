@@ -62,19 +62,8 @@ int image_descriptor_build(fma_engine_t* e, int tier, std::vector<char>* out) {
     return FMA_OK;
 }
 
-namespace {
-
-// Parsed + validated descriptor, matched against the engine's segments for `tag_mask` (same order rule as fma_sleep).
-struct ParsedImage {
-    ImageHeader hd;
-    std::vector<ImageSegDesc> ds;
-    std::vector<size_t> order;          // engine segment index of descriptor entry i
-    std::vector<uint64_t> page_off;     // version 2: the PACKED image's page table
-    std::vector<uint32_t> page_bytes;
-};
-
-int image_descriptor_parse(fma_engine_t* e, const char* tail, size_t tail_bytes, size_t store_cap, uint64_t tag_mask, ParsedImage* out) {
-    ParsedImage& pi = *out;
+int image_descriptor_read(const char* tail, size_t tail_bytes, size_t store_cap, ImageDescriptor* out) {
+    ImageDescriptor& pi = *out;
     if (tail_bytes < sizeof(ImageHeader)) return fail(FMA_EINVAL, "image descriptor missing or corrupt");
     memcpy(&pi.hd, tail, sizeof(pi.hd));
     const ImageHeader& hd = pi.hd;
@@ -98,6 +87,29 @@ int image_descriptor_parse(fma_engine_t* e, const char* tail, size_t tail_bytes,
         }
         if (total > store_cap) return fail(FMA_EINVAL, "packed image: stored pages exceed the store");
     }
+    pi.ds.resize(hd.n_segments);
+    uint64_t off = 0;
+    for (size_t i = 0; i < pi.ds.size(); ++i) {
+        memcpy(&pi.ds[i], tail + sizeof(hd) + i * sizeof(ImageSegDesc), sizeof(ImageSegDesc));
+        if (pi.ds[i].tag_len >= sizeof(pi.ds[i].tag) || pi.ds[i].digest_valid > 1) return fail(FMA_EINVAL, "image descriptor is malformed (tag length / digest flag)");
+        if (pi.ds[i].packed_off != off || pi.ds[i].bytes > hd.image_bytes - off) return fail(FMA_EINVAL, "image descriptor is malformed (segment offsets)");
+        off += pi.ds[i].bytes;
+    }
+    if (off != hd.image_bytes) return fail(FMA_EINVAL, "image size mismatch");
+    return FMA_OK;
+}
+
+namespace {
+
+// A descriptor matched against the engine's segments for `tag_mask` (same order rule as fma_sleep).
+struct ParsedImage : ImageDescriptor {
+    std::vector<size_t> order;          // engine segment index of descriptor entry i
+};
+
+int image_descriptor_parse(fma_engine_t* e, const char* tail, size_t tail_bytes, size_t store_cap, uint64_t tag_mask, ParsedImage* out) {
+    ParsedImage& pi = *out;
+    RC(image_descriptor_read(tail, tail_bytes, store_cap, &pi));
+    const ImageHeader& hd = pi.hd;
     std::lock_guard<std::mutex> lk(e->mu);
     for (size_t i = 0; i < e->segs.size(); ++i)
         if (tag_bit_set(tag_mask, e->segs[i].tag)) pi.order.push_back(i);
@@ -106,13 +118,9 @@ int image_descriptor_parse(fma_engine_t* e, const char* tail, size_t tail_bytes,
         return x.arena != y.arena ? x.arena < y.arena : x.va < y.va;
     });
     if (pi.order.size() != hd.n_segments) return fail(FMA_EINVAL, "image and engine disagree on the number of segments");
-    pi.ds.resize(hd.n_segments);
     uint64_t off = 0;
     for (size_t i = 0; i < pi.ds.size(); ++i) {
-        memcpy(&pi.ds[i], tail + sizeof(hd) + i * sizeof(ImageSegDesc), sizeof(ImageSegDesc));
         const Segment& s = e->segs[pi.order[i]];
-        // the descriptor comes from a file or another process: bound what it claims before using it as a length
-        if (pi.ds[i].tag_len >= sizeof(pi.ds[i].tag) || pi.ds[i].digest_valid > 1) return fail(FMA_EINVAL, "image descriptor is malformed (tag length / digest flag)");
         if (pi.ds[i].bytes != s.bytes || pi.ds[i].packed_off != off || std::string(pi.ds[i].tag, pi.ds[i].tag_len) != e->tags[s.tag])
             return fail(FMA_EINVAL, "image and engine disagree on a segment's size, offset or tag");
         off += s.bytes;
@@ -691,18 +699,9 @@ int fma_image_adopt_file(fma_engine_t* e, const char* path, uint64_t tag_mask, u
     if (!path || !tag_mask) return fail(FMA_EINVAL, "adopt needs the file and the tag mask the image was slept with");
     RC(adopt_needs_awake(e));
     FileFd f;
-    f.fd = open(path, O_RDONLY | O_CLOEXEC);
-    if (f.fd < 0) return fail(FMA_EIO, "cannot open %s: %s", path, strerror(errno));
-    struct stat sb;
-    if (fstat(f.fd, &sb) != 0 || (size_t)sb.st_size <= kImageTail) return fail(FMA_EINVAL, "%s is not an image file", path);
-    const size_t cap = (size_t)sb.st_size - kImageTail;
-    std::vector<char> tail(kImageTail);
-    for (size_t got = 0; got < kImageTail;) {
-        const ssize_t n = pread(f.fd, tail.data() + got, kImageTail - got, (off_t)(cap + got));
-        if (n < 0 && errno == EINTR) continue;
-        if (n <= 0) return fail(FMA_EIO, "cannot read the descriptor of %s: %s", path, n < 0 ? strerror(errno) : "the file ends early");
-        got += (size_t)n;
-    }
+    size_t cap = 0;
+    std::vector<char> tail;
+    RC(ImageFile::read_tail(path, FMA_EINVAL, &f, &cap, &tail));
     RC(adopt(e, tail.data(), kImageTail, cap, tag_mask, flags, FMA_TIER_FILE, [&] {
         if (!e->load_ring) RC(ensure_io_windows(e));
         invalidate_shadows(e);

@@ -167,7 +167,7 @@ struct HostStore {
 
 // Descriptor of a packed image, stored in the last 2 MiB of a memfd-backed store (fma_image_export / fma_image_adopt).
 constexpr uint64_t kImageMagic = 0x31304d49414d46ull;  // "FMAIM01"
-constexpr size_t kImageTail = (size_t)2 << 20;
+constexpr size_t kImageTail = FMA_IMAGE_TAIL_BYTES;
 struct ImageSegDesc {
     uint64_t bytes;
     uint64_t packed_off;
@@ -449,6 +449,17 @@ inline HbmPart hbm_part(const fma_engine_t* e) {
 CUmemAllocationProp device_prop(int device);
 // ---- image descriptor (fma_image.cu): what a sleeping image is made of, so another engine / process can adopt it ----
 int image_descriptor_build(fma_engine_t* e, int tier, std::vector<char>* out);
+// A descriptor as its format defines it, before any engine is matched against it: header, one entry per segment and, for
+// version 2 (PACKED), the page table.
+struct ImageDescriptor {
+    ImageHeader hd;
+    std::vector<ImageSegDesc> ds;
+    std::vector<uint64_t> page_off;     // version 2: the PACKED image's page table
+    std::vector<uint32_t> page_bytes;
+};
+// Reads the descriptor in `tail` for a store of `store_cap` bytes.  It comes from a file or another process, so everything it
+// claims is bounded before it is used as a length.  Torn, foreign or malformed: FMA_EINVAL.  Every adoption parses through it.
+int image_descriptor_read(const char* tail, size_t tail_bytes, size_t store_cap, ImageDescriptor* out);
 void invalidate_shadows(fma_engine_t* e);   // the host store no longer holds a usable copy of any segment
 // ---- file I/O (fma_load.cu) ----
 int ensure_io_windows(fma_engine_t* e);   // pin the I/O windows for the current load_* options (and their events)
@@ -557,6 +568,9 @@ class ImageFile {
     // in the kImageTail bytes behind the image, then fdatasync again, so a torn file fails descriptor parsing; then the row.
     int seal(int tier);
     int fd() const { return file_.fd; }
+    // The kImageTail bytes at the end of the image file `path` (opened into *f): *store_cap is what lies before them.  No engine.
+    // Cannot open or read it: FMA_EIO; too short to hold a descriptor: `short_code`.
+    static int read_tail(const char* path, int short_code, FileFd* f, size_t* store_cap, std::vector<char>* tail);
 
   private:
     int row(uint64_t bytes);

@@ -140,6 +140,23 @@ int ImageFile::row(uint64_t bytes) {
     return FMA_OK;
 }
 
+int ImageFile::read_tail(const char* path, int short_code, FileFd* f, size_t* store_cap, std::vector<char>* tail) {
+    f->fd = open(path, O_RDONLY | O_CLOEXEC);
+    if (f->fd < 0) return fail(FMA_EIO, "cannot open %s: %s", path, strerror(errno));
+    struct stat sb;
+    if (fstat(f->fd, &sb) != 0) return fail(FMA_EIO, "fstat(%s) failed: %s", path, strerror(errno));
+    if ((size_t)sb.st_size <= kImageTail) return fail(short_code, "%s is not an image file: %llu bytes, no room for an image and its descriptor", path, (unsigned long long)sb.st_size);
+    *store_cap = (size_t)sb.st_size - kImageTail;
+    tail->assign(kImageTail, 0);
+    for (size_t got = 0; got < kImageTail;) {
+        const ssize_t n = pread(f->fd, tail->data() + got, kImageTail - got, (off_t)(*store_cap + got));
+        if (n < 0 && errno == EINTR) continue;
+        if (n <= 0) return fail(FMA_EIO, "cannot read the descriptor of %s: %s", path, n < 0 ? strerror(errno) : "the file ends early");
+        got += (size_t)n;
+    }
+    return FMA_OK;
+}
+
 std::vector<FileIO::Item> FileIO::cut(const fma_engine_t* e, const std::vector<Item>& ranges, std::vector<size_t>* ends) {
     const uint64_t piece = max_item(e);
     std::vector<Item> items;
@@ -299,6 +316,35 @@ int FileIO::finish() { return stop() == FMA_OK ? FMA_OK : fail(error_, "%s", msg
 using namespace fma_impl;
 
 extern "C" {
+
+int fma_image_file_info(const char* path, fma_image_file_info_t* out) {
+    if (!path || !out) return fail(FMA_EINVAL, "NULL path or out");
+    FileFd f;
+    size_t cap = 0;
+    std::vector<char> tail;
+    RC(ImageFile::read_tail(path, FMA_EIO, &f, &cap, &tail));   // a file that short cannot hold an image and its descriptor
+    ImageDescriptor d;
+    RC(image_descriptor_read(tail.data(), tail.size(), SIZE_MAX, &d));   // the store's size is checked below, as a short file
+    uint64_t stored = d.hd.image_bytes;
+    if (d.hd.version == 2) stored = d.page_off.empty() ? 0 : d.page_off.back() + d.page_bytes.back();
+    if (stored > cap)
+        return fail(FMA_EIO, "%s holds %zu bytes in front of its descriptor, the image needs %llu", path, cap, (unsigned long long)stored);
+    memset(out, 0, sizeof(*out));
+    out->image_bytes = stored;
+    out->weight_bytes = d.hd.image_bytes;
+    out->n_segments = d.hd.n_segments;
+    out->version = d.hd.version;
+    out->packed = d.hd.version == 2;
+    out->digests = d.ds.empty() ? 0 : 1;
+    for (const ImageSegDesc& s : d.ds) {
+        out->digests &= (int32_t)s.digest_valid;
+        const std::string tag(s.tag, s.tag_len);
+        uint32_t t = 0;
+        while (t < out->n_tags && tag != out->tags[t]) ++t;
+        if (t == out->n_tags && t < FMA_MAX_TAGS) memcpy(out->tags[out->n_tags++], tag.c_str(), tag.size() + 1);
+    }
+    return FMA_OK;
+}
 
 int fma_load_file(fma_engine_t* e, const char* path, const fma_load_span_t* spans, uint32_t n_spans, uint32_t flags,
                   fma_load_stats_t* out_stats) {

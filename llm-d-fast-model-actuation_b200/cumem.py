@@ -103,6 +103,7 @@ class CuMemAllocator:
         self.allocator_and_pools: dict[str, Any] = {}
         self._reserve_thread: threading.Thread | None = None
         self._file_path: str | None = None     # FMA_TIER=file: this rank's image file, once named
+        self._file_deposited = False           # FMA_DEPOSIT_FILE_IMAGE=1: the node agent holds a standing deposit of that file
         # MULTI-PATH wake across processes (FMA_REMOTE_PATHS=k): the node agent's helper GPUs pull for this instance; that needs the
         # host store as a memfd the agent can map, so the switch is thrown before the store is first reserved
         self._remote = None
@@ -160,9 +161,10 @@ class CuMemAllocator:
                     logger.warning("fma_b200: GPU %d cannot take %.2f GiB right now (%s): sleeping to the host tier instead", peer, nbytes / 1024**3, e.message)
                     tier = L.FMA_TIER_HOST
         elif tier == L.FMA_TIER_FILE and self._file_path is None:
+            # (also after adopting a kept file: that file is the node agent's and is only read, never written)
             self._file_path = _file_tier_path()
             self.engine.file_store(self._file_path)
-            atexit.register(_remove_file, self._file_path)
+            atexit.register(self._remove_own_file)
         deposit_host = (tier == L.FMA_TIER_HOST and os.environ.get("FMA_DEPOSIT_HOST_IMAGE") == "1" and os.environ.get("FMA_NODE_AGENT_SOCK")
                         and os.environ.get("FMA_HOST_STORE_SHM") == "1")
         if deposit_host:
@@ -171,7 +173,10 @@ class CuMemAllocator:
                 logger.warning("fma_b200: FMA_DEPOSIT_HOST_IMAGE=1 takes precedence over FMA_RESIDENT_MIB: the whole image goes to the host store")
             self.engine.set_option("resident_bytes", 0)
         try:
-            self.engine.sleep(offload_tags, tier=tier)
+            # a deposited image (file, or host memfd the node agent may spill to a kept file) is adopted by another process, whose
+            # wake checks it against these digests
+            deposits = deposit_host or (tier == L.FMA_TIER_FILE and _deposits_file())
+            self.engine.sleep(offload_tags, tier=tier, flags=L.FMA_FLAG_VERIFY if deposits else 0)
         except L.FmaError as e:
             # the file tier refused before releasing anything (no room on the disk, no HBM for its staging ring): the host tier works
             if tier != L.FMA_TIER_FILE or e.code not in (L.FMA_EIO, L.FMA_ENOMEM) or self.engine.is_sleeping():
@@ -187,6 +192,8 @@ class CuMemAllocator:
             from .parking import ParkingClient
 
             ParkingClient().deposit_host(self.engine, _instance_id(), _rank())
+        elif _deposits_file() and self.engine.stats()["tier"] == L.FMA_TIER_FILE and self.engine.stats()["sleep_bytes_copied"]:
+            self._deposit_file()
         st = self.engine.stats()
         total = st["sleep_bytes_offloaded"] + st["sleep_bytes_discarded"]
         # same INFO line the reference emits (cumem.py:215-222; parsed by llm-d-benchmark), plus GB/s
@@ -210,6 +217,15 @@ class CuMemAllocator:
                 self._remote.request_pull(self.engine, _instance_id(), _rank())
             except Exception as e:      # noqa: BLE001
                 logger.warning("fma_b200: pull request to the node agent failed (%s): waking over the own link only", e)
+        if self._file_deposited and (tags is None or "weights" in tags):
+            # the weights are about to serve, and may change: the file is no image to keep once this process exits
+            self._file_deposited = False
+            try:
+                from .parking import ParkingClient
+
+                ParkingClient().withdraw_file(_instance_id(), _rank())
+            except Exception as e:      # noqa: BLE001
+                logger.warning("fma_b200: cannot withdraw the image file from the node agent (%s)", e)
         self.engine.wake(tags)
         st = self.engine.stats()
         if st["wake_copy_seconds"] > 0:
@@ -225,7 +241,7 @@ class CuMemAllocator:
             if self._file_path is None:
                 self._file_path = _file_tier_path()
                 self.engine.file_store(self._file_path)
-                atexit.register(_remove_file, self._file_path)
+                atexit.register(self._remove_own_file)
             self.engine.move_image(L.FMA_TIER_FILE)
             self.engine.host_release()
         elif tier == "host":
@@ -299,8 +315,11 @@ class CuMemAllocator:
             logger.info("fma_b200: weights pool closed: %s", json.dumps({"segments": len(segs), "bytes": sum(sg.bytes for sg in segs),
                                                                           "first_mib": [sg.bytes >> 20 for sg in segs[:6]],
                                                                           "mib_histogram": {str(k): v for k, v in sorted(hist.items())}}))
+        adopted = False
         if tag == "weights" and os.environ.get("FMA_ADOPT_PARKED") == "1" and os.environ.get("FMA_NODE_AGENT_SOCK"):
-            self._adopt_parked_image()
+            adopted = self._adopt_parked_image()
+        if tag == "weights" and not adopted and os.environ.get("FMA_ADOPT_FILE") == "1" and os.environ.get("FMA_NODE_AGENT_SOCK"):
+            self._adopt_kept_file()
         if tag == "weights" and self._remote is None and int(os.environ.get("FMA_REMOTE_PATHS", "0") or 0) > 0 \
                 and os.environ.get("FMA_NODE_AGENT_SOCK") and _tier_from_env() == L.FMA_TIER_HOST:
             try:
@@ -315,7 +334,7 @@ class CuMemAllocator:
         if tag == "weights" and os.environ.get("FMA_PREPIN", "1") != "0" and _tier_from_env() == L.FMA_TIER_HOST:
             self._start_reserve()
 
-    def _adopt_parked_image(self) -> None:
+    def _adopt_parked_image(self) -> bool:
         """Warm start (SURVEY §8f-1): an earlier instance with this instance ID parked its weights with the node agent and died
         (or was deleted) asleep — the controller would cold-start here (inference-server.go:416-448).  The weights pool has just
         been filled by the loader (``--load-format dummy`` is enough: contents are about to be replaced); if the owner holds an image
@@ -331,16 +350,79 @@ class CuMemAllocator:
             if not cli.adopt(self.engine, _instance_id(), _rank(), tags=("weights",)) and \
                     not cli.adopt_host(self.engine, _instance_id(), _rank(), tags=("weights",)):
                 logger.info("fma_b200: no parked image for instance %s rank %d: keeping the loaded weights", _instance_id(), _rank())
-                return
+                return False
             self.engine.wake(["weights"], flags=L.FMA_FLAG_VERIFY)
             st = self.engine.stats()
             logger.info("fma_b200: adopted the parked image of instance %s rank %d: %.2f GiB restored from %s in %.3f s (digests verified)",
                         _instance_id(), _rank(), st["wake_bytes_restored"] / 1024**3, {L.FMA_TIER_HOST: "the host store", L.FMA_TIER_PEER: "peer HBM"}.get(st["tier"], f"tier {st['tier']}"),
                         time.perf_counter() - t0)
+            return True
         except L.FmaError as e:
             if self.engine.is_sleeping():
                 raise                                   # half way: do not serve from unmapped weights
             logger.warning("fma_b200: parked image not adopted (%s): keeping the loaded weights", e)
+            return False
+
+    def _adopt_kept_file(self) -> bool:
+        """Warm start from disk (FMA_ADOPT_FILE=1): an earlier instance with this instance ID slept to the file tier, deposited its
+        image file with the node agent and was deleted; the agent kept the file.  The weights pool has just been filled by the
+        loader (``--load-format dummy`` is enough): adopt the kept file and wake with its digests verified.  A miss or a refusal
+        before the wake (another segment sequence, an unreadable file) keeps the loaded weights; weights that fail their digests
+        raise, and the agent drops the file.  The kept file is only read: this rank's own file-tier sleeps write its own path."""
+        import time
+
+        from .parking import ParkingClient
+
+        t0 = time.perf_counter()
+        iid, rank = _instance_id(), _rank()
+        try:
+            cli = ParkingClient()
+            path = cli.lookup_file(iid, rank)
+        except (RuntimeError, OSError) as e:
+            logger.warning("fma_b200: cannot ask the node agent for a kept image file (%s): keeping the loaded weights", e)
+            return False
+        if path is None:
+            logger.info("fma_b200: no kept image file for instance %s rank %d: keeping the loaded weights", iid, rank)
+            return False
+        drop = False
+        try:
+            try:
+                self.engine.image_adopt_file(path, ("weights",))
+            except L.FmaError as e:
+                if self.engine.is_sleeping():
+                    raise
+                logger.warning("fma_b200: kept image file %s not adopted (%s): keeping the loaded weights", path, e)
+                return False
+            try:
+                self.engine.wake(["weights"], flags=L.FMA_FLAG_VERIFY)
+            except L.FmaError as e:
+                drop = e.code == L.FMA_EINTEGRITY       # never serve weights that failed their digests; the file goes
+                raise
+            st = self.engine.stats()
+            logger.info("fma_b200: adopted the kept image file of instance %s rank %d: %.2f GiB restored from %s in %.3f s (digests verified)",
+                        iid, rank, st["wake_bytes_restored"] / 1024**3, path, time.perf_counter() - t0)
+            return True
+        finally:
+            try:
+                cli.lookup_done(iid, rank, drop=drop)
+            except (RuntimeError, OSError) as e:
+                logger.warning("fma_b200: cannot end the lease on %s with the node agent (%s)", path, e)
+
+    def _deposit_file(self) -> None:
+        """FMA_DEPOSIT_FILE_IMAGE=1: the file this sleep wrote goes to the node agent, which keeps it if the process exits asleep.
+        If the agent cannot take it, the file is removed at exit as usual; the sleep itself never fails for that."""
+        from .parking import ParkingClient
+
+        try:
+            ParkingClient().deposit_file(_instance_id(), _rank(), self._file_path)
+            self._file_deposited = True
+        except (RuntimeError, OSError) as e:
+            logger.warning("fma_b200: cannot deposit %s with the node agent (%s): it is removed when this process exits", self._file_path, e)
+
+    def _remove_own_file(self) -> None:
+        """At exit: this rank's image file goes, unless a deposit with the node agent stands (the agent owns the file then)."""
+        if self._file_path is not None and not self._file_deposited:
+            _remove_file(self._file_path)
 
     # ---- pre-pinning off the critical path -----------------------------------------------
     def _start_reserve(self) -> None:
@@ -369,6 +451,11 @@ def _instance_id() -> str:
     """The controller's instance ID (``"I" + base64url(sha256(...)) + "i"``, inference-server.go:801-829): the node agent passes it to
     its children as FMA_INSTANCE_ID; a bare process falls back to its pid."""
     return os.environ.get("FMA_INSTANCE_ID") or f"pid{os.getpid()}"
+
+
+def _deposits_file() -> bool:
+    """FMA_DEPOSIT_FILE_IMAGE=1 (with FMA_TIER=file and a node agent): file-tier images are deposited with the agent."""
+    return os.environ.get("FMA_DEPOSIT_FILE_IMAGE") == "1" and bool(os.environ.get("FMA_NODE_AGENT_SOCK")) and _tier_from_env() == L.FMA_TIER_FILE
 
 
 def _rank() -> int:

@@ -342,6 +342,18 @@ class Engine:
         engine must hold the same segment sequence for ``tags``.  Reads only the descriptor; ``wake`` streams the data."""
         check(self._lib.fma_image_adopt_file(self._h, path.encode(), self.tag_mask(tags), flags))
 
+    @staticmethod
+    def image_file_info(path: str) -> dict:
+        """What the image file at ``path`` holds, from its descriptor tail alone (fma_image_file_info): no engine, no GPU.  Keys:
+        image_bytes (stored), weight_bytes, n_segments, version, packed, digests (every segment carries one) and tags (names).
+        Raises FmaError: FMA_EIO for a file that cannot be read or is shorter than its image, FMA_EINVAL for a torn or foreign
+        tail."""
+        lib = L.load_library()
+        out = L.fma_image_file_info_t()
+        check(lib.fma_image_file_info(path.encode(), C.byref(out)))
+        return {"image_bytes": out.image_bytes, "weight_bytes": out.weight_bytes, "n_segments": out.n_segments, "version": out.version,
+                "packed": bool(out.packed), "digests": bool(out.digests), "tags": [out.tags[i].value.decode() for i in range(out.n_tags)]}
+
     def move_image(self, tier: int) -> None:
         """Move the sleeping image to ``tier`` without waking it (fma_image_move): host DRAM, a file (``file_store`` first), a peer's
         parking buffer (``peer_reserve`` first) or this GPU's.  The source store stays allocated until ``host_release`` /

@@ -22,6 +22,7 @@ independent controller reconciles never do (SURVEY.md §3.4):
     GET  /v2/vllm/instances/{id}/is_sleeping
     POST /v2/node/swap {"sleep": idA, "wake": idB}     sleep(A) || wake(B): D2H of A and H2D of B on opposite PCIe directions
     GET  /v2/node/sleepers                             who sleeps where (for sleeper budgets)
+    GET  /v2/node/images                               images kept for dead instances: peer HBM, host DRAM, disk (parking.py)
 
 Design differences from the reference (this is not a port): instances are forked by a single-threaded *fork server*
 that has pre-imported the serving stack (the reference forks from its asyncio server process), exits are observed by
@@ -212,6 +213,11 @@ class NodeAgent:
             if self.parking is not None:   # the instance's allocator shim parks on buffers THIS process owns (parking.py)
                 extra_env["FMA_NODE_AGENT_SOCK"] = self.parking.sock_path
                 extra_env["FMA_INSTANCE_ID"] = instance_id
+                if self.parking.keep_dir:
+                    extra_env["FMA_KEEP_DIR"] = self.parking.keep_dir
+                    for var, n in (("FMA_KEEP_DISK_GIB", self.parking.keep_disk_bytes), ("FMA_KEEP_DRAM_GIB", self.parking.keep_dram_bytes)):
+                        if n is not None:
+                            extra_env[var] = str(n / (1 << 30))
             inst = _Instance(instance_id, cfg, self.log_dir)
             open(inst.log_path, "wb").close()
             inst.proc = self._ctx.Process(target=_child_main, args=(cfg.model_dump(exclude_none=True), inst.log_path, extra_env), daemon=False)
@@ -224,8 +230,18 @@ class NodeAgent:
         threading.Thread(target=self._wait_exit, args=(inst,), name=f"exit-{instance_id}", daemon=True).start()
         return result
 
+    def _exited(self, inst: _Instance) -> None:
+        """The instance's process is gone: the parking service settles the image files it deposited and the leases it held."""
+        if self.parking is not None:
+            try:
+                self.parking.instance_exited(inst.id)
+            except Exception as e:      # noqa: BLE001 — bookkeeping must not break the instance's lifecycle
+                logger.warning("exit hook of instance %s failed: %s", inst.id, e)
+
     def _wait_exit(self, inst: _Instance) -> None:
         inst.proc.join()
+        if not inst.deleting:
+            self._exited(inst)
         with self._lock:
             if inst.deleting or self._instances.get(inst.id) is not inst:
                 return                                                # a DELETE is reporting this exit
@@ -251,6 +267,7 @@ class NodeAgent:
                 except ProcessLookupError:
                     pass
                 inst.proc.join()
+        self._exited(inst)
         try:
             os.unlink(inst.log_path)
         except FileNotFoundError:
@@ -358,6 +375,12 @@ class NodeAgent:
             res.update(self.parking.stats())
         return res
 
+    def images(self) -> dict:
+        """Images kept for dead or future instances and the DRAM / disk budgets they count against (parking.py ``kept``)."""
+        if self.parking is None:
+            return {"images": [], "dram_bytes": 0, "dram_budget_bytes": None, "disk_bytes": 0, "disk_budget_bytes": None, "keep_dir": None}
+        return self.parking.kept()
+
 
 class LogRangeNotAvailable(Exception):
     def __init__(self, available: int):
@@ -408,7 +431,8 @@ def create_app(agent: NodeAgent) -> FastAPI:
                                            "watch_instances": "GET /v2/vllm/instances/watch",
                                            "sleep_instance": "POST /v2/vllm/instances/{instance_id}/sleep",
                                            "wake_instance": "POST /v2/vllm/instances/{instance_id}/wake_up",
-                                           "swap": "POST /v2/node/swap", "sleepers": "GET /v2/node/sleepers"}})
+                                           "swap": "POST /v2/node/swap", "sleepers": "GET /v2/node/sleepers",
+                                           "images": "GET /v2/node/images"}})
 
     @app.get("/v2/vllm/instances/watch")
     async def watch(since: Optional[int] = Query(None)):
@@ -523,7 +547,19 @@ def create_app(agent: NodeAgent) -> FastAPI:
     def sleepers():
         return JSONResponse(agent.sleepers())
 
+    @app.get("/v2/node/images")
+    def images():
+        return JSONResponse(agent.images())
+
     return app
+
+
+def keep_settings(env) -> dict:
+    """Kept image files (parking.py), opt-in: FMA_KEEP_DIR (default: ``kept`` under FMA_FILE_DIR, the children's file-tier directory,
+    so a kept file is a rename away), FMA_KEEP_DISK_GIB and FMA_KEEP_DRAM_GIB (unset: no bound)."""
+    keep_dir = env.get("FMA_KEEP_DIR") or (os.path.join(env["FMA_FILE_DIR"], "kept") if env.get("FMA_FILE_DIR") else None)
+    gib = lambda v: int(float(env[v]) * (1 << 30)) if env.get(v) else None    # noqa: E731
+    return {"keep_dir": keep_dir, "keep_disk_bytes": gib("FMA_KEEP_DISK_GIB"), "keep_dram_bytes": gib("FMA_KEEP_DRAM_GIB")}
 
 
 def main() -> None:
@@ -551,7 +587,7 @@ def main() -> None:
 
             pynvml.nvmlInit()
             n_dev = pynvml.nvmlDeviceGetCount()
-        parking = ParkingService(os.path.join(a.log_dir, f"fma_node_agent.{os.getpid()}.sock"), n_devices=n_dev)
+        parking = ParkingService(os.path.join(a.log_dir, f"fma_node_agent.{os.getpid()}.sock"), n_devices=n_dev, **keep_settings(os.environ))
         parking.start()
     agent = NodeAgent(mock_gpus=a.mock_gpus, log_dir=a.log_dir, parking=parking)
     uvicorn.run(create_app(agent), host=a.host, port=a.port, log_level=a.log_level)
