@@ -220,6 +220,30 @@ func (e *Engine) ImageAdoptParked(desc []byte, tagMask uint64) error {
 	return nil
 }
 
+// FlagWriteBehind makes a file-tier SleepFlags (or swap) return once the image is in the engine's host store: a background job
+// writes the file and then moves the image to the file tier (Writeback).  Ignored for other tiers.
+const FlagWriteBehind = uint32(C.FMA_FLAG_WRITE_BEHIND)
+
+// SleepFlags is Sleep with fma_sleep's flags (FMA_FLAG_VERIFY, FlagWriteBehind, ...).
+func (e *Engine) SleepFlags(offloadMask uint64, tier int, flags uint32) error {
+	if rc := C.fma_sleep(e.h, C.uint64_t(offloadMask), C.int(tier), C.uint32_t(flags)); rc != 0 {
+		return lastErr(rc)
+	}
+	return nil
+}
+
+// Writeback waits up to timeoutS seconds (0 polls, negative waits until it ends) for the last write-behind job: writing is true,
+// with the image bytes not yet written, while it writes; false once it committed, was pre-empted by another call, or none was
+// started.  A job whose write failed returns its error once; the image then still sleeps in the host tier.
+func (e *Engine) Writeback(timeoutS float64) (writing bool, pendingBytes uint64, err error) {
+	var pending C.uint64_t
+	rc := C.fma_image_writeback(e.h, C.double(timeoutS), &pending)
+	if rc < 0 {
+		return false, 0, lastErr(rc)
+	}
+	return rc == 1, uint64(pending), nil
+}
+
 // FileStore names the file the next file-tier sleep (Sleep(mask, C.FMA_TIER_FILE)) writes; "" forgets it.  The caller owns the file.
 func (e *Engine) FileStore(path string) error {
 	var cs *C.char

@@ -82,6 +82,8 @@ extern "C" {
 /* ---- flags for fma_sleep / fma_wake ----------------------------------------------- */
 #define FMA_FLAG_VERIFY   (1u << 0)  /* K3 digest before sleep, re-check after wake       */
 #define FMA_FLAG_KEEP_BACKUP (1u << 1) /* wake does not drop the backup (tests, re-wake)  */
+#define FMA_FLAG_WRITE_BEHIND (1u << 2) /* fma_sleep / fma_swap to FMA_TIER_FILE: sleep into the host store at PCIe speed and
+                                          write the file after the call returns (see fma_image_writeback); other tiers: ignored */
 
 typedef struct fma_engine fma_engine_t;
 
@@ -281,6 +283,35 @@ FMA_API int  fma_file_store(fma_engine_t* e, const char* path);
  * else; the engine is then asleep in FMA_TIER_FILE and a wake streams the data from `path`.  A file whose descriptor does not
  * parse (torn, foreign) is refused with FMA_EINVAL and nothing touched. */
 FMA_API int  fma_image_adopt_file(fma_engine_t* e, const char* path, uint64_t tag_mask, uint32_t flags);
+/* WRITE-BEHIND: a file-tier sleep whose time is not bound by the disk.  A file-tier sleep holds the GPU's HBM until its last pwrite
+ * has returned, so a hot swap's wake waits for the sleeper's disk.  With FMA_FLAG_WRITE_BEHIND a full file-tier sleep runs as a
+ * host-tier sleep (the STAGED pipeline, plain or PACKED) into the engine's pinned host store and returns at PCIe speed; a background
+ * job (one thread per engine) then pwrites the store to the fma_file_store file and seals it (fdatasync, descriptor, fdatasync) as
+ * fma_image_move(FMA_TIER_FILE) does.  Once the file is complete the job takes the operation lock and commits: every backed-up
+ * segment and fma_stats_t.tier report FMA_TIER_FILE, and the host store is released (after the lock, so a wake does not wait for
+ * its cudaHostUnregister + munmap) — the state fma_image_move(FMA_TIER_FILE) followed by fma_host_release leaves.
+ * Taken only when the engine already holds a private (not shared) host store of at least the image's stored bytes: one from
+ * fma_host_reserve, or kept from an earlier host-tier sleep or wake.  The sleep never pins one.  Otherwise, and for a sleep that
+ * writes nothing (a clean INCREMENTAL sleep), the sleep is the ordinary file-tier sleep and its timeline has a "wb_fallback" row
+ * whose idx says why: 1 no host store, 2 too small, 3 shared, 4 nothing to write.  The cost is a pinned image-sized store while
+ * awake and until the commit.  The free-space check and the file's creation come before anything is released (FMA_EIO, fully
+ * awake, as in the file tier); a sleep that fails otherwise fails as a host-tier sleep, and nothing is written behind it.
+ * Until the commit the image is a host-tier image in every respect (fma_stats_t.tier, fma_segment_info tier, host_store_bytes).
+ * Pre-emption: every call that takes the operation lock (sleep, wake, swap, move, verify, prefetch, export / describe / share,
+ * adoptions, host / peer reserve and release, paths, fma_file_store, fma_engine_destroy) first cancels a job still writing and
+ * joins it — waiting at most for the pwrite each writer has in flight (one load_chunk_bytes item) or an fdatasync — then sees the
+ * host-tier image: a wake during the write is a host-tier wake.  The file is emptied (it never carries a descriptor) and the store
+ * kept, so the next write-behind sleep reuses it.  A commit that loses the race for the lock is cancelled the same way, even with
+ * every byte written.  A job whose write fails leaves the image in the host tier and the store kept, empties the file and reports
+ * the error once, through fma_image_writeback.  fma_stats and fma_image_writeback do not pre-empt.
+ * Timeline: the sleep's host-tier rows and "wb_start"; at commit or cancel op "writeback" with rows file_io and total (idx 1
+ * committed, 0 cancelled; bytes written); a call that cancelled a job starts its own timeline with a "wb_cancel" row (how long the
+ * cancel took; its times are before the call's own entry). */
+/* Waits up to timeout_s (0: polls; a negative value waits as long as it takes) for the last write-behind job.  Returns 1 while it
+ * still writes (*out_pending_bytes, if given: the image bytes not yet written), 0 when none is pending (it committed, was
+ * cancelled, or none was started), or the negative code of a job that failed — once per failure, with fma_last_error set on
+ * the caller's thread. */
+FMA_API int  fma_image_writeback(fma_engine_t* e, double timeout_s, uint64_t* out_pending_bytes);
 /* What an image file holds, read from its descriptor tail alone: no engine, no driver and no CUDA call, so a node-level owner can
  * judge a dead instance's image file (keep it for a warm start, or delete it) on any host.  The tail is read by the same parser
  * every adoption uses.  Tags are reported by name, in image order of first appearance: tag ids belong to one engine

@@ -19,7 +19,7 @@ ERROR_NAMES = {
 FMA_TIER_HOST, FMA_TIER_PEER, FMA_TIER_LOCAL, FMA_TIER_FILE = 0, 1, 2, 3
 FMA_MODE_AUTO, FMA_MODE_DIRECT, FMA_MODE_STAGED, FMA_MODE_KERNEL = 0, 1, 2, 3
 FMA_KERNEL_TMA, FMA_KERNEL_LDG = 0, 1
-FMA_FLAG_VERIFY, FMA_FLAG_KEEP_BACKUP = 1, 2
+FMA_FLAG_VERIFY, FMA_FLAG_KEEP_BACKUP, FMA_FLAG_WRITE_BEHIND = 1, 2, 4
 NO_OFFSET = (1 << 64) - 1
 
 
@@ -145,6 +145,7 @@ _PROTOTYPES = {
     "fma_image_adopt": (C.c_int, [C.c_void_p, C.c_int, C.c_uint64, C.c_uint32]),
     "fma_file_store": (C.c_int, [C.c_void_p, C.c_char_p]),
     "fma_image_adopt_file": (C.c_int, [C.c_void_p, C.c_char_p, C.c_uint64, C.c_uint32]),
+    "fma_image_writeback": (C.c_int, [C.c_void_p, C.c_double, C.POINTER(C.c_uint64)]),
     "fma_image_file_info": (C.c_int, [C.c_char_p, C.POINTER(fma_image_file_info_t)]),
     "fma_image_move": (C.c_int, [C.c_void_p, C.c_int]),
     "fma_image_verify": (C.c_int, [C.c_void_p, C.POINTER(C.c_int), C.c_int]),

@@ -922,6 +922,8 @@ int fma_engine_destroy(fma_engine_t* e) {
         std::lock_guard<std::mutex> lk(g_current_mu);
         if (g_current == e) g_current = nullptr;
     }
+    { OpLock op(e); }    // a write-behind job still writing is cancelled (its file emptied) ...
+    writeback_join(e);   // ... and a committed one has freed its store
     DeviceGuard guard(e->device);
     cudaDeviceSynchronize();
     for (auto& kv : e->units) g_drv.MemUnmap(kv.second.va, kv.second.bytes);
@@ -1095,13 +1097,13 @@ uint64_t fma_current_usage(fma_engine_t* e) {
 // nothing left to do (idempotence, abstract.py:336-338).
 int fma_sleep(fma_engine_t* e, uint64_t offload_tag_mask, int tier, uint32_t flags) {
     if (check_engine(e) != FMA_OK) return FMA_EINVAL;
-    std::lock_guard<std::mutex> op(e->op_mu);
+    OpLock op(e);
     return do_sleep(e, offload_tag_mask, tier, flags);
 }
 
 int fma_wake(fma_engine_t* e, uint64_t tag_mask, uint32_t flags) {
     if (check_engine(e) != FMA_OK) return FMA_EINVAL;
-    std::lock_guard<std::mutex> op(e->op_mu);
+    OpLock op(e);
     return do_wake(e, tag_mask, flags);
 }
 
@@ -1148,13 +1150,13 @@ int fma_swap(fma_engine_t* out_e, uint64_t offload_tag_mask, int tier, fma_engin
     int rc_sleep = FMA_OK;
     char sleep_msg[512] = "";
     std::thread t([&] {
-        std::lock_guard<std::mutex> op(out_e->op_mu);
+        OpLock op(out_e);
         rc_sleep = do_sleep(out_e, offload_tag_mask, tier, flags);
         if (rc_sleep != FMA_OK) snprintf(sleep_msg, sizeof(sleep_msg), "%s", tl_err);
     });
     int rc_wake;
     {
-        std::lock_guard<std::mutex> op(in_e->op_mu);
+        OpLock op(in_e);
         rc_wake = do_wake(in_e, wake_tag_mask, flags);
     }
     t.join();
@@ -1168,7 +1170,7 @@ int fma_swap(fma_engine_t* out_e, uint64_t offload_tag_mask, int tier, fma_engin
 // only ever walked under e->mu (torch may be allocating the kv_cache pool on another thread at that moment).
 int fma_host_reserve(fma_engine_t* e, size_t bytes) {
     if (check_engine(e) != FMA_OK) return FMA_EINVAL;
-    std::lock_guard<std::mutex> op(e->op_mu);
+    OpLock op(e);
     if (e->host.cap < bytes && image_in(e, ImageIn::Host)) return fail(FMA_ESTATE, "cannot regrow the host store while it holds a sleeping image");
     DeviceGuard guard(e->device);
     return host_store_reserve(e, bytes);
@@ -1176,7 +1178,7 @@ int fma_host_reserve(fma_engine_t* e, size_t bytes) {
 
 int fma_host_release(fma_engine_t* e) {
     if (check_engine(e) != FMA_OK) return FMA_EINVAL;
-    std::lock_guard<std::mutex> op(e->op_mu);
+    OpLock op(e);
     if (image_in(e, ImageIn::Host)) return fail(FMA_ESTATE, "host store holds a sleeping image");
     DeviceGuard guard(e->device);
     cudaDeviceSynchronize();
@@ -1197,7 +1199,7 @@ int fma_host_store_view(fma_engine_t* e, const void** base, uint64_t* bytes) {
 
 int fma_peer_reserve(fma_engine_t* e, int peer_device, size_t bytes) {
     if (check_engine(e) != FMA_OK) return FMA_EINVAL;
-    std::lock_guard<std::mutex> op(e->op_mu);
+    OpLock op(e);
     if (image_in(e, ImageIn::NotHost)) return fail(FMA_ESTATE, "parking buffer holds a sleeping image");
     DeviceGuard guard(e->device);
     return park_reserve(e, peer_device, bytes);
@@ -1205,7 +1207,7 @@ int fma_peer_reserve(fma_engine_t* e, int peer_device, size_t bytes) {
 
 int fma_peer_release(fma_engine_t* e) {
     if (check_engine(e) != FMA_OK) return FMA_EINVAL;
-    std::lock_guard<std::mutex> op(e->op_mu);
+    OpLock op(e);
     if (image_in(e, ImageIn::NotHost)) return fail(FMA_ESTATE, "parking buffer holds a sleeping image");
     DeviceGuard guard(e->device);
     return park_release(e);
@@ -1283,7 +1285,7 @@ int fma_parking_destroy(uint64_t handle) {
 int fma_peer_attach(fma_engine_t* e, int fd, size_t bytes) {
     if (check_engine(e) != FMA_OK) return FMA_EINVAL;
     if (fd < 0 || bytes == 0 || bytes % FMA_PAGE_BYTES) return fail(FMA_EINVAL, "attach needs the owner's fd and the buffer's size (a multiple of 2 MiB)");
-    std::lock_guard<std::mutex> op(e->op_mu);
+    OpLock op(e);
     if (image_in(e, ImageIn::NotHost)) return fail(FMA_ESTATE, "parking buffer holds a sleeping image");
     DeviceGuard guard(e->device);
     RC(park_release(e));
@@ -1314,7 +1316,7 @@ static int replace_store_for_paths(fma_engine_t* e) {
 int fma_paths_set(fma_engine_t* e, const int* helper_devices, int n, size_t slot_bytes, int slots) {
     if (check_engine(e) != FMA_OK) return FMA_EINVAL;
     if (n < 0 || n > kMaxPaths - 1 || (n && !helper_devices)) return fail(FMA_EINVAL, "0..%d helper devices", kMaxPaths - 1);
-    std::lock_guard<std::mutex> op(e->op_mu);
+    OpLock op(e);
     DeviceGuard guard(e->device);
     cudaDeviceSynchronize();
     paths_release(e);
@@ -1641,9 +1643,9 @@ int fma_stats(fma_engine_t* e, fma_stats_t* out) {
         DeviceGuard guard(e->device);
         RC(flush_kernel_times(e));
     }
-    *out = e->st;
     {
-        std::lock_guard<std::mutex> lk(e->mu);
+        std::lock_guard<std::mutex> lk(e->mu);   // (a write-behind commit changes tier and host_store_bytes under it)
+        *out = e->st;
         uint64_t mapped = 0;
         for (const auto& kv : e->units) mapped += kv.second.bytes;
         out->hbm_mapped_bytes = mapped;

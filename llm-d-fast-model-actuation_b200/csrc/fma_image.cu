@@ -635,14 +635,187 @@ int prefetch_copy(fma_engine_t* e, const PrefetchPlan& p, char* dst) {
     });
 }
 
+// ---- WRITE-BEHIND: the file of a file-tier sleep written after the sleep returned (see include/fma_engine.h) ----------------
+
+// Under op_mu, once the file is complete: the image moves to the file tier as fma_image_move(FMA_TIER_FILE) moves it, and the host
+// store is detached for the job to free after the lock.  A descriptor that no longer describes the sleeping image (a segment freed
+// while the job wrote) is not committed.
+bool writeback_commit(fma_engine_t* e, const std::string& path, const std::vector<char>& desc, HostStore* detached) {
+    std::vector<char> now;
+    if (image_descriptor_build(e, FMA_TIER_HOST, &now) != FMA_OK || now != desc) return false;
+    {
+        std::lock_guard<std::mutex> lk(e->mu);   // (fma_segment_info and fma_stats read these without op_mu)
+        for (Segment& s : e->segs)
+            if (s.has_backup && !s.mapped) s.backup_tier = FMA_TIER_FILE;
+        e->st.tier = FMA_TIER_FILE;
+        e->st.host_store_bytes = 0;
+    }
+    e->image_tier = FMA_TIER_FILE;
+    e->image_file = path;
+    invalidate_shadows(e);   // (the copy a clean sleep may keep lay in the store the image left)
+    *detached = e->host;
+    e->host = HostStore{};
+    return true;
+}
+
+// The job's thread: the FileIO writers pwrite the store straight into the file, the descriptor seals it, and the commit takes op_mu
+// unless a call that holds it has cancelled the job meanwhile.  The file keeps no descriptor unless the image moved to it.
+void writeback_run(fma_engine_t* e, std::unique_ptr<ImageFile> file, std::vector<char> desc, std::vector<FileIO::Item> items, char* store,
+                   int item_delay_ms) {
+    WriteBehind& wb = e->wb;
+    cudaSetDevice(e->device);
+    auto cancelled = [&] {
+        std::lock_guard<std::mutex> lk(wb.mu);
+        return wb.cancel;
+    };
+    file->restart_clock();
+    std::optional<FileIO> io;
+    file->write(std::move(items), &io, store, item_delay_ms);
+    {
+        std::lock_guard<std::mutex> lk(wb.mu);
+        wb.io = &*io;
+        if (wb.cancel) io->cancel();
+    }
+    int rc = io->finish();   // every writer has left
+    {
+        std::lock_guard<std::mutex> lk(wb.mu);
+        wb.written = std::min<uint64_t>(io->written() * wb.piece, wb.bytes);
+        wb.io = nullptr;
+    }
+    io.reset();
+    if (rc == FMA_OK && !cancelled()) rc = file->seal_with(desc);
+    const double t_file = now_s();
+    char msg[512];
+    snprintf(msg, sizeof(msg), "write-behind of %.200s: %.280s", file->path().c_str(), tl_err);
+    bool locked = false;   // the commit's op_mu, or the cancel of the call that holds it
+    while (rc == FMA_OK && !locked) {
+        locked = e->op_mu.try_lock();
+        if (locked) break;
+        std::unique_lock<std::mutex> lk(wb.mu);
+        if (wb.cv.wait_for(lk, std::chrono::milliseconds(1), [&] { return wb.cancel; })) break;
+    }
+    HostStore detached;
+    bool committed = false;
+    if (locked) {
+        committed = writeback_commit(e, file->path(), desc, &detached);
+        DeviceGuard guard(e->device);
+        flush_kernel_times(e);   // (the sleep's kernel rows belong to the sleep's timeline)
+        e->tl_begin("writeback", wb.t_entry);
+        ImageFile::file_io_row(e, file->direct(), file->started(), t_file, wb.written + (committed ? kImageTail : 0));
+        e->tl_add("total", committed ? 1 : 0, wb.t_entry, now_s(), wb.written);
+    }
+    if (!committed) {   // cancelled or failed: what was written goes (without its descriptor the file is refused anyway)
+        const int r = ftruncate(file->fd(), 0);
+        (void)r;
+    }
+    {
+        std::lock_guard<std::mutex> lk(wb.mu);
+        wb.direct = file->direct();
+        wb.file_t0 = file->started();
+        wb.file_t1 = t_file;
+        if (committed) {
+            wb.state = WriteBehind::Committed;
+        } else if (rc != FMA_OK && rc != FileIO::kCancelled) {
+            wb.state = WriteBehind::Failed;
+            wb.error = rc;
+            wb.reported = false;
+            snprintf(wb.msg, sizeof(wb.msg), "%s", msg);
+        } else {
+            wb.state = WriteBehind::Cancelled;
+        }
+    }
+    wb.cv.notify_all();
+    if (locked) e->op_mu.unlock();
+    file.reset();
+    host_store_free(detached);   // after the lock: a wake does not wait for cudaHostUnregister + munmap
+    cudaGetLastError();
+}
+
 }  // namespace
+
+void writeback_join(fma_engine_t* e) {
+    if (e->wb.th.joinable()) e->wb.th.join();
+}
+
+void writeback_start(fma_engine_t* e, std::unique_ptr<ImageFile> file) {
+    WriteBehind& wb = e->wb;
+    writeback_join(e);   // a committed job may still be freeing its store
+    const uint64_t bytes = e->image_store_bytes;
+    std::vector<FileIO::Item> items = move_host_file(e, bytes);
+    std::vector<char> desc;   // built now, under op_mu: the job reads nothing of the engine's records
+    const int rc = image_descriptor_build(e, FMA_TIER_HOST, &desc);
+    std::lock_guard<std::mutex> lk(wb.mu);
+    wb.cancel = false;
+    wb.io = nullptr;
+    wb.bytes = bytes;
+    wb.piece = items.empty() ? 0 : items[0].bytes;
+    wb.written = 0;
+    wb.t_entry = now_s();
+    if (rc != FMA_OK) {   // the image stays in the host tier; the file, emptied by the sleep, stays empty
+        wb.state = WriteBehind::Failed;
+        wb.error = rc;
+        wb.reported = false;
+        snprintf(wb.msg, sizeof(wb.msg), "write-behind of %.200s: %.280s", file->path().c_str(), tl_err);
+        return;
+    }
+    wb.state = WriteBehind::Writing;
+    wb.error = FMA_OK;
+    wb.reported = true;
+    wb.th = std::thread(writeback_run, e, std::move(file), std::move(desc), std::move(items), static_cast<char*>(e->host.base),
+                        env_int("FMA_WB_ITEM_DELAY_MS", 0));
+}
+
+void writeback_preempt(fma_engine_t* e) {
+    WriteBehind& wb = e->wb;
+    {
+        std::lock_guard<std::mutex> lk(wb.mu);
+        if (wb.state != WriteBehind::Writing) return;
+        wb.cancel = true;
+        if (wb.io) wb.io->cancel();
+    }
+    wb.cv.notify_all();
+    const double t0 = now_s();
+    wb.th.join();   // at most the pwrite each writer has in flight, or an fdatasync
+    const double t1 = now_s();
+    if (wb.state != WriteBehind::Cancelled) return;   // (failed first: fma_image_writeback reports it)
+    DeviceGuard guard(e->device);
+    flush_kernel_times(e);
+    e->tl_begin("writeback", wb.t_entry);
+    ImageFile::file_io_row(e, wb.direct, wb.file_t0, wb.file_t1, wb.written);
+    e->tl_add("total", 0, wb.t_entry, t1, wb.written);
+    e->tl_add("wb_cancel", 0, t0, t1, wb.written);
+    e->tl_carry = true;   // the caller's own timeline, if it starts one, opens with this row
+    e->tl_carry_t0 = t0;
+    e->tl_carry_t1 = t1;
+    e->tl_carry_bytes = wb.written;
+}
+
 }  // namespace fma_impl
 
 extern "C" {
 
+int fma_image_writeback(fma_engine_t* e, double timeout_s, uint64_t* out_pending_bytes) {
+    if (check_engine(e) != FMA_OK) return FMA_EINVAL;
+    WriteBehind& wb = e->wb;
+    std::unique_lock<std::mutex> lk(wb.mu);
+    const auto settled = [&] { return wb.state != WriteBehind::Writing; };
+    if (timeout_s < 0 || std::isinf(timeout_s)) wb.cv.wait(lk, settled);
+    else if (timeout_s > 0) wb.cv.wait_for(lk, std::chrono::duration<double>(timeout_s), settled);
+    if (out_pending_bytes) *out_pending_bytes = 0;
+    if (wb.state == WriteBehind::Writing) {
+        if (out_pending_bytes) *out_pending_bytes = wb.bytes - (wb.io ? std::min<uint64_t>(wb.io->written() * wb.piece, wb.bytes) : wb.written);
+        return 1;
+    }
+    if (wb.state == WriteBehind::Failed && !wb.reported) {   // once per failure, on the caller's thread
+        wb.reported = true;
+        return fail(wb.error, "%s", wb.msg);
+    }
+    return FMA_OK;
+}
+
 int fma_image_export(fma_engine_t* e, int* out_fd) {
     if (check_engine(e) != FMA_OK) return FMA_EINVAL;
-    std::lock_guard<std::mutex> op(e->op_mu);
+    OpLock op(e);
     if (!out_fd) return fail(FMA_EINVAL, "out_fd is NULL");
     RC(refuse_resident_handover(e));
     if (e->image_tier == FMA_TIER_FILE && image_in(e, ImageIn::AnyAsleep)) return fail(FMA_ESTATE, "the sleeping image is in a file: the file itself is the hand-over");
@@ -661,7 +834,7 @@ int fma_image_export(fma_engine_t* e, int* out_fd) {
 
 int fma_image_adopt(fma_engine_t* e, int fd, uint64_t tag_mask, uint32_t flags) {
     if (check_engine(e) != FMA_OK) return FMA_EINVAL;
-    std::lock_guard<std::mutex> op(e->op_mu);
+    OpLock op(e);
     if (!tag_mask) return fail(FMA_EINVAL, "adopt needs the tag mask the image was slept with");
     RC(adopt_needs_awake(e));
     struct stat sb;
@@ -681,7 +854,7 @@ int fma_image_adopt(fma_engine_t* e, int fd, uint64_t tag_mask, uint32_t flags) 
 
 int fma_file_store(fma_engine_t* e, const char* path) {
     if (check_engine(e) != FMA_OK) return FMA_EINVAL;
-    std::lock_guard<std::mutex> op(e->op_mu);
+    OpLock op(e);
     if (!path) {
         e->file_path.clear();
         return FMA_OK;
@@ -695,7 +868,7 @@ int fma_file_store(fma_engine_t* e, const char* path) {
 
 int fma_image_adopt_file(fma_engine_t* e, const char* path, uint64_t tag_mask, uint32_t flags) {
     if (check_engine(e) != FMA_OK) return FMA_EINVAL;
-    std::lock_guard<std::mutex> op(e->op_mu);
+    OpLock op(e);
     if (!path || !tag_mask) return fail(FMA_EINVAL, "adopt needs the file and the tag mask the image was slept with");
     RC(adopt_needs_awake(e));
     FileFd f;
@@ -716,7 +889,7 @@ int fma_image_adopt_file(fma_engine_t* e, const char* path, uint64_t tag_mask, u
 
 int fma_image_describe(fma_engine_t* e, int tier, void* buf, size_t cap) {
     if (check_engine(e) != FMA_OK) return FMA_EINVAL;
-    std::lock_guard<std::mutex> op(e->op_mu);
+    OpLock op(e);
     RC(refuse_resident_handover(e));
     if (tier != e->image_tier) return fail(FMA_ESTATE, "no image sleeps in tier %d", tier);
     if (tier == FMA_TIER_FILE) return fail(FMA_ESTATE, "the sleeping image is in a file: the file itself is the hand-over (its descriptor is its tail)");
@@ -728,7 +901,7 @@ int fma_image_describe(fma_engine_t* e, int tier, void* buf, size_t cap) {
 
 int fma_image_adopt_parked(fma_engine_t* e, const void* desc, size_t desc_bytes, uint64_t tag_mask, uint32_t flags) {
     if (check_engine(e) != FMA_OK) return FMA_EINVAL;
-    std::lock_guard<std::mutex> op(e->op_mu);
+    OpLock op(e);
     if (!desc || !tag_mask) return fail(FMA_EINVAL, "adopt needs the descriptor and the tag mask the image was slept with");
     if (!e->park.va || e->park.device == e->device) return fail(FMA_ESTATE, "adopt_parked needs an attached / reserved peer parking buffer first");
     RC(adopt_needs_awake(e));
@@ -741,7 +914,7 @@ int fma_image_adopt_parked(fma_engine_t* e, const void* desc, size_t desc_bytes,
 // ---- moving a sleeping image to another tier (see include/fma_engine.h) -------------------------------------------------
 int fma_image_move(fma_engine_t* e, int tier) {
     if (check_engine(e) != FMA_OK) return FMA_EINVAL;
-    std::lock_guard<std::mutex> op(e->op_mu);
+    OpLock op(e);
     const int from = e->image_tier;
     fma_layout::MoveFacts facts{};
     sleep_state(e, &facts.asleep, &facts.backup_mapped);
@@ -782,7 +955,7 @@ int fma_image_move(fma_engine_t* e, int tier) {
 // ---- checking a sleeping image against its digests where it lies (see include/fma_engine.h) ------------------------------
 int fma_image_verify(fma_engine_t* e, int* out_bad, int cap) {
     if (check_engine(e) != FMA_OK) return FMA_EINVAL;
-    std::lock_guard<std::mutex> op(e->op_mu);
+    OpLock op(e);
     if (cap < 0 || (cap > 0 && !out_bad)) return fail(FMA_EINVAL, "out_bad is NULL or cap is negative");
     Verifier v(e);
     std::vector<size_t> main, res, pf;   // positions in v.segs: the image's own store, the resident share, the prefetched copy
@@ -824,7 +997,7 @@ int fma_image_verify(fma_engine_t* e, int* out_bad, int cap) {
 // ---- prefetching part of a sleeping image into HBM ahead of a wake (see include/fma_engine.h) ------------------------------
 int fma_image_prefetch(fma_engine_t* e, uint64_t bytes) {
     if (check_engine(e) != FMA_OK) return FMA_EINVAL;
-    std::lock_guard<std::mutex> op(e->op_mu);
+    OpLock op(e);
     DeviceGuard guard(e->device);
     if (!bytes) {   // the hand-back: nothing on the device reads the buffer between operations
         prefetch_release(e);

@@ -5,7 +5,8 @@
 //   fma_wake.cu     WAKE pipeline (do_wake)
 //   fma_load.cu     file I/O: reader / writer threads over the pinned I/O windows (cold load fma_load_file, FILE tier)
 //   fma_image.cu    image hand-over between engines / processes (fma_image_export / fma_image_adopt), moves between tiers (fma_image_move),
-//                  checks in place (fma_image_verify), prefetch into HBM (fma_image_prefetch)
+//                  checks in place (fma_image_verify), prefetch into HBM (fma_image_prefetch), the write-behind job of a file-tier sleep
+//                  (fma_image_writeback)
 //
 // Everything below lives in namespace fma_impl; the library is built with -fvisibility=hidden, so none of it is exported.
 #pragma once
@@ -14,6 +15,7 @@
 
 #include <algorithm>
 #include <cctype>
+#include <cmath>
 #include <atomic>
 #include <chrono>
 #include <condition_variable>
@@ -25,6 +27,7 @@
 #include <initializer_list>
 #include <iterator>
 #include <map>
+#include <memory>
 #include <mutex>
 #include <optional>
 #include <string>
@@ -225,6 +228,30 @@ struct TimelineEv {
     uint64_t bytes;
 };
 
+class FileIO;
+
+// WRITE-BEHIND (FMA_FLAG_WRITE_BEHIND): the background job that writes a file-tier sleep's image from the host store to its file
+// after the sleep returned (fma_image.cu).  One per engine.  It holds no op_mu while it writes: every call that takes op_mu first
+// cancels a job still writing and joins it (OpLock), and the job takes op_mu only to commit, giving up when a call cancels it.
+struct WriteBehind {
+    enum State { Idle, Writing, Committed, Cancelled, Failed };
+    std::mutex mu;                    // guards everything below but `th`
+    std::condition_variable cv;       // `cancel` was set
+    std::thread th;                   // joined by a pre-emption while Writing, else by the next job or fma_engine_destroy (a
+                                      // committed job may still be freeing the store it detached)
+    State state = Idle;
+    bool cancel = false;
+    bool reported = true;             // a failure has been returned by fma_image_writeback
+    int error = 0;                    // FMA_OK, or the failed job's code and message
+    char msg[512] = "";
+    FileIO* io = nullptr;             // the writers, while they run
+    uint64_t bytes = 0, piece = 0;    // the image's stored bytes; the bytes of one write item (the last may be shorter)
+    uint64_t written = 0;             // image bytes written, once the writers have finished
+    double t_entry = 0;               // the job's start: the origin of its "writeback" timeline
+    double file_t0 = 0, file_t1 = 0;  // its "file_io" row (idx: `direct`), for the call that cancels it
+    bool direct = false;
+};
+
 }  // namespace fma_impl
 
 using namespace fma_impl;  // internal header: only the engine's own translation units include it
@@ -332,6 +359,7 @@ struct fma_engine {
     // FILE tier
     std::string file_path;               // fma_file_store: where the next file-tier sleep writes ("" = nowhere)
     std::string image_file;              // the file the last file-tier image was written to / adopted from (read by the wake)
+    WriteBehind wb;                      // WRITE-BEHIND: the job that writes a host-tier image to file_path after its sleep
 
     fma_k_tma_cfg tma = fma_k_default_tma_cfg();
     fma_stats_t st{};
@@ -346,6 +374,10 @@ struct fma_engine {
     char tl_op[16] = "";
     double tl_entry = 0;               // now_s() at the operation's entry
     double tl_dev_base = 0;            // host time (since entry) at which ev_start was recorded: origin of the device-side events
+    // the "wb_cancel" row of the pre-emption that opened the current call (OpLock): its timeline starts with it
+    bool tl_carry = false;
+    double tl_carry_t0 = 0, tl_carry_t1 = 0;
+    uint64_t tl_carry_bytes = 0;
     void tl_begin(const char* op, double t_entry) {
         std::lock_guard<std::mutex> lk(tl_mu);
         tl.clear();
@@ -354,6 +386,7 @@ struct fma_engine {
         snprintf(tl_op, sizeof(tl_op), "%s", op);
         tl_entry = t_entry;
         tl_dev_base = 0;
+        if (tl_carry) tl.push_back(TimelineEv{"wb_cancel", 0, tl_carry_t0 - t_entry, tl_carry_t1 - t_entry, tl_carry_bytes});
     }
     void tl_add(const char* kind, int idx, double t0_abs, double t1_abs, uint64_t bytes) {
         std::lock_guard<std::mutex> lk(tl_mu);
@@ -488,8 +521,14 @@ class FileIO {
     static uint64_t max_item(const fma_engine_t* e) { return e->io_window_bytes - 8192; }
     // `ranges` cut into items of at most one window each, in order; (*ends)[r]: one past the last item of range r
     static std::vector<Item> cut(const fma_engine_t* e, const std::vector<Item>& ranges, std::vector<size_t>* ends = nullptr);
-    FileIO(fma_engine_t* e, int fd, bool write, bool direct, std::vector<Item> items, uint64_t file_bytes, const char* path, char* mem = nullptr);
+    // item_delay_ms: each thread waits that long before each item (FMA_WB_ITEM_DELAY_MS, a test knob of the write-behind job);
+    // cancel() ends the wait
+    FileIO(fma_engine_t* e, int fd, bool write, bool direct, std::vector<Item> items, uint64_t file_bytes, const char* path, char* mem = nullptr,
+           int item_delay_ms = 0);
     ~FileIO();
+    static constexpr int kCancelled = 1;   // the error of a cancelled I/O (never returned by the C-ABI)
+    // The threads leave after the item each is doing (with `mem`; the write-behind job); finish() then returns kCancelled
+    void cancel() { set_error(kCancelled, "file I/O of %s was cancelled", path_); }
     int copy(size_t k, void* dev, cudaStream_t stream);   // FMA_OK, a CUDA error, or (the I/O failed) finish()'s error
     // read: copy() without the copy.  enqueue(window) puts work on `stream` that reads item k in place in its pinned window (a
     // kernel reading it over the link, fma_image_verify), and the window is handed back behind that work.
@@ -536,6 +575,7 @@ class FileIO {
     const char* path_;
     char* mem_;
     int n_;
+    int item_delay_ms_;
     std::mutex mu_;
     std::condition_variable cv_;
     std::vector<char> ready_, posted_, done_;   // read: item read; both: copy enqueued; write: pwrite returned
@@ -561,16 +601,25 @@ class ImageFile {
     // Opens `path` (created if need be) to write an image of `bytes`, and empties it only once its filesystem has room for the
     // image and its descriptor (fstatvfs).  Short of room, the file is left untouched.
     int create(const std::string& path, uint64_t bytes);
-    void write(std::vector<FileIO::Item> items, std::optional<FileIO>* io, char* mem = nullptr);   // *io's writers of `items`
+    void write(std::vector<FileIO::Item> items, std::optional<FileIO>* io, char* mem = nullptr, int item_delay_ms = 0);   // *io's writers of `items`
     // Read: every read has returned and every copy out of a window has finished (io.finish()), then the row.
     int finish(FileIO& io);
     // Write, after the last item: fdatasync, then the descriptor of the image sleeping in `tier`'s store (image_descriptor_build)
     // in the kImageTail bytes behind the image, then fdatasync again, so a torn file fails descriptor parsing; then the row.
     int seal(int tier);
+    // The same with a descriptor built before, and no row: the write-behind job writes the file outside the operation lock and
+    // records its row at the end (restart_clock: the row starts when its write does, after the sleep that created the file)
+    int seal_with(const std::vector<char>& desc);
+    void restart_clock() { t0_ = now_s(); }
+    double started() const { return t0_; }
+    bool direct() const { return direct_; }
     int fd() const { return file_.fd; }
+    const std::string& path() const { return path_; }
     // The kImageTail bytes at the end of the image file `path` (opened into *f): *store_cap is what lies before them.  No engine.
     // Cannot open or read it: FMA_EIO; too short to hold a descriptor: `short_code`.
     static int read_tail(const char* path, int short_code, FileFd* f, size_t* store_cap, std::vector<char>* tail);
+    // The "file_io" timeline row (idx 1 with O_DIRECT) of an I/O over [t0, t1): the write-behind job records its own at its end
+    static void file_io_row(fma_engine_t* e, bool direct, double t0, double t1, uint64_t bytes);
 
   private:
     int row(uint64_t bytes);
@@ -580,6 +629,23 @@ class ImageFile {
     bool direct_ = false;
     double t0_ = 0;
     uint64_t bytes_ = 0;   // read: every item's; write: the image's
+};
+
+// ---- WRITE-BEHIND (fma_image.cu) ----
+// Starts the job that writes the host-tier image a write-behind sleep just made to `file` (created and emptied by that sleep) and,
+// once every byte and the descriptor are on disk, moves the image to the file tier (caller: that sleep, under op_mu).
+void writeback_start(fma_engine_t* e, std::unique_ptr<ImageFile> file);
+// A job still writing is cancelled and joined (caller holds op_mu): its file is emptied, its store stays the engine's host store,
+// and the caller sees an ordinary host-tier image.  The time it took becomes a "wb_cancel" row.
+void writeback_preempt(fma_engine_t* e);
+void writeback_join(fma_engine_t* e);   // whatever the job's state, its thread has ended (the next job, fma_engine_destroy)
+
+// One sleep / wake / swap / image or store operation per engine at a time, and a write-behind job still writing pre-empted first
+struct OpLock {
+    fma_engine_t* e;
+    std::lock_guard<std::mutex> lk;
+    explicit OpLock(fma_engine_t* eng) : e(eng), lk(eng->op_mu) { writeback_preempt(e); }
+    ~OpLock() { e->tl_carry = false; }
 };
 
 // ---- pipelines ----

@@ -268,21 +268,47 @@ struct SleepFacts {
     // are re-coded in place (PACKED image: their stored sizes held, and a staging ring was had for them)
     bool clean, partial, partial_packed;
     bool multipath_env, ring = true, worth_packing = true;  // FMA_MULTIPATH_SLEEP; a staging ring is available; K4p found it worth packing
+    // WRITE-BEHIND (FMA_FLAG_WRITE_BEHIND, file tier only): the sleep fills the engine's host store and a job writes the file later
+    bool write_behind = false;        // the flag was passed
+    bool host_store = false, store_shared = false;   // the engine holds a host store; somebody else may hold it too (read-only)
+    uint64_t store_cap = 0, stored = 0;              // its capacity; the image's stored bytes (plain size until K4p has run)
 };
+
+// Why a write-behind sleep was not taken (the timeline's "wb_fallback" row carries it as idx); 0: taken, or not asked for
+enum WbFallback { kWbTaken = 0, kWbNoStore = 1, kWbSmallStore = 2, kWbSharedStore = 3, kWbNothingToWrite = 4 };
+
 struct SleepRoute {
     SleepPipeKind pipe;
     int mode;                  // what fma_stats_t.mode reports
     bool wants_ring, wants_probe;  // `ring` / `worth_packing` decide the pipe
+    bool write_behind = false;     // a file-tier sleep that runs as a host-tier sleep into the host store (pipe Staged / StagedPacked)
+    int wb_fallback = kWbTaken;    // asked for write-behind and not taken: why
 };
 
+// The host store a write-behind sleep fills is one the engine already holds: private, and big enough for the stored image.  The
+// engine never pins a store inside a sleep.  A sleep that writes nothing (adopted, clean INCREMENTAL) keeps its path.
+inline int write_behind_fallback(const SleepFacts& f) {
+    if (f.adopt || f.clean || f.partial || f.partial_packed) return kWbNothingToWrite;
+    if (!f.host_store) return kWbNoStore;
+    if (f.store_shared) return kWbSharedStore;
+    if (f.store_cap < f.stored) return kWbSmallStore;
+    return kWbTaken;
+}
+
 inline SleepRoute sleep_route(const SleepFacts& f) {
-    if (f.adopt || f.clean) return SleepRoute{SleepPipeKind::Adopt, f.mode, false, false};
+    const bool wb_asked = f.write_behind && f.tier == FMA_TIER_FILE;   // (ignored for the other tiers)
+    const int wb_why = wb_asked ? write_behind_fallback(f) : kWbTaken;
+    if (f.adopt || f.clean) return SleepRoute{SleepPipeKind::Adopt, f.mode, false, false, false, wb_why};
     if (f.partial_packed) return SleepRoute{SleepPipeKind::PartialPacked, f.mode, false, false};
     if (f.partial) return SleepRoute{SleepPipeKind::PartialDirect, FMA_MODE_DIRECT, false, false};
-    // FILE: the ring-staged pipeline with a disk stage behind it, PACKED when asked and worth it; without a ring nothing moves
+    // FILE: the ring-staged pipeline with a disk stage behind it, PACKED when asked and worth it; without a ring nothing moves.
+    // WRITE-BEHIND: the host tier's ring-staged pipeline into the host store, under the same ring and PACKED rules
     if (f.tier == FMA_TIER_FILE) {
-        const SleepPipeKind k = !f.ring ? SleepPipeKind::NoRing : f.pack && f.worth_packing ? SleepPipeKind::FilePacked : SleepPipeKind::File;
-        return SleepRoute{k, FMA_MODE_STAGED, true, f.pack};
+        const bool packed = f.pack && f.worth_packing, wb = wb_asked && wb_why == kWbTaken;
+        const SleepPipeKind k = !f.ring ? SleepPipeKind::NoRing
+                              : wb      ? (packed ? SleepPipeKind::StagedPacked : SleepPipeKind::Staged)
+                                        : (packed ? SleepPipeKind::FilePacked : SleepPipeKind::File);
+        return SleepRoute{k, FMA_MODE_STAGED, true, f.pack, wb && f.ring, wb_why};
     }
     SleepRoute r{SleepPipeKind::Staged, f.mode, false, false};
     // MULTI-PATH: a full, plain host-tier sleep is striped over the paths' links, each with its own staging slots

@@ -119,8 +119,8 @@ int ImageFile::create(const std::string& path, uint64_t bytes) {
     return open_file_store(file_.fd, bytes, path_.c_str());
 }
 
-void ImageFile::write(std::vector<FileIO::Item> items, std::optional<FileIO>* io, char* mem) {
-    io->emplace(e_, file_.fd, true, direct_, std::move(items), 0, path_.c_str(), mem);
+void ImageFile::write(std::vector<FileIO::Item> items, std::optional<FileIO>* io, char* mem, int item_delay_ms) {
+    io->emplace(e_, file_.fd, true, direct_, std::move(items), 0, path_.c_str(), mem, item_delay_ms);
 }
 
 int ImageFile::finish(FileIO& io) {
@@ -131,14 +131,18 @@ int ImageFile::finish(FileIO& io) {
 int ImageFile::seal(int tier) {
     std::vector<char> desc;
     RC(image_descriptor_build(e_, tier, &desc));
-    RC(close_file_store(file_.fd, bytes_, path_.c_str(), direct_, desc));
+    RC(seal_with(desc));
     return row(bytes_ + kImageTail);
 }
 
+int ImageFile::seal_with(const std::vector<char>& desc) { return close_file_store(file_.fd, bytes_, path_.c_str(), direct_, desc); }
+
 int ImageFile::row(uint64_t bytes) {
-    e_->tl_add("file_io", direct_ ? 1 : 0, t0_, now_s(), bytes);
+    file_io_row(e_, direct_, t0_, now_s(), bytes);
     return FMA_OK;
 }
+
+void ImageFile::file_io_row(fma_engine_t* e, bool direct, double t0, double t1, uint64_t bytes) { e->tl_add("file_io", direct ? 1 : 0, t0, t1, bytes); }
 
 int ImageFile::read_tail(const char* path, int short_code, FileFd* f, size_t* store_cap, std::vector<char>* tail) {
     f->fd = open(path, O_RDONLY | O_CLOEXEC);
@@ -167,9 +171,10 @@ std::vector<FileIO::Item> FileIO::cut(const fma_engine_t* e, const std::vector<I
     return items;
 }
 
-FileIO::FileIO(fma_engine_t* e, int fd, bool write, bool direct, std::vector<Item> items, uint64_t file_bytes, const char* path, char* mem)
+FileIO::FileIO(fma_engine_t* e, int fd, bool write, bool direct, std::vector<Item> items, uint64_t file_bytes, const char* path, char* mem,
+               int item_delay_ms)
     : e_(e), fd_(fd), write_(write), direct_(direct), items_(std::move(items)), file_bytes_(file_bytes), path_(path), mem_(mem), n_(e->io_windows),
-      ready_(items_.size(), 0), posted_(items_.size(), mem ? 1 : 0), done_(items_.size(), 0) {
+      item_delay_ms_(item_delay_ms), ready_(items_.size(), 0), posted_(items_.size(), mem ? 1 : 0), done_(items_.size(), 0) {
     if (mem_) {   // nothing is copied into or out of a window: every item is "posted" from the start
         n_posted_items_ = items_.size();
         for (const Item& it : items_)
@@ -226,8 +231,9 @@ void FileIO::worker() {
             }
             abuf = window(k);
         } else {
-            std::lock_guard<std::mutex> lk(mu_);
-            if (error_ != FMA_OK) break;   // another item failed: the I/O stops
+            std::unique_lock<std::mutex> lk(mu_);
+            if (item_delay_ms_ > 0) cv_.wait_for(lk, std::chrono::milliseconds(item_delay_ms_), [&] { return error_ != FMA_OK; });
+            if (error_ != FMA_OK) break;   // another item failed, or the I/O was cancelled: it stops
         }
         const double t0 = now_s();
         uint64_t done = 0;

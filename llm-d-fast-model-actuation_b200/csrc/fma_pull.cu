@@ -299,7 +299,7 @@ int fma_paths_attach(fma_engine_t* e, const int* staging_fds, int n, size_t slot
     if (check_engine(e) != FMA_OK) return FMA_EINVAL;
     if (n < 1 || n > (int)kPullMaxPaths - 1 || !staging_fds || !out_mailbox_fd) return fail(FMA_EINVAL, "1..%d staging fds and an out pointer", (int)kPullMaxPaths - 1);
     if (slot_bytes == 0 || slot_bytes % FMA_PAGE_BYTES || slots < 1 || slots > (int)kPullMaxSlots) return fail(FMA_EINVAL, "attach needs the slot shape the owner created");
-    std::lock_guard<std::mutex> op(e->op_mu);
+    OpLock op(e);
     DeviceGuard guard(e->device);
     cudaDeviceSynchronize();
     paths_release(e);
@@ -344,7 +344,7 @@ uint64_t fma_pull_next_generation(fma_engine_t* e) { return e ? e->pull_generati
 int fma_host_store_share(fma_engine_t* e, int* out_fd) {
     if (check_engine(e) != FMA_OK) return FMA_EINVAL;
     if (!out_fd) return fail(FMA_EINVAL, "out_fd is NULL");
-    std::lock_guard<std::mutex> op(e->op_mu);
+    OpLock op(e);
     RC(refuse_resident_handover(e));
     if (e->image_tier == FMA_TIER_FILE && image_in(e, ImageIn::AnyAsleep)) return fail(FMA_ESTATE, "the sleeping image is in a file: the file itself is the hand-over");
     if (e->host.fd < 0 || !e->host.base) return fail(FMA_ESTATE, "the host store is not shareable (set FMA_HOST_STORE_SHM=1 before the first sleep / host_reserve)");

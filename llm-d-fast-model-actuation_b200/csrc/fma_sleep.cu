@@ -501,13 +501,23 @@ struct SleepPlan {
     uint32_t copy_ops = 0;
     double copy_s = 0;
     ImageFile file;                   // FILE tier: the file this sleep writes, opened by size_store
+    // WRITE-BEHIND (the route's write_behind): from route_sleep on, `tier` is the host tier this sleep runs as, and wb_file the file
+    // the job will write, created and emptied by size_store
+    bool write_behind = false;
+    std::unique_ptr<ImageFile> wb_file;
     SleepPlan(fma_engine_t* e, int t, uint32_t f) : tier(t), flags(f), timer{e}, kt{e}, file(e) {}
     bool adopt() const { return (flags & kFlagAdopt) || clean || !W; }  // not a byte moves (the route is then Adopt)
 };
 
 fma_layout::SleepFacts sleep_facts(const fma_engine_t* e, const SleepPlan& p) {
-    return fma_layout::SleepFacts{p.tier, fma_layout::resolve_mode(e->cfg.mode, p.tier), e->cfg.pack != 0, !e->paths.empty(), e->mbox != nullptr,
-                                  (p.flags & kFlagAdopt) || !p.W, p.clean, p.partial, p.partial_packed, env_int("FMA_MULTIPATH_SLEEP", 1) != 0};
+    fma_layout::SleepFacts f{p.tier, fma_layout::resolve_mode(e->cfg.mode, p.tier), e->cfg.pack != 0, !e->paths.empty(), e->mbox != nullptr,
+                             (p.flags & kFlagAdopt) || !p.W, p.clean, p.partial, p.partial_packed, env_int("FMA_MULTIPATH_SLEEP", 1) != 0};
+    f.write_behind = (p.flags & FMA_FLAG_WRITE_BEHIND) != 0;
+    f.host_store = e->host.base != nullptr;
+    f.store_shared = e->host.shared;
+    f.store_cap = e->host.cap;
+    f.stored = p.W;   // (the PACKED size once K4p has run: route_sleep)
+    return f;
 }
 
 // `path` is a file of an image of store_bytes (plus the descriptor tail)
@@ -678,6 +688,7 @@ int route_sleep(fma_engine_t* e, SleepPlan& p) {
     } else if (p.route.wants_probe) {
         if (!p.pre_planned) RC(plan_packed_image(e, p.ex, p.W, &p.pk_off, &p.pk_bytes, &p.Wp, &p.packed));
         f.worth_packing = p.packed;
+        f.stored = p.Wp;
         p.route = fma_layout::sleep_route(f);
     } else {  // (a plan of the resident split is dropped)
         p.packed = false;
@@ -690,6 +701,11 @@ int route_sleep(fma_engine_t* e, SleepPlan& p) {
         e->img_bytes = p.packed ? std::move(p.pk_bytes) : std::vector<uint32_t>();
     }
     if (kept || p.packed) e->image_bytes = p.W;  // the layout is indexed by image page: valid from here on, also if the sleep fails
+    if (p.route.wb_fallback != fma_layout::kWbTaken) e->tl_add("wb_fallback", p.route.wb_fallback, now_s(), now_s(), p.Wp);
+    if (p.route.write_behind) {   // a host-tier sleep from here on; the file is written behind it
+        p.write_behind = true;
+        p.tier = FMA_TIER_HOST;
+    }
     return FMA_OK;
 }
 
@@ -702,12 +718,20 @@ int open_sleep_file(fma_engine_t* e, SleepPlan& p) {
     return FMA_OK;
 }
 
+// WRITE-BEHIND: the file the job writes is checked for room and emptied now, before anything is released, as the file tier does
+int open_write_behind_file(fma_engine_t* e, SleepPlan& p) {
+    if (e->file_path.empty()) return fail(FMA_ESTATE, "the file tier needs fma_file_store(path) first");
+    p.wb_file = std::make_unique<ImageFile>(e);
+    return p.wb_file->create(e->file_path, p.Wp);
+}
+
 // 5. a store of the tier that holds Wp bytes
 int size_store(fma_engine_t* e, SleepPlan& p) {
     if (!p.W) return FMA_OK;
     if (p.tier == FMA_TIER_HOST && p.adopt()) {
         if (!e->host.base) return fail(FMA_ESTATE, "adopt without a store");  // the adopted store IS the image: never re-sized
     } else if (p.tier == FMA_TIER_HOST) {
+        if (p.write_behind) RC(open_write_behind_file(e, p));   // (the route saw a private store that fits: nothing is pinned below)
         if (e->host.shared) {  // this sleep writes: leave the shared image to its other holders and take a private store
             invalidate_shadows(e);
             host_store_free(e->host);
@@ -881,11 +905,16 @@ int do_sleep(fma_engine_t* e, uint64_t offload_mask, int tier, uint32_t flags) {
 
     // ---- unmapper thread (types above): cuMemUnmap runs UNDER the copy pipeline instead of after it ----
     Unmapper un(e);
-    ApplyUnmapped apply_unmapped{&un, e, &p.ex, tier};
+    ApplyUnmapped apply_unmapped{&un, e, &p.ex, p.tier};
     un.plan(p.ex, p.route.mode == FMA_MODE_STAGED);
     if (env_int("FMA_OVERLAP_UNMAP", 1) != 0) un.th = std::thread([&un] { un.run(); });
     RC(run_pipeline(e, p, un));
-    return finish_sleep(e, p, un, apply_unmapped, t_entry);
+    RC(finish_sleep(e, p, un, apply_unmapped, t_entry));
+    if (p.write_behind) {   // asleep in the host store: the file is written behind the call (nothing is, behind a failed sleep)
+        e->tl_add("wb_start", 0, now_s(), now_s(), p.Wp);
+        writeback_start(e, std::move(p.wb_file));
+    }
+    return FMA_OK;
 }
 
 }  // namespace fma_impl

@@ -129,6 +129,7 @@ class CuMemAllocator:
             offload_tags = (offload_tags,)
         assert isinstance(offload_tags, tuple)
         self._join_reserve()
+        self._check_writeback()
         import torch
 
         tier = _tier_from_env()
@@ -165,6 +166,7 @@ class CuMemAllocator:
             self._file_path = _file_tier_path()
             self.engine.file_store(self._file_path)
             atexit.register(self._remove_own_file)
+            atexit.register(self._finish_writeback)   # (runs first)
         deposit_host = (tier == L.FMA_TIER_HOST and os.environ.get("FMA_DEPOSIT_HOST_IMAGE") == "1" and os.environ.get("FMA_NODE_AGENT_SOCK")
                         and os.environ.get("FMA_HOST_STORE_SHM") == "1")
         if deposit_host:
@@ -176,7 +178,9 @@ class CuMemAllocator:
             # a deposited image (file, or host memfd the node agent may spill to a kept file) is adopted by another process, whose
             # wake checks it against these digests
             deposits = deposit_host or (tier == L.FMA_TIER_FILE and _deposits_file())
-            self.engine.sleep(offload_tags, tier=tier, flags=L.FMA_FLAG_VERIFY if deposits else 0)
+            # FMA_FILE_WRITE_BEHIND=1: into the host store pinned after load (or kept), the file written behind the sleep
+            behind = tier == L.FMA_TIER_FILE and _write_behind()
+            self.engine.sleep(offload_tags, tier=tier, flags=(L.FMA_FLAG_VERIFY if deposits else 0) | (L.FMA_FLAG_WRITE_BEHIND if behind else 0))
         except L.FmaError as e:
             # the file tier refused before releasing anything (no room on the disk, no HBM for its staging ring): the host tier works
             if tier != L.FMA_TIER_FILE or e.code not in (L.FMA_EIO, L.FMA_ENOMEM) or self.engine.is_sleeping():
@@ -192,7 +196,8 @@ class CuMemAllocator:
             from .parking import ParkingClient
 
             ParkingClient().deposit_host(self.engine, _instance_id(), _rank())
-        elif _deposits_file() and self.engine.stats()["tier"] == L.FMA_TIER_FILE and self.engine.stats()["sleep_bytes_copied"]:
+        elif _deposits_file() and ((self.engine.stats()["tier"] == L.FMA_TIER_FILE and self.engine.stats()["sleep_bytes_copied"])
+                                   or self._writing_behind()):
             self._deposit_file()
         st = self.engine.stats()
         total = st["sleep_bytes_offloaded"] + st["sleep_bytes_discarded"]
@@ -226,11 +231,16 @@ class CuMemAllocator:
                 ParkingClient().withdraw_file(_instance_id(), _rank())
             except Exception as e:      # noqa: BLE001
                 logger.warning("fma_b200: cannot withdraw the image file from the node agent (%s)", e)
+        self._check_writeback()
         self.engine.wake(tags)
         st = self.engine.stats()
         if st["wake_copy_seconds"] > 0:
             logger.info("fma_b200: wake %.3f s, H2D %.1f GB/s", st["wake_seconds"],
                         st["wake_bytes_restored"] / st["wake_copy_seconds"] / 1e9)
+        if _write_behind() and not st["host_store_bytes"] and not self.engine.is_sleeping():
+            # the write-behind committed and released the store: the next sleep needs one again, pinned off its critical path
+            self._join_reserve()
+            self._start_reserve()
 
     def move_image(self, tier: str) -> None:
         """Move this rank's sleeping image without waking it.  ``"file"`` demotes it to ``<FMA_FILE_DIR>/<instance id>-r<rank>.fmaimg``
@@ -331,7 +341,7 @@ class CuMemAllocator:
                 logger.info("fma_b200: %d remote wake path(s) through the node agent's helper GPUs", n)
             except Exception as e:      # noqa: BLE001
                 logger.warning("fma_b200: no remote wake paths (%s): host-tier wakes use the own link only", e)
-        if tag == "weights" and os.environ.get("FMA_PREPIN", "1") != "0" and _tier_from_env() == L.FMA_TIER_HOST:
+        if tag == "weights" and ((os.environ.get("FMA_PREPIN", "1") != "0" and _tier_from_env() == L.FMA_TIER_HOST) or _write_behind()):
             self._start_reserve()
 
     def _adopt_parked_image(self) -> bool:
@@ -419,6 +429,38 @@ class CuMemAllocator:
         except (RuntimeError, OSError) as e:
             logger.warning("fma_b200: cannot deposit %s with the node agent (%s): it is removed when this process exits", self._file_path, e)
 
+    def _writing_behind(self) -> bool:
+        """A write-behind job of the last sleep is writing this rank's file, or has moved the image there already."""
+        if not _write_behind():
+            return False
+        try:
+            return self.engine.writeback(0.0)[0] == 1 or self.engine.stats()["tier"] == L.FMA_TIER_FILE
+        except L.FmaError as e:
+            self._warn_writeback(e)
+            return False
+
+    def _check_writeback(self) -> None:
+        """A failed write-behind is reported once: the image then sleeps on in host DRAM."""
+        if not _write_behind():
+            return
+        try:
+            self.engine.writeback(0.0)
+        except L.FmaError as e:
+            self._warn_writeback(e)
+
+    def _warn_writeback(self, e: L.FmaError) -> None:
+        logger.warning("fma_b200: the sleeping image could not be written to %s (%s): it stays in host DRAM (%.2f GiB pinned)",
+                       self._file_path, e.message, self.engine.stats()["host_store_bytes"] / 1024**3)
+
+    def _finish_writeback(self) -> None:
+        """At exit, before the engine goes: a deposited file a write-behind job still writes is completed (destroying the engine
+        would cancel the job, and the node agent would find an empty file)."""
+        if self._file_deposited:
+            try:
+                self.engine.writeback(None)
+            except L.FmaError as e:
+                self._warn_writeback(e)
+
     def _remove_own_file(self) -> None:
         """At exit: this rank's image file goes, unless a deposit with the node agent stands (the agent owns the file then)."""
         if self._file_path is not None and not self._file_deposited:
@@ -456,6 +498,12 @@ def _instance_id() -> str:
 def _deposits_file() -> bool:
     """FMA_DEPOSIT_FILE_IMAGE=1 (with FMA_TIER=file and a node agent): file-tier images are deposited with the agent."""
     return os.environ.get("FMA_DEPOSIT_FILE_IMAGE") == "1" and bool(os.environ.get("FMA_NODE_AGENT_SOCK")) and _tier_from_env() == L.FMA_TIER_FILE
+
+
+def _write_behind() -> bool:
+    """FMA_FILE_WRITE_BEHIND=1 (with FMA_TIER=file): sleeps return once the image is in the host store, pinned in the background after
+    load and after a wake whose store was released; the file is written behind them (FMA_FLAG_WRITE_BEHIND)."""
+    return os.environ.get("FMA_FILE_WRITE_BEHIND") == "1" and _tier_from_env() == L.FMA_TIER_FILE
 
 
 def _rank() -> int:

@@ -342,6 +342,15 @@ class Engine:
         engine must hold the same segment sequence for ``tags``.  Reads only the descriptor; ``wake`` streams the data."""
         check(self._lib.fma_image_adopt_file(self._h, path.encode(), self.tag_mask(tags), flags))
 
+    def writeback(self, timeout_s: float | None = 0.0) -> tuple[int, int]:
+        """The last write-behind job (``sleep(tier=FMA_TIER_FILE, flags=FMA_FLAG_WRITE_BEHIND)``), after waiting up to ``timeout_s``
+        seconds for it (0 polls, None waits until it ends): (1, bytes not yet written) while it writes, (0, 0) once it committed
+        (the image sleeps in the file tier), was pre-empted by another call, or when none was started.  Raises FmaError, once, for
+        a job whose write failed: the image then still sleeps in the host tier."""
+        pending = C.c_uint64()
+        state = check(self._lib.fma_image_writeback(self._h, -1.0 if timeout_s is None else float(timeout_s), C.byref(pending)))
+        return state, int(pending.value)
+
     @staticmethod
     def image_file_info(path: str) -> dict:
         """What the image file at ``path`` holds, from its descriptor tail alone (fma_image_file_info): no engine, no GPU.  Keys:
