@@ -304,6 +304,15 @@ func (e *Engine) MoveImage(tier int) error {
 	return nil
 }
 
+// MoveImageFlags is MoveImage with fma_image_move_flags' flags.  FlagWriteBehind demotes a host-tier image to the file tier behind
+// the call: the write-behind job writes the file and commits, Writeback waits for it, and any later call pre-empts it.
+func (e *Engine) MoveImageFlags(tier int, flags uint32) error {
+	if rc := C.fma_image_move_flags(e.h, C.int(tier), C.uint32_t(flags)); rc != 0 {
+		return lastErr(rc)
+	}
+	return nil
+}
+
 // PrefetchImage copies the tail of the sleeping image, up to `bytes` of stored bytes (rounded down to 2 MiB), from host DRAM or
 // its file into this GPU's HBM ahead of a wake, without waking it; the next Wake moves only the rest over the link.  0 frees that
 // HBM again.  Stats().prefetched_bytes reports what the copy holds.

@@ -356,8 +356,25 @@ FMA_API int  fma_image_file_info(const char* path, fma_image_file_info_t* out);
  * the host store or parking buffer (a peer's or an attached one included) that it would have replaced kept, a destination file
  * emptied (never with a descriptor).  A replaced store or buffer is released only once the move has succeeded.  Only the engine's own streams and events are synchronised, so another
  * engine of the process may serve meanwhile; host <-> file moves make no CUDA call beyond pinning a host store they create.  fma_timeline: op "move", rows file_io,
- * copies_landed (the copy engines ran) and total (bytes = image_store_bytes). */
+ * copies_landed (the copy engines ran) and total (bytes = image_store_bytes).
+ * fma_image_move(e, tier) is fma_image_move_flags(e, tier, 0). */
 FMA_API int  fma_image_move(fma_engine_t* e, int tier);
+/* fma_image_move with flags.  0: fma_image_move.  FMA_FLAG_WRITE_BEHIND (the only other flag; any other bit: FMA_EINVAL): a
+ * DEMOTION that does not hold the operation lock for the disk write.  A host-tier image goes to FMA_TIER_FILE behind the call: the
+ * synchronous move's refusals come first, with its codes and the engine unchanged (nothing asleep, a mapped backed-up segment, a
+ * resident share, no fma_file_store, no room on the filesystem (fstatvfs), a file that cannot be created); then a shared host store
+ * (fma_host_store_share, fma_image_export) is refused with FMA_ESTATE, because its bytes are not this engine's alone to release.
+ * The flag with any other pair of tiers is FMA_EINVAL.  Otherwise the file is emptied, the write-behind job of a write-behind sleep
+ * (see FMA_FLAG_WRITE_BEHIND) starts over the host store that already holds the image, and the call returns: no byte is copied on
+ * the caller's thread.  The job pwrites the store, seals the file (fdatasync, descriptor, fdatasync) and commits under the operation
+ * lock to the state fma_image_move(FMA_TIER_FILE) followed by fma_host_release leaves: every backed-up segment and fma_stats_t.tier
+ * report FMA_TIER_FILE, host_store_bytes is 0, K3 digests travel with the image, and a prefetched copy is kept.  Until then the image
+ * is a host-tier image in every respect.  Pre-emption, failures and fma_image_writeback are exactly those of a write-behind sleep: a
+ * call that takes the operation lock cancels the job and sees a host-tier image with its store kept and the file emptied (a wake
+ * during the demotion is a host-tier wake); a failed write leaves the image in the host tier, the store kept, the file emptied, and
+ * is reported once by fma_image_writeback.  fma_timeline: op "move", rows wb_start and total (bytes 0); the commit or cancel records
+ * op "writeback". */
+FMA_API int  fma_image_move_flags(fma_engine_t* e, int tier, uint32_t flags);
 
 /* Check the sleeping image against the K3 digests it carries, where it lies (host store, parking buffer, resident share, file),
  * without mapping a segment.  Returns the number of segments whose stored bytes do not match (0 = intact) and writes up to `cap`

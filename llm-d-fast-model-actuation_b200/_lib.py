@@ -148,6 +148,7 @@ _PROTOTYPES = {
     "fma_image_writeback": (C.c_int, [C.c_void_p, C.c_double, C.POINTER(C.c_uint64)]),
     "fma_image_file_info": (C.c_int, [C.c_char_p, C.POINTER(fma_image_file_info_t)]),
     "fma_image_move": (C.c_int, [C.c_void_p, C.c_int]),
+    "fma_image_move_flags": (C.c_int, [C.c_void_p, C.c_int, C.c_uint32]),
     "fma_image_verify": (C.c_int, [C.c_void_p, C.POINTER(C.c_int), C.c_int]),
     "fma_image_prefetch": (C.c_int, [C.c_void_p, C.c_uint64]),
     "fma_set_option": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int64]),

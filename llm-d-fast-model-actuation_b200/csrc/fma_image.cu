@@ -912,8 +912,11 @@ int fma_image_adopt_parked(fma_engine_t* e, const void* desc, size_t desc_bytes,
 }
 
 // ---- moving a sleeping image to another tier (see include/fma_engine.h) -------------------------------------------------
-int fma_image_move(fma_engine_t* e, int tier) {
+int fma_image_move(fma_engine_t* e, int tier) { return fma_image_move_flags(e, tier, 0); }
+
+int fma_image_move_flags(fma_engine_t* e, int tier, uint32_t flags) {
     if (check_engine(e) != FMA_OK) return FMA_EINVAL;
+    if (flags & ~FMA_FLAG_WRITE_BEHIND) return fail(FMA_EINVAL, "an image move takes no flag but FMA_FLAG_WRITE_BEHIND");
     OpLock op(e);
     const int from = e->image_tier;
     fma_layout::MoveFacts facts{};
@@ -922,6 +925,8 @@ int fma_image_move(fma_engine_t* e, int tier) {
     facts.prepared = tier == FMA_TIER_PEER ? e->park.va && e->park.device != e->device && e->park.bytes >= e->image_store_bytes
                    : tier == FMA_TIER_FILE ? !e->file_path.empty()
                                            : true;
+    facts.write_behind = (flags & FMA_FLAG_WRITE_BEHIND) != 0;
+    facts.store_shared = e->host.shared || e->host.fd_handed_out;
     const fma_layout::MoveRoute route = fma_layout::move_route(from, tier, facts);
     if (route.error != FMA_OK) return fail(route.error, "image move from tier %d to tier %d: %s", from, tier, route.why);
 
@@ -929,6 +934,14 @@ int fma_image_move(fma_engine_t* e, int tier) {
     RC(flush_kernel_times(e));
     const double t_entry = now_s();
     e->tl_begin("move", t_entry);
+    if (route.pipe == fma_layout::MovePipeKind::HostFileBehind) {   // the file checked for room and emptied, then written behind the call
+        auto file = std::make_unique<ImageFile>(e);
+        RC(file->create(e->file_path, e->image_store_bytes));
+        e->tl_add("wb_start", 0, now_s(), now_s(), e->image_store_bytes);
+        writeback_start(e, std::move(file));
+        e->tl_add("total", 0, t_entry, now_s(), 0);
+        return FMA_OK;
+    }
     MoveState ms(e);
     const int rc = run_move(e, route.pipe, from, tier, ms);
     if (rc != FMA_OK) {

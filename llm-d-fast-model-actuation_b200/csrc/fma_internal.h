@@ -160,6 +160,8 @@ struct HostStore {
     int fd = -1;                // memfd backing (FMA_HOST_STORE_SHM=1 or an adopted image); -1 = anonymous memory
     bool shared = false;        // somebody else may hold this image too (exported, or adopted in place): it is READ-ONLY from
                                 // now on — a sleep that has to write gets a fresh private store first (copy-on-write per store)
+    bool fd_handed_out = false; // fma_host_store_share gave its memfd to a node-level owner, who may read it: a demotion
+                                // (fma_image_move_flags, FMA_FLAG_WRITE_BEHIND) may not release it
     size_t map_bytes = 0;       // bytes mapped at base (cap + descriptor tail for memfd stores)
     // NUMA placement by byte range (MULTI-PATH wake: each path pulls the part of the image that lives on ITS GPU's node, so no
     // path drags its share across the socket interconnect); one range covering everything otherwise

@@ -357,13 +357,16 @@ inline WakeRoute wake_route(const WakeFacts& f) {
 
 // ---- which copy a move of a sleeping image between tiers runs (fma_image_move) ----
 // Park: the parking buffer, of the peer tier or the local one.  Every tier stores the image in one layout, so a move is a byte copy.
-enum class MovePipeKind { HostPark, ParkHost, HostFile, FileHost, ParkFile, FilePark, Refused };
+// HostFileBehind: host -> file with FMA_FLAG_WRITE_BEHIND, the write-behind job writing the host store after the call returns.
+enum class MovePipeKind { HostPark, ParkHost, HostFile, FileHost, ParkFile, FilePark, Refused, HostFileBehind };
 
 struct MoveFacts {
     bool asleep;          // a segment with a backup is unmapped
     bool backup_mapped;   // a segment with a backup is mapped (a KEEP_BACKUP wake, a partly woken image)
     bool resident;        // part of the image sleeps in a resident share
     bool prepared;        // the destination is ready: PEER, a peer parking buffer that holds the image; FILE, a path (HOST and LOCAL: always)
+    bool write_behind = false;   // FMA_FLAG_WRITE_BEHIND was passed (fma_image_move_flags)
+    bool store_shared = false;   // the host store is shared (fma_host_store_share, a deposit): not this engine's alone to release
 };
 struct MoveRoute {
     MovePipeKind pipe;
@@ -382,9 +385,14 @@ inline MoveRoute move_route(int from, int to, const MoveFacts& f) {
     if (from < FMA_TIER_HOST || from > FMA_TIER_FILE) return refuse(FMA_EINVAL, "the image's tier is unknown");
     if (to == from) return refuse(FMA_EINVAL, "the image already sleeps in that tier");
     if (is_park_tier(from) && is_park_tier(to)) return refuse(FMA_EINVAL, "there is one parking buffer: no move between the peer and local tiers");
+    if (f.write_behind && !(from == FMA_TIER_HOST && to == FMA_TIER_FILE)) return refuse(FMA_EINVAL, "a write-behind move takes a host-tier image to the file tier only");
     if (!f.prepared)
         return refuse(FMA_ESTATE, to == FMA_TIER_FILE ? "a move to the file tier needs fma_file_store(path) first"
                                                       : "a move to the peer tier needs a peer parking buffer that holds the image (fma_peer_reserve / fma_peer_attach)");
+    if (f.write_behind) {
+        if (f.store_shared) return refuse(FMA_ESTATE, "the host store is shared: its bytes are not this engine's alone to release behind a write");
+        return MoveRoute{MovePipeKind::HostFileBehind, FMA_OK, ""};
+    }
     if (from == FMA_TIER_HOST) return MoveRoute{to == FMA_TIER_FILE ? MovePipeKind::HostFile : MovePipeKind::HostPark, FMA_OK, ""};
     if (from == FMA_TIER_FILE) return MoveRoute{to == FMA_TIER_HOST ? MovePipeKind::FileHost : MovePipeKind::FilePark, FMA_OK, ""};
     return MoveRoute{to == FMA_TIER_HOST ? MovePipeKind::ParkHost : MovePipeKind::ParkFile, FMA_OK, ""};

@@ -350,6 +350,7 @@ int fma_host_store_share(fma_engine_t* e, int* out_fd) {
     if (e->host.fd < 0 || !e->host.base) return fail(FMA_ESTATE, "the host store is not shareable (set FMA_HOST_STORE_SHM=1 before the first sleep / host_reserve)");
     const int fd = dup(e->host.fd);
     if (fd < 0) return fail(FMA_ENOMEM, "dup failed: %s", strerror(errno));
+    e->host.fd_handed_out = true;
     *out_fd = fd;
     return FMA_OK;
 }

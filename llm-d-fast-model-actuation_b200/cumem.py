@@ -30,7 +30,9 @@ import gc
 import json
 import logging
 import os
+import socket
 import threading
+import time
 from contextlib import contextmanager
 from typing import Any
 
@@ -107,6 +109,12 @@ class CuMemAllocator:
         # MULTI-PATH wake across processes (FMA_REMOTE_PATHS=k): the node agent's helper GPUs pull for this instance; that needs the
         # host store as a memfd the agent can map, so the switch is thrown before the store is first reserved
         self._remote = None
+        # FMA_NODE_SLEEPER_DRAM_GIB (with a node agent): the agent's host-memory budget may demote / promote this rank's image
+        self._ctl_lock = threading.Lock()          # this rank's sleep and wake against the agent's commands
+        self._channel: "_SleeperChannel | None" = None
+        self._slept_at = 0.0
+        self._report_lock = threading.Lock()       # one report at a time, each read and sent together: the agent sees them in order
+        self._waiting = False                      # a waiter thread reports the end of the write-behind job (under _report_lock)
         if int(os.environ.get("FMA_REMOTE_PATHS", "0") or 0) > 0 and os.environ.get("FMA_NODE_AGENT_SOCK"):
             os.environ["FMA_HOST_STORE_SHM"] = "1"
 
@@ -123,6 +131,17 @@ class CuMemAllocator:
 
     # ---- hot path ----------------------------------------------------------------------
     def sleep(self, offload_tags: tuple[str, ...] | str | None = None) -> None:
+        if self._channel is None and os.environ.get("FMA_NODE_AGENT_SOCK") and os.environ.get("FMA_NODE_SLEEPER_DRAM_GIB"):
+            try:
+                self._channel = _SleeperChannel(self)
+            except OSError as e:
+                logger.warning("fma_b200: cannot reach the node agent's sleeper budget (%s): this rank is not demoted", e)
+        with self._ctl_lock:
+            self._sleep(offload_tags)
+            self._slept_at = time.time()
+        self._report()
+
+    def _sleep(self, offload_tags: tuple[str, ...] | str | None) -> None:
         if offload_tags is None:
             offload_tags = (CuMemAllocator.default_tag,)
         elif isinstance(offload_tags, str):
@@ -216,6 +235,11 @@ class CuMemAllocator:
         torch.cuda.empty_cache()
 
     def wake_up(self, tags: list[str] | None = None) -> None:
+        with self._ctl_lock:
+            self._wake_up(tags)
+        self._report()
+
+    def _wake_up(self, tags: list[str] | None) -> None:
         moves_an_image = tags is None or any(t != "kv_cache" for t in tags)   # the kv cache is discarded on sleep: waking it copies nothing
         if self._remote is not None and moves_an_image and self.engine.is_sleeping() and _tier_from_env() == L.FMA_TIER_HOST:
             try:    # the owner's helpers serve the wake that follows; if the request fails, the instance's own link does it all
@@ -248,10 +272,7 @@ class CuMemAllocator:
         host DRAM ahead of a wake and leaves the file to the exit hook."""
         self._join_reserve()
         if tier == "file":
-            if self._file_path is None:
-                self._file_path = _file_tier_path()
-                self.engine.file_store(self._file_path)
-                atexit.register(self._remove_own_file)
+            self._name_own_file()
             self.engine.move_image(L.FMA_TIER_FILE)
             self.engine.host_release()
         elif tier == "host":
@@ -259,6 +280,90 @@ class CuMemAllocator:
         else:
             raise L.FmaError(L.FMA_EINVAL, f"move_image: tier {tier!r} is not 'host' or 'file'")
         logger.info("fma_b200: sleeping image moved to the %s tier (%.2f GiB)", tier, self.engine.stats()["image_store_bytes"] / 1024**3)
+        self._report()
+
+    def _name_own_file(self) -> None:
+        if self._file_path is None:
+            self._file_path = _file_tier_path()
+            self.engine.file_store(self._file_path)
+            atexit.register(self._remove_own_file)
+
+    # ---- the node agent's host-memory budget (FMA_NODE_SLEEPER_DRAM_GIB) --------------------------------------------------
+    def _agent_command(self, op: str) -> None:
+        """``demote``: the image goes to this rank's file behind the call (``move_image(file, behind=True)``), and the state is
+        reported again when the write commits, is cancelled or fails.  ``promote``: back to host DRAM (synchronous).  A command
+        that finds the rank awake is a no-op.  The lock only orders the command against a sleep or wake in progress; the engine
+        call runs outside it, so a wake that comes meanwhile pre-empts a demotion (or waits for a promotion) in the engine."""
+        with self._ctl_lock:
+            asleep = self.engine.is_sleeping()
+        if not asleep or op not in ("demote", "promote"):
+            self._report(answer=op)
+            return
+        try:
+            if op == "demote":
+                self._name_own_file()
+                self.engine.move_image(L.FMA_TIER_FILE, behind=True)
+            else:
+                self.engine.move_image(L.FMA_TIER_HOST)
+        except L.FmaError as e:
+            logger.info("fma_b200: the node agent's %s of this rank's image was refused: %s", op, e)
+            self._report(answer=op, error=e)
+            return
+        self._report(answer=op)
+
+    def _await_writeback(self) -> None:
+        """A write-behind job is writing (a write-behind sleep's, or a demotion's): report again once it has committed, been
+        cancelled or failed, so the agent's books never keep a rank demoting."""
+        while True:
+            failed = None
+            try:
+                self.engine.writeback(None)     # (waits without pre-empting)
+            except L.FmaError as e:
+                self._warn_writeback(e)
+                failed = "demote"
+            if not self._report(failed=failed, waiter=True):   # (a job started meanwhile: wait for that one too)
+                return
+
+    def _report(self, answer: str | None = None, error: L.FmaError | None = None, failed: str | None = None, waiter: bool = False) -> bool:
+        """This rank's sleeper_state for the agent's budget: host_bytes is the pinned host store, a write-behind reserve held
+        while awake included.  ``failed``: a write-behind write failed (the agent does not demote this rank again until it sleeps
+        again).  While a job writes, a waiter reports its end."""
+        ch = self._channel
+        if ch is None:
+            if waiter:
+                self._waiting = False
+            return False
+        with self._report_lock:
+            return self._send_report(ch, answer, error, failed, waiter)
+
+    def _send_report(self, ch: "_SleeperChannel", answer, error, failed, waiter: bool) -> bool:
+        try:
+            demoting = self.engine.writeback(0.0)[0] == 1
+        except L.FmaError as e:
+            self._warn_writeback(e)
+            demoting, failed = False, "demote"
+        if waiter:
+            self._waiting = demoting
+        elif demoting and not self._waiting:
+            self._waiting = True
+            threading.Thread(target=self._await_writeback, name="fma-writeback-waiter", daemon=True).start()
+        st = self.engine.stats()
+        msg = {"op": "sleeper_state", "instance": _instance_id(), "rank": _rank(), "asleep": self.engine.is_sleeping(),
+               "tier": _TIER_NAMES.get(st["tier"], str(st["tier"])), "host_bytes": st["host_store_bytes"], "image_bytes": st["image_store_bytes"],
+               "slept_at": self._slept_at, "demoting": demoting, "file_dir": os.environ.get("FMA_FILE_DIR", ""),
+               "shared": os.environ.get("FMA_DEPOSIT_HOST_IMAGE") == "1"}
+        if answer:
+            msg["answer"] = answer
+        if error is not None:
+            msg["error"], msg["code"] = error.message[:200], error.code
+        if failed:
+            msg["failed"] = failed
+        try:
+            ch.send(msg)
+        except OSError as e:
+            logger.warning("fma_b200: the node agent's sleeper budget is gone (%s)", e)
+            self._channel = None
+        return demoting
 
     def verify_image(self) -> bool:
         """Check this rank's sleeping image where it lies (host DRAM, disk or parking HBM) against the digests recorded when it
@@ -479,6 +584,7 @@ class CuMemAllocator:
                 self.engine.host_reserve(nbytes)
             except L.FmaError as e:  # sleep will retry and report
                 logger.warning("background host_reserve failed: %s", e)
+            self._report()   # (the node agent's budget counts the pinned store)
 
         self._reserve_thread = threading.Thread(target=run, name="fma-prepin", daemon=True)
         self._reserve_thread.start()
@@ -493,6 +599,38 @@ def _instance_id() -> str:
     """The controller's instance ID (``"I" + base64url(sha256(...)) + "i"``, inference-server.go:801-829): the node agent passes it to
     its children as FMA_INSTANCE_ID; a bare process falls back to its pid."""
     return os.environ.get("FMA_INSTANCE_ID") or f"pid{os.getpid()}"
+
+
+_TIER_NAMES = {L.FMA_TIER_HOST: "host", L.FMA_TIER_PEER: "peer", L.FMA_TIER_LOCAL: "local", L.FMA_TIER_FILE: "file"}
+
+
+class _SleeperChannel:
+    """This rank's persistent connection to the node agent's host-memory budget (parking.py ``sleeper`` op): sleeper_state reports
+    go up, demote / promote commands come down and are run by a daemon thread, which owns the connection's reading end."""
+
+    def __init__(self, alloc: CuMemAllocator):
+        self._alloc = alloc
+        self._send_lock = threading.Lock()
+        self._sock = socket.socket(socket.AF_UNIX, socket.SOCK_STREAM)
+        self._sock.connect(os.environ["FMA_NODE_AGENT_SOCK"])
+        self._sock.sendall((json.dumps({"op": "sleeper", "instance": _instance_id(), "rank": _rank()}) + "\n").encode())
+        self._rfile = self._sock.makefile("rb")
+        rep = json.loads(self._rfile.readline() or b"{}")
+        if not rep.get("ok"):
+            self._sock.close()
+            raise OSError(rep.get("error", "the node agent keeps no sleeper budget"))
+        threading.Thread(target=self._run, name="fma-sleeper-channel", daemon=True).start()
+
+    def send(self, msg: dict) -> None:
+        with self._send_lock:
+            self._sock.sendall((json.dumps(msg) + "\n").encode())
+
+    def _run(self) -> None:
+        try:
+            for line in self._rfile:
+                self._alloc._agent_command(json.loads(line).get("op", ""))
+        except (OSError, ValueError) as e:
+            logger.warning("fma_b200: the node agent's sleeper channel closed (%s)", e)
 
 
 def _deposits_file() -> bool:

@@ -363,11 +363,19 @@ class Engine:
         return {"image_bytes": out.image_bytes, "weight_bytes": out.weight_bytes, "n_segments": out.n_segments, "version": out.version,
                 "packed": bool(out.packed), "digests": bool(out.digests), "tags": [out.tags[i].value.decode() for i in range(out.n_tags)]}
 
-    def move_image(self, tier: int) -> None:
+    def move_image(self, tier: int, behind: bool = False) -> None:
         """Move the sleeping image to ``tier`` without waking it (fma_image_move): host DRAM, a file (``file_store`` first), a peer's
         parking buffer (``peer_reserve`` first) or this GPU's.  The source store stays allocated until ``host_release`` /
-        ``peer_release``; a source file is never touched."""
-        check(self._lib.fma_image_move(self._h, tier))
+        ``peer_release``; a source file is never touched.
+
+        ``behind=True`` (host tier to FMA_TIER_FILE only, fma_image_move_flags with FMA_FLAG_WRITE_BEHIND): returns once the file is
+        checked and emptied; the write-behind job writes it from the host store, then moves the image to the file tier and frees
+        the store.  ``writeback`` waits for it; any later call that takes the operation lock (a wake included) pre-empts it and
+        sees the host-tier image.  A shared host store is refused (FMA_ESTATE)."""
+        if behind:
+            check(self._lib.fma_image_move_flags(self._h, tier, L.FMA_FLAG_WRITE_BEHIND))
+        else:
+            check(self._lib.fma_image_move(self._h, tier))
 
     def verify_image(self) -> list[int]:
         """Check the sleeping image against the digests it carries, where it lies, without waking it (fma_image_verify): the

@@ -23,6 +23,8 @@ independent controller reconciles never do (SURVEY.md §3.4):
     POST /v2/node/swap {"sleep": idA, "wake": idB}     sleep(A) || wake(B): D2H of A and H2D of B on opposite PCIe directions
     GET  /v2/node/sleepers                             who sleeps where (for sleeper budgets)
     GET  /v2/node/images                               images kept for dead instances: peer HBM, host DRAM, disk (parking.py)
+    POST /v2/node/sleepers/{id}/promote                FMA_NODE_SLEEPER_DRAM_GIB: bring a demoted sleeper's image back to host DRAM ahead
+                                                       of an expected wake (409: it does not fit under the budget)
 
 Design differences from the reference (this is not a port): instances are forked by a single-threaded *fork server*
 that has pre-imported the serving stack (the reference forks from its asyncio server process), exits are observed by
@@ -218,6 +220,8 @@ class NodeAgent:
                     for var, n in (("FMA_KEEP_DISK_GIB", self.parking.keep_disk_bytes), ("FMA_KEEP_DRAM_GIB", self.parking.keep_dram_bytes)):
                         if n is not None:
                             extra_env[var] = str(n / (1 << 30))
+                if self.parking.sleeper_budget is not None:
+                    extra_env["FMA_NODE_SLEEPER_DRAM_GIB"] = str(self.parking.sleeper_budget.budget / (1 << 30))
             inst = _Instance(instance_id, cfg, self.log_dir)
             open(inst.log_path, "wb").close()
             inst.proc = self._ctx.Process(target=_child_main, args=(cfg.model_dump(exclude_none=True), inst.log_path, extra_env), daemon=False)
@@ -373,7 +377,20 @@ class NodeAgent:
             # what a sleeper costs in HBM, per GPU index, in MiB — the unit accelMemoryIsLowEnough compares against
             # (inference-server.go:1609-1636; budget = count x 4096 MiB, cmd/dual-pods-controller/main.go:72-74)
             res.update(self.parking.stats())
+        budget = self.parking.sleeper_budget if self.parking is not None else None
+        if budget is not None:   # FMA_NODE_SLEEPER_DRAM_GIB: what each live sleeper pins in host DRAM, and the node's sum
+            books = budget.sleepers()
+            for s in out:
+                s.update(books.get(s["instance_id"], {"tier": None, "host_bytes": 0, "demoting": False}))
+            res["sleeper_dram_bytes"] = budget.used()
+            res["sleeper_dram_budget_bytes"] = budget.budget
         return res
+
+    def promote(self, instance_id: str):
+        """Ask the ranks of a demoted sleeper to bring its image back to host DRAM (None: not a known sleeper; False: no room; else
+        the ranks asked, empty when none sleeps in the file tier)."""
+        budget = self.parking.sleeper_budget if self.parking is not None else None
+        return None if budget is None else budget.promote(instance_id)
 
     def images(self) -> dict:
         """Images kept for dead or future instances and the DRAM / disk budgets they count against (parking.py ``kept``)."""
@@ -551,6 +568,17 @@ def create_app(agent: NodeAgent) -> FastAPI:
     def images():
         return JSONResponse(agent.images())
 
+    @app.post("/v2/node/sleepers/{instance_id}/promote")
+    def promote(instance_id: str):
+        ranks = agent.promote(instance_id)
+        if ranks is None:
+            raise HTTPException(status_code=404, detail=f"no sleeper {instance_id} in the host-memory budget's books")
+        if ranks is False:
+            raise HTTPException(status_code=409, detail=f"the image of {instance_id} does not fit under FMA_NODE_SLEEPER_DRAM_GIB")
+        if not ranks:
+            return JSONResponse({"instance_id": instance_id, "promoting": False, "why": "no rank sleeps in the file tier (awake, or in host DRAM)"})
+        return JSONResponse({"instance_id": instance_id, "promoting": True, "ranks": ranks})
+
     return app
 
 
@@ -560,6 +588,12 @@ def keep_settings(env) -> dict:
     keep_dir = env.get("FMA_KEEP_DIR") or (os.path.join(env["FMA_FILE_DIR"], "kept") if env.get("FMA_FILE_DIR") else None)
     gib = lambda v: int(float(env[v]) * (1 << 30)) if env.get(v) else None    # noqa: E731
     return {"keep_dir": keep_dir, "keep_disk_bytes": gib("FMA_KEEP_DISK_GIB"), "keep_dram_bytes": gib("FMA_KEEP_DRAM_GIB")}
+
+
+def sleeper_budget_settings(env) -> dict:
+    """FMA_NODE_SLEEPER_DRAM_GIB (unset: no bound): the host bytes of live sleepers, demoted to disk and promoted back (parking.py
+    SleeperDramBudget)."""
+    return {"sleeper_dram_bytes": int(float(env["FMA_NODE_SLEEPER_DRAM_GIB"]) * (1 << 30)) if env.get("FMA_NODE_SLEEPER_DRAM_GIB") else None}
 
 
 def main() -> None:
@@ -587,7 +621,8 @@ def main() -> None:
 
             pynvml.nvmlInit()
             n_dev = pynvml.nvmlDeviceGetCount()
-        parking = ParkingService(os.path.join(a.log_dir, f"fma_node_agent.{os.getpid()}.sock"), n_devices=n_dev, **keep_settings(os.environ))
+        parking = ParkingService(os.path.join(a.log_dir, f"fma_node_agent.{os.getpid()}.sock"), n_devices=n_dev, **keep_settings(os.environ),
+                                 **sleeper_budget_settings(os.environ))
         parking.start()
     agent = NodeAgent(mock_gpus=a.mock_gpus, log_dir=a.log_dir, parking=parking)
     uvicorn.run(create_app(agent), host=a.host, port=a.port, log_level=a.log_level)

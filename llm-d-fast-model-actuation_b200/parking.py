@@ -30,6 +30,13 @@ Kept image files (opt-in: ``keep_dir``), so a deleted sleeper's next instance wa
     {"op": "lookup_done",   "instance": id, "rank": r[, "drop": true]}       -> {"ok": true}   ends the lease; drop: the file failed its digests
     {"op": "kept"}                                                           -> {"ok": true, "images": [...], "dram_bytes": ..., ...}
 
+Live sleepers' host memory (opt-in: ``sleeper_dram_bytes``, FMA_NODE_SLEEPER_DRAM_GIB; SleeperDramBudget), one persistent
+connection per rank, JSON lines both ways:
+
+    {"op": "sleeper", "instance": id, "rank": r}                             -> {"ok": true}, then the connection stays open:
+    up:   {"op": "sleeper_state", "asleep", "tier", "host_bytes", "image_bytes", "slept_at", "demoting", "file_dir", "shared"[, "answer", "error", "code"][, "failed"]}
+    down: {"op": "demote"} | {"op": "promote"}
+
 When an instance exits (``instance_exited``, from the node agent's child-exit path) with a file deposit standing, the file is kept
 if ``fma_image_file_info`` accepts it and every segment carries a digest: it is renamed into ``keep_dir``.  Any other file the
 instance deposited is unlinked.  Host memfds beyond ``keep_dram_bytes`` are spilled to kept files, oldest first; kept files beyond
@@ -94,14 +101,138 @@ def _parse_kept_name(name: str) -> Optional[Tuple[str, int]]:
     return urllib.parse.unquote(stem), int(rank)
 
 
+class SleeperDramBudget:
+    """FMA_NODE_SLEEPER_DRAM_GIB: the pinned host memory of a node's LIVE sleepers, the sum of the ``host_bytes`` each rank reports,
+    kept within a budget.  Each rank is its own sleeper, keyed (instance, rank).  Pure bookkeeping over the ranks' ``sleeper_state``
+    reports: ``send(key, op)`` delivers "demote" (the rank runs ``move_image(file, behind=True)``) or "promote" (``move_image(host)``)
+    and the rank answers with a report that carries ``answer``.
+
+    Demotion: while the sum is over budget, host-tier sleepers are demoted, least recently slept first; never an awake rank, one
+    already demoting or with a command in flight, one whose store is shared or deposited (``shared``), or one whose demotion was
+    refused or whose write failed since it last slept.  One demotion per file-tier directory (``file_dir``) at a time, so they do not split a disk.  A
+    rank's bytes stop counting only when it reports the commit (tier "file", host_bytes 0); while a demotion writes, its bytes are
+    set against the excess only so that no further rank is demoted for the same bytes.  A cancelled demotion (a wake cut it short)
+    reports host_bytes again, and the policy re-runs on every report.
+    Promotion: with no demotion writing and none needed, the most recently slept file-tier sleeper is promoted if its whole image
+    fits under the budget; one at a time (a promotion is synchronous in the rank); never one whose promotion failed since it last
+    slept.
+    A failure is remembered per operation until the rank sleeps again (a new ``slept_at``): a command answered with ``error``, or a
+    report with ``failed`` (a write-behind write that failed).  So neither a refusal nor a failing disk or pin is retried in a loop."""
+
+    def __init__(self, budget_bytes: int, send: Callable[[Tuple[str, int], str], None]):
+        self.budget = int(budget_bytes)
+        self._send = send
+        self._lock = threading.Lock()
+        self._books: Dict[Tuple[str, int], dict] = {}     # (instance, rank) -> its last report
+        self._pending: Dict[Tuple[str, int], str] = {}    # a command sent and not yet answered
+
+    def used(self) -> int:
+        with self._lock:
+            return sum(int(s["host_bytes"]) for s in self._books.values())
+
+    def report(self, state: dict) -> None:
+        key = (str(state["instance"]), int(state.get("rank", 0)))
+        with self._lock:
+            old = self._books.get(key, {})
+            s = dict(state)
+            # operations that failed since this sleep: not asked again until the rank sleeps again
+            s["failed_ops"] = set(old.get("failed_ops", ())) if old.get("slept_at") == s.get("slept_at") else set()
+            if state.get("answer") and state.get("error"):
+                s["failed_ops"].add(state["answer"])
+            if state.get("failed"):
+                s["failed_ops"].add(state["failed"])
+            self._books[key] = s
+            if state.get("answer"):
+                self._pending.pop(key, None)
+            cmds = self._plan()
+        self._deliver(cmds)
+
+    def drop(self, key: Tuple[str, int]) -> None:
+        """The rank's connection closed (its process exited): its bytes leave the books, which may leave room for a promotion."""
+        with self._lock:
+            self._books.pop(key, None)
+            self._pending.pop(key, None)
+            cmds = self._plan()
+        self._deliver(cmds)
+
+    def promote(self, instance: str):
+        """Promote every file-tier rank of ``instance`` ahead of an expected wake (an explicit request: also one whose promotion
+        failed before).  None: no such sleeper; False: its images do not fit under the budget (nothing is sent); else the ranks being
+        promoted (asked now or already), empty when none sleeps in the file tier (awake, or already in host DRAM)."""
+        with self._lock:
+            keys = [k for k in self._books if k[0] == instance]
+            if not keys:
+                return None
+            asleep_in_file = [k for k in keys if self._books[k].get("asleep") and self._books[k].get("tier") == "file"]
+            todo = [k for k in asleep_in_file if k not in self._pending]   # (a promotion in flight is not asked twice)
+            need = sum(int(self._books[k].get("image_bytes", 0)) for k in todo)
+            if sum(int(s["host_bytes"]) for s in self._books.values()) + need > self.budget:
+                return False
+            for k in todo:
+                self._pending[k] = "promote"
+        self._deliver([(k, "promote") for k in todo])
+        return [k[1] for k in asleep_in_file]
+
+    def sleepers(self) -> Dict[str, dict]:
+        """Per instance: the tier of its rank 0, its ranks' host bytes, and whether one of them is demoting."""
+        out: Dict[str, dict] = {}
+        with self._lock:
+            for (inst, rank), s in sorted(self._books.items()):
+                o = out.setdefault(inst, {"tier": s.get("tier"), "host_bytes": 0, "demoting": False})
+                o["host_bytes"] += int(s["host_bytes"])
+                o["demoting"] = o["demoting"] or bool(s.get("demoting")) or self._pending.get((inst, rank)) == "demote"
+        return out
+
+    def _in_flight(self, key) -> bool:
+        return bool(self._books[key].get("demoting")) or self._pending.get(key) == "demote"
+
+    def _plan(self) -> list:
+        cmds = []
+        used = sum(int(s["host_bytes"]) for s in self._books.values())
+        writing = [k for k in self._books if self._in_flight(k)]
+        excess = used - sum(int(self._books[k]["host_bytes"]) for k in writing) - self.budget
+        if excess > 0:
+            busy = {self._books[k].get("file_dir") for k in writing}
+            for k, s in sorted(self._books.items(), key=lambda kv: (kv[1].get("slept_at", 0), kv[0])):
+                if excess <= 0:
+                    break
+                if (not s.get("asleep") or s.get("tier") != "host" or k in self._pending or self._in_flight(k) or s.get("shared")
+                        or "demote" in s["failed_ops"] or s.get("file_dir") in busy or not int(s["host_bytes"])):
+                    continue
+                cmds.append((k, "demote"))
+                self._pending[k] = "demote"
+                busy.add(s.get("file_dir"))
+                excess -= int(s["host_bytes"])
+            return cmds
+        if writing or self._pending:
+            return cmds
+        for k, s in sorted(self._books.items(), key=lambda kv: (kv[1].get("slept_at", 0), kv[0]), reverse=True):
+            if (s.get("asleep") and s.get("tier") == "file" and "promote" not in s["failed_ops"]
+                    and used + int(s.get("image_bytes", 0)) <= self.budget):
+                cmds.append((k, "promote"))
+                self._pending[k] = "promote"
+                break
+        return cmds
+
+    def _deliver(self, cmds) -> None:
+        for key, op in cmds:
+            try:
+                self._send(key, op)
+            except OSError as e:            # the rank is gone: its connection's close drops it
+                logger.warning("fma_b200: cannot send %s to %s rank %d: %s", op, key[0], key[1], e)
+                with self._lock:
+                    self._pending.pop(key, None)
+
+
 class ParkingService:
     """Owner side.  ``make_buffer(device, nbytes)`` must return an object with ``.nbytes``, ``.device``, ``.export_fd()`` and
     ``.close()`` — ``fma_b200.ParkingBuffer`` in production."""
 
     def __init__(self, sock_path: str, n_devices: int, make_buffer: Optional[Callable] = None, keep_dir: Optional[str] = None,
-                 keep_disk_bytes: Optional[int] = None, keep_dram_bytes: Optional[int] = None):
+                 keep_disk_bytes: Optional[int] = None, keep_dram_bytes: Optional[int] = None, sleeper_dram_bytes: Optional[int] = None):
         """``keep_dir`` turns on kept image files (None: the file ops are refused and host deposits are unbounded, as before);
-        ``keep_disk_bytes`` / ``keep_dram_bytes`` bound the kept files and the deposited host memfds (None: no bound)."""
+        ``keep_disk_bytes`` / ``keep_dram_bytes`` bound the kept files and the deposited host memfds (None: no bound).
+        ``sleeper_dram_bytes`` bounds the host bytes of live sleepers (SleeperDramBudget; None: no bound, as before)."""
         self.sock_path = sock_path
         self.n_devices = n_devices
         if make_buffer is None:
@@ -133,6 +264,41 @@ class ParkingService:
         self._srv: Optional[socket.socket] = None
         self._thread: Optional[threading.Thread] = None
         self._stop = False
+        # live sleepers' host memory (opt-in): one persistent connection per rank ("sleeper" op), commands sent down it
+        self._sleeper_conns: Dict[Tuple[str, int], Tuple[socket.socket, threading.Lock]] = {}
+        self.sleeper_budget = SleeperDramBudget(sleeper_dram_bytes, self._send_sleeper) if sleeper_dram_bytes is not None else None
+
+    def _send_sleeper(self, key: Tuple[str, int], op: str) -> None:
+        if key not in self._sleeper_conns:
+            raise OSError(f"no connection from {key[0]} rank {key[1]}")
+        conn, lock = self._sleeper_conns[key]
+        with lock:
+            conn.sendall((json.dumps({"op": op}) + "\n").encode())
+
+    def _serve_sleeper(self, conn: socket.socket, instance: str, rank: int) -> None:
+        """A rank's persistent connection: its sleeper_state reports come up, demote / promote go down; its close (the process
+        exited) drops the rank from the budget's books."""
+        key = (instance, int(rank))
+        self._sleeper_conns[key] = (conn, threading.Lock())
+        conn.sendall((json.dumps({"ok": True}) + "\n").encode())
+        buf = b""
+        try:
+            while True:
+                more = conn.recv(1 << 16)
+                if not more:
+                    break
+                buf += more
+                while b"\n" in buf:
+                    line, buf = buf.split(b"\n", 1)
+                    msg = json.loads(line.decode())
+                    if msg.get("op") == "sleeper_state":
+                        self.sleeper_budget.report(dict(msg, instance=instance, rank=int(rank)))
+        except OSError:
+            pass
+        finally:
+            if self._sleeper_conns.get(key, (None,))[0] is conn:
+                del self._sleeper_conns[key]
+            self.sleeper_budget.drop(key)
 
     # ---- bookkeeping ------------------------------------------------------------------------------------------
     def parked_bytes_per_device(self) -> Dict[int, int]:
@@ -629,6 +795,9 @@ class ParkingService:
                 rep = {"ok": True}
             elif op == "kept":
                 rep = {"ok": True, **self.kept()}
+            elif op == "sleeper" and self.sleeper_budget is not None:
+                self._serve_sleeper(conn, req["instance"], req.get("rank", 0))
+                return
             else:
                 rep = {"ok": False, "error": f"unknown op {op!r}"}
             socket.send_fds(conn, [(json.dumps(rep) + "\n").encode()], fds)
